@@ -105,6 +105,8 @@ int mp3b200_encode_streams(int channels, int samplerate, int kbps, int nstreams,
  * quantizer passes; first pass by kernel: [8] k_q_prepare, [9] k_q_search (gr0 + gr1), [10] k_q_outer (gr0 + gr1),
  * [11] k_q_finish (gr0 + gr1), [12] k_q_pack, [13] the re-validation folded into the first pass (verify + repaired
  * searches / rate loops of the few frames whose speculated start did not stand); [14..15] reserved (0).
+ * More than 65535 streams run as consecutive launches of at most 65535 streams: the times are summed over them, [7] is the
+ * largest pass count of any of them.
  * The call runs on a stream of its own that first waits for work already queued on the legacy default stream (where torch /
  * plain CUDA callers produced d_pcm) and returns after that stream has drained. */
 int mp3b200_encode_streams_device(int channels, int samplerate, int kbps, int nstreams, const int16_t* d_pcm,

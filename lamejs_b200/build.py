@@ -25,9 +25,10 @@ def needs_build():
     return any(os.path.getmtime(os.path.join(CSRC, d)) > t for d in DEPS)
 
 
-def build(force=False, verbose=False, variant=None, defines=()):
-    """variant/defines: tuning builds (libmp3b200_<variant>.so with -D flags), selected at run time by MP3B200_LIB."""
-    out = LIB if variant is None else os.path.join(HERE, "libmp3b200_%s.so" % variant)
+def build(force=False, verbose=False, variant=None, defines=(), out_dir=None):
+    """variant/defines: tuning or test builds (libmp3b200_<variant>.so with -D flags, in out_dir or next to the default
+    library), selected at run time by MP3B200_LIB."""
+    out = LIB if variant is None else os.path.join(out_dir or HERE, "libmp3b200_%s.so" % variant)
     if variant is None and not force and not needs_build():
         return LIB
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

@@ -460,6 +460,18 @@ __global__ void k_attack_prepass(const Mp3Tables* __restrict__ T, const StreamDe
  * The result equals the sequential scan exactly; the worst case degenerates to it.  One block per stream. */
 #define SCAN_FRAMES 16
 #define SCAN_THREADS 1024
+/* The in-state every chunk but a stream's first starts from: lastAttacks and blocktype_old of both channels, and the ATH
+ * (adjust, adjustLimit) pair.  Only the number of redo rounds depends on it (tests/test_gpu_speculation.py builds the
+ * library with wrong guesses and checks the bytes). */
+#ifndef SCAN_GUESS_LA
+#define SCAN_GUESS_LA 0
+#endif
+#ifndef SCAN_GUESS_BT
+#define SCAN_GUESS_BT BT_NORM
+#endif
+#ifndef SCAN_GUESS_ATH
+#define SCAN_GUESS_ATH 1.0
+#endif
 struct ScanChunk { int fsm_in, fsm_out, dirty_fsm, dirty_ath; double ath_in[2], ath_out[2]; };
 
 __device__ __forceinline__ int fsm_pack(int la0, int la1, int o0, int o1) { return la0 | (la1 << 2) | (o0 << 4) | (o1 << 6); }
@@ -565,9 +577,9 @@ k_stream_scan(const Mp3Tables* __restrict__ T, StreamDesc* __restrict__ streams,
   const int tid = threadIdx.x;
   for (int c = tid; c < nchunks; c += SCAN_THREADS) {
     ck[c].fsm_in = c == 0 ? fsm_pack(sd.last_attacks[0], sd.last_attacks[1], sd.blocktype_old[0], sd.blocktype_old[1])
-                          : fsm_pack(0, 0, BT_NORM, BT_NORM);
-    ck[c].ath_in[0] = c == 0 ? sd.ath_adjust : 1.0;
-    ck[c].ath_in[1] = c == 0 ? sd.ath_adjust_limit : 1.0;
+                          : fsm_pack(SCAN_GUESS_LA, SCAN_GUESS_LA, SCAN_GUESS_BT, SCAN_GUESS_BT);
+    ck[c].ath_in[0] = c == 0 ? sd.ath_adjust : SCAN_GUESS_ATH;
+    ck[c].ath_in[1] = c == 0 ? sd.ath_adjust_limit : SCAN_GUESS_ATH;
     ck[c].dirty_fsm = ck[c].dirty_ath = 1;
   }
   for (;;) {

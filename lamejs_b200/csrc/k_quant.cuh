@@ -194,6 +194,12 @@ __device__ unsigned long long g_qstats[16];
 #ifndef Q_SPEC_STEP
 #define Q_SPEC_STEP 32
 #endif
+#ifndef Q_SPEC_GR1_STEP
+#define Q_SPEC_GR1_STEP 2      /* the start step a speculated MPEG-1 frame hands its gr1 search (k_q_search) */
+#endif
+#ifndef Q_SPEC_FOLD
+#define Q_SPEC_FOLD 1          /* 0: no re-validation / repair inside the first pass; the fixed-point loop does all of it */
+#endif
 #ifndef Q_MIN_BLOCKS
 #define Q_MIN_BLOCKS 14
 #endif
@@ -1822,7 +1828,7 @@ k_q_search(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ strea
       /* a frame encoded from a guessed in-state also guesses the step gr1's search starts with: 2, what a stationary
        * signal produces (the formula would give 4 whenever the guessed start lies 4 above the landing gain); the value
        * used is recorded, and re-validation re-runs gr1's search only when the true step differs from it */
-      if (gr == 0 && fg.f != 0 && T->mode_gr == 2) cs = 2;
+      if (gr == 0 && fg.f != 0 && T->mode_gr == 2) cs = Q_SPEC_GR1_STEP;
       if (lane == 0) {
         q->bs_hash[gr][ch] = h;
         if (gr == 0) { q->bs_gain0[ch] = ov; q->bs_step0[ch] = cs; }
@@ -2189,7 +2195,7 @@ static int quant_run(const Mp3Tables* dT, const Mp3Tables& hT, StreamDesc* d_str
     search(1, nullptr, nullptr, F, 0); mark(QE_S1);
   }
   bool forked = false;
-  if (speculated) {
+  if (Q_SPEC_FOLD && speculated) {
     verify(G == 1 ? 1 : 0);
     search(0, list1, B.counter, F, 1);
     if (G == 2) {

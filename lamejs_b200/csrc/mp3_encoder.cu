@@ -184,6 +184,8 @@ struct Workspace {
  * or batches never serialise on the legacy default stream), events, workspace and staging buffers.  Bound to one device;
  * re-created when the thread is used with a configuration of another device. */
 enum { MP3_MAX_PCM_CHUNKS = 8 };
+/* The stream index is a grid y / z coordinate of several kernels (CUDA limit 65535): larger batches run in groups */
+enum { MP3_MAX_LAUNCH_STREAMS = 65535 };
 struct ThreadCtx {
   int device = -1;
   cudaStream_t st = nullptr, up_st = nullptr, aux_st = nullptr;   /* main, PCM upload, quantizer repair chain */
@@ -308,6 +310,7 @@ int run_pipeline(Config* cfg, Workspace& ws, std::vector<StreamDesc>& h_streams,
     scan_rows += (s.nframes + SCAN_FRAMES - 1) / SCAN_FRAMES;
   }
   if (S == 0 || total_frames == 0) { if (tm) *tm = Timings(); return 0; }   /* empty batch: nothing to launch */
+  if (S > MP3_MAX_LAUNCH_STREAMS) { g_err = "internal: more streams in one pipeline launch than a grid dimension holds"; return MP3B200_ERR_CUDA; }
   CK(cudaEventRecord(t_ctx.ev_in, cudaStreamLegacy));
   CK(cudaStreamWaitEvent(st, t_ctx.ev_in, 0));
   CK(cudaMemcpyAsync(ws.d_streams, h_streams.data(), sizeof(StreamDesc) * S, cudaMemcpyHostToDevice, st));
@@ -510,37 +513,42 @@ int encode_streams_device_impl(Config* cfg, int channels, int nstreams, const in
                                const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off, float* timings_ms,
                                const PcmArrival* arrival) {
   int rc = 0;
-  std::vector<StreamDesc> sds(nstreams);
-  long long U = 0, F = 0;
-  for (int s = 0; s < nstreams; s++) {
-    StreamDesc& sd = sds[s];
-    memset(&sd, 0, sizeof sd);
-    sd.pcm[0] = d_pcm + pcm_off[s];
-    sd.pcm[1] = channels == 2 ? d_pcm + pcm_off[s] + nsamples[s] : sd.pcm[0];
-    sd.pcm_base = 0; sd.pcm_end = nsamples[s];
-    sd.frame0 = 0; sd.nframes = (int)frames_for(nsamples[s], cfg->host.mode_gr);
-    sd.unit_base = (int)U; sd.frame_base = (int)F;
-    sd.out_base = out_off[s];
-    init_stream_state(sd);
-    U += (long long)cfg->host.mode_gr * sd.nframes; F += sd.nframes;
-  }
-  if (nstreams == 0 || F == 0) {            /* empty batch: success, nothing launched */
-    if (timings_ms) for (int i = 0; i < 16; i++) timings_ms[i] = 0.0f;
-    return MP3B200_OK;
-  }
-  Workspace& ws = t_ctx.ws;
-  if (ws.units < U || ws.frames < F || ws.nstreams < nstreams || ws.nch != cfg->host.nch) {
-    rc = ws.alloc(nstreams, cfg->host.nch, U, F, false);
+  if (timings_ms) for (int i = 0; i < 16; i++) timings_ms[i] = 0.0f;
+  /* Streams are independent: a batch wider than one launch can hold runs as consecutive groups on the thread's stream.
+   * The times add up over the groups; the pass count is the largest any group needed. */
+  for (int g0 = 0; g0 < nstreams; g0 += MP3_MAX_LAUNCH_STREAMS) {
+    const int n = nstreams - g0 < MP3_MAX_LAUNCH_STREAMS ? nstreams - g0 : MP3_MAX_LAUNCH_STREAMS;
+    std::vector<StreamDesc> sds(n);
+    long long U = 0, F = 0;
+    for (int i = 0; i < n; i++) {
+      const int s = g0 + i;
+      StreamDesc& sd = sds[i];
+      memset(&sd, 0, sizeof sd);
+      sd.pcm[0] = d_pcm + pcm_off[s];
+      sd.pcm[1] = channels == 2 ? d_pcm + pcm_off[s] + nsamples[s] : sd.pcm[0];
+      sd.pcm_base = 0; sd.pcm_end = nsamples[s];
+      sd.frame0 = 0; sd.nframes = (int)frames_for(nsamples[s], cfg->host.mode_gr);
+      sd.unit_base = (int)U; sd.frame_base = (int)F;
+      sd.out_base = out_off[s];
+      init_stream_state(sd);
+      U += (long long)cfg->host.mode_gr * sd.nframes; F += sd.nframes;
+    }
+    if (F == 0) continue;                     /* empty group: nothing to launch */
+    Workspace& ws = t_ctx.ws;
+    if (ws.units < U || ws.frames < F || ws.nstreams < n || ws.nch != cfg->host.nch) {
+      rc = ws.alloc(n, cfg->host.nch, U, F, false);
+      if (rc) return rc;
+    }
+    Timings tm;
+    rc = run_pipeline(cfg, ws, sds, d_out, nullptr, false, &tm, arrival);
     if (rc) return rc;
-  }
-  Timings tm;
-  rc = run_pipeline(cfg, ws, sds, d_out, nullptr, false, &tm, arrival);
-  if (rc) return rc;
-  if (timings_ms) {
-    timings_ms[0] = tm.psy; timings_ms[1] = tm.scan; timings_ms[2] = tm.mask; timings_ms[3] = tm.fb;
-    timings_ms[4] = tm.q1; timings_ms[5] = tm.qn; timings_ms[6] = tm.total; timings_ms[7] = (float)tm.passes;
-    timings_ms[8] = tm.q_prepare; timings_ms[9] = tm.q_search; timings_ms[10] = tm.q_outer; timings_ms[11] = tm.q_finish; timings_ms[12] = tm.q_pack;
-    timings_ms[13] = tm.q_mid; timings_ms[14] = timings_ms[15] = 0.0f;
+    arrival = nullptr;                        /* the later groups run behind the first one, after every upload landed */
+    if (timings_ms) {
+      const float t[16] = {tm.psy, tm.scan, tm.mask, tm.fb, tm.q1, tm.qn, tm.total, 0.0f,
+                           tm.q_prepare, tm.q_search, tm.q_outer, tm.q_finish, tm.q_pack, tm.q_mid, 0.0f, 0.0f};
+      for (int i = 0; i < 16; i++) timings_ms[i] += t[i];
+      if ((float)tm.passes > timings_ms[7]) timings_ms[7] = (float)tm.passes;
+    }
   }
   return 0;
 }

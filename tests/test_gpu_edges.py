@@ -1,0 +1,42 @@
+"""The edge corpus (tests/edge_signals.py: full scale, -32768, DC, Nyquist, +-1 LSB, click trains over every attack sub-block
+and across the 16-frame chunks of the block-type scan, a silent channel, L = -R, level jumps, tones near 20 kHz) through
+the CUDA path: every stage tap and all side-info columns bit-equal to the oracle, MPEG-1 and LSF, mono and stereo; and
+the whole corpus once more as one ragged batch per configuration."""
+import pytest
+
+import edge_signals
+import stage_taps
+
+pytestmark = pytest.mark.gpu
+
+
+@pytest.fixture(scope="module")
+def M():
+    import lamejs_b200
+
+    return lamejs_b200
+
+
+@pytest.mark.parametrize("case", edge_signals.CASES, ids=[edge_signals.case_id(c) for c in edge_signals.CASES])
+def test_edge_stage_parity(M, oracle, case):
+    kind, ch, sr, kbps, frames = case
+    l, r = edge_signals.signal(case)
+    G = M.granules_per_frame(ch, sr, kbps)
+    F = M.stream_frames(len(l), ch, sr, kbps)
+    ref, _, tr = oracle.encode_stream(ch, sr, kbps, l, r, trace_frames=F + 2)
+    assert len(tr) == F
+    g = M.debug_stages(ch, sr, kbps, l, r, want=stage_taps.ALL_TAPS)
+    stage_taps.compare(g, tr, ref, G, ch, edge_signals.case_id(case))
+
+
+def test_edge_corpus_as_batches(M, oracle):
+    """Each configuration's cases in one encode_streams call, together with prefixes of themselves (other chunk phases)."""
+    by_cfg = {}
+    for c in edge_signals.CASES:
+        by_cfg.setdefault(c[1:4], []).append(c)
+    for (ch, sr, kbps), cases in by_cfg.items():
+        sigs = [edge_signals.signal(c) for c in cases]
+        sigs += [(l[:len(l) * 2 // 3 + 17], None if r is None else r[:len(r) * 2 // 3 + 17]) for l, r in sigs]
+        outs = M.encode_streams(ch, sr, kbps, [s[0] for s in sigs], [s[1] for s in sigs] if ch == 2 else None)
+        for (l, r), o in zip(sigs, outs):
+            assert o == oracle.encode_stream(ch, sr, kbps, l, r)[0], (ch, sr, kbps, len(l))

@@ -7,6 +7,8 @@ import numpy as np
 import pytest
 
 import mp3_parse
+import stage_taps
+from stage_taps import bits_equal
 from synth import make_signal, white, octave_hold, bursts
 
 pytestmark = pytest.mark.gpu
@@ -19,11 +21,6 @@ def M():
     return lamejs_b200
 
 
-def bits_equal(a, b):
-    a, b = np.ascontiguousarray(a), np.ascontiguousarray(b)
-    return a.shape == b.shape and np.array_equal(a.view(np.uint32), b.view(np.uint32))
-
-
 @pytest.mark.parametrize("kind,ch,sr,kbps,frames", [
     ("noise", 2, 44100, 128, 60), ("burst", 2, 44100, 128, 80), ("white", 2, 48000, 320, 50), ("sine", 1, 44100, 128, 40),
     ("octave", 1, 44100, 128, 60), ("sweep", 2, 44100, 128, 120), ("noise", 2, 32000, 160, 40), ("white", 1, 48000, 320, 30),
@@ -33,15 +30,8 @@ def test_stage_parity(M, oracle, kind, ch, sr, kbps, frames):
     r = r if ch == 2 else None
     F = M.stream_frames(len(l))
     ref, _, tr = oracle.encode_stream(ch, sr, kbps, l, r, trace_frames=F + 2)
-    g = M.debug_stages(ch, sr, kbps, l, r, want=("xr", "blocktype", "en_l", "thm_l", "en_s", "thm_s", "ath_adjust", "l3_enc", "ginfo", "bytes"))
-    assert np.array_equal(g["blocktype"], tr["blocktype"][:, :, :ch])
-    assert np.array_equal(g["ath_adjust"], tr["ath_adjust"])
-    for k in ("xr", "en_l", "thm_l", "en_s", "thm_s"):
-        assert bits_equal(g[k], tr[k][:, :, :ch]), k          # relative tolerance: 0
-    assert np.array_equal(g["l3_enc"], tr["l3_enc"][:, :, :ch])
-    for j, k in enumerate(["global_gain", "part2_3_length", "part2_length", "big_values", "count1", "scalefac_compress"]):
-        assert np.array_equal(g["ginfo"][..., j], tr[k][:, :, :ch]), k
-    assert g["bytes"].tobytes() == ref
+    g = M.debug_stages(ch, sr, kbps, l, r, want=stage_taps.ALL_TAPS)
+    stage_taps.compare(g, tr, ref, 2, ch)      # every tap, all 15 side-info columns, relative tolerance 0
 
 
 def test_mdct_alone_with_forced_block_types(M, oracle):
@@ -269,15 +259,8 @@ def test_stage_parity_lsf(M, oracle, kind, ch, sr, kbps, frames):
     F = M.stream_frames(len(l), ch, sr, kbps)
     ref, _, tr = oracle.encode_stream(ch, sr, kbps, l, r, trace_frames=F + 2)
     assert len(tr) == F
-    g = M.debug_stages(ch, sr, kbps, l, r, want=("xr", "blocktype", "en_l", "thm_l", "en_s", "thm_s", "ath_adjust", "l3_enc", "ginfo", "bytes"))
-    assert np.array_equal(g["blocktype"], tr["blocktype"][:, :1, :ch])
-    assert np.array_equal(g["ath_adjust"], tr["ath_adjust"])
-    for k in ("xr", "en_l", "thm_l", "en_s", "thm_s"):
-        assert bits_equal(g[k], tr[k][:, :1, :ch]), k
-    assert np.array_equal(g["l3_enc"], tr["l3_enc"][:, :1, :ch])
-    for j, k in enumerate(["global_gain", "part2_3_length", "part2_length", "big_values", "count1", "scalefac_compress"]):
-        assert np.array_equal(g["ginfo"][..., j], tr[k][:, :1, :ch]), k
-    assert g["bytes"].tobytes() == ref
+    g = M.debug_stages(ch, sr, kbps, l, r, want=stage_taps.ALL_TAPS)
+    stage_taps.compare(g, tr, ref, 1, ch)
 
 
 def test_lsf_batches_and_handles(M, oracle):
