@@ -54,7 +54,12 @@ void mp3b200_destroy(mp3b200_encoder* h);
  * calling mp3b200_encode / mp3b200_flush on every handle in turn, but the frames all handles complete in this call
  * are encoded by ONE pipeline launch (handle i = stream i).  left[i]/right[i]: nsamples[i] Int16 (right or right[i]
  * NULL: mono / duplicate left); out[i] receives out_bytes[i] bytes (cap[i] >= trunc(1.25 * nsamples[i] + 7200) like
- * lamejs, 0 = unchecked); out_bytes[i] < 0 reports a per-handle error (NULL handle -3, buffer too small -1).
+ * lamejs, 0 = unchecked); out_bytes[i] < 0 reports a per-handle error (NULL handle -3, buffer too small -1, a handle of
+ * another configuration than the batch's first one with frames to encode -1).  A handle whose call failed keeps its
+ * samples and its completed frames: its next call hands them out first.
+ * A handle may be listed more than once: the call then runs as consecutive rounds, round k taking the k-th occurrence of
+ * every handle, so each handle's entries run in list order (a repeated flush returns 0 bytes, like a second flush); a
+ * call without repeats is one round.
  * A JS caller loops over its encoders instead (worker-example/worker.js, worker-realtime.js:46). */
 int mp3b200_encode_batch(mp3b200_encoder* const* handles, const int16_t* const* left, const int16_t* const* right,
                          const int* nsamples, uint8_t* const* out, const int* cap, int nstreams, int* out_bytes);
@@ -66,7 +71,9 @@ int mp3b200_flush_batch(mp3b200_encoder* const* handles, uint8_t* const* out, co
  *   export_state  writes everything the handle carries between calls (scalars, the previous unit's masking row from device
  *                 memory, the PCM tail later frames still read, FIFO accounting); buf == NULL returns the size.  Two handles
  *                 that encoded the same frames from the same samples export identical bytes.
- *   import_state  makes a handle of the same configuration continue exactly where the exporting one stood.
+ *   import_state  makes a handle of the same configuration continue exactly where the exporting one stood.  A blob whose
+ *                 retained samples do not start at max(0, framesize*frames_done - 1104) is refused (-1), and the handle is
+ *                 left as it was.
  *   seek          positions a FRESH handle at frame `frame` >= 1 with the sequential state of a stream start: the start of
  *                 a warm-up.  A segment encoder seeks W frames before its first frame, encodes them (discarding the bytes)
  *                 and compares its state with the predecessor segment's exported end state: equal blobs prove its frames are

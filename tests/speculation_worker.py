@@ -11,6 +11,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 import edge_signals  # noqa: E402
+import handle_schedule as HS  # noqa: E402
 import oracle_lib as O  # noqa: E402
 from synth import make_signal, white  # noqa: E402
 
@@ -72,6 +73,11 @@ def main():
                 fail.append("handles %d/%d/%d stream %d flush" % (ch, sr, kbps, i))
         for e, r in zip(encs, refs):
             e.close(); r.close()
+
+    # one reduced call schedule per configuration family (tests/handle_schedule.py), with many calls of up to 200 frames
+    for cfg, seed in (((2, 44100, 128), 7), ((2, 22050, 64), 8)):
+        s = HS.make_schedule(cfg, 8, 40, seed, big=0.3)
+        fail += ["schedule %d/%d/%d: %s" % (cfg + (f,)) for f in HS.run(M, s, HS.replay(s))]
 
     # the edge corpus, one batch per configuration
     by_cfg = {}

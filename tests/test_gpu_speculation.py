@@ -3,7 +3,8 @@ speed, never the bytes.  The library is rebuilt with deliberately bad guesses --
 step (Q_SPEC_START, Q_SPEC_STEP), the start step handed to gr1 (Q_SPEC_GR1_STEP), the in-state of the block-type / ATH scan
 chunks (SCAN_GUESS_LA, SCAN_GUESS_BT, SCAN_GUESS_ATH) -- and with the re-validation folded into the first pass switched off
 (Q_SPEC_FOLD=0), so that every wrong guess is repaired by the fixed-point loop.  Each variant encodes ragged MPEG-1 and LSF
-batches, live handles fed 5000-sample calls and the edge corpus, all byte-equal to the oracle (tests/speculation_worker.py,
+batches, live handles fed 5000-sample calls, one MPEG-1 and one LSF handle call schedule (tests/handle_schedule.py) with many
+calls of up to 200 frames, and the edge corpus, all byte-equal to the oracle (tests/speculation_worker.py,
 one subprocess per library because the library is loaded once per process)."""
 import json
 import os
