@@ -217,6 +217,33 @@ int mp3b200_debug_stages(int channels, int samplerate, int kbps, const int16_t* 
                          float* en_l, float* thm_l, float* en_s, float* thm_s, double* ath_adjust,
                          int32_t* l3_enc, int32_t* ginfo, uint8_t* bytes_out, int64_t bytes_cap);
 
+/* The same taps, and the quantizer's state, through one struct (mp3b200_debug_stages is a thin wrapper of it).  `size` must
+ * be sizeof(mp3b200_debug_taps).  Inputs and the first outputs are those of mp3b200_debug_stages; in addition ([G] granules
+ * per frame):
+ *   scalefac       int32 [F][G][nch][39]  final scalefactors; gr1 bands that scfsi shares with gr0 hold -1 (as in lamejs)
+ *   subblock_gain  int32 [F][G][nch][3]
+ *   xmin           float [F][G][nch][39]  calc_xmin's output as the rate loop receives it: the psymax bands (21 long, 36 short),
+ *                                         0 above them and for granules without energy (where lamejs skips the rate loop)
+ *   max_nonzero_coeff int32 [F][G][nch], xrpow_max double [F][G][nch]   after init_xrpow / calc_xmin, before the rate loop
+ *   scfsi          int32 [F][nch][4]
+ *   old_value, cur_step  int32 [F][3][nch]: gfc.OldValue / CurrentStep at the frame's start [0], after gr0 [1] (MPEG-1; 0 for
+ *                  LSF) and after the frame [2], read from the speculation bookkeeping once the fixed-point loop has ended.
+ *                  These are the states the final bytes were encoded from: the last verification found every frame's start
+ *                  state equal to its predecessor's end state, and a search result kept from an earlier, speculated start
+ *                  was kept only because the search from this start landed on the same gain and granule info.
+ * Any output pointer may be NULL. */
+typedef struct mp3b200_debug_taps {
+  int32_t size, channels, samplerate, kbps;
+  const int16_t *left, *right;
+  int64_t nsamples;
+  const int32_t* force_blocktype;
+  float* xr; int32_t* blocktype; float *en_l, *thm_l, *en_s, *thm_s; double* ath_adjust;
+  int32_t *l3_enc, *ginfo; uint8_t* bytes_out; int64_t bytes_cap;
+  int32_t *scalefac, *subblock_gain; float* xmin; int32_t* max_nonzero_coeff; double* xrpow_max;
+  int32_t *scfsi, *old_value, *cur_step;
+} mp3b200_debug_taps;
+int mp3b200_debug_stages_ex(const mp3b200_debug_taps* t);
+
 const char* mp3b200_last_error(void);
 /* total number of kernel launches issued by this library since load (bench.py "gpu_launches") */
 int64_t mp3b200_launch_count(void);

@@ -625,8 +625,28 @@ int mp3b200_debug_stages(int channels, int samplerate, int kbps, const int16_t* 
                          int64_t nsamples, const int32_t* force_blocktype, float* xr, int32_t* blocktype,
                          float* en_l, float* thm_l, float* en_s, float* thm_s, double* ath_adjust,
                          int32_t* l3_enc, int32_t* ginfo, uint8_t* bytes_out, int64_t bytes_cap) {
+  mp3b200_debug_taps t;
+  memset(&t, 0, sizeof t);
+  t.size = (int32_t)sizeof t; t.channels = channels; t.samplerate = samplerate; t.kbps = kbps;
+  t.left = left; t.right = right; t.nsamples = nsamples; t.force_blocktype = force_blocktype;
+  t.xr = xr; t.blocktype = blocktype; t.en_l = en_l; t.thm_l = thm_l; t.en_s = en_s; t.thm_s = thm_s; t.ath_adjust = ath_adjust;
+  t.l3_enc = l3_enc; t.ginfo = ginfo; t.bytes_out = bytes_out; t.bytes_cap = bytes_cap;
+  return mp3b200_debug_stages_ex(&t);
+}
+
+int mp3b200_debug_stages_ex(const mp3b200_debug_taps* tp) {
+  if (!tp || tp->size != (int32_t)sizeof(mp3b200_debug_taps)) { g_err = "mp3b200_debug_taps: size must be sizeof(mp3b200_debug_taps)"; return MP3B200_ERR_HANDLE; }
+  const int channels = tp->channels;
+  const int16_t *left = tp->left, *right = tp->right;
+  const int64_t nsamples = tp->nsamples;
+  const int32_t* force_blocktype = tp->force_blocktype;
+  float *xr = tp->xr, *en_l = tp->en_l, *thm_l = tp->thm_l, *en_s = tp->en_s, *thm_s = tp->thm_s;
+  int32_t *blocktype = tp->blocktype, *l3_enc = tp->l3_enc, *ginfo = tp->ginfo;
+  double* ath_adjust = tp->ath_adjust;
+  uint8_t* bytes_out = tp->bytes_out;
+  const int64_t bytes_cap = tp->bytes_cap;
   Config* cfg;
-  int rc = get_config(channels, samplerate, kbps, &cfg);
+  int rc = get_config(channels, tp->samplerate, tp->kbps, &cfg);
   if (rc) return rc;
   rc = t_ctx.use(cfg->device);
   if (rc) return rc;
@@ -649,7 +669,10 @@ int mp3b200_debug_stages(int channels, int samplerate, int kbps, const int16_t* 
   Workspace ws;
   rc = ws.alloc(1, nch, U, F, true);
   if (rc) { cudaFree(d_pcm); cudaFree(d_out); return rc; }
-  const bool only_mdct = (l3_enc == nullptr && ginfo == nullptr && bytes_out == nullptr);
+  const bool want_gi = ginfo || tp->scalefac || tp->subblock_gain;
+  const bool want_prep = tp->xmin || tp->max_nonzero_coeff || tp->xrpow_max;
+  const bool want_q = tp->scfsi || tp->old_value || tp->cur_step;
+  const bool only_mdct = !(l3_enc || bytes_out || want_gi || want_prep || want_q);
   rc = run_pipeline(cfg, ws, sds, d_out, force_blocktype, only_mdct, nullptr);
   if (rc == 0) {
     if (xr) CK(cudaMemcpy(xr, ws.d_xr, sizeof(float) * (size_t)U * nch * 576, cudaMemcpyDeviceToHost));
@@ -676,15 +699,50 @@ int mp3b200_debug_stages(int channels, int samplerate, int kbps, const int16_t* 
       CK(cudaMemcpy(t.data(), ws.d_l3enc, sizeof(short) * t.size(), cudaMemcpyDeviceToHost));
       for (size_t i = 0; i < t.size(); i++) l3_enc[i] = t[i];
     }
-    if (ginfo) {
+    if (want_gi) {
       std::vector<GranuleInfoDev> g((size_t)U * nch);
       CK(cudaMemcpy(g.data(), ws.d_ginfo, sizeof(GranuleInfoDev) * g.size(), cudaMemcpyDeviceToHost));
       for (size_t i = 0; i < g.size(); i++) {
-        int32_t* o = ginfo + i * 16;
-        o[0] = g[i].global_gain; o[1] = g[i].part2_3_length; o[2] = g[i].part2_length; o[3] = g[i].big_values;
-        o[4] = g[i].count1; o[5] = g[i].scalefac_compress; o[6] = g[i].table_select[0]; o[7] = g[i].table_select[1];
-        o[8] = g[i].table_select[2]; o[9] = g[i].region0_count; o[10] = g[i].region1_count; o[11] = g[i].preflag;
-        o[12] = g[i].scalefac_scale; o[13] = g[i].count1table_select; o[14] = g[i].block_type; o[15] = 0;
+        if (ginfo) {
+          int32_t* o = ginfo + i * 16;
+          o[0] = g[i].global_gain; o[1] = g[i].part2_3_length; o[2] = g[i].part2_length; o[3] = g[i].big_values;
+          o[4] = g[i].count1; o[5] = g[i].scalefac_compress; o[6] = g[i].table_select[0]; o[7] = g[i].table_select[1];
+          o[8] = g[i].table_select[2]; o[9] = g[i].region0_count; o[10] = g[i].region1_count; o[11] = g[i].preflag;
+          o[12] = g[i].scalefac_scale; o[13] = g[i].count1table_select; o[14] = g[i].block_type; o[15] = 0;
+        }
+        if (tp->scalefac) memcpy(tp->scalefac + i * MP3_SFBMAX, g[i].scalefac, sizeof(int32_t) * MP3_SFBMAX);
+        if (tp->subblock_gain) for (int k = 0; k < 3; k++) tp->subblock_gain[i * 3 + k] = g[i].subblock_gain[k];
+      }
+    }
+    if (want_prep) {
+      /* the prepared granule-channel as k_q_prepare left it for the searches and rate loops; xmin is defined for the psymax
+       * bands of granules with energy only (the others never reach calc_xmin) */
+      std::vector<GcPrep> p((size_t)U * nch);
+      CK(cudaMemcpy(p.data(), ws.d_prep, sizeof(GcPrep) * p.size(), cudaMemcpyDeviceToHost));
+      for (size_t i = 0; i < p.size(); i++) {
+        if (tp->xmin) {
+          const int psymax = p[i].block_type == BT_SHORT ? 36 : 21;
+          for (int k = 0; k < MP3_SFBMAX; k++) tp->xmin[i * MP3_SFBMAX + k] = (p[i].have && k < psymax) ? p[i].xmin[k] : 0.0f;
+        }
+        if (tp->max_nonzero_coeff) tp->max_nonzero_coeff[i] = p[i].mnz;
+        if (tp->xrpow_max) tp->xrpow_max[i] = p[i].xrpow_max;
+      }
+    }
+    if (want_q) {
+      std::vector<QuantFrameState> q((size_t)F);
+      CK(cudaMemcpy(q.data(), ws.d_qstate, sizeof(QuantFrameState) * q.size(), cudaMemcpyDeviceToHost));
+      for (long long f = 0; f < F; f++) {
+        const QuantFrameState& s = q[(size_t)f];
+        for (int c = 0; c < nch; c++) {
+          if (tp->scfsi) for (int b = 0; b < 4; b++) tp->scfsi[(f * nch + c) * 4 + b] = s.scfsi[c][b];
+          /* [in, after gr0 (MPEG-1 only: bs_* is the state gr1's search started from), out] */
+          const int ov[3] = {s.in_old[c], G == 2 ? s.bs_gain0[c] : 0, s.out_old[c]};
+          const int cs[3] = {s.in_step[c], G == 2 ? s.bs_step0[c] : 0, s.out_step[c]};
+          for (int k = 0; k < 3; k++) {
+            if (tp->old_value) tp->old_value[(f * 3 + k) * nch + c] = ov[k];
+            if (tp->cur_step) tp->cur_step[(f * 3 + k) * nch + c] = cs[k];
+          }
+        }
       }
     }
     if (bytes_out) {

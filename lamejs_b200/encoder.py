@@ -13,6 +13,17 @@ class Mp3B200Error(RuntimeError):
     pass
 
 
+class DebugTaps(ctypes.Structure):
+    """mp3b200_debug_taps (include/mp3b200.h)"""
+    _vp = ctypes.c_void_p
+    _fields_ = [("size", ctypes.c_int32), ("channels", ctypes.c_int32), ("samplerate", ctypes.c_int32), ("kbps", ctypes.c_int32),
+                ("left", _vp), ("right", _vp), ("nsamples", ctypes.c_int64), ("force_blocktype", _vp),
+                ("xr", _vp), ("blocktype", _vp), ("en_l", _vp), ("thm_l", _vp), ("en_s", _vp), ("thm_s", _vp), ("ath_adjust", _vp),
+                ("l3_enc", _vp), ("ginfo", _vp), ("bytes_out", _vp), ("bytes_cap", ctypes.c_int64),
+                ("scalefac", _vp), ("subblock_gain", _vp), ("xmin", _vp), ("max_nonzero_coeff", _vp), ("xrpow_max", _vp),
+                ("scfsi", _vp), ("old_value", _vp), ("cur_step", _vp)]
+
+
 def lib():
     """Load (building if needed) libmp3b200.so and declare the C-ABI of include/mp3b200.h."""
     global _lib
@@ -58,6 +69,7 @@ def lib():
     L.mp3b200_wav_read_header.argtypes = [vp, c_i64, vp]
     L.mp3b200_debug_music_crc.argtypes = [vp, vp, vp, c_int, vp, vp]
     L.mp3b200_debug_stages.argtypes = [c_int, c_int, c_int, vp, vp, c_i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, c_i64]
+    L.mp3b200_debug_stages_ex.argtypes = [ctypes.POINTER(DebugTaps)]
     _lib = L
     return L
 
@@ -378,7 +390,9 @@ def encode_streams_device(channels, samplerate, kbps, d_pcm_ptr, pcm_off, nsampl
 
 
 def debug_stages(channels, samplerate, kbps, left, right=None, force_blocktype=None, want=("xr",)):
-    """Stage taps for parity tests: returns a dict of numpy arrays (see include/mp3b200.h)."""
+    """Stage taps for parity tests: returns a dict of numpy arrays (see include/mp3b200.h).  `want` names any of xr,
+    blocktype, en_l, thm_l, en_s, thm_s, ath_adjust, l3_enc, ginfo, bytes, scalefac, subblock_gain, xmin, max_nonzero_coeff,
+    xrpow_max, scfsi, old_value and cur_step (the last two [F][3][nch]: frame start, after gr0, frame end)."""
     L = lib()
     left = np.ascontiguousarray(left, dtype=np.int16)
     right = left if (right is None or channels == 1) else np.ascontiguousarray(right, dtype=np.int16)
@@ -413,7 +427,13 @@ def debug_stages(channels, samplerate, kbps, left, right=None, force_blocktype=N
     if nb < 0:
         raise Mp3B200Error("unsupported configuration: channels=%d samplerate=%d kbps=%d" % (channels, samplerate, kbps))
     p_by = alloc("bytes", (nb,), np.uint8)
-    _check(L.mp3b200_debug_stages(channels, samplerate, kbps, left.ctypes.data, right.ctypes.data, n,
-                                  fb.ctypes.data if fb is not None else None, p_xr, p_bt, p_enl, p_thl, p_ens, p_ths, p_ath,
-                                  p_l3, p_gi, p_by, nb))
+    t = DebugTaps(size=ctypes.sizeof(DebugTaps), channels=channels, samplerate=samplerate, kbps=kbps, left=left.ctypes.data,
+                  right=right.ctypes.data, nsamples=n, force_blocktype=fb.ctypes.data if fb is not None else None,
+                  xr=p_xr, blocktype=p_bt, en_l=p_enl, thm_l=p_thl, en_s=p_ens, thm_s=p_ths, ath_adjust=p_ath,
+                  l3_enc=p_l3, ginfo=p_gi, bytes_out=p_by, bytes_cap=nb,
+                  scalefac=alloc("scalefac", (F, G, nch, 39), np.int32), subblock_gain=alloc("subblock_gain", (F, G, nch, 3), np.int32),
+                  xmin=alloc("xmin", (F, G, nch, 39), np.float32), max_nonzero_coeff=alloc("max_nonzero_coeff", (F, G, nch), np.int32),
+                  xrpow_max=alloc("xrpow_max", (F, G, nch), np.float64), scfsi=alloc("scfsi", (F, nch, 4), np.int32),
+                  old_value=alloc("old_value", (F, 3, nch), np.int32), cur_step=alloc("cur_step", (F, 3, nch), np.int32))
+    _check(L.mp3b200_debug_stages_ex(ctypes.byref(t)))
     return res

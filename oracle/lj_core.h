@@ -115,4 +115,24 @@ struct LjFrameTrace {
   int   old_value_in[2], old_value_out[2], cur_step_in[2], cur_step_out[2];
 };
 
+/* per-frame record of the quantizer's inputs (lj_set_quant_trace), row k belonging to LjFrameTrace row k.  A record of its own,
+ * so that the layout of LjFrameTrace, which callers size their buffers by, stays as it was.
+ * What outer_loop receives (lj_iteration_loop): calc_xmin's l3_xmin (psymax bands; 0 elsewhere and for granules without
+ * energy), max_nonzero_coeff after calc_xmin, xrpow_max after init_xrpow (before the rate loop raises it). */
+struct LjQuantTrace {
+  float xmin[2][2][SFBMAX];
+  int   max_nonzero_coeff[2][2];
+  double xrpow_max[2][2];
+  int   old_value_mid[2], cur_step_mid[2];   /* MPEG-1: OldValue / CurrentStep after gr0, where gr1's search starts; 0 for LSF */
+};
+
+/* what an encoder carries from one call to the next (lj_get_state) */
+struct LjState {
+  double ath_adjust, ath_adjust_limit;
+  int   blocktype_old[2], last_attacks[2], old_value[2], current_step[2];
+  int   frames_done, mf_size, mf_samples_to_encode, pad_;
+  /* gfc.en / gfc.thm: the masking the psy model hands the next granule */
+  float en_l[2][SBMAX_l], thm_l[2][SBMAX_l], en_s[2][SBMAX_s][3], thm_s[2][SBMAX_s][3];
+};
+
 #endif

@@ -100,6 +100,8 @@ struct LjEnc {
   int ancillary_flag;
   /* trace */
   LjFrameTrace* trace; int trace_cap, trace_n;
+  LjQuantTrace* qtrace; int qtrace_cap;
+  LjQuantTrace* qtrace_cur;      /* the quantizer row of the frame being encoded while tracing, else NULL (lj_quant.cpp) */
   /* Xing / LAME tag state (VBRSeekInfo.js, LameInternalFlags.js:170; lj_vbrtag.cpp).  nMusicCRC and nBytesWritten are
    * maintained by copy_buffer on every call whether or not a tag is written (BitStream.js:924-935). */
   int nMusicCRC; long long nBytesWritten;

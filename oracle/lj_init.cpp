@@ -422,7 +422,10 @@ static int encode_mp3_frame(LjEnc* e, uint8_t* mp3buf, int mp3buf_size) {
     f = (670 * 5 * e->mode_gr * e->channels_out) / f;
     for (int gr = 0; gr < e->mode_gr; gr++) for (int ch = 0; ch < e->channels_out; ch++) pe_use[gr][ch] *= f;
   }
+  e->qtrace_cur = (tracing && e->qtrace && e->trace_n < e->qtrace_cap) ? &e->qtrace[e->trace_n] : NULL;
+  if (e->qtrace_cur) memset(e->qtrace_cur, 0, sizeof *e->qtrace_cur);
   lj_iteration_loop(e, pe_use, ms_ener_ratio, masking);
+  e->qtrace_cur = NULL;
   lj_format_bitstream(e);
   int mp3count = lj_copy_buffer(e, mp3buf, mp3buf_size, 1);
   lj_add_vbr_frame(e);             /* Encoder.js:640-641 */
@@ -687,8 +690,26 @@ int lj_flush(LjEnc* e, uint8_t* out, int cap) {
 }
 
 void lj_set_trace(LjEnc* e, LjFrameTrace* buf, int cap) { e->trace = buf; e->trace_cap = cap; e->trace_n = 0; }
+/* quantizer rows next to the frame trace: row k is filled together with lj_set_trace's row k (call it after lj_set_trace) */
+void lj_set_quant_trace(LjEnc* e, LjQuantTrace* buf, int cap) { e->qtrace = buf; e->qtrace_cap = cap; }
+int lj_quant_trace_size(void) { return (int)sizeof(LjQuantTrace); }
 int lj_trace_count(const LjEnc* e) { return e->trace_n; }
 int lj_trace_size(void) { return (int)sizeof(LjFrameTrace); }
+int lj_state_size(void) { return (int)sizeof(LjState); }
+/* the state an encoder carries into its next call (the counterpart of a handle's state blob) */
+int lj_get_state(const LjEnc* e, LjState* s) {
+  memset(s, 0, sizeof *s);
+  s->ath_adjust = e->ath_adjust; s->ath_adjust_limit = e->ath_adjustLimit;
+  for (int ch = 0; ch < 2; ch++) {
+    s->blocktype_old[ch] = e->blocktype_old[ch]; s->last_attacks[ch] = e->lastAttacks[ch];
+    s->old_value[ch] = e->OldValue[ch]; s->current_step[ch] = e->CurrentStep[ch];
+    for (int sb = 0; sb < SBMAX_l; sb++) { s->en_l[ch][sb] = e->en[ch].l[sb].v; s->thm_l[ch][sb] = e->thm[ch].l[sb].v; }
+    for (int sb = 0; sb < SBMAX_s; sb++)
+      for (int b = 0; b < 3; b++) { s->en_s[ch][sb][b] = e->en[ch].s[sb][b].v; s->thm_s[ch][sb][b] = e->thm[ch].s[sb][b].v; }
+  }
+  s->frames_done = e->frameNum; s->mf_size = e->mf_size; s->mf_samples_to_encode = e->mf_samples_to_encode;
+  return (int)sizeof *s;
+}
 int lj_frame_bytes_for(const LjEnc* e, int padding) {
   return framebits(e->version, e->bitrate_index, e->out_samplerate, padding) / 8;
 }

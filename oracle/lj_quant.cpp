@@ -1357,12 +1357,19 @@ void lj_iteration_loop(LjEnc* e, double pe[2][2], const double* ms_ener_ratio, P
       else masking_lower_db = e->mask_adjust_short - 0;
       e->masking_lower = js_pow(10.0, masking_lower_db * 0.1);
       init_outer_loop(e, cod_info);
-      if (init_xrpow(e, cod_info, xrpow)) {
-        calc_xmin(e, &ratio[gr][ch], cod_info, l3_xmin);
-        outer_loop(e, cod_info, l3_xmin, xrpow, ch, targ_bits[ch]);
+      const bool have = init_xrpow(e, cod_info, xrpow);
+      if (have) calc_xmin(e, &ratio[gr][ch], cod_info, l3_xmin);
+      if (e->qtrace_cur) {                     /* test tap: what outer_loop starts from */
+        LjQuantTrace* t = e->qtrace_cur;
+        t->max_nonzero_coeff[gr][ch] = cod_info->max_nonzero_coeff;
+        t->xrpow_max[gr][ch] = cod_info->xrpow_max;
+        for (int i = 0; i < SFBMAX; i++) t->xmin[gr][ch][i] = (have && i < cod_info->psymax) ? l3_xmin[i].v : 0.0f;
       }
+      if (have) outer_loop(e, cod_info, l3_xmin, xrpow, ch, targ_bits[ch]);
       iteration_finish_one(e, gr, ch);
     }
+    if (e->qtrace_cur && gr == 0 && e->mode_gr == 2)
+      for (int ch = 0; ch < 2; ch++) { e->qtrace_cur->old_value_mid[ch] = e->OldValue[ch]; e->qtrace_cur->cur_step_mid[ch] = e->CurrentStep[ch]; }
   }
   ResvFrameEnd(e, mean_bits);
 }

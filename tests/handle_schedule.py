@@ -11,7 +11,9 @@ decay.
 
 The expected bytes of every call come from one OracleEncoder per logical stream that replays that stream's calls in order,
 which is how include/mp3b200.h defines a batch call.  A call that fails for a too small buffer hands out nothing and keeps
-its frames: the stream's next call returns them in front of its own.  tests/test_gpu_handle_soak.py and
+its frames: the stream's next call returns them in front of its own.  After every operation the runner also compares the
+state blob of each stream it named -- header and halo, including after hand-overs and flushes -- with that stream's
+OracleEncoder.state().  tests/test_gpu_handle_soak.py and
 tests/speculation_worker.py run schedules on the GPU; tests/test_handle_schedule_cpu.py checks what they reach."""
 import ctypes
 from collections import namedtuple
@@ -123,7 +125,8 @@ class Expected:
     """What a schedule must produce.  results[i][j]: bytes, or the negative error, of entry j of operation i (None for a
     hand-over).  raw[s]: the oracle's bytes of stream s call by call (including those a failed call held back).  epochs[s]:
     the sample ranges of stream s that a flush ended.  tags[s]: tag_on, tag frame, music CRC and bytes written after the last
-    flush.  With tracing, calls lists (s, frames the call completed, block types of its last granule) for every oracle call."""
+    flush.  states[i]: {s: OracleEncoder.state()} after operation i for every stream it names.  With tracing, calls lists
+    (s, frames the call completed, block types of its last granule) for every oracle call."""
 
 
 def replay(sched, trace=False):
@@ -162,9 +165,13 @@ def replay(sched, trace=False):
         return b
 
     pos = [0] * K
+    ex.states = []
     for kind, entries in sched.ops:
+        # what each stream the operation touches carries into its next call, after the operation
+        ex.states.append({c.s: None for c in entries if c.s is not None})
         if kind == "handover":
             ex.results.append([None])
+            ex.states[-1] = {s: encs[s].state() for s in ex.states[-1]}
             continue
         res = []
         for c in entries:
@@ -186,6 +193,7 @@ def replay(sched, trace=False):
                 res.append(total)
                 backlog[c.s] = b""
         ex.results.append(res)
+        ex.states[-1] = {s: encs[s].state() for s in ex.states[-1]}
     assert not any(backlog), "the schedule's last flush must deliver everything"
     ex.tags = [{"tag_on": e.tag_on, "tag": e.lametag_frame(), "music_crc": e.music_crc(), "bytes_written": e.bytes_written()}
                for e in encs]
@@ -229,6 +237,58 @@ def reached(sched, ex):
 
 # ---- the library side ----
 
+# StateBlobHeader (lamejs_b200/csrc/mp3_handle.inc), followed by the halo (per channel the PsyRatioDev row en_l[22],
+# thm_l[22], en_s[13][3], thm_s[13][3]) once a frame has been encoded, then the retained PCM
+BLOB_HEADER = np.dtype([("magic", "<u4"), ("channels", "<i4"), ("samplerate", "<i4"), ("kbps", "<i4"),
+                        ("frames_pending", "<i4"), ("mf_size", "<i4"), ("mf_samples_to_encode", "<i4"), ("halo_floats", "<i4"),
+                        ("hist_base", "<i8"), ("fed", "<i8"), ("frames_done", "<i8"), ("pcm_samples", "<i8"),
+                        ("ath_adjust", "<f8"), ("ath_adjust_limit", "<f8"), ("blocktype_old", "<i4", (2,)),
+                        ("last_attacks", "<i4", (2,)), ("old_value", "<i4", (2,)), ("current_step", "<i4", (2,))])
+
+
+def _bits(a):
+    a = np.ascontiguousarray(a)
+    return a.view(np.uint64 if a.dtype.itemsize == 8 else np.uint32) if a.dtype.kind == "f" else a
+
+
+def blob_state_diff(blob, st, nch):
+    """Names of the fields in which a handle's exported state blob differs from the oracle's state `st` (OracleEncoder.state())
+    for the same stream after the same calls.  Floats are compared as bit patterns.  A handle whose last call failed still
+    holds frames the oracle has encoded (frames_pending > 0): its fill level must agree, its sequential state is checked after
+    the call that delivers them."""
+    h = np.frombuffer(bytes(blob[:BLOB_HEADER.itemsize]), dtype=BLOB_HEADER)[0]
+    bad = []
+    if h["frames_done"] + h["frames_pending"] != st["frames_done"]:
+        bad.append("frames_done")
+    for k in ("mf_size", "mf_samples_to_encode"):
+        if h[k] != st[k]:
+            bad.append(k)
+    if h["frames_pending"] > 0:
+        return bad
+    for k in ("ath_adjust", "ath_adjust_limit"):
+        if _bits(h[k]) != _bits(st[k]):
+            bad.append(k)
+    for k in ("blocktype_old", "last_attacks", "old_value", "current_step"):
+        if not np.array_equal(h[k][:nch], st[k][:nch]):
+            bad.append(k)
+    if h["frames_done"] > 0:
+        if h["halo_floats"] != nch * 122:
+            return bad + ["halo_floats"]
+        halo = np.frombuffer(bytes(blob[BLOB_HEADER.itemsize:BLOB_HEADER.itemsize + 4 * nch * 122]), dtype="<f4").reshape(nch, 122)
+        want = np.concatenate([st["en_l"][:nch], st["thm_l"][:nch], st["en_s"][:nch].reshape(nch, 39),
+                               st["thm_s"][:nch].reshape(nch, 39)], axis=1)
+        if not np.array_equal(_bits(halo), _bits(want)):
+            bad.append("halo (en/thm handed to the next granule)")
+    return bad
+
+
+def export_blob(L, h):
+    n = L.mp3b200_export_state(h, None, 0)
+    blob = np.empty(n, dtype=np.uint8)
+    assert L.mp3b200_export_state(h, blob.ctypes.data, n) == n
+    return blob
+
+
 SENTINEL = 0xA5
 TAIL = 16               # sentinel bytes behind every output buffer
 
@@ -265,17 +325,24 @@ def run(M, sched, ex):
         return h
 
     hs = [create(s) for s in range(sched.nstreams)]
+
+    def check_states(i, kind):
+        """the state every stream named by operation i carries into its next call equals the oracle's"""
+        for s, st in ex.states[i].items():
+            bad = blob_state_diff(export_blob(L, hs[s]), st, ch)
+            if bad:
+                fails.append("op %d %s: state of stream %d differs in %s" % (i, kind, s, ", ".join(bad)))
+
     for i, ((kind, entries), want) in enumerate(zip(sched.ops, ex.results)):
         if kind == "handover":
             s = entries[0].s
-            n = L.mp3b200_export_state(hs[s], None, 0)
-            blob = np.empty(n, dtype=np.uint8)
-            assert L.mp3b200_export_state(hs[s], blob.ctypes.data, n) == n
+            blob = export_blob(L, hs[s])
             h = create(s)
-            if L.mp3b200_import_state(h, blob.ctypes.data, n) != 0:
+            if L.mp3b200_import_state(h, blob.ctypes.data, len(blob)) != 0:
                 fails.append("op %d: import_state refused a blob of stream %d" % (i, s))
             L.mp3b200_destroy(hs[s])
             hs[s] = h
+            check_states(i, kind)
             continue
         m = len(entries)
         bufs = [_buffer(w) for w in want]
@@ -311,6 +378,7 @@ def run(M, sched, ex):
                 what = g if isinstance(g, str) else ("%d bytes" % len(g) if isinstance(g, bytes) else "error %d" % g)
                 wwhat = "%d bytes" % len(w) if isinstance(w, bytes) else "error %d" % w
                 fails.append("op %d %s entry %d (stream %s, samples %d..%d): got %s, want %s" % (i, kind, j, c.s, c.lo, c.hi, what, wwhat))
+        check_states(i, kind)
     for s, t in enumerate(ex.tags):
         if not t["tag_on"]:
             continue

@@ -48,6 +48,43 @@ TRACE_DTYPE = np.dtype(
     align=True,
 )
 
+# lj_set_quant_trace: the quantizer's inputs, one row per TRACE_DTYPE row
+QTRACE_DTYPE = np.dtype(
+    [
+        ("xmin", np.float32, (2, 2, SFBMAX)),             # calc_xmin's output as outer_loop receives it (psymax bands)
+        ("max_nonzero_coeff", np.int32, (2, 2)),
+        ("xrpow_max", np.float64, (2, 2)),                # after init_xrpow, before the rate loop
+        ("old_value_mid", np.int32, (2,)),                # MPEG-1: the state gr1's search starts from (0 for LSF)
+        ("cur_step_mid", np.int32, (2,)),
+    ],
+    align=True,
+)
+
+# what OracleEncoder.traces() returns: the fields of both records
+FULL_TRACE_DTYPE = np.dtype([(n, TRACE_DTYPE.fields[n][0]) for n in TRACE_DTYPE.names] +
+                            [(n, QTRACE_DTYPE.fields[n][0]) for n in QTRACE_DTYPE.names])
+
+# lj_get_state: what an encoder carries from one call to the next
+STATE_DTYPE = np.dtype(
+    [
+        ("ath_adjust", np.float64),
+        ("ath_adjust_limit", np.float64),
+        ("blocktype_old", np.int32, (2,)),
+        ("last_attacks", np.int32, (2,)),
+        ("old_value", np.int32, (2,)),
+        ("current_step", np.int32, (2,)),
+        ("frames_done", np.int32),
+        ("mf_size", np.int32),
+        ("mf_samples_to_encode", np.int32),
+        ("pad_", np.int32),
+        ("en_l", np.float32, (2, SBMAX_l)),               # gfc.en / gfc.thm: the masking handed to the next granule
+        ("thm_l", np.float32, (2, SBMAX_l)),
+        ("en_s", np.float32, (2, SBMAX_s, 3)),
+        ("thm_s", np.float32, (2, SBMAX_s, 3)),
+    ],
+    align=True,
+)
+
 _lib = None
 
 
@@ -84,7 +121,11 @@ def lib():
         L.lj_get_lametag_frame.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]
         L.lj_crc16.argtypes = [ctypes.c_void_p, ctypes.c_longlong, ctypes.c_int]
         L.lj_wav_read_header.argtypes = [ctypes.c_void_p, ctypes.c_longlong, ctypes.c_void_p]
+        L.lj_get_state.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
+        L.lj_set_quant_trace.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]
         assert L.lj_trace_size() == TRACE_DTYPE.itemsize, (L.lj_trace_size(), TRACE_DTYPE.itemsize)
+        assert L.lj_quant_trace_size() == QTRACE_DTYPE.itemsize, (L.lj_quant_trace_size(), QTRACE_DTYPE.itemsize)
+        assert L.lj_state_size() == STATE_DTYPE.itemsize, (L.lj_state_size(), STATE_DTYPE.itemsize)
         _lib = L
     return _lib
 
@@ -110,10 +151,12 @@ class OracleEncoder:
         elif reservoir:                    # gfp.disable_reservoir = false (SURVEY 8(f2); Mp3Encoder never does this)
             assert self.L.lj_enable_reservoir(self.h) == 0
         self.tag_on = bool(write_vbr_tag) and self.L.lj_enable_vbr_tag(self.h) == 1   # gfp.bWriteVbrTag (InitVbrTag may refuse)
-        self.trace = None
+        self.trace = self.qtrace = None
         if trace_frames:
             self.trace = np.zeros(trace_frames, dtype=TRACE_DTYPE)
+            self.qtrace = np.zeros(trace_frames, dtype=QTRACE_DTYPE)
             self.L.lj_set_trace(self.h, self.trace.ctypes.data, trace_frames)
+            self.L.lj_set_quant_trace(self.h, self.qtrace.ctypes.data, trace_frames)
 
     def encode_buffer(self, left, right=None):
         left = np.ascontiguousarray(left, dtype=np.int16)
@@ -135,7 +178,20 @@ class OracleEncoder:
         return buf[:k].tobytes()
 
     def traces(self):
-        return self.trace[: self.L.lj_trace_count(self.h)]
+        """the traced frames so far: FULL_TRACE_DTYPE rows (the frame trace and the quantizer trace side by side)"""
+        n = self.L.lj_trace_count(self.h)
+        out = np.empty(n, dtype=FULL_TRACE_DTYPE)
+        for rec in (self.trace, self.qtrace):
+            for k in rec.dtype.names:
+                out[k] = rec[k][:n]
+        return out
+
+    def state(self):
+        """The state carried into the next call: one STATE_DTYPE record (ATH adjust and its limit, blocktype_old,
+        lastAttacks, OldValue, CurrentStep, frames done, the mfbuf fill level and samples to encode, and gfc.en / gfc.thm)."""
+        s = np.zeros((), dtype=STATE_DTYPE)
+        self.L.lj_get_state(self.h, s.ctypes.data)
+        return s
 
     # gfc.nMusicCRC / VBR_seek_table.nBytesWritten: kept by copy_buffer on every call (BitStream.js:924-935)
     def music_crc(self):

@@ -13,6 +13,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import edge_signals  # noqa: E402
 import handle_schedule as HS  # noqa: E402
 import oracle_lib as O  # noqa: E402
+import stage_taps  # noqa: E402
 from synth import make_signal, white  # noqa: E402
 
 
@@ -43,6 +44,19 @@ def main():
             if o != O.encode_stream(ch, sr, kbps, l, r if ch == 2 else None)[0]:
                 fail.append("%s stream %d (%d samples)" % (tag, i, len(l)))
 
+    def check_taps(tag, ch, sr, kbps, sigs):
+        """every stage tap of each stream, the quantizer's carried state included: where a stale speculated state would
+        show although the bytes agree"""
+        G = M.granules_per_frame(ch, sr, kbps)
+        for i, (l, r) in enumerate(sigs):
+            r = r if ch == 2 else None
+            F = M.stream_frames(len(l), ch, sr, kbps)
+            ref, _, tr = O.encode_stream(ch, sr, kbps, l, r, trace_frames=F + 2)
+            try:
+                stage_taps.compare(M.debug_stages(ch, sr, kbps, l, r, want=stage_taps.ALL_TAPS), tr, ref, G, ch)
+            except AssertionError as e:
+                fail.append("%s stream %d taps: %s" % (tag, i, str(e)[:300]))
+
     # ragged batches through the device entry point (the pass count is reported there): MPEG-1 (verify, repair stream)
     # and LSF (verify(1) with predict_step)
     for tag, ch, sr, kbps, frame in (("mpeg1", 2, 44100, 128, 1152), ("lsf", 2, 22050, 64, 576), ("lsf_mono", 1, 16000, 24, 576)):
@@ -55,6 +69,7 @@ def main():
         check(tag, got, ch, sr, kbps, sigs)
         check(tag + " host", M.encode_streams(ch, sr, kbps, [s[0] for s in sigs], [s[1] for s in sigs] if ch == 2 else None),
               ch, sr, kbps, sigs)
+        check_taps(tag, ch, sr, kbps, sigs)
 
     # live handles fed 5000-sample calls: several frames per call, so the handle path speculates too
     for ch, sr, kbps in ((2, 44100, 128), (1, 24000, 48)):
@@ -89,6 +104,7 @@ def main():
         got, p = device_encode(M, torch, ch, sr, kbps, sigs)
         edge_passes = max(edge_passes, p)
         check("edge %d/%d/%d" % (ch, sr, kbps), got, ch, sr, kbps, sigs)
+        check_taps("edge %d/%d/%d" % (ch, sr, kbps), ch, sr, kbps, sigs)
     passes["edge"] = edge_passes
     print(json.dumps({"fail": fail, "passes": passes}))
 

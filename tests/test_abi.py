@@ -3,6 +3,7 @@ closed-form stream geometry (no compute) matches the oracle; host-side logic fai
 import ctypes
 import os
 import re
+import subprocess
 
 import numpy as np
 import pytest
@@ -37,6 +38,39 @@ def test_stream_geometry_matches_oracle(M, oracle, n):
         assert len(data) == M.stream_bytes(2, 44100, 128, n)
     else:
         assert F == (n - 1376) // 1152 + 1 + 2 or F == (n - 1376) // 1152 + 1 + 1
+
+
+DEBUG_TAPS_FIELDS = ["size", "channels", "samplerate", "kbps", "left", "right", "nsamples", "force_blocktype", "xr", "blocktype",
+                     "en_l", "thm_l", "en_s", "thm_s", "ath_adjust", "l3_enc", "ginfo", "bytes_out", "bytes_cap", "scalefac",
+                     "subblock_gain", "xmin", "max_nonzero_coeff", "xrpow_max", "scfsi", "old_value", "cur_step"]
+
+
+def test_debug_taps_layout(M, tmp_path):
+    """mp3b200_debug_taps: the Python binding's ctypes struct has the C header's field order, offsets and size, and both are
+    pinned (16 bytes of int32 header, then 8-byte pointers / int64; 200 bytes on LP64)."""
+    from lamejs_b200.encoder import DebugTaps
+
+    assert [f[0] for f in DebugTaps._fields_] == DEBUG_TAPS_FIELDS
+    want = {n: 4 * i for i, n in enumerate(DEBUG_TAPS_FIELDS[:4])}
+    want.update({n: 16 + 8 * i for i, n in enumerate(DEBUG_TAPS_FIELDS[4:])})
+    assert {n: getattr(DebugTaps, n).offset for n in DEBUG_TAPS_FIELDS} == want
+    assert ctypes.sizeof(DebugTaps) == 200
+    src = tmp_path / "layout.c"
+    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "mp3b200.h"\nint main(void) {\n' +
+                   "".join('  printf("%%s %%zu\\n", "%s", offsetof(mp3b200_debug_taps, %s));\n' % (n, n) for n in DEBUG_TAPS_FIELDS) +
+                   '  printf("sizeof %zu\\n", sizeof(mp3b200_debug_taps));\n  return 0;\n}\n')
+    exe = tmp_path / "layout"
+    subprocess.check_call(["cc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
+    got = dict(line.split() for line in subprocess.check_output([str(exe)], text=True).splitlines())
+    assert {n: int(got[n]) for n in DEBUG_TAPS_FIELDS} == want and int(got["sizeof"]) == 200
+
+
+def test_debug_taps_size_is_checked(M):
+    """A struct of another size is refused before any device work (no GPU needed)."""
+    from lamejs_b200.encoder import DebugTaps
+
+    t = DebugTaps(size=ctypes.sizeof(DebugTaps) - 8)
+    assert M.lib().mp3b200_debug_stages_ex(ctypes.byref(t)) == -3
 
 
 def test_config_errors(M):

@@ -1,6 +1,9 @@
 """The streaming handle API under random call schedules (tests/handle_schedule.py) and at its per-handle error paths: every
 call's bytes and byte count, and the tag of the tagged streams, equal what one lamejs encoder per stream would hand out for
-the same calls (the oracle).  The directed tests cover a handle listed twice in one batch call, a failed handle inside a batch,
+the same calls (the oracle); after every operation, the state each named handle carries into its next call (its exported
+blob's header and halo: ATH adjust, block-type state, OldValue / CurrentStep, frame count, FIFO fill, the masking handed to
+the next granule) equals that stream's OracleEncoder.state(), through hand-overs and flush-then-reuse.  The directed tests
+cover a handle listed twice in one batch call, a failed handle inside a batch,
 NULL handles, a handle of another configuration, state blobs of different chunkings, and blobs whose bookkeeping was
 tampered with."""
 import ctypes
