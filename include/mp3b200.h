@@ -98,7 +98,8 @@ int64_t mp3b200_stream_frames_cfg(int channels, int samplerate, int kbps, int64_
 /* granules per frame: 2 (MPEG-1: 32 / 44.1 / 48 kHz) or 1 (MPEG-2 / 2.5: 8 .. 24 kHz); -1 if rejected */
 int mp3b200_granules_per_frame(int channels, int samplerate, int kbps);
 
-/* Host buffers.  left[s]/right[s]: nsamples[s] Int16 each (right NULL or ignored for mono).  out[s] receives
+/* Host buffers.  left[s]/right[s]: nsamples[s] Int16 each; right ignored for mono; with stereo input, right == NULL or
+ * right[s] == NULL encodes left[s] on both channels.  out[s] receives
  * out_bytes[s] = mp3b200_stream_bytes(...) bytes (cap[s] must be >= that).  Returns 0 or a negative error. */
 int mp3b200_encode_streams(int channels, int samplerate, int kbps, int nstreams, const int16_t* const* left,
                            const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
@@ -136,8 +137,9 @@ int mp3b200_encode_streams_device(int channels, int samplerate, int kbps, int ns
  *   lametag_size        the tag frame's size for a configuration (0: does not fit; negative: rejected configuration).
  *   lametag_build       the same frame from numbers instead of a handle (pure host arithmetic, no device needed): for callers
  *                       that encode one stream in segments and combine counts and CRCs themselves.
- *   encode_streams_tagged   mp3b200_encode_streams with the tag on: out[s] = finished tag frame ++ audio frames
- *                       (cap[s] >= mp3b200_stream_bytes + mp3b200_lametag_size); one k_music_crc launch for the batch. */
+ *   encode_streams_tagged   mp3b200_encode_streams with the tag on (same input rules and PCM upload): out[s] = finished
+ *                       tag frame ++ audio frames (cap[s] >= mp3b200_stream_bytes + mp3b200_lametag_size); one k_music_crc
+ *                       launch for the batch. */
 int mp3b200_set_write_vbr_tag(mp3b200_encoder* h, int on);
 int mp3b200_get_lametag_frame(mp3b200_encoder* h, uint8_t* buf, int cap);
 int mp3b200_music_crc(mp3b200_encoder* h);

@@ -2145,7 +2145,6 @@ static int quant_run(const Mp3Tables* dT, const Mp3Tables& hT, StreamDesc* d_str
   int* const list1 = B.list;                     /* frames listed by k_qstate_verify */
   int* const list2 = B.list + (F + 1);           /* short list built by the re-validating gr0 search: any flag */
   int* const list3 = B.list + 2 * (F + 1);       /* repair list: frames whose gr0 must be redone */
-  const int gq_all = grid_for(F * nch, Q_BLOCKS_PER_SM), gp_all = grid_for(F, 8);
   auto search = [&](int gr, const int* list, const int* cptr, long long count, int reval) {
     k_q_search<<<grid_for(count * nch, Q_SLIM_BLOCKS), Q_THREADS, smem_slim, st>>>(dT, d_streams, B.qs, B.ginfo, B.l3enc, B.xrpow, B.prep, gr, list, cptr, (int)count,
                                                                              reval, fresh_counter(), list2, B.counter + 1, list3, B.counter + 2);
@@ -2177,7 +2176,6 @@ static int quant_run(const Mp3Tables* dT, const Mp3Tables& hT, StreamDesc* d_str
     k_qstate_verify<<<(int)((F + 255) / 256), 256, 0, st>>>(d_streams, B.qs, F, list1, B.counter, predict_step);
     (*launches)++;
   };
-  (void)gq_all; (void)gp_all;
   const int G = hT.mode_gr;
   /* every stream contributes at most its first frame of this launch (a live encoder advancing one frame per call): all
    * in-states are the true ones, nothing is speculated, nothing to verify -- no extra launches, no host round trip */

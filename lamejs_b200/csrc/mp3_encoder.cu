@@ -49,7 +49,7 @@ bool g_fb_attr_done[MP3_MAX_DEVICES] = {};
 
 struct Config { Mp3Tables host; Mp3Tables* dev; int device; };
 std::map<std::tuple<int, int, int, int>, Config*> g_configs;   /* (device, ch, sr, kbps) */
-struct ByteGeom { int frame_bytes_nopad, frac_SpF, mode_gr; };
+struct ByteGeom { int frame_bytes_nopad, frac_SpF, mode_gr, samplerate; };
 std::map<std::tuple<int, int, int>, ByteGeom> g_byte_geom;   /* (ch, sr, kbps) -> byte geometry; frame_bytes_nopad < 0: unsupported */
 
 /* g_mu held.  Makes `dev` current for the calling thread and uploads the constant tables once per device. */
@@ -90,93 +90,117 @@ int get_config(int ch, int sr, int kbps, Config** out) {
   return 0;
 }
 
-/* frames produced by encodeBuffer(n samples) + flush()  (Lame.js:1592-1663 + :1393-1443 in closed form).
- * framesize = 576 * mode_gr; a frame is encoded whenever the FIFO holds framesize + 752 samples (calcNeeded, Lame.js:1516);
- * the FIFO starts with 528 zeros; ENCDELAY + POSTDELAY = 576 + 1152 regardless of the frame size. */
-long long frames_for(long long n, int mode_gr) {
-  const long long fs = 576LL * mode_gr, need = fs + 752;
-  const long long f_enc = 528 + n >= need ? (528 + n - need) / fs + 1 : 0;
-  long long mf_size = 528 + n - fs * f_enc;
-  const long long ste = 576 + n - fs * f_enc;            /* mf_samples_to_encode - POSTDELAY */
-  long long end_padding = fs - (ste % fs);
-  if (end_padding < 576) end_padding += fs;
-  long long frames_left = (ste + end_padding) / fs, frames = f_enc;
-  /* lame_encode_flush feeds zero bunches of min(1152, need - mf_size) samples and counts ONE frame per bunch that completed
-   * any (Lame.js:1416-1443); with 576-sample frames a bunch can complete two, so the loop is replayed, not closed-formed */
-  while (frames_left > 0) {
-    long long bunch = need - mf_size;
-    if (bunch > 1152) bunch = 1152;
-    if (bunch < 1) bunch = 1;
-    int got = 0;
-    while (bunch > 0) {
-      const long long c = bunch < fs ? bunch : fs;
-      bunch -= c; mf_size += c;
-      if (mf_size >= need) { got++; mf_size -= fs; }
-    }
-    frames += got;
-    frames_left -= got > 0 ? 1 : 0;
+/* lamejs's input FIFO (gfc.mf_size / mf_samples_to_encode), counted without the samples.  framesize = 576 * mode_gr samples
+ * enter per step of lame_encode_buffer_sample (Lame.js:1592-1663); a frame is encoded whenever the FIFO holds
+ * framesize + 752 (calcNeeded, Lame.js:1516).  A fresh encoder's FIFO holds 576 - 48 zeros and has ENCDELAY + POSTDELAY =
+ * 576 + 1152 samples to encode, whatever the frame size. */
+struct FifoFlush { long long frames, zeros, end_padding; };
+struct LameFifo {
+  static constexpr long long ENC_POST_DELAY = 576 + 1152;     /* ENCDELAY + POSTDELAY */
+  long long framesize, mf_size = 576 - 48, mf_samples_to_encode = ENC_POST_DELAY;
+  explicit LameFifo(int mode_gr) : framesize(576LL * mode_gr) {}
+  /* frames completed by feeding n samples.  Closed form of the step loop: a step adds at most framesize and takes at most
+   * one frame, so mf_size stays below framesize + 752 and the frames are the crossings of that level. */
+  long long feed(long long n) {
+    if (n <= 0) return 0;
+    const long long need = framesize + 752;
+    const long long frames = mf_size + n >= need ? (mf_size + n - need) / framesize + 1 : 0;
+    if (mf_samples_to_encode < 1) mf_samples_to_encode = ENC_POST_DELAY;
+    mf_size += n - frames * framesize;
+    mf_samples_to_encode += n - frames * framesize;
+    return frames;
   }
-  return frames;
+  /* lame_encode_flush (Lame.js:1393-1443): feeds zero bunches of min(1152, what the next frame needs) until the padded end
+   * is out; all zero once flushed (Lame.js:1397-1399).  end_padding is gfp.encoder_padding (Lame.js:1412). */
+  FifoFlush flush() {
+    FifoFlush r = {0, 0, 0};
+    if (mf_samples_to_encode < 1) return r;
+    const long long samples_to_encode = mf_samples_to_encode - 1152;     /* POSTDELAY */
+    r.end_padding = framesize - samples_to_encode % framesize;
+    if (r.end_padding < 576) r.end_padding += framesize;
+    long long frames_left = (samples_to_encode + r.end_padding) / framesize;
+    while (frames_left > 0) {
+      long long bunch = framesize + 752 - mf_size;
+      if (bunch > 1152) bunch = 1152;
+      if (bunch < 1) bunch = 1;
+      const long long got = feed(bunch);
+      r.zeros += bunch;
+      r.frames += got;
+      frames_left -= got > 0 ? 1 : 0;     /* sic (Lame.js:1443): one per bunch that completed a frame, even when a 1152-sample
+                                             bunch completed two 576-sample frames */
+    }
+    mf_samples_to_encode = 0;
+    return r;
+  }
+};
+
+/* frames produced by encodeBuffer(n samples) + flush() on a fresh encoder */
+long long frames_for(long long n, int mode_gr) {
+  LameFifo f(mode_gr);
+  const long long fed = f.feed(n);
+  return fed + f.flush().frames;
 }
 
-/* ------------------------------------------------------------------------------------------------ */
-/* Per-batch device workspace.                                                                         */
-struct Workspace {
-  int nstreams = 0, nch = 0;
-  long long units = 0, frames = 0;        /* granule rows / frame rows */
-  StreamDesc* d_streams = nullptr;
-  signed char* d_bt_final = nullptr;      /* [units][2] final block type used by MDCT + quantizer */
-  signed char* d_bt_prev = nullptr;       /* [units][2] blocktype_old seen by the masking of this granule */
-  float* d_xr = nullptr;                  /* [units][nch][576] */
-  float* d_slab = nullptr;                /* [units + nstreams][nch][18][32] subband samples (gfc.sb_sample), psy row numbering */
-  PsyUnit* d_psy = nullptr;               /* [units + nstreams][nch]  (one halo unit per stream in front) */
-  ScanIn* d_scan_in = nullptr;            /* [units + nstreams][nch] attack candidates + loudness for the scans */
-  PsyRatioDev* d_ratio = nullptr;         /* [units + nstreams][nch]  masking of unit c (used by granule c+1) */
-  double* d_ath_psy = nullptr;            /* [frames] ATH.adjust seen by the psy calls of the frame */
-  double* d_ath_q = nullptr;              /* [frames] ATH.adjust after adjust_ATH (quantizer) */
-  QuantFrameState* d_qstate = nullptr;    /* [frames] speculation bookkeeping */
-  GranuleInfoDev* d_ginfo = nullptr;      /* [units][nch] side info of the final quantization */
-  short* d_l3enc = nullptr;               /* [units][nch][576] quantised lines of a gc: after the search, parked best, final */
-  float* d_xrq = nullptr;                 /* [units][nch][576] xr as the quantizer sees it (reordered, analog silence zeroed) */
-  float* d_xrpow = nullptr;               /* [units][nch][576] |xr|^(3/4) */
-  unsigned* d_neg = nullptr;              /* [units][nch][18] sign mask of d_xrq (what the packer needs of it) */
-  GcPrep* d_prep = nullptr;               /* [units][nch] xmin + scalars of the prepared granule-channel */
-  int* d_dirty = nullptr;                 /* [frames] work list for re-quantization passes */
-  int* d_counter = nullptr;               /* [4] */
-  ScanChunk* d_scan = nullptr;            /* [frames / SCAN_FRAMES + nstreams] */
-  ~Workspace() { release(); }
+/* bytes of frames k0 .. k0 + n - 1 of a stream (g: Mp3Tables or ByteGeom): frame k is padded when pad_count steps at k */
+template <class Geom> long long bytes_of_frames(const Geom& g, long long k0, long long n) {
+  return n * g.frame_bytes_nopad + pad_count(k0 + n - 1, g.frac_SpF, g.samplerate) - pad_count(k0 - 1, g.frac_SpF, g.samplerate);
+}
+
+/* Grow-only buffer (device memory, or pinned host memory): when a call needs more than it holds, it is reallocated to
+ * max(need, 2 x capacity) elements, so a steady run of calls of one shape allocates once.  Contents are not kept. */
+template <class T, bool Pinned = false> struct Buf {
+  T* p = nullptr;
+  size_t cap = 0;
   void release() {
-    cudaFree(d_streams); cudaFree(d_bt_final); cudaFree(d_bt_prev); cudaFree(d_xr); cudaFree(d_slab); d_slab = nullptr; cudaFree(d_psy); cudaFree(d_scan_in); d_scan_in = nullptr;
-    cudaFree(d_ratio); cudaFree(d_ath_psy); cudaFree(d_ath_q); cudaFree(d_qstate); cudaFree(d_ginfo);
-    cudaFree(d_l3enc); cudaFree(d_xrq); d_xrq = nullptr; cudaFree(d_xrpow); d_xrpow = nullptr; cudaFree(d_neg); d_neg = nullptr; cudaFree(d_prep); d_prep = nullptr; cudaFree(d_dirty); cudaFree(d_counter); cudaFree(d_scan); d_scan = nullptr;
-    d_streams = nullptr; d_bt_final = d_bt_prev = nullptr; d_xr = nullptr; d_psy = nullptr; d_ratio = nullptr;
-    d_ath_psy = d_ath_q = nullptr; d_qstate = nullptr; d_ginfo = nullptr; d_l3enc = nullptr; d_dirty = nullptr; d_counter = nullptr;
+    if (Pinned) cudaFreeHost(p); else cudaFree(p);
+    p = nullptr; cap = 0;
   }
-  int alloc(int S, int nch_, long long U, long long F, bool want_l3enc) {
+  int fit(size_t n) {
+    if (n <= cap) return 0;
+    if (n < 2 * cap) n = 2 * cap;
     release();
-    nstreams = S; nch = nch_; units = U; frames = F;
-    CK(cudaMalloc(&d_streams, sizeof(StreamDesc) * S));
-    CK(cudaMalloc(&d_bt_final, (size_t)U * 2 + 16));
-    CK(cudaMalloc(&d_bt_prev, (size_t)U * 2 + 16));
-    CK(cudaMalloc(&d_xr, sizeof(float) * (size_t)U * nch * 576));
-    CK(cudaMalloc(&d_slab, sizeof(float) * (size_t)(U + S) * nch * 576));
-    CK(cudaMalloc(&d_psy, sizeof(PsyUnit) * (size_t)(U + S) * nch));
-    CK(cudaMalloc(&d_scan_in, sizeof(ScanIn) * (size_t)(U + S) * nch));
-    CK(cudaMalloc(&d_ratio, sizeof(PsyRatioDev) * (size_t)(U + S) * nch));
-    CK(cudaMalloc(&d_ath_psy, sizeof(double) * (size_t)(F + 1)));
-    CK(cudaMalloc(&d_ath_q, sizeof(double) * (size_t)(F + 1)));
-    CK(cudaMalloc(&d_qstate, sizeof(QuantFrameState) * (size_t)(F + 1)));
-    CK(cudaMalloc(&d_ginfo, sizeof(GranuleInfoDev) * (size_t)U * nch));
-    (void)want_l3enc;
-    CK(cudaMalloc(&d_l3enc, sizeof(short) * (size_t)U * nch * 576));
-    CK(cudaMalloc(&d_xrq, sizeof(float) * (size_t)U * nch * 576));
-    CK(cudaMalloc(&d_xrpow, sizeof(float) * (size_t)U * nch * 576));
-    CK(cudaMalloc(&d_neg, sizeof(unsigned) * (size_t)U * nch * 18));
-    CK(cudaMalloc(&d_prep, sizeof(GcPrep) * (size_t)U * nch));
-    CK(cudaMalloc(&d_dirty, sizeof(int) * 3 * (size_t)(F + 1)));
-    CK(cudaMalloc(&d_counter, sizeof(int) * Q_NCOUNTERS));
-    CK(cudaMalloc(&d_scan, sizeof(ScanChunk) * (size_t)(F / SCAN_FRAMES + S + 1)));
+    CK(Pinned ? cudaMallocHost((void**)&p, sizeof(T) * n) : cudaMalloc((void**)&p, sizeof(T) * n));
+    cap = n;
     return 0;
+  }
+};
+
+/* ------------------------------------------------------------------------------------------------ */
+/* Per-launch device workspace (U granule rows, F frame rows, S streams of nch channels).                */
+struct Workspace {
+  Buf<StreamDesc> streams;
+  Buf<signed char> bt_final;              /* [U][2] final block type used by MDCT + quantizer */
+  Buf<signed char> bt_prev;               /* [U][2] blocktype_old seen by the masking of this granule */
+  Buf<float> xr;                          /* [U][nch][576] */
+  Buf<float> slab;                        /* [U + S][nch][18][32] subband samples (gfc.sb_sample), psy row numbering */
+  Buf<PsyUnit> psy;                       /* [U + S][nch]  (one halo unit per stream in front) */
+  Buf<ScanIn> scan_in;                    /* [U + S][nch] attack candidates + loudness for the scans */
+  Buf<PsyRatioDev> ratio;                 /* [U + S][nch]  masking of unit c (used by granule c+1) */
+  Buf<double> ath_psy;                    /* [F] ATH.adjust seen by the psy calls of the frame */
+  Buf<double> ath_q;                      /* [F] ATH.adjust after adjust_ATH (quantizer) */
+  Buf<QuantFrameState> qstate;            /* [F] speculation bookkeeping */
+  Buf<GranuleInfoDev> ginfo;              /* [U][nch] side info of the final quantization */
+  Buf<short> l3enc;                       /* [U][nch][576] quantised lines of a gc: after the search, parked best, final */
+  Buf<float> xrq;                         /* [U][nch][576] xr as the quantizer sees it (reordered, analog silence zeroed) */
+  Buf<float> xrpow;                       /* [U][nch][576] |xr|^(3/4) */
+  Buf<unsigned> neg;                      /* [U][nch][18] sign mask of xrq (what the packer needs of it) */
+  Buf<GcPrep> prep;                       /* [U][nch] xmin + scalars of the prepared granule-channel */
+  Buf<int> dirty;                         /* [3][F] work lists for re-quantization passes */
+  Buf<int> counter;                       /* [Q_NCOUNTERS] */
+  Buf<ScanChunk> scan;                    /* [F / SCAN_FRAMES + S] */
+  int fit(int S, int nch, long long U, long long F) {
+    const size_t gc = (size_t)U * nch, rows = (size_t)(U + S) * nch, f = (size_t)F + 1;
+    const bool failed = streams.fit(S) || bt_final.fit((size_t)U * 2 + 16) || bt_prev.fit((size_t)U * 2 + 16) ||
+                        xr.fit(gc * 576) || slab.fit(rows * 576) || psy.fit(rows) || scan_in.fit(rows) || ratio.fit(rows) ||
+                        ath_psy.fit(f) || ath_q.fit(f) || qstate.fit(f) || ginfo.fit(gc) || l3enc.fit(gc * 576) ||
+                        xrq.fit(gc * 576) || xrpow.fit(gc * 576) || neg.fit(gc * 18) || prep.fit(gc) || dirty.fit(3 * f) ||
+                        counter.fit(Q_NCOUNTERS) || scan.fit((size_t)(F / SCAN_FRAMES + S + 1));
+    return failed ? MP3B200_ERR_CUDA : 0;
+  }
+  void release() {
+    streams.release(); bt_final.release(); bt_prev.release(); xr.release(); slab.release(); psy.release(); scan_in.release();
+    ratio.release(); ath_psy.release(); ath_q.release(); qstate.release(); ginfo.release(); l3enc.release(); xrq.release();
+    xrpow.release(); neg.release(); prep.release(); dirty.release(); counter.release(); scan.release();
   }
 };
 
@@ -192,18 +216,15 @@ struct ThreadCtx {
   cudaEvent_t ev[8] = {}, evq[QE_COUNT] = {}, ev_in = nullptr, ev_fork = nullptr, ev_join = nullptr, ready[MP3_MAX_PCM_CHUNKS] = {};
   Workspace ws;
   int evq_pred[QE_COUNT] = {};
-  int16_t* d_pcm = nullptr; size_t d_pcm_cap = 0;
-  uint8_t* d_out = nullptr; size_t d_out_cap = 0;
-  uint8_t* h_pin = nullptr; size_t h_pin_cap = 0;       /* pinned host staging */
-  long long* d_crc_ranges = nullptr; unsigned* d_crc = nullptr; int crc_cap = 0;   /* music CRC: [2][cap] offsets / lengths, [cap] results */
+  Buf<int16_t> pcm;                       /* staged PCM of host callers */
+  Buf<uint8_t> out;                       /* encoded bytes of host callers */
+  Buf<uint8_t, true> pin;                 /* pinned host staging */
+  Buf<long long> crc_ranges;              /* music CRC: [2][R] offsets / lengths */
+  Buf<unsigned> crc;                      /* music CRC: [R] results */
   void release() {
     if (device < 0) return;
     cudaSetDevice(device);
-    ws.release(); ws.units = ws.frames = 0; ws.nstreams = 0;
-    cudaFree(d_pcm); d_pcm = nullptr; d_pcm_cap = 0;
-    cudaFree(d_out); d_out = nullptr; d_out_cap = 0;
-    cudaFreeHost(h_pin); h_pin = nullptr; h_pin_cap = 0;
-    cudaFree(d_crc_ranges); d_crc_ranges = nullptr; cudaFree(d_crc); d_crc = nullptr; crc_cap = 0;
+    ws.release(); pcm.release(); out.release(); pin.release(); crc_ranges.release(); crc.release();
     for (auto& e : ev) if (e) { cudaEventDestroy(e); e = nullptr; }
     for (auto& e : evq) if (e) { cudaEventDestroy(e); e = nullptr; }
     for (auto& e : ready) if (e) { cudaEventDestroy(e); e = nullptr; }
@@ -236,35 +257,6 @@ struct ThreadCtx {
     device = dev;
     return 0;
   }
-  int need_pcm(size_t samples) {
-    if (d_pcm_cap >= samples) return 0;
-    cudaFree(d_pcm); d_pcm = nullptr; d_pcm_cap = 0;
-    CK(cudaMalloc(&d_pcm, sizeof(int16_t) * samples));
-    d_pcm_cap = samples;
-    return 0;
-  }
-  int need_out(size_t bytes) {
-    if (d_out_cap >= bytes) return 0;
-    cudaFree(d_out); d_out = nullptr; d_out_cap = 0;
-    CK(cudaMalloc(&d_out, bytes));
-    d_out_cap = bytes;
-    return 0;
-  }
-  int need_crc(int ranges) {
-    if (crc_cap >= ranges) return 0;
-    cudaFree(d_crc_ranges); d_crc_ranges = nullptr; cudaFree(d_crc); d_crc = nullptr; crc_cap = 0;
-    CK(cudaMalloc(&d_crc_ranges, sizeof(long long) * 2 * (size_t)ranges));
-    CK(cudaMalloc(&d_crc, sizeof(unsigned) * (size_t)ranges));
-    crc_cap = ranges;
-    return 0;
-  }
-  int need_pin(size_t bytes) {
-    if (h_pin_cap >= bytes) return 0;
-    cudaFreeHost(h_pin); h_pin = nullptr; h_pin_cap = 0;
-    CK(cudaMallocHost(&h_pin, bytes));
-    h_pin_cap = bytes;
-    return 0;
-  }
 };
 thread_local ThreadCtx t_ctx;
 
@@ -282,38 +274,47 @@ bool debug_sync() { static int v = -1; if (v < 0) { const char* e = getenv("MP3B
 struct Timings { float psy = 0, scan = 0, mask = 0, fb = 0, q1 = 0, qn = 0, total = 0; int passes = 0;
                  float q_prepare = 0, q_search = 0, q_outer = 0, q_finish = 0, q_pack = 0, q_mid = 0; };
 
-/* Runs the whole pipeline for the streams described in `h_streams` (device pointers already set).
- * d_out: device output buffer.  force_bt: optional host array [units][nch] of block types (debug). */
-/* pcm_chunks > 1: the caller uploads each stream's PCM in that many time slices on another stream and records
- * pcm_ready[j] after slice j; the psy analysis of slice j starts as soon as it has landed. */
+/* chunks > 1: the caller uploads each stream's PCM in that many time slices on another stream and records ready[j] after
+ * slice j; the psy analysis of slice j starts as soon as it has landed. */
 struct PcmArrival { int chunks = 1; cudaEvent_t* ready = nullptr; };
 
-/* All launches go to the calling thread's stream (t_ctx.st), which first waits for whatever the caller queued on the
- * legacy default stream (torch and plain CUDA callers produce their device buffers there); the call returns after the
- * stream has drained, so the results are visible to any stream afterwards. */
-int run_pipeline(Config* cfg, Workspace& ws, std::vector<StreamDesc>& h_streams, uint8_t* d_out, const int32_t* force_bt,
-                 bool stop_after_mdct, Timings* tm, const PcmArrival* arrival = nullptr, bool sync = true) {
+/* Options of launch_streams */
+struct LaunchOpts {
+  const int32_t* force_bt = nullptr;     /* debug: host [units][nch] block types overriding the psy model's decision */
+  bool stop_after_mdct = false;          /* debug: no quantizer, no bytes */
+  const PcmArrival* arrival = nullptr;   /* PCM still landing on the upload stream */
+  float* timings_ms = nullptr;           /* the 16 timing slots of include/mp3b200.h */
+  bool sync = true;                      /* false: return with the work queued on t_ctx.st (no timings) */
+  StreamDesc* committed = nullptr;       /* host: each stream's descriptor as the pipeline left it (the carried state),
+                                            valid once t_ctx.st has drained */
+};
+
+/* One pipeline launch for the streams sds[0 .. S) (at most MP3_MAX_LAUNCH_STREAMS, unit / frame bases set, the workspace
+ * large enough).  All launches go to the calling thread's stream (t_ctx.st), which first waits for whatever the caller
+ * queued on the legacy default stream (torch and plain CUDA callers produce their device buffers there); with o.sync the
+ * call returns after the stream has drained, so the results are visible to any stream afterwards. */
+int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, const LaunchOpts& o, const PcmArrival* arrival,
+                 Timings* tm) {
   cudaStream_t st = t_ctx.st;
   cudaEvent_t* ev = t_ctx.ev;
+  Workspace& ws = t_ctx.ws;
 
-  const int S = (int)h_streams.size();
   const int nch = cfg->host.nch;
   int max_frames = 0;
   long long total_frames = 0;          /* rows actually used this launch (the workspace may be larger) */
   int scan_rows = 0;
   int streams_with_frames = 0;
-  for (auto& s : h_streams) {
+  for (int i = 0; i < S; i++) {
+    StreamDesc& s = h_streams[i];
     max_frames = s.nframes > max_frames ? s.nframes : max_frames;
     total_frames += s.nframes;
     streams_with_frames += s.nframes > 0 ? 1 : 0;
     s.scan_base = scan_rows;
     scan_rows += (s.nframes + SCAN_FRAMES - 1) / SCAN_FRAMES;
   }
-  if (S == 0 || total_frames == 0) { if (tm) *tm = Timings(); return 0; }   /* empty batch: nothing to launch */
-  if (S > MP3_MAX_LAUNCH_STREAMS) { g_err = "internal: more streams in one pipeline launch than a grid dimension holds"; return MP3B200_ERR_CUDA; }
   CK(cudaEventRecord(t_ctx.ev_in, cudaStreamLegacy));
   CK(cudaStreamWaitEvent(st, t_ctx.ev_in, 0));
-  CK(cudaMemcpyAsync(ws.d_streams, h_streams.data(), sizeof(StreamDesc) * S, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ws.streams.p, h_streams, sizeof(StreamDesc) * S, cudaMemcpyHostToDevice, st));
   CK(cudaEventRecord(ev[0], st));
 
   /* K2: psy analysis, one block per (granule incl. 1 halo, channel, stream) */
@@ -325,7 +326,8 @@ int run_pipeline(Config* cfg, Workspace& ws, std::vector<StreamDesc>& h_streams,
     const int G = cfg->host.mode_gr;     /* granules ("units") per frame */
     for (int j = 0; j < nchunks; j++) { u_lo[j] = G * max_frames; u_hi[j] = -1; }
     if (nchunks > 1) {
-      for (const auto& sd : h_streams) {
+      for (int s = 0; s < S; s++) {
+        const StreamDesc& sd = h_streams[s];
         const long long n = sd.pcm_end - sd.pcm_base;
         for (int u = -1; u < G * sd.nframes; u++) {
           long long last = 576 * ((long long)G * sd.frame0 + u) - 224 + 1023 - sd.pcm_base;
@@ -341,7 +343,7 @@ int run_pipeline(Config* cfg, Workspace& ws, std::vector<StreamDesc>& h_streams,
       if (arrival) CK(cudaStreamWaitEvent(st, arrival->ready[j], 0));
       if (u_hi[j] <= u_lo[j]) continue;
       dim3 gridj(u_hi[j] - u_lo[j], nch, S);
-      k_psy_analysis<<<gridj, PSY_THREADS, 0, st>>>(cfg->dev, ws.d_streams, ws.d_psy, j, nchunks, u_lo[j]);
+      k_psy_analysis<<<gridj, PSY_THREADS, 0, st>>>(cfg->dev, ws.streams.p, ws.psy.p, j, nchunks, u_lo[j]);
       g_launches++;
       DBG("k_psy_analysis");
     }
@@ -350,9 +352,9 @@ int run_pipeline(Config* cfg, Workspace& ws, std::vector<StreamDesc>& h_streams,
   /* K3a: attack pre-pass (parallel) + sequential per-stream scans */
   {
     dim3 grid((cfg->host.mode_gr * max_frames + 127) / 128, 1, S);
-    k_attack_prepass<<<grid, 128, 0, st>>>(cfg->dev, ws.d_streams, ws.d_psy, ws.d_scan_in);
+    k_attack_prepass<<<grid, 128, 0, st>>>(cfg->dev, ws.streams.p, ws.psy.p, ws.scan_in.p);
     DBG("k_attack_prepass");
-    k_stream_scan<<<S, SCAN_THREADS, 0, st>>>(cfg->dev, ws.d_streams, S, ws.d_scan_in, ws.d_bt_final, ws.d_bt_prev, ws.d_ath_psy, ws.d_ath_q, ws.d_scan);
+    k_stream_scan<<<S, SCAN_THREADS, 0, st>>>(cfg->dev, ws.streams.p, S, ws.scan_in.p, ws.bt_final.p, ws.bt_prev.p, ws.ath_psy.p, ws.ath_q.p, ws.scan.p);
     g_launches += 2;
     DBG("k_stream_scan");
     /* K1a: subband analysis, programmatic dependent of the scan (reads nothing the scan writes; see k_stream_scan) */
@@ -370,23 +372,24 @@ int run_pipeline(Config* cfg, Workspace& ws, std::vector<StreamDesc>& h_streams,
       at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
       at[0].val.programmaticStreamSerializationAllowed = 1;
       lc.attrs = at; lc.numAttrs = 1;
-      CK(cudaLaunchKernelEx(&lc, k_subband_analysis, (const Mp3Tables*)cfg->dev, (const StreamDesc*)ws.d_streams, ws.d_slab));
+      CK(cudaLaunchKernelEx(&lc, k_subband_analysis, (const Mp3Tables*)cfg->dev, (const StreamDesc*)ws.streams.p, ws.slab.p));
       g_launches++;
       DBG("k_subband_analysis");
     }
   }
   CK(cudaEventRecord(ev[2], st));
-  if (force_bt) {   /* debug: override block decision for the filterbank */
-    std::vector<signed char> bt((size_t)ws.units * 2, 0);
-    for (long long u = 0; u < ws.units; u++)
-      for (int c = 0; c < nch; c++) bt[u * 2 + c] = (signed char)force_bt[u * nch + c];
-    CK(cudaMemcpyAsync(ws.d_bt_final, bt.data(), bt.size(), cudaMemcpyHostToDevice, st));
+  if (o.force_bt) {   /* debug: override block decision for the filterbank */
+    const long long units = (long long)cfg->host.mode_gr * total_frames;
+    std::vector<signed char> bt((size_t)units * 2, 0);
+    for (long long u = 0; u < units; u++)
+      for (int c = 0; c < nch; c++) bt[u * 2 + c] = (signed char)o.force_bt[u * nch + c];
+    CK(cudaMemcpyAsync(ws.bt_final.p, bt.data(), bt.size(), cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));
   }
   /* K3b: masking thresholds */
   {
     dim3 grid(cfg->host.mode_gr * max_frames + 1, 1, S);
-    k_psy_masking<<<grid, MASK_THREADS, 0, st>>>(cfg->dev, ws.d_streams, ws.d_psy, ws.d_bt_prev, ws.d_ath_psy, ws.d_ratio);
+    k_psy_masking<<<grid, MASK_THREADS, 0, st>>>(cfg->dev, ws.streams.p, ws.psy.p, ws.bt_prev.p, ws.ath_psy.p, ws.ratio.p);
     g_launches++;
     DBG("k_psy_masking");
   }
@@ -395,23 +398,23 @@ int run_pipeline(Config* cfg, Workspace& ws, std::vector<StreamDesc>& h_streams,
    * it saves only a few microseconds for the pair -- not worth losing the per-kernel times.) */
   {
     dim3 grid((cfg->host.mode_gr * max_frames + FB_G - 1) / FB_G, nch, S);
-    k_mdct<<<grid, FB_G * 32, 0, st>>>(cfg->dev, ws.d_streams, ws.d_slab, ws.d_bt_final, ws.d_xr);
+    k_mdct<<<grid, FB_G * 32, 0, st>>>(cfg->dev, ws.streams.p, ws.slab.p, ws.bt_final.p, ws.xr.p);
     g_launches++;
     DBG("k_mdct");
   }
   CK(cudaEventRecord(ev[4], st));
   int passes = 0;
-  if (!stop_after_mdct) {
+  if (!o.stop_after_mdct) {
     QuantBuffers qb;
-    qb.xr = ws.d_xr; qb.ratio = ws.d_ratio; qb.bt = ws.d_bt_final; qb.ath_q = ws.d_ath_q; qb.qs = ws.d_qstate; qb.ginfo = ws.d_ginfo;
-    qb.l3enc = ws.d_l3enc; qb.xrq = ws.d_xrq; qb.xrpow = ws.d_xrpow; qb.neg = ws.d_neg; qb.prep = ws.d_prep; qb.list = ws.d_dirty; qb.counter = ws.d_counter;
-    int rc = quant_run(cfg->dev, cfg->host, ws.d_streams, S, streams_with_frames, max_frames, total_frames, qb, d_out, st, t_ctx.aux_st, t_ctx.ev_fork, t_ctx.ev_join, ev[5], t_ctx.evq, t_ctx.evq_pred, &passes, &g_launches);
+    qb.xr = ws.xr.p; qb.ratio = ws.ratio.p; qb.bt = ws.bt_final.p; qb.ath_q = ws.ath_q.p; qb.qs = ws.qstate.p; qb.ginfo = ws.ginfo.p;
+    qb.l3enc = ws.l3enc.p; qb.xrq = ws.xrq.p; qb.xrpow = ws.xrpow.p; qb.neg = ws.neg.p; qb.prep = ws.prep.p; qb.list = ws.dirty.p; qb.counter = ws.counter.p;
+    int rc = quant_run(cfg->dev, cfg->host, ws.streams.p, S, streams_with_frames, max_frames, total_frames, qb, d_out, st, t_ctx.aux_st, t_ctx.ev_fork, t_ctx.ev_join, ev[5], t_ctx.evq, t_ctx.evq_pred, &passes, &g_launches);
     if (rc) { g_err = "quantizer stage failed: " + std::string(cudaGetErrorString(cudaGetLastError())); return rc; }
   } else {
     CK(cudaEventRecord(ev[5], st));
   }
   CK(cudaEventRecord(ev[6], st));
-  if (!sync) return 0;                     /* the caller queues its copies behind the kernels and synchronises once */
+  if (!o.sync) return 0;                   /* the caller queues its copies behind the kernels and synchronises once */
   CK(cudaStreamSynchronize(st));
   CK(cudaGetLastError());
   if (tm) {
@@ -423,7 +426,7 @@ int run_pipeline(Config* cfg, Workspace& ws, std::vector<StreamDesc>& h_streams,
     cudaEventElapsedTime(&tm->qn, ev[5], ev[6]);
     cudaEventElapsedTime(&tm->total, ev[0], ev[6]);
     tm->passes = passes;
-    if (!stop_after_mdct && passes > 0) {
+    if (!o.stop_after_mdct && passes > 0) {
       auto span = [&](int slot) { float v = 0; const int p = t_ctx.evq_pred[slot]; if (p >= 0) cudaEventElapsedTime(&v, t_ctx.evq[p], t_ctx.evq[slot]); return v; };
       tm->q_prepare = span(QE_PREP);
       tm->q_search = span(QE_S0) + span(QE_S1);
@@ -444,8 +447,40 @@ void init_stream_state(StreamDesc& sd) {   /* lame_init_old + psymodel_init star
   sd.current_step[0] = sd.current_step[1] = 4;
 }
 
-long long bytes_for(const Mp3Tables& t, long long frames) {
-  return frames * t.frame_bytes_nopad + pad_count(frames - 1, t.frac_SpF, t.samplerate);
+/* Encodes the streams `sds` into d_out: the caller sets each descriptor's PCM, pcm_base / pcm_end, frame0, nframes,
+ * out_base and carried state; this assigns unit_base / frame_base, grows the thread's workspace and runs the pipeline.
+ * The stream index is a grid y / z coordinate of several kernels (CUDA limit 65535): a larger batch runs as consecutive
+ * launches of at most MP3_MAX_LAUNCH_STREAMS streams on the thread's stream, the later ones behind every PCM upload.
+ * Timings add up over the launches; the pass count is the largest any of them needed. */
+int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, const LaunchOpts& o) {
+  if (o.timings_ms) for (int i = 0; i < 16; i++) o.timings_ms[i] = 0.0f;
+  const PcmArrival* arrival = o.arrival;
+  const int nstreams = (int)sds.size();
+  for (int g0 = 0; g0 < nstreams; g0 += MP3_MAX_LAUNCH_STREAMS) {
+    const int n = nstreams - g0 < MP3_MAX_LAUNCH_STREAMS ? nstreams - g0 : MP3_MAX_LAUNCH_STREAMS;
+    StreamDesc* group = sds.data() + g0;
+    long long U = 0, F = 0;
+    for (int i = 0; i < n; i++) {
+      group[i].unit_base = (int)U; group[i].frame_base = (int)F;
+      U += (long long)cfg->host.mode_gr * group[i].nframes; F += group[i].nframes;
+    }
+    if (F == 0) continue;                     /* empty group: nothing to launch */
+    int rc = t_ctx.ws.fit(n, cfg->host.nch, U, F);
+    if (rc) return rc;
+    Timings tm;
+    rc = run_pipeline(cfg, group, n, d_out, o, arrival, &tm);
+    if (rc) return rc;
+    arrival = nullptr;
+    if (o.committed)
+      CK(cudaMemcpyAsync(o.committed + g0, t_ctx.ws.streams.p, sizeof(StreamDesc) * n, cudaMemcpyDeviceToHost, t_ctx.st));
+    if (o.timings_ms) {
+      const float t[16] = {tm.psy, tm.scan, tm.mask, tm.fb, tm.q1, tm.qn, tm.total, 0.0f,
+                           tm.q_prepare, tm.q_search, tm.q_outer, tm.q_finish, tm.q_pack, tm.q_mid, 0.0f, 0.0f};
+      for (int i = 0; i < 16; i++) o.timings_ms[i] += t[i];
+      if ((float)tm.passes > o.timings_ms[7]) o.timings_ms[7] = (float)tm.passes;
+    }
+  }
+  return 0;
 }
 
 }  // namespace
@@ -481,7 +516,7 @@ ByteGeom byte_geom(int channels, int samplerate, int kbps) {
   if (it != g_byte_geom.end()) return it->second;
   Mp3Tables* t = new Mp3Tables();
   const int rc = mp3_build_tables(channels, samplerate, kbps, t);
-  ByteGeom g = rc == 0 ? ByteGeom{t->frame_bytes_nopad, t->frac_SpF, t->mode_gr} : ByteGeom{-1, 0, 2};
+  ByteGeom g = rc == 0 ? ByteGeom{t->frame_bytes_nopad, t->frac_SpF, t->mode_gr, t->samplerate} : ByteGeom{-1, 0, 2, samplerate};
   delete t;
   g_byte_geom[key] = g;
   return g;
@@ -491,8 +526,7 @@ ByteGeom byte_geom(int channels, int samplerate, int kbps) {
 int64_t mp3b200_stream_bytes(int channels, int samplerate, int kbps, int64_t nsamples) {
   const ByteGeom g = byte_geom(channels, samplerate, kbps);
   if (g.frame_bytes_nopad < 0 || nsamples < 0) return -1;
-  const long long frames = frames_for(nsamples, g.mode_gr);
-  return frames * g.frame_bytes_nopad + pad_count(frames - 1, g.frac_SpF, samplerate);
+  return bytes_of_frames(g, 0, frames_for(nsamples, g.mode_gr));
 }
 
 int64_t mp3b200_stream_frames_cfg(int channels, int samplerate, int kbps, int64_t nsamples) {
@@ -509,48 +543,73 @@ int mp3b200_granules_per_frame(int channels, int samplerate, int kbps) {
 }  // extern "C"
 
 namespace {
-int encode_streams_device_impl(Config* cfg, int channels, int nstreams, const int16_t* d_pcm, const int64_t* pcm_off,
-                               const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off, float* timings_ms,
-                               const PcmArrival* arrival) {
-  int rc = 0;
-  if (timings_ms) for (int i = 0; i < 16; i++) timings_ms[i] = 0.0f;
-  /* Streams are independent: a batch wider than one launch can hold runs as consecutive groups on the thread's stream.
-   * The times add up over the groups; the pass count is the largest any group needed. */
-  for (int g0 = 0; g0 < nstreams; g0 += MP3_MAX_LAUNCH_STREAMS) {
-    const int n = nstreams - g0 < MP3_MAX_LAUNCH_STREAMS ? nstreams - g0 : MP3_MAX_LAUNCH_STREAMS;
-    std::vector<StreamDesc> sds(n);
-    long long U = 0, F = 0;
-    for (int i = 0; i < n; i++) {
-      const int s = g0 + i;
-      StreamDesc& sd = sds[i];
-      memset(&sd, 0, sizeof sd);
-      sd.pcm[0] = d_pcm + pcm_off[s];
-      sd.pcm[1] = channels == 2 ? d_pcm + pcm_off[s] + nsamples[s] : sd.pcm[0];
-      sd.pcm_base = 0; sd.pcm_end = nsamples[s];
-      sd.frame0 = 0; sd.nframes = (int)frames_for(nsamples[s], cfg->host.mode_gr);
-      sd.unit_base = (int)U; sd.frame_base = (int)F;
-      sd.out_base = out_off[s];
-      init_stream_state(sd);
-      U += (long long)cfg->host.mode_gr * sd.nframes; F += sd.nframes;
-    }
-    if (F == 0) continue;                     /* empty group: nothing to launch */
-    Workspace& ws = t_ctx.ws;
-    if (ws.units < U || ws.frames < F || ws.nstreams < n || ws.nch != cfg->host.nch) {
-      rc = ws.alloc(n, cfg->host.nch, U, F, false);
-      if (rc) return rc;
-    }
-    Timings tm;
-    rc = run_pipeline(cfg, ws, sds, d_out, nullptr, false, &tm, arrival);
-    if (rc) return rc;
-    arrival = nullptr;                        /* the later groups run behind the first one, after every upload landed */
-    if (timings_ms) {
-      const float t[16] = {tm.psy, tm.scan, tm.mask, tm.fb, tm.q1, tm.qn, tm.total, 0.0f,
-                           tm.q_prepare, tm.q_search, tm.q_outer, tm.q_finish, tm.q_pack, tm.q_mid, 0.0f, 0.0f};
-      for (int i = 0; i < 16; i++) timings_ms[i] += t[i];
-      if ((float)tm.passes > timings_ms[7]) timings_ms[7] = (float)tm.passes;
-    }
+/* Whole streams (encodeBuffer(everything) + flush() on fresh encoders): stream s reads nsamples[s] samples per channel at
+ * d_pcm + pcm_off[s] (stereo: the right channel follows the left) and writes its bytes at out_off[s]. */
+std::vector<StreamDesc> whole_streams(Config* cfg, int nstreams, const int16_t* d_pcm, const int64_t* pcm_off,
+                                      const int64_t* nsamples, const int64_t* out_off) {
+  std::vector<StreamDesc> sds(nstreams);
+  for (int s = 0; s < nstreams; s++) {
+    StreamDesc& sd = sds[s];
+    memset(&sd, 0, sizeof sd);
+    sd.pcm[0] = d_pcm + pcm_off[s];
+    sd.pcm[1] = cfg->host.nch == 2 ? sd.pcm[0] + nsamples[s] : sd.pcm[0];
+    sd.pcm_base = 0; sd.pcm_end = nsamples[s];
+    sd.frame0 = 0; sd.nframes = (int)frames_for(nsamples[s], cfg->host.mode_gr);
+    sd.out_base = out_off[s];
+    init_stream_state(sd);
   }
-  return 0;
+  return sds;
+}
+
+/* Whole streams from host buffers: checks that out[s] has room for the stream's audio[s] bytes plus `extra`
+ * (out_bytes[s] = their sum), stages the PCM in the thread's buffers and encodes the batch into t_ctx.out, stream s at
+ * out_off[s].  Stereo input with right == NULL or right[s] == NULL encodes left[s] on both channels. */
+int encode_host_streams(Config* cfg, int nstreams, const int16_t* const* left, const int16_t* const* right,
+                        const int64_t* nsamples, const int64_t* cap, int extra, int64_t* out_bytes,
+                        std::vector<int64_t>& out_off, std::vector<long long>& audio) {
+  const int nch = cfg->host.nch;
+  std::vector<int64_t> pcm_off(nstreams);
+  out_off.assign(nstreams, 0);
+  audio.assign(nstreams, 0);
+  long long tot_samples = 0, tot_bytes = 0;
+  for (int s = 0; s < nstreams; s++) {
+    pcm_off[s] = tot_samples;
+    tot_samples += nsamples[s] * nch;
+    out_off[s] = tot_bytes;
+    audio[s] = bytes_of_frames(cfg->host, 0, frames_for(nsamples[s], cfg->host.mode_gr));
+    if (cap[s] < audio[s] + extra) { g_err = "output buffer too small"; return MP3B200_ERR_BUFFER; }
+    out_bytes[s] = audio[s] + extra;
+    tot_bytes += audio[s];
+  }
+  if (nstreams == 0) return MP3B200_OK;
+  int rc = t_ctx.use(cfg->device);
+  if (rc) return rc;
+  rc = t_ctx.pcm.fit((size_t)tot_samples + 8);
+  if (rc) return rc;
+  rc = t_ctx.out.fit((size_t)tot_bytes + 8);
+  if (rc) return rc;
+  int16_t* d_pcm = t_ctx.pcm.p;
+  /* Upload in time slices on a copy stream; the psy analysis of a slice starts when it has landed, so only the first
+   * slice's transfer is exposed.  Many small streams are uploaded whole (one slice): per-copy overhead would win. */
+  PcmArrival arr;
+  arr.chunks = (nstreams <= 8 && tot_samples >= (1 << 20)) ? MP3_MAX_PCM_CHUNKS : 1;
+  arr.ready = t_ctx.ready;
+  for (int j = 0; j < arr.chunks; j++) {
+    for (int s = 0; s < nstreams; s++) {
+      const int64_t lo = nsamples[s] * j / arr.chunks, hi = nsamples[s] * (j + 1) / arr.chunks;
+      if (hi <= lo) continue;
+      CK(cudaMemcpyAsync(d_pcm + pcm_off[s] + lo, left[s] + lo, sizeof(int16_t) * (hi - lo), cudaMemcpyHostToDevice, t_ctx.up_st));
+      if (nch == 2) {
+        const int16_t* r = (right && right[s]) ? right[s] : left[s];
+        CK(cudaMemcpyAsync(d_pcm + pcm_off[s] + nsamples[s] + lo, r + lo, sizeof(int16_t) * (hi - lo), cudaMemcpyHostToDevice, t_ctx.up_st));
+      }
+    }
+    CK(cudaEventRecord(t_ctx.ready[j], t_ctx.up_st));
+  }
+  std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off.data(), nsamples, out_off.data());
+  LaunchOpts o;
+  o.arrival = &arr;
+  return launch_streams(cfg, sds, t_ctx.out.p, o);
 }
 
 }  // namespace
@@ -566,7 +625,10 @@ int mp3b200_encode_streams_device(int channels, int samplerate, int kbps, int ns
   if (rc) return rc;
   rc = t_ctx.use(cfg->device);
   if (rc) return rc;
-  return encode_streams_device_impl(cfg, channels, nstreams, d_pcm, pcm_off, nsamples, d_out, out_off, timings_ms, nullptr);
+  std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off, nsamples, out_off);
+  LaunchOpts o;
+  o.timings_ms = timings_ms;
+  return launch_streams(cfg, sds, d_out, o);
 }
 
 int mp3b200_encode_streams(int channels, int samplerate, int kbps, int nstreams, const int16_t* const* left,
@@ -576,48 +638,13 @@ int mp3b200_encode_streams(int channels, int samplerate, int kbps, int nstreams,
   Config* cfg;
   int rc = get_config(channels, samplerate, kbps, &cfg);
   if (rc) return rc;
-  std::vector<int64_t> pcm_off(nstreams), out_off(nstreams);
-  long long tot_samples = 0, tot_bytes = 0;
-  for (int s = 0; s < nstreams; s++) {
-    pcm_off[s] = tot_samples;
-    tot_samples += nsamples[s] * channels;
-    out_off[s] = tot_bytes;
-    const long long b = bytes_for(cfg->host, frames_for(nsamples[s], cfg->host.mode_gr));
-    if (cap[s] < b) { g_err = "output buffer too small"; return MP3B200_ERR_BUFFER; }
-    out_bytes[s] = b;
-    tot_bytes += b;
-  }
-  if (nstreams == 0) return MP3B200_OK;
-  rc = t_ctx.use(cfg->device);
-  if (rc) return rc;
-  /* grow-only staging buffers: a steady stream of batches does not pay cudaMalloc/cudaFree per call */
-  rc = t_ctx.need_pcm((size_t)tot_samples + 8);
-  if (rc) return rc;
-  rc = t_ctx.need_out((size_t)tot_bytes + 8);
-  if (rc) return rc;
-  int16_t* d_pcm = t_ctx.d_pcm;
-  uint8_t* d_out = t_ctx.d_out;
-  /* Upload in time slices on a copy stream; the psy analysis of a slice starts when it has landed, so only the first
-   * slice's transfer is exposed.  Many small streams are uploaded whole (one slice): per-copy overhead would win. */
-  PcmArrival arr;
-  arr.chunks = (nstreams <= 8 && tot_samples >= (1 << 20)) ? MP3_MAX_PCM_CHUNKS : 1;
-  arr.ready = t_ctx.ready;
-  for (int j = 0; j < arr.chunks; j++) {
-    for (int s = 0; s < nstreams; s++) {
-      const int64_t lo = nsamples[s] * j / arr.chunks, hi = nsamples[s] * (j + 1) / arr.chunks;
-      if (hi <= lo) continue;
-      CK(cudaMemcpyAsync(d_pcm + pcm_off[s] + lo, left[s] + lo, sizeof(int16_t) * (hi - lo), cudaMemcpyHostToDevice, t_ctx.up_st));
-      if (channels == 2)
-        CK(cudaMemcpyAsync(d_pcm + pcm_off[s] + nsamples[s] + lo, right[s] + lo, sizeof(int16_t) * (hi - lo), cudaMemcpyHostToDevice, t_ctx.up_st));
-    }
-    CK(cudaEventRecord(t_ctx.ready[j], t_ctx.up_st));
-  }
-  rc = encode_streams_device_impl(cfg, channels, nstreams, d_pcm, pcm_off.data(), nsamples, d_out, out_off.data(), nullptr, &arr);
-  if (rc == 0) {
-    for (int s = 0; s < nstreams; s++)
-      if (cudaMemcpyAsync(out[s], d_out + out_off[s], (size_t)out_bytes[s], cudaMemcpyDeviceToHost, t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
-    if (cudaStreamSynchronize(t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
-  }
+  std::vector<int64_t> out_off;
+  std::vector<long long> audio;
+  rc = encode_host_streams(cfg, nstreams, left, right, nsamples, cap, 0, out_bytes, out_off, audio);
+  if (rc || nstreams == 0) return rc;
+  for (int s = 0; s < nstreams; s++)
+    if (cudaMemcpyAsync(out[s], t_ctx.out.p + out_off[s], (size_t)audio[s], cudaMemcpyDeviceToHost, t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
+  if (cudaStreamSynchronize(t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
   return rc;
 }
 
@@ -653,38 +680,42 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* tp) {
   const int nch = cfg->host.nch;
   const int G = cfg->host.mode_gr;
   const long long F = frames_for(nsamples, G), U = G * F;
-  int16_t* d_pcm = nullptr; uint8_t* d_out = nullptr;
-  CK(cudaMalloc(&d_pcm, sizeof(int16_t) * (size_t)(nsamples * nch + 8)));
-  CK(cudaMemcpy(d_pcm, left, sizeof(int16_t) * nsamples, cudaMemcpyHostToDevice));
-  if (nch == 2) CK(cudaMemcpy(d_pcm + nsamples, right, sizeof(int16_t) * nsamples, cudaMemcpyHostToDevice));
-  const long long nbytes = bytes_for(cfg->host, F);
-  CK(cudaMalloc(&d_out, (size_t)nbytes + 8));
-  CK(cudaMemset(d_out, 0, (size_t)nbytes + 8));
-  std::vector<StreamDesc> sds(1);
-  StreamDesc& sd = sds[0];
-  memset(&sd, 0, sizeof sd);
-  sd.pcm[0] = d_pcm; sd.pcm[1] = nch == 2 ? d_pcm + nsamples : d_pcm;
-  sd.pcm_end = nsamples; sd.nframes = (int)F;
-  init_stream_state(sd);
-  Workspace ws;
-  rc = ws.alloc(1, nch, U, F, true);
-  if (rc) { cudaFree(d_pcm); cudaFree(d_out); return rc; }
+  /* one whole stream, staged and encoded like a batch of host streams of one */
+  const long long nbytes = bytes_of_frames(cfg->host, 0, F);
+  rc = t_ctx.pcm.fit((size_t)(nsamples * nch + 8));
+  if (rc) return rc;
+  rc = t_ctx.out.fit((size_t)nbytes + 8);
+  if (rc) return rc;
+  int16_t* d_pcm = t_ctx.pcm.p;
+  uint8_t* d_out = t_ctx.out.p;
+  CK(cudaMemcpyAsync(d_pcm, left, sizeof(int16_t) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
+  if (nch == 2) CK(cudaMemcpyAsync(d_pcm + nsamples, right, sizeof(int16_t) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
+  const int64_t zero = 0;
+  std::vector<StreamDesc> sds = whole_streams(cfg, 1, d_pcm, &zero, &nsamples, &zero);
   const bool want_gi = ginfo || tp->scalefac || tp->subblock_gain;
   const bool want_prep = tp->xmin || tp->max_nonzero_coeff || tp->xrpow_max;
   const bool want_q = tp->scfsi || tp->old_value || tp->cur_step;
-  const bool only_mdct = !(l3_enc || bytes_out || want_gi || want_prep || want_q);
-  rc = run_pipeline(cfg, ws, sds, d_out, force_blocktype, only_mdct, nullptr);
+  LaunchOpts opts;
+  opts.force_bt = force_blocktype;
+  opts.stop_after_mdct = !(l3_enc || bytes_out || want_gi || want_prep || want_q);
+  rc = launch_streams(cfg, sds, d_out, opts);
+  /* read-back on the thread's stream (the launch has drained it) */
+  auto fetch = [](void* dst, const void* src, size_t bytes) {
+    const cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, t_ctx.st);
+    return e != cudaSuccess ? e : cudaStreamSynchronize(t_ctx.st);
+  };
+  const Workspace& ws = t_ctx.ws;
   if (rc == 0) {
-    if (xr) CK(cudaMemcpy(xr, ws.d_xr, sizeof(float) * (size_t)U * nch * 576, cudaMemcpyDeviceToHost));
+    if (xr) CK(fetch(xr, ws.xr.p, sizeof(float) * (size_t)U * nch * 576));
     if (blocktype) {
       std::vector<signed char> bt((size_t)U * 2);
-      CK(cudaMemcpy(bt.data(), ws.d_bt_final, bt.size(), cudaMemcpyDeviceToHost));
+      CK(fetch(bt.data(), ws.bt_final.p, bt.size()));
       for (long long u = 0; u < U; u++) for (int c = 0; c < nch; c++) blocktype[u * nch + c] = bt[u * 2 + c];
     }
     if (en_l || thm_l || en_s || thm_s) {
       /* masking used by granule u is the ratio of psy unit u-1: row (u + 1 - 1) of the halo-shifted array */
       std::vector<PsyRatioDev> r((size_t)(U + 1) * nch);
-      CK(cudaMemcpy(r.data(), ws.d_ratio, sizeof(PsyRatioDev) * r.size(), cudaMemcpyDeviceToHost));
+      CK(fetch(r.data(), ws.ratio.p, sizeof(PsyRatioDev) * r.size()));
       for (long long u = 0; u < U; u++) for (int c = 0; c < nch; c++) {
         const PsyRatioDev& q = r[(size_t)u * nch + c];
         if (en_l) memcpy(en_l + (u * nch + c) * 22, q.en_l, sizeof q.en_l);
@@ -693,15 +724,15 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* tp) {
         if (thm_s) memcpy(thm_s + (u * nch + c) * 39, q.thm_s, sizeof q.thm_s);
       }
     }
-    if (ath_adjust) CK(cudaMemcpy(ath_adjust, ws.d_ath_q, sizeof(double) * (size_t)F, cudaMemcpyDeviceToHost));
+    if (ath_adjust) CK(fetch(ath_adjust, ws.ath_q.p, sizeof(double) * (size_t)F));
     if (l3_enc) {
       std::vector<short> t((size_t)U * nch * 576);
-      CK(cudaMemcpy(t.data(), ws.d_l3enc, sizeof(short) * t.size(), cudaMemcpyDeviceToHost));
+      CK(fetch(t.data(), ws.l3enc.p, sizeof(short) * t.size()));
       for (size_t i = 0; i < t.size(); i++) l3_enc[i] = t[i];
     }
     if (want_gi) {
       std::vector<GranuleInfoDev> g((size_t)U * nch);
-      CK(cudaMemcpy(g.data(), ws.d_ginfo, sizeof(GranuleInfoDev) * g.size(), cudaMemcpyDeviceToHost));
+      CK(fetch(g.data(), ws.ginfo.p, sizeof(GranuleInfoDev) * g.size()));
       for (size_t i = 0; i < g.size(); i++) {
         if (ginfo) {
           int32_t* o = ginfo + i * 16;
@@ -718,7 +749,7 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* tp) {
       /* the prepared granule-channel as k_q_prepare left it for the searches and rate loops; xmin is defined for the psymax
        * bands of granules with energy only (the others never reach calc_xmin) */
       std::vector<GcPrep> p((size_t)U * nch);
-      CK(cudaMemcpy(p.data(), ws.d_prep, sizeof(GcPrep) * p.size(), cudaMemcpyDeviceToHost));
+      CK(fetch(p.data(), ws.prep.p, sizeof(GcPrep) * p.size()));
       for (size_t i = 0; i < p.size(); i++) {
         if (tp->xmin) {
           const int psymax = p[i].block_type == BT_SHORT ? 36 : 21;
@@ -730,7 +761,7 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* tp) {
     }
     if (want_q) {
       std::vector<QuantFrameState> q((size_t)F);
-      CK(cudaMemcpy(q.data(), ws.d_qstate, sizeof(QuantFrameState) * q.size(), cudaMemcpyDeviceToHost));
+      CK(fetch(q.data(), ws.qstate.p, sizeof(QuantFrameState) * q.size()));
       for (long long f = 0; f < F; f++) {
         const QuantFrameState& s = q[(size_t)f];
         for (int c = 0; c < nch; c++) {
@@ -747,10 +778,9 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* tp) {
     }
     if (bytes_out) {
       if (bytes_cap < nbytes) { g_err = "output buffer too small"; rc = MP3B200_ERR_BUFFER; }
-      else CK(cudaMemcpy(bytes_out, d_out, (size_t)nbytes, cudaMemcpyDeviceToHost));
+      else CK(fetch(bytes_out, d_out, (size_t)nbytes));
     }
   }
-  cudaFree(d_pcm); cudaFree(d_out);
   return rc;
 }
 
@@ -783,23 +813,25 @@ int music_crc_ranges(int device, const uint8_t* d_buf, const std::vector<long lo
     }
   }
   ThreadCtx& sc = t_ctx;
-  int rc = sc.need_crc(R);
+  int rc = sc.crc_ranges.fit((size_t)2 * R);
+  if (rc) return rc;
+  rc = sc.crc.fit((size_t)R);
   if (rc) return rc;
   std::vector<long long> ranges((size_t)2 * R);
   long long longest = 0;
   for (int i = 0; i < R; i++) { ranges[i] = off[i]; ranges[(size_t)R + i] = len[i]; longest = len[i] > longest ? len[i] : longest; }
-  CK(cudaMemcpyAsync(sc.d_crc_ranges, ranges.data(), sizeof(long long) * ranges.size(), cudaMemcpyHostToDevice, sc.st));
-  CK(cudaMemsetAsync(sc.d_crc, 0, sizeof(unsigned) * (size_t)R, sc.st));
+  CK(cudaMemcpyAsync(sc.crc_ranges.p, ranges.data(), sizeof(long long) * ranges.size(), cudaMemcpyHostToDevice, sc.st));
+  CK(cudaMemsetAsync(sc.crc.p, 0, sizeof(unsigned) * (size_t)R, sc.st));
   if (longest > 0) {
     const long long pieces = (longest + CRC_PIECE_BYTES - 1) / CRC_PIECE_BYTES;
     for (int r0 = 0; r0 < R; r0 += 65535) {
       const int nr = R - r0 < 65535 ? R - r0 : 65535;
       dim3 grid((unsigned)((pieces + CRC_WARPS - 1) / CRC_WARPS), (unsigned)nr);
-      k_music_crc<<<grid, CRC_WARPS * 32, 0, sc.st>>>(d_buf, sc.d_crc_ranges + r0, sc.d_crc_ranges + R + r0, g_crc_dev[device], sc.d_crc + r0);
+      k_music_crc<<<grid, CRC_WARPS * 32, 0, sc.st>>>(d_buf, sc.crc_ranges.p + r0, sc.crc_ranges.p + R + r0, g_crc_dev[device], sc.crc.p + r0);
       g_launches++;
     }
   }
-  CK(cudaMemcpyAsync(crc.data(), sc.d_crc, sizeof(unsigned) * (size_t)R, cudaMemcpyDeviceToHost, sc.st));
+  CK(cudaMemcpyAsync(crc.data(), sc.crc.p, sizeof(unsigned) * (size_t)R, cudaMemcpyDeviceToHost, sc.st));
   CK(cudaStreamSynchronize(sc.st));
   CK(cudaGetLastError());
   return 0;
@@ -887,51 +919,28 @@ int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int ns
   Mp3TagParams p;
   if (mp3_tag_params(channels, samplerate, kbps, &p) != 0) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
   const int tfs = p.fits ? p.frame_bytes : 0;
-  std::vector<int64_t> pcm_off(nstreams), out_off(nstreams);
-  std::vector<long long> frames(nstreams), audio(nstreams);
-  long long tot_samples = 0, tot_bytes = 0;
-  for (int s = 0; s < nstreams; s++) {
-    pcm_off[s] = tot_samples; tot_samples += nsamples[s] * channels;
-    out_off[s] = tot_bytes;
-    frames[s] = frames_for(nsamples[s], cfg->host.mode_gr);
-    audio[s] = bytes_for(cfg->host, frames[s]);
-    if (cap[s] < audio[s] + tfs) { g_err = "output buffer too small"; return MP3B200_ERR_BUFFER; }
-    out_bytes[s] = audio[s] + tfs;
-    tot_bytes += audio[s];
-  }
-  if (nstreams == 0) return MP3B200_OK;
-  rc = t_ctx.use(cfg->device);
-  if (rc) return rc;
-  rc = t_ctx.need_pcm((size_t)tot_samples + 8);
-  if (rc) return rc;
-  rc = t_ctx.need_out((size_t)tot_bytes + 8);
-  if (rc) return rc;
-  for (int s = 0; s < nstreams; s++) {
-    if (nsamples[s] <= 0) continue;
-    CK(cudaMemcpyAsync(t_ctx.d_pcm + pcm_off[s], left[s], sizeof(int16_t) * nsamples[s], cudaMemcpyHostToDevice, t_ctx.up_st));
-    if (channels == 2)
-      CK(cudaMemcpyAsync(t_ctx.d_pcm + pcm_off[s] + nsamples[s], (right && right[s]) ? right[s] : left[s], sizeof(int16_t) * nsamples[s], cudaMemcpyHostToDevice, t_ctx.up_st));
-  }
-  PcmArrival arr;
-  arr.chunks = 1; arr.ready = t_ctx.ready;
-  CK(cudaEventRecord(t_ctx.ready[0], t_ctx.up_st));
-  rc = encode_streams_device_impl(cfg, channels, nstreams, t_ctx.d_pcm, pcm_off.data(), nsamples, t_ctx.d_out, out_off.data(), nullptr, &arr);
-  if (rc) return rc;
+  std::vector<int64_t> out_off;
+  std::vector<long long> audio;
+  rc = encode_host_streams(cfg, nstreams, left, right, nsamples, cap, tfs, out_bytes, out_off, audio);
+  if (rc || nstreams == 0) return rc;
   /* the music CRC of every stream, where the bytes are */
   std::vector<long long> off(out_off.begin(), out_off.end());
   std::vector<unsigned> crc;
-  rc = music_crc_ranges(cfg->device, t_ctx.d_out, off, audio, crc);
+  rc = music_crc_ranges(cfg->device, t_ctx.out.p, off, audio, crc);
   if (rc) return rc;
   Mp3SeekBag* bag = new Mp3SeekBag();
   for (int s = 0; s < nstreams; s++) {
     int wrote = 0;
-    if (tfs > 0 && frames[s] > 0) {
+    LameFifo fifo(cfg->host.mode_gr);
+    const long long frames = fifo.feed(nsamples[s]);
+    const FifoFlush fl = fifo.flush();
+    if (tfs > 0 && frames + fl.frames > 0) {
       bag->reset();
-      bag->add_frames(frames[s], p.kbps);
-      wrote = mp3_tag_frame(p, *bag, audio[s], crc[s], mp3_encoder_padding(nsamples[s], cfg->host.mode_gr), out[s]);
+      bag->add_frames(frames + fl.frames, p.kbps);
+      wrote = mp3_tag_frame(p, *bag, audio[s], crc[s], (int)fl.end_padding, out[s]);
     }
     out_bytes[s] = audio[s] + wrote;
-    if (audio[s] > 0 && cudaMemcpyAsync(out[s] + wrote, t_ctx.d_out + out_off[s], (size_t)audio[s], cudaMemcpyDeviceToHost, t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
+    if (audio[s] > 0 && cudaMemcpyAsync(out[s] + wrote, t_ctx.out.p + out_off[s], (size_t)audio[s], cudaMemcpyDeviceToHost, t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
   }
   delete bag;
   if (cudaStreamSynchronize(t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;

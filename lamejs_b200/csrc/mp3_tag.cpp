@@ -101,17 +101,6 @@ int mp3_tag_frame(const Mp3TagParams& p, const Mp3SeekBag& bag, long long music_
   return p.frame_bytes;
 }
 
-/* lame_encode_flush's end padding for a stream of n samples per channel (Lame.js:1393-1412; see frames_for in
- * mp3_encoder.cu for the same walk) */
-int mp3_encoder_padding(long long n, int mode_gr) {
-  const long long fs = 576LL * mode_gr, need = fs + 752;
-  const long long f_enc = 528 + n >= need ? (528 + n - need) / fs + 1 : 0;
-  const long long ste = 576 + n - fs * f_enc;
-  long long end_padding = fs - (ste % fs);
-  if (end_padding < 576) end_padding += fs;
-  return (int)end_padding;
-}
-
 namespace {
 bool rd(const uint8_t* d, long long n, long long pos, int nbytes, bool little, unsigned long long* v) {
   if (pos < 0 || pos + nbytes > n) return false;

@@ -18,7 +18,6 @@ void mp3_tag_header(const Mp3TagParams& p, int mode_ext, uint8_t* h4);
 int mp3_tag_placeholder(const Mp3TagParams& p, uint8_t* out);
 /* getLameTagFrame: p.frame_bytes bytes, or 0 (tag off / no frame counted yet) */
 int mp3_tag_frame(const Mp3TagParams& p, const Mp3SeekBag& bag, long long music_bytes, unsigned music_crc, int encoder_padding, uint8_t* out);
-int mp3_encoder_padding(long long nsamples, int mode_gr);
 /* WavHeader.readHeader: 1 ok, 0 `return undefined`, -1 throws 'extended fmt chunk not implemented', -2 DataView RangeError */
 int mp3_wav_read_header(const uint8_t* d, long long n, long long* data_offset, long long* data_len, int* channels, unsigned* sample_rate);
 /* VBRTagData (reference src/main/java/mp3/VBRTagData.java; `new VBRTagData()` in VBRTag.js:376) */

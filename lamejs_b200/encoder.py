@@ -322,10 +322,8 @@ def flush_batch(encoders):
     return [o[: int(g)].tobytes() for o, g in zip(outs, got)]
 
 
-def encode_streams(channels, samplerate, kbps, lefts, rights=None):
-    """Batch extension: encodeBuffer(whole stream) + flush() for many independent streams in one launch sequence.
-    Host buffers in, list of bytes out."""
-    L = lib()
+def _encode_host_streams(fn, channels, samplerate, kbps, lefts, rights, room):
+    """Marshalling of the whole-stream host calls: out[s] has room for the stream's bytes plus `room`."""
     S = len(lefts)
     if S == 0:
         return []
@@ -335,36 +333,28 @@ def encode_streams(channels, samplerate, kbps, lefts, rights=None):
     nb = [stream_bytes(channels, samplerate, kbps, int(n)) for n in ns]
     if any(b < 0 for b in nb):
         raise Mp3B200Error("unsupported configuration: channels=%d samplerate=%d kbps=%d (lame_init_params would resample)" % (channels, samplerate, kbps))
+    nb = [b + room for b in nb]
     outs = [np.empty(b, dtype=np.uint8) for b in nb]
     lp = (ctypes.c_void_p * S)(*[x.ctypes.data for x in lefts])
     rp = (ctypes.c_void_p * S)(*[x.ctypes.data for x in rights])
     op = (ctypes.c_void_p * S)(*[x.ctypes.data for x in outs])
     caps = np.array(nb, dtype=np.int64)
     got = np.zeros(S, dtype=np.int64)
-    _check(L.mp3b200_encode_streams(channels, samplerate, kbps, S, lp, rp, ns.ctypes.data, op, caps.ctypes.data, got.ctypes.data))
+    _check(fn(channels, samplerate, kbps, S, lp, rp, ns.ctypes.data, op, caps.ctypes.data, got.ctypes.data))
     return [o[: int(g)].tobytes() for o, g in zip(outs, got)]
+
+
+def encode_streams(channels, samplerate, kbps, lefts, rights=None):
+    """Batch extension: encodeBuffer(whole stream) + flush() for many independent streams in one launch sequence.
+    Host buffers in, list of bytes out."""
+    return _encode_host_streams(lib().mp3b200_encode_streams, channels, samplerate, kbps, lefts, rights, 0)
 
 
 def encode_streams_tagged(channels, samplerate, kbps, lefts, rights=None):
     """encode_streams with gfp.bWriteVbrTag on: every returned stream starts with its finished Info / LAME tag frame (frame
     and byte counts, seek table, encoder delay / padding, CRC-16 of the audio bytes computed on the GPU)."""
-    L = lib()
-    S = len(lefts)
-    if S == 0:
-        return []
-    lefts = [np.ascontiguousarray(x, dtype=np.int16) for x in lefts]
-    rights = lefts if (rights is None or channels == 1) else [np.ascontiguousarray(x, dtype=np.int16) for x in rights]
-    ns = np.array([len(x) for x in lefts], dtype=np.int64)
-    room = lametag_size(channels, samplerate, kbps)
-    nb = [stream_bytes(channels, samplerate, kbps, int(n)) + room for n in ns]
-    outs = [np.empty(b, dtype=np.uint8) for b in nb]
-    lp = (ctypes.c_void_p * S)(*[x.ctypes.data for x in lefts])
-    rp = (ctypes.c_void_p * S)(*[x.ctypes.data for x in rights])
-    op = (ctypes.c_void_p * S)(*[x.ctypes.data for x in outs])
-    caps = np.array(nb, dtype=np.int64)
-    got = np.zeros(S, dtype=np.int64)
-    _check(L.mp3b200_encode_streams_tagged(channels, samplerate, kbps, S, lp, rp, ns.ctypes.data, op, caps.ctypes.data, got.ctypes.data))
-    return [o[: int(g)].tobytes() for o, g in zip(outs, got)]
+    return _encode_host_streams(lib().mp3b200_encode_streams_tagged, channels, samplerate, kbps, lefts, rights,
+                                lametag_size(channels, samplerate, kbps))
 
 
 def debug_music_crc(d_buf_ptr, offsets, lengths, timed=False):

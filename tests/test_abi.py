@@ -40,6 +40,16 @@ def test_stream_geometry_matches_oracle(M, oracle, n):
         assert F == (n - 1376) // 1152 + 1 + 2 or F == (n - 1376) // 1152 + 1 + 1
 
 
+@pytest.mark.parametrize("samplerate,kbps", [(44100, 128), (22050, 32)])
+def test_stream_geometry_sweep_matches_oracle(M, oracle, samplerate, kbps):
+    """Every length from 0 to 4 frames + 1500 samples, MPEG-1 (1152-sample frames) and MPEG-2 (576): the frame count and byte
+    length of encodeBuffer(n) + flush() match the oracle across the first-frame and flush boundaries of both frame sizes."""
+    framesize = 576 * M.granules_per_frame(1, samplerate, kbps)
+    for n in range(4 * framesize + 1500 + 1):
+        data, _, tr = oracle.encode_stream(1, samplerate, kbps, np.zeros(n, dtype=np.int16), None, trace_frames=16)
+        assert (M.stream_frames(n, 1, samplerate, kbps), M.stream_bytes(1, samplerate, kbps, n)) == (len(tr), len(data)), n
+
+
 DEBUG_TAPS_FIELDS = ["size", "channels", "samplerate", "kbps", "left", "right", "nsamples", "force_blocktype", "xr", "blocktype",
                      "en_l", "thm_l", "en_s", "thm_s", "ath_adjust", "l3_enc", "ginfo", "bytes_out", "bytes_cap", "scalefac",
                      "subblock_gain", "xmin", "max_nonzero_coeff", "xrpow_max", "scfsi", "old_value", "cur_step"]

@@ -40,3 +40,27 @@ def test_edge_corpus_as_batches(M, oracle):
         outs = M.encode_streams(ch, sr, kbps, [s[0] for s in sigs], [s[1] for s in sigs] if ch == 2 else None)
         for (l, r), o in zip(sigs, outs):
             assert o == oracle.encode_stream(ch, sr, kbps, l, r)[0], (ch, sr, kbps, len(l))
+
+
+@pytest.mark.parametrize("tagged", [False, True])
+def test_stereo_host_streams_without_right(M, tagged):
+    """Stereo whole streams from host buffers: right == NULL, or right[s] == NULL, encodes left[s] on both channels."""
+    import ctypes
+
+    import numpy as np
+    from synth import make_signal
+
+    L = M.lib()
+    fn = L.mp3b200_encode_streams_tagged if tagged else L.mp3b200_encode_streams
+    lefts = [np.ascontiguousarray(make_signal("noise", n, 44100, seed=n)[0], dtype=np.int16) for n in (5000, 12345)]
+    want = (M.encode_streams_tagged if tagged else M.encode_streams)(2, 44100, 128, lefts, lefts)
+    room = M.lametag_size(2, 44100, 128) if tagged else 0
+    ns = np.array([len(x) for x in lefts], dtype=np.int64)
+    caps = np.array([M.stream_bytes(2, 44100, 128, int(n)) + room for n in ns], dtype=np.int64)
+    lp = (ctypes.c_void_p * 2)(*[x.ctypes.data for x in lefts])
+    for rp in (None, (ctypes.c_void_p * 2)(lefts[0].ctypes.data, None)):
+        outs = [np.zeros(int(c), dtype=np.uint8) for c in caps]
+        op = (ctypes.c_void_p * 2)(*[o.ctypes.data for o in outs])
+        got = np.zeros(2, dtype=np.int64)
+        assert fn(2, 44100, 128, 2, lp, rp, ns.ctypes.data, op, caps.ctypes.data, got.ctypes.data) == 0
+        assert [o[: int(g)].tobytes() for o, g in zip(outs, got)] == want
