@@ -32,11 +32,27 @@ int mp3b200_set_device(int device);
  * 32000|44100|48000 (MPEG-1); kbps snapped to the nearest legal rate of that MPEG version like FindNearestBitrate
  * (src/js/Lame.js:408-423).  Configurations for which lamejs would RESAMPLE (lame_init_params picks out_samplerate !=
  * in_samplerate from the bitrate's low-pass, Lame.js:285-364 -- e.g. 44.1 kHz stereo below 112 kbps) return
- * MP3B200_ERR_CONFIG: the CPU oracle models lamejs's resampler byte for byte (all 306 reference fixtures), but lamejs
- * reads its input with fractional / out-of-range typed-array indices there (whole-buffer calls and every flush of a
- * non-integer rate ratio put NaN samples into the stream, oracle/lj_init.cpp fill_buffer_resample), so that row is not
- * offered as a drop-in. */
+ * MP3B200_ERR_CONFIG here; mp3b200_create_ex with MP3B200_RESAMPLE accepts those whose rate ratio is an integer.
+ * This call is mp3b200_create_ex with flags = 0. */
 int mp3b200_create(int channels, int samplerate, int kbps, mp3b200_encoder** out);
+
+/* ---- resampling (lamejs fill_buffer_resample, Lame.js:1719-1843) -------------------------------------------------------
+ * MP3B200_RESAMPLE also accepts a configuration for which lamejs resamples, when its output rate divides the input rate
+ * (lamejs's own test, |in / out - round(in / out)| < 1e-4): 48000 -> 24000, 44100 -> 22050, 48000 / 32000 -> 16000 and
+ * 48000 / 32000 / 24000 / 16000 -> 8000, e.g. `new Mp3Encoder(2, 48000, 64)`, which encodes at 24 kHz.  The caller feeds
+ * samples at the input rate; the GPU resamples them (k_resample: one 33-tap filter, bit-exact with lamejs) and encodes at the
+ * output rate, byte-identical to lamejs however the input is split into calls.  Non-integer ratios return MP3B200_ERR_CONFIG
+ * with or without the flag: lamejs reads its input with fractional typed-array indices there, so NaN samples enter its
+ * stream and its bytes depend on the call sizes.  Without the flag nothing changes; with it, configurations that encode at
+ * their input rate behave exactly as without it.
+ * On a resampled handle every handle call works as documented, with sample counts in input samples (state blobs carry their
+ * own magic and both rates and are refused by a handle of another rate pair), except mp3b200_seek, which returns -2.
+ * The _ex entry points below take the flags; the others are the same calls with flags = 0. */
+#define MP3B200_RESAMPLE 1
+int mp3b200_create_ex(int channels, int samplerate, int kbps, int flags, mp3b200_encoder** out);
+/* the output rate lamejs encodes a configuration at (Lame.js:285-364; != samplerate: it resamples), 0 for a channel count
+ * other than 1 or 2.  Pure host code. */
+int mp3b200_out_samplerate(int channels, int samplerate, int kbps);
 
 /* Replaces `encodeBuffer(left, right)` (src/js/index.js:117-130 -> Lame.js:1490-1667).  `right` may be NULL
  * for mono.  Writes the bytes of the frames completed by this call (possibly 0) into `out` and returns their
@@ -80,7 +96,7 @@ int mp3b200_flush_batch(mp3b200_encoder* const* handles, uint8_t* const* out, co
  *                 the ones a single encoder would produce; otherwise it imports the predecessor's state and encodes again
  *                 (lamejs_b200/sharding.py encode_stream_segments).  `hist`: the stream samples
  *                 [max(0, frame*framesize - 1104), frame*framesize + 224), framesize = 576 * granules per frame; feeding
- *                 continues with sample frame*framesize + 224.
+ *                 continues with sample frame*framesize + 224.  Not supported on a resampled handle (returns -2).
  * Return MP3B200_OK / bytes written, or a negative error (wrong configuration -2, buffer -1, handle -3). */
 int mp3b200_export_state(mp3b200_encoder* h, void* buf, int cap);
 int mp3b200_import_state(mp3b200_encoder* h, const void* buf, int len);
@@ -92,6 +108,8 @@ int mp3b200_seek(mp3b200_encoder* h, int64_t frame, const int16_t* left_hist, co
 
 /* Number of bytes / frames that stream of `nsamples` per channel produces (closed form: CBR, no reservoir). */
 int64_t mp3b200_stream_bytes(int channels, int samplerate, int kbps, int64_t nsamples);
+/* the same with flags (MP3B200_RESAMPLE: nsamples are input samples) */
+int64_t mp3b200_stream_bytes_ex(int channels, int samplerate, int kbps, int flags, int64_t nsamples);
 int64_t mp3b200_stream_frames(int64_t nsamples);                 /* MPEG-1 configurations (1152-sample frames) */
 /* any accepted configuration (MPEG-2 / 2.5 frames carry 576 samples); -1 if the configuration is rejected */
 int64_t mp3b200_stream_frames_cfg(int channels, int samplerate, int kbps, int64_t nsamples);
@@ -104,6 +122,10 @@ int mp3b200_granules_per_frame(int channels, int samplerate, int kbps);
 int mp3b200_encode_streams(int channels, int samplerate, int kbps, int nstreams, const int16_t* const* left,
                            const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
                            const int64_t* cap, int64_t* out_bytes);
+/* the same with flags (MP3B200_RESAMPLE: input samples in, out_bytes[s] = mp3b200_stream_bytes_ex(...)) */
+int mp3b200_encode_streams_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
+                              const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
+                              const int64_t* cap, int64_t* out_bytes);
 
 /* Device-resident variant for benchmarking kernel throughput: d_pcm is ONE device allocation holding, per
  * stream s, nsamples[s] Int16 of the left channel at sample offset pcm_off[s] and (stereo) the right channel at
@@ -120,6 +142,11 @@ int mp3b200_encode_streams(int channels, int samplerate, int kbps, int nstreams,
 int mp3b200_encode_streams_device(int channels, int samplerate, int kbps, int nstreams, const int16_t* d_pcm,
                                   const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
                                   const int64_t* out_off, float* timings_ms);
+/* the same with flags.  With MP3B200_RESAMPLE, d_pcm / nsamples hold input samples, and timings_ms[14] receives the
+ * resampler's time (k_resample; 0 for a configuration that encodes at its input rate).  [6] does not include it. */
+int mp3b200_encode_streams_device_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
+                                     const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
+                                     const int64_t* out_off, float* timings_ms);
 
 /* ---- container / metadata step after the path (SURVEY.md 8(f3)) ------------------------------------------------------
  * lamejs carries LAME's Xing / Info / LAME tag writer (src/js/VBRTag.js) and keeps its two inputs up to date on every
@@ -145,6 +172,7 @@ int mp3b200_get_lametag_frame(mp3b200_encoder* h, uint8_t* buf, int cap);
 int mp3b200_music_crc(mp3b200_encoder* h);
 int64_t mp3b200_bytes_written(mp3b200_encoder* h);
 int mp3b200_lametag_size(int channels, int samplerate, int kbps);
+int mp3b200_lametag_size_ex(int channels, int samplerate, int kbps, int flags);   /* with flags: MP3B200_RESAMPLE handles */
 int mp3b200_lametag_build(int channels, int samplerate, int kbps, int64_t nframes, int64_t music_bytes, int music_crc,
                           int encoder_padding, uint8_t* buf, int cap);
 int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int nstreams, const int16_t* const* left,
@@ -245,6 +273,12 @@ typedef struct mp3b200_debug_taps {
   int32_t *scfsi, *old_value, *cur_step;
 } mp3b200_debug_taps;
 int mp3b200_debug_stages_ex(const mp3b200_debug_taps* t);
+
+/* Test tap of k_resample: y[c * ny + m], m < ny, = output m of channel c (nch rows) of the resampler of a configuration that
+ * MP3B200_RESAMPLE accepts with resampling, for the input left / right (nsamples each; right NULL: left) extended with zeros
+ * on both sides.  MP3B200_ERR_CONFIG for a configuration that does not resample. */
+int mp3b200_debug_resample(int channels, int samplerate, int kbps, const int16_t* left, const int16_t* right, int64_t nsamples,
+                           float* y, int64_t ny);
 
 const char* mp3b200_last_error(void);
 /* total number of kernel launches issued by this library since load (bench.py "gpu_launches") */

@@ -308,6 +308,7 @@ __device__ __forceinline__ void mdct_short_dev(f32s* io) {
 #define FB_MIN_BLOCKS 3
 #endif
 #define FB_SLABS (FB_G + 1)
+template <bool F32_PCM>     /* as k_psy_analysis: Float32 samples of the resampler instead of Int16 input */
 __global__ void __launch_bounds__(FB_THREADS, FB_MIN_BLOCKS)
 k_subband_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ streams, float* __restrict__ slab_out) {
   const int z = blockIdx.z;
@@ -332,7 +333,25 @@ k_subband_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict
   const int scale_applied = T->scale_applied;
   const double scale = T->scale;
   const int span = 576 * (scount - 1) + 1055;
-  {
+  if constexpr (F32_PCM) {
+    const float* __restrict__ pbuf = reinterpret_cast<const float*>(sd.pcm[ch]);
+    const long long pbase = sd.pcm_base, pend = sd.pcm_end;
+#pragma unroll 1
+    for (int j0 = tid; j0 < span; j0 += FB_THREADS * 8) {
+      float v[8];
+#pragma unroll
+      for (int k = 0; k < 8; k++) {
+        const int j = j0 + k * FB_THREADS;
+        const long long i = lo + j;
+        v[k] = (j < span && i >= 0 && i < pend) ? __ldg(&pbuf[i - pbase]) : 0.0f;
+      }
+#pragma unroll
+      for (int k = 0; k < 8; k++) {
+        const int j = j0 + k * FB_THREADS;
+        if (j < span) pcm[fb_pad(j)] = (double)v[k];
+      }
+    }
+  } else {
     /* 8 independent Int16 loads per thread in flight (one dependent load per iteration left this phase, a third of the
      * kernel's samples in the round-2 profile, waiting for HBM latency) */
     const int16_t* __restrict__ pbuf = sd.pcm[ch];

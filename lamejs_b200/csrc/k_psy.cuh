@@ -160,10 +160,12 @@ __device__ __forceinline__ void fht_task(f32w* fz, int stage, int task, const do
 /* psy row of (stream z, relative unit u >= -1): unit_base + z + u + 1 */
 __device__ __forceinline__ size_t psy_row(const StreamDesc& sd, int z, int u) { return (size_t)sd.unit_base + z + u + 1; }
 
-/* grid (max_units + 1, nch, nstreams) */
+/* grid (max_units + 1, nch, nstreams).  F32_PCM: sd.pcm[ch] points at Float32 samples already at the encoding rate and
+ * scaled (the resampler's output, k_resample) instead of Int16 input. */
 #ifndef PSY_MIN_BLOCKS
 #define PSY_MIN_BLOCKS 12     /* C2 step on an H100 SXM (400 W): 8 / 10 / 12 blocks -> 5.18 / 5.15 / 5.13 ms */
 #endif
+template <bool F32_PCM>
 __global__ void __launch_bounds__(PSY_THREADS, PSY_MIN_BLOCKS)
 k_psy_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ streams, PsyUnit* __restrict__ out,
                int chunk, int nchunks, int u_base) {
@@ -225,7 +227,24 @@ k_psy_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ s
   const int scale_applied = T->scale_applied;
   const double scale = T->scale;
   const long long x0 = 576 * c - 224;                /* stream sample of bufPos */
-  {
+  if constexpr (F32_PCM) {
+    /* the resampler's Float32 output: scaled before the filter, widened without scaling */
+    const float* __restrict__ pbuf = reinterpret_cast<const float*>(sd.pcm[ch]);
+    const long long pbase = sd.pcm_base, pend = sd.pcm_end;
+    constexpr int NB = (1024 + PSY_THREADS - 1) / PSY_THREADS;
+    float v[NB];
+#pragma unroll
+    for (int k = 0; k < NB; k++) {
+      const int j = tid + k * PSY_THREADS;
+      const long long i = x0 + j;
+      v[k] = (j < 1024 && i >= 0 && i < pend) ? __ldg(&pbuf[i - pbase]) : 0.0f;
+    }
+#pragma unroll
+    for (int k = 0; k < NB; k++) {
+      const int j = tid + k * PSY_THREADS;
+      if (j < 1024) xs[j] = (double)v[k];
+    }
+  } else {
     /* all of a thread's Int16 loads in flight at once (they were one dependent HBM round trip per iteration) */
     const int16_t* __restrict__ pbuf = sd.pcm[ch];
     const long long pbase = sd.pcm_base, pend = sd.pcm_end;

@@ -1,0 +1,58 @@
+/* k_resample.cuh -- the resampler lamejs runs in front of the encoder when the output rate divides the input rate.
+ *
+ * Included after every other kernel header: its __constant__ table then sits behind theirs, and their constant-bank
+ * addresses (and code) stay as they were.
+ */
+#ifndef MP3B200_K_RESAMPLE_CUH
+#define MP3B200_K_RESAMPLE_CUH
+#include "mp3_device.cuh"
+
+/* ---- resampler: lamejs fill_buffer_resample (Lame.js:1719-1843) for an integer rate ratio r = in / out ----
+ * With out | in the filter bank has one row in use (bpc = 1, offset 0) and the input position of output m is r m exactly,
+ * whatever the call sizes, so output m of a stream is
+ *   y[m] = Float32( sum_{i=0..32} (double)h[i] * xs[r m - 16 + i] ),  summed in double in tap order from 0.0,
+ * xs = Float32(Int16 * scale) (lamejs scales its Float32Array before resampling), 0 before the stream and past its end
+ * (inbuf_old starts zeroed; flush feeds zeros).  y then stands where the input would: the rest of the pipeline reads it
+ * like PCM at the output rate (k_psy_analysis<true>, k_subband_analysis<true>). */
+#define RS_THREADS 256
+#define RS_MAX_RATIO 6                          /* 48 kHz -> 8 kHz */
+__constant__ float c_rs_h[RS_MAX_RATIO + 1][MP3_RS_TAPS];   /* row r: the filter of ratio r (the taps depend on r only) */
+
+struct ResampleDesc {
+  const int16_t* x[2];      /* input of each channel, at stream sample x_base */
+  long long x_base, x_end;  /* input samples [x_base, x_end) are there; samples >= x_end (and < 0) read as 0 */
+  float* y[2];              /* outputs y_base .. y_base + ny - 1 of each channel */
+  long long y_base, ny;
+};
+
+/* grid (ceil(max ny / RS_THREADS), nch, nstreams); thread = one output */
+__global__ void __launch_bounds__(RS_THREADS)
+k_resample(const ResampleDesc* __restrict__ descs, int ratio, int scale_applied, double scale) {
+  __shared__ double xs[RS_MAX_RATIO * RS_THREADS + MP3_RS_TAPS];
+  const ResampleDesc& d = descs[blockIdx.z];
+  const int ch = blockIdx.y, tid = threadIdx.x;
+  const long long m0 = (long long)blockIdx.x * RS_THREADS;     /* first output of the block, relative to y_base */
+  if (m0 >= d.ny) return;
+  /* the block's input span: r * RS_THREADS + 32 samples from r (y_base + m0) - 16, widened once */
+  const long long k0 = (long long)ratio * (d.y_base + m0) - MP3_RS_HALF;
+  const int span = ratio * RS_THREADS + MP3_RS_TAPS - 1;
+  const int16_t* __restrict__ x = d.x[ch];
+  for (int j = tid; j < span; j += RS_THREADS) {
+    const long long k = k0 + j;
+    const int v = (k >= 0 && k < d.x_end) ? (int)__ldg(&x[k - d.x_base]) : 0;
+    double s = (double)v;
+    if (scale_applied) s = (double)(float)(s * scale);
+    xs[j] = s;
+  }
+  __syncthreads();
+  const long long m = m0 + tid;
+  if (m >= d.ny) return;
+  const double* w = xs + ratio * tid;
+  const float* h = c_rs_h[ratio];
+  double acc = 0.;
+#pragma unroll
+  for (int i = 0; i < MP3_RS_TAPS; i++) acc += w[i] * (double)h[i];
+  d.y[ch][m] = (float)acc;
+}
+
+#endif

@@ -193,14 +193,55 @@ float snr_norm(double bval, double a, double b) {  /* PsyModel.js:2609-2614 / 26
 
 }  // namespace
 
-int mp3_build_tables(int channels, int samplerate, int kbps, Mp3Tables* t) {
+namespace {
+
+/* blackman() of the resampler (Lame.js:1691-1714) */
+double rs_blackman(double x, double fcn, int l) {
+  const double PI = 3.141592653589793;
+  const double wcn = PI * fcn;
+  x /= l;
+  if (x < 0) x = 0;
+  if (x > 1) x = 1;
+  const double x2 = x - .5;
+  const double bkwn = 0.42 - 0.5 * cos(2 * x * PI) + 0.08 * cos(4 * x * PI);
+  if (fabs(x2) < 1e-9) return wcn / PI;
+  return bkwn * sin(l * wcn * x2) / (PI * l * x2);
+}
+
+/* the filter row an integer ratio uses (Lame.js:1746-1760 with bpc = 1, j = 1: offset 0, filter_l = 32).  Each tap is stored
+ * to the Float32Array, the sum adds the unrounded double, and the normalised tap is stored again. */
+void rs_filter(double resample_ratio, float* h) {
+  double fcn = 1.00 / resample_ratio;
+  if (fcn > 1.00) fcn = 1.00;
+  double sum = 0.;
+  for (int i = 0; i < MP3_RS_TAPS; i++) {
+    const double v = rs_blackman(i, fcn, MP3_RS_TAPS - 1);
+    h[i] = (float)v;
+    sum += v;
+  }
+  for (int i = 0; i < MP3_RS_TAPS; i++) h[i] = (float)((double)h[i] / sum);
+}
+
+}  // namespace
+
+int mp3_out_samplerate(int channels, int samplerate, int kbps) {
+  if (channels != 1 && channels != 2) return 0;
+  double lowpass = kLowpassHz[ladder_index(kbps)];
+  if (channels == 1) lowpass *= 1.5;
+  double lp = (double)to_i32(lowpass);
+  if (2 * lp > samplerate) lp = samplerate / 2.0;
+  return suggested_out_rate(to_i32(lp), samplerate);
+}
+
+int mp3_build_tables(int channels, int samplerate, int kbps, Mp3Tables* t, int flags, Mp3Resample* rs) {
   memset(t, 0, sizeof *t);
+  if (rs) { memset(rs, 0, sizeof *rs); rs->in_rate = samplerate; rs->ratio = 1; }
   if (channels != 1 && channels != 2) return -1;
   t->nch = channels;
   t->mono = channels == 1;
 
   /* ---- rate / bandwidth decisions (Lame.js:838-896, 1044-1061) ---- */
-  const int ladder_raw = ladder_index(kbps);          /* optimum_bandwidth sees the UNSNAPPED kbps */
+  const int ladder_raw = ladder_index(kbps);          /* optimum_bandwidth sees the UNSNAPPED kbps and the INPUT rate */
   double lowpass = kLowpassHz[ladder_raw];
   if (t->mono) lowpass *= 1.5;
   double lp = (double)to_i32(lowpass);
@@ -208,7 +249,12 @@ int mp3_build_tables(int channels, int samplerate, int kbps, Mp3Tables* t) {
   const int out_rate = suggested_out_rate(to_i32(lp), samplerate);
   lp = dmin(20500, lp);
   lp = dmin(out_rate / 2.0, lp);
-  if (out_rate != samplerate) return -1;               /* would need fill_buffer_resample */
+  if (out_rate != samplerate) {                        /* fill_buffer_resample */
+    const double ratio = (double)samplerate / out_rate;
+    if (!(flags & 1) || !(fabs(ratio - floor(.5 + ratio)) < .0001)) return -1;   /* intratio (Lame.js:1735) */
+    if (rs) { rs->ratio = samplerate / out_rate; rs_filter(ratio, rs->h); }
+    samplerate = out_rate;                             /* everything below is at the rate lamejs encodes at */
+  }
   switch (samplerate) {                                /* SmpFrqIndex (Lame.js:369-402) */
     case 44100: t->version = 1; t->samplerate_index = 0; break;
     case 48000: t->version = 1; t->samplerate_index = 1; break;
@@ -491,11 +537,12 @@ int mp3_build_tables(int channels, int samplerate, int kbps, Mp3Tables* t) {
 /* The tag's view of a configuration: lowpassfreq as lame_init_params leaves it (Lame.js:838-896), the preset's safejoint
  * bit (Presets.js:262-263), and the "non optimal settings" rule of putLameVBR (VBRTag.js:722-731), which for Mp3Encoder
  * reduces to: reservoir disabled below 320 kbps, or a source rate of 32 kHz and below. */
-int mp3_tag_params(int channels, int samplerate, int kbps, Mp3TagParams* p) {
+int mp3_tag_params(int channels, int samplerate, int kbps, Mp3TagParams* p, int flags) {
   memset(p, 0, sizeof *p);
   Mp3Tables* t = new Mp3Tables();
-  const int rc = mp3_build_tables(channels, samplerate, kbps, t);
+  const int rc = mp3_build_tables(channels, samplerate, kbps, t, flags);
   if (rc == 0) {
+    /* with resampling, the low-pass and the source-rate fields see the input rate, the rest the output rate */
     p->version = t->version; p->mpeg25 = t->mpeg25; p->samplerate = t->samplerate; p->kbps = t->kbps; p->mono = t->mono;
     p->bitrate_index = t->bitrate_index; p->samplerate_index = t->samplerate_index; p->sideinfo_len = t->sideinfo_len;
     p->frame_bytes = t->frame_bytes_nopad;
@@ -505,7 +552,7 @@ int mp3_tag_params(int channels, int samplerate, int kbps, Mp3TagParams* p) {
     double lp = (double)to_i32(lowpass);
     if (2 * lp > samplerate) lp = samplerate / 2.0;
     lp = dmin(20500, lp);
-    lp = dmin(samplerate / 2.0, lp);
+    lp = dmin(t->samplerate / 2.0, lp);
     const double lb = lp / 100.0 + .5;
     p->lowpass_byte = to_i32(lb > 255 ? 255 : lb);
     p->quality_byte = 100 - 10 * 4 - 3;

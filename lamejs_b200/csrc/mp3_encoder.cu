@@ -6,6 +6,7 @@
  * No CPU fallback exists: if CUDA is unavailable every entry point returns MP3B200_ERR_CUDA.
  */
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -24,6 +25,7 @@
 #include "k_psy.cuh"
 #include "k_quant.cuh"
 #include "k_tag.cuh"
+#include "k_resample.cuh"
 #include "mp3_tag.h"
 
 namespace {
@@ -34,7 +36,7 @@ int g_device = 0;                         /* device of configurations / handles 
 std::atomic<long long> g_launches{0};
 enum { MP3_MAX_DEVICES = 64 };
 bool g_consts_ready[MP3_MAX_DEVICES] = {};   /* __constant__ / __device__ tables are per device */
-bool g_fb_attr_done[MP3_MAX_DEVICES] = {};
+bool g_fb_attr_done[MP3_MAX_DEVICES][2] = {};   /* k_subband_analysis<false / true> */
 
 #define CK(call)                                                                                  \
   do {                                                                                            \
@@ -47,10 +49,19 @@ bool g_fb_attr_done[MP3_MAX_DEVICES] = {};
     }                                                                                             \
   } while (0)
 
-struct Config { Mp3Tables host; Mp3Tables* dev; int device; };
-std::map<std::tuple<int, int, int, int>, Config*> g_configs;   /* (device, ch, sr, kbps) */
-struct ByteGeom { int frame_bytes_nopad, frac_SpF, mode_gr, samplerate; };
-std::map<std::tuple<int, int, int>, ByteGeom> g_byte_geom;   /* (ch, sr, kbps) -> byte geometry; frame_bytes_nopad < 0: unsupported */
+/* host.samplerate is the rate lamejs encodes at; with resampling (rs.ratio > 1) the caller's samples arrive at rs.in_rate
+ * and k_resample turns them into samples at host.samplerate on the device */
+struct Config { Mp3Tables host; Mp3Tables* dev; int device; int flags, kbps_asked; Mp3Resample rs; };
+std::map<std::tuple<int, int, int, int, int>, Config*> g_configs;   /* (device, ch, sr, kbps, flags) */
+struct ByteGeom { int frame_bytes_nopad, frac_SpF, mode_gr, samplerate, ratio; };
+std::map<std::tuple<int, int, int, int>, ByteGeom> g_byte_geom;   /* (ch, sr, kbps, flags) -> byte geometry; frame_bytes_nopad < 0: unsupported */
+
+/* the flags that select a configuration: MP3B200_RESAMPLE only matters where lamejs resamples, so a flagged configuration
+ * that encodes at its input rate is the unflagged one.  -1: unknown flag bits. */
+int config_flags(int ch, int sr, int kbps, int flags) {
+  if (flags & ~MP3B200_RESAMPLE) return -1;
+  return (flags & MP3B200_RESAMPLE) && mp3_out_samplerate(ch, sr, kbps) != sr ? MP3B200_RESAMPLE : 0;
+}
 
 /* g_mu held.  Makes `dev` current for the calling thread and uploads the constant tables once per device. */
 int ensure_device(int dev) {
@@ -72,17 +83,23 @@ int ensure_device(int dev) {
   return 0;
 }
 
-int get_config(int ch, int sr, int kbps, Config** out) {
+int get_config(int ch, int sr, int kbps, int flags, Config** out) {
+  flags = config_flags(ch, sr, kbps, flags);
+  if (flags < 0) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
   std::lock_guard<std::mutex> lk(g_mu);
   const int dev = g_device;
   int rc = ensure_device(dev);
   if (rc) return rc;
-  auto key = std::make_tuple(dev, ch, sr, kbps);
+  auto key = std::make_tuple(dev, ch, sr, kbps, flags);
   auto it = g_configs.find(key);
   if (it != g_configs.end()) { *out = it->second; return 0; }
   Config* c = new Config();
-  if (mp3_build_tables(ch, sr, kbps, &c->host) != 0) { delete c; g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
-  c->device = dev;
+  if (mp3_build_tables(ch, sr, kbps, &c->host, flags, &c->rs) != 0 || c->rs.ratio > RS_MAX_RATIO) {
+    delete c; g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG;
+  }
+  c->device = dev; c->flags = flags; c->kbps_asked = kbps;
+  if (c->rs.ratio > 1)     /* the ratio's filter row (the same taps for every configuration of that ratio) */
+    CK(cudaMemcpyToSymbol(c_rs_h, c->rs.h, sizeof(float) * MP3_RS_TAPS, sizeof(float) * MP3_RS_TAPS * c->rs.ratio));
   CK(cudaMalloc(&c->dev, sizeof(Mp3Tables)));
   CK(cudaMemcpy(c->dev, &c->host, sizeof(Mp3Tables), cudaMemcpyHostToDevice));
   g_configs[key] = c;
@@ -93,38 +110,54 @@ int get_config(int ch, int sr, int kbps, Config** out) {
 /* lamejs's input FIFO (gfc.mf_size / mf_samples_to_encode), counted without the samples.  framesize = 576 * mode_gr samples
  * enter per step of lame_encode_buffer_sample (Lame.js:1592-1663); a frame is encoded whenever the FIFO holds
  * framesize + 752 (calcNeeded, Lame.js:1516).  A fresh encoder's FIFO holds 576 - 48 zeros and has ENCDELAY + POSTDELAY =
- * 576 + 1152 samples to encode, whatever the frame size. */
-struct FifoFlush { long long frames, zeros, end_padding; };
+ * 576 + 1152 samples to encode, whatever the frame size.
+ * With an integer resampling ratio r (Config::rs) the FIFO fills with the resampler's outputs: after P input samples
+ * lamejs has made outputs(P) = max(0, ceil((P - 16) / r)) of them (output m needs input r m + 16), however P was split
+ * into calls.  Sample counts of feed() and flush() are input samples; mf_size and mf_samples_to_encode count outputs. */
+struct FifoFlush { long long frames, zeros; int end_padding; };
 struct LameFifo {
   static constexpr long long ENC_POST_DELAY = 576 + 1152;     /* ENCDELAY + POSTDELAY */
   long long framesize, mf_size = 576 - 48, mf_samples_to_encode = ENC_POST_DELAY;
-  explicit LameFifo(int mode_gr) : framesize(576LL * mode_gr) {}
-  /* frames completed by feeding n samples.  Closed form of the step loop: a step adds at most framesize and takes at most
-   * one frame, so mf_size stays below framesize + 752 and the frames are the crossings of that level. */
+  int ratio = 1;
+  long long in_fed = 0;                   /* input samples fed so far (resampling only) */
+  explicit LameFifo(int mode_gr, int r = 1) : framesize(576LL * mode_gr), ratio(r) {}
+  long long outputs(long long p) const {
+    if (ratio == 1) return p;
+    return p > MP3_RS_HALF ? (p - MP3_RS_HALF + ratio - 1) / ratio : 0;
+  }
+  /* frames completed by feeding n input samples.  Closed form of the step loop: a step adds at most framesize outputs and
+   * takes at most one frame, so mf_size stays below framesize + 752 and the frames are the crossings of that level. */
   long long feed(long long n) {
     if (n <= 0) return 0;
+    const long long k = outputs(in_fed + n) - outputs(in_fed);
+    in_fed += n;
     const long long need = framesize + 752;
-    const long long frames = mf_size + n >= need ? (mf_size + n - need) / framesize + 1 : 0;
+    const long long frames = mf_size + k >= need ? (mf_size + k - need) / framesize + 1 : 0;
     if (mf_samples_to_encode < 1) mf_samples_to_encode = ENC_POST_DELAY;
-    mf_size += n - frames * framesize;
-    mf_samples_to_encode += n - frames * framesize;
+    mf_size += k - frames * framesize;
+    mf_samples_to_encode += k - frames * framesize;
     return frames;
   }
-  /* lame_encode_flush (Lame.js:1393-1443): feeds zero bunches of min(1152, what the next frame needs) until the padded end
-   * is out; all zero once flushed (Lame.js:1397-1399).  end_padding is gfp.encoder_padding (Lame.js:1412). */
+  /* lame_encode_flush (Lame.js:1393-1443), in JS numbers: feeds zero bunches of min(1152, the input the next frame needs)
+   * until the padded end is out; all zero once flushed (Lame.js:1397-1399).  end_padding is gfp.encoder_padding
+   * (Lame.js:1412).  With resampling, samples_to_encode gains 16 * out / in (16 / r: the same correctly rounded quotient),
+   * so end_padding and frames_left are fractional: frames_left = 3 + eps encodes a fourth frame, as lamejs does. */
   FifoFlush flush() {
     FifoFlush r = {0, 0, 0};
     if (mf_samples_to_encode < 1) return r;
-    const long long samples_to_encode = mf_samples_to_encode - 1152;     /* POSTDELAY */
-    r.end_padding = framesize - samples_to_encode % framesize;
-    if (r.end_padding < 576) r.end_padding += framesize;
-    long long frames_left = (samples_to_encode + r.end_padding) / framesize;
+    double samples_to_encode = (double)(mf_samples_to_encode - 1152);     /* POSTDELAY */
+    if (ratio > 1) samples_to_encode += 16. / ratio;
+    double end_padding = framesize - fmod(samples_to_encode, (double)framesize);
+    if (end_padding < 576) end_padding += framesize;
+    r.end_padding = (int)end_padding;                                    /* ToInt32 of a small positive number */
+    double frames_left = (samples_to_encode + end_padding) / framesize;
     while (frames_left > 0) {
-      long long bunch = framesize + 752 - mf_size;
+      double bunch = (double)(framesize + 752 - mf_size);
+      bunch *= ratio;                                                    /* * in / out: exact for out | in */
       if (bunch > 1152) bunch = 1152;
       if (bunch < 1) bunch = 1;
-      const long long got = feed(bunch);
-      r.zeros += bunch;
+      const long long got = feed((long long)bunch);                      /* an integer: (need) * r or a clamp bound */
+      r.zeros += (long long)bunch;
       r.frames += got;
       frames_left -= got > 0 ? 1 : 0;     /* sic (Lame.js:1443): one per bunch that completed a frame, even when a 1152-sample
                                              bunch completed two 576-sample frames */
@@ -135,8 +168,8 @@ struct LameFifo {
 };
 
 /* frames produced by encodeBuffer(n samples) + flush() on a fresh encoder */
-long long frames_for(long long n, int mode_gr) {
-  LameFifo f(mode_gr);
+long long frames_for(long long n, int mode_gr, int ratio = 1) {
+  LameFifo f(mode_gr, ratio);
   const long long fed = f.feed(n);
   return fed + f.flush().frames;
 }
@@ -188,6 +221,8 @@ struct Workspace {
   Buf<int> dirty;                         /* [3][F] work lists for re-quantization passes */
   Buf<int> counter;                       /* [Q_NCOUNTERS] */
   Buf<ScanChunk> scan;                    /* [F / SCAN_FRAMES + S] */
+  Buf<ResampleDesc> rs_desc;              /* resampled batches: [S] */
+  Buf<float> rs_y;                        /* resampled batches: the resampler's output rows, the PCM the pipeline reads */
   int fit(int S, int nch, long long U, long long F) {
     const size_t gc = (size_t)U * nch, rows = (size_t)(U + S) * nch, f = (size_t)F + 1;
     const bool failed = streams.fit(S) || bt_final.fit((size_t)U * 2 + 16) || bt_prev.fit((size_t)U * 2 + 16) ||
@@ -201,6 +236,7 @@ struct Workspace {
     streams.release(); bt_final.release(); bt_prev.release(); xr.release(); slab.release(); psy.release(); scan_in.release();
     ratio.release(); ath_psy.release(); ath_q.release(); qstate.release(); ginfo.release(); l3enc.release(); xrq.release();
     xrpow.release(); neg.release(); prep.release(); dirty.release(); counter.release(); scan.release();
+    rs_desc.release(); rs_y.release();
   }
 };
 
@@ -214,6 +250,7 @@ struct ThreadCtx {
   int device = -1;
   cudaStream_t st = nullptr, up_st = nullptr, aux_st = nullptr;   /* main, PCM upload, quantizer repair chain */
   cudaEvent_t ev[8] = {}, evq[QE_COUNT] = {}, ev_in = nullptr, ev_fork = nullptr, ev_join = nullptr, ready[MP3_MAX_PCM_CHUNKS] = {};
+  cudaEvent_t ev_rs[2] = {};              /* around k_resample */
   Workspace ws;
   int evq_pred[QE_COUNT] = {};
   Buf<int16_t> pcm;                       /* staged PCM of host callers */
@@ -228,6 +265,7 @@ struct ThreadCtx {
     for (auto& e : ev) if (e) { cudaEventDestroy(e); e = nullptr; }
     for (auto& e : evq) if (e) { cudaEventDestroy(e); e = nullptr; }
     for (auto& e : ready) if (e) { cudaEventDestroy(e); e = nullptr; }
+    for (auto& e : ev_rs) if (e) { cudaEventDestroy(e); e = nullptr; }
     if (ev_in) { cudaEventDestroy(ev_in); ev_in = nullptr; }
     if (ev_fork) { cudaEventDestroy(ev_fork); ev_fork = nullptr; }
     if (ev_join) { cudaEventDestroy(ev_join); ev_join = nullptr; }
@@ -246,6 +284,7 @@ struct ThreadCtx {
     for (auto& e : ev) CK(cudaEventCreate(&e));
     for (auto& e : evq) CK(cudaEventCreate(&e));
     for (auto& e : ready) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    for (auto& e : ev_rs) CK(cudaEventCreate(&e));
     CK(cudaEventCreateWithFlags(&ev_in, cudaEventDisableTiming));
     CK(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
     CK(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
@@ -300,6 +339,7 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
   Workspace& ws = t_ctx.ws;
 
   const int nch = cfg->host.nch;
+  const bool f32_pcm = cfg->rs.ratio > 1;   /* the streams read the resampler's Float32 output */
   int max_frames = 0;
   long long total_frames = 0;          /* rows actually used this launch (the workspace may be larger) */
   int scan_rows = 0;
@@ -343,7 +383,8 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
       if (arrival) CK(cudaStreamWaitEvent(st, arrival->ready[j], 0));
       if (u_hi[j] <= u_lo[j]) continue;
       dim3 gridj(u_hi[j] - u_lo[j], nch, S);
-      k_psy_analysis<<<gridj, PSY_THREADS, 0, st>>>(cfg->dev, ws.streams.p, ws.psy.p, j, nchunks, u_lo[j]);
+      if (f32_pcm) k_psy_analysis<true><<<gridj, PSY_THREADS, 0, st>>>(cfg->dev, ws.streams.p, ws.psy.p, j, nchunks, u_lo[j]);
+      else k_psy_analysis<false><<<gridj, PSY_THREADS, 0, st>>>(cfg->dev, ws.streams.p, ws.psy.p, j, nchunks, u_lo[j]);
       g_launches++;
       DBG("k_psy_analysis");
     }
@@ -361,9 +402,10 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
     {
       const int G = cfg->host.mode_gr;
       const size_t smem = sizeof(double) * FB_PCM_WORDS + sizeof(float) * (FB_SLABS * 18 * FB_SLAB_STRIDE);
+      void (*const k_fb)(const Mp3Tables*, const StreamDesc*, float*) = f32_pcm ? k_subband_analysis<true> : k_subband_analysis<false>;
       {
         std::lock_guard<std::mutex> lk(g_mu);   /* the attribute is per device */
-        if (!g_fb_attr_done[cfg->device]) { CK(cudaFuncSetAttribute(k_subband_analysis, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); g_fb_attr_done[cfg->device] = true; }
+        if (!g_fb_attr_done[cfg->device][f32_pcm]) { CK(cudaFuncSetAttribute(k_fb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); g_fb_attr_done[cfg->device][f32_pcm] = true; }
       }
       cudaLaunchConfig_t lc = {};
       lc.gridDim = dim3((G * max_frames + 1 + FB_SLABS - 1) / FB_SLABS, nch, S);
@@ -372,7 +414,7 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
       at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
       at[0].val.programmaticStreamSerializationAllowed = 1;
       lc.attrs = at; lc.numAttrs = 1;
-      CK(cudaLaunchKernelEx(&lc, k_subband_analysis, (const Mp3Tables*)cfg->dev, (const StreamDesc*)ws.streams.p, ws.slab.p));
+      CK(cudaLaunchKernelEx(&lc, k_fb, (const Mp3Tables*)cfg->dev, (const StreamDesc*)ws.streams.p, ws.slab.p));
       g_launches++;
       DBG("k_subband_analysis");
     }
@@ -447,11 +489,70 @@ void init_stream_state(StreamDesc& sd) {   /* lame_init_old + psymodel_init star
   sd.current_step[0] = sd.current_step[1] = 4;
 }
 
+/* first sample (at the encoding rate) that frame `frame` and later frames read: the filterbank slab of the granule before
+ * frame k starts at framesize * k - 1104 */
+long long hist_base_at(int mode_gr, long long frame) {
+  const long long b = 576LL * mode_gr * frame - 1104;
+  return b > 0 ? b : 0;
+}
+
+/* Resampled launches: the descriptors sds[0 .. S) hold the caller's input (Int16 at rs.in_rate; pcm_base / pcm_end count
+ * input samples, and pcm_base is at most max(0, r * hist_base_at(frame0) - 16), the first input the outputs below read).
+ * Queues k_resample for the outputs the streams' frames read -- from hist_base_at(frame0) up to the last output the input
+ * reaches; later outputs are 0 -- into the workspace, and points the descriptors at them: from then on pcm_base / pcm_end
+ * count outputs, and the stream reads like PCM at the output rate. */
+int resample_streams(Config* cfg, StreamDesc* sds, int S) {
+  const int r = cfg->rs.ratio, nch = cfg->host.nch;
+  Workspace& ws = t_ctx.ws;
+  std::vector<ResampleDesc> rd((size_t)S);
+  long long tot = 0, max_ny = 0;
+  for (int i = 0; i < S; i++) {
+    const StreamDesc& sd = sds[i];
+    const long long yb = hist_base_at(cfg->host.mode_gr, sd.frame0);
+    const long long xb = r * yb - MP3_RS_HALF > 0 ? r * yb - MP3_RS_HALF : 0;
+    if (sd.pcm_base > xb) { g_err = "resampler input starts after the first sample it reads"; return MP3B200_ERR_HANDLE; }
+    long long ye = (sd.pcm_end + MP3_RS_HALF - 1) / r + 1;      /* y[m] reads input up to r m + 16 */
+    if (sd.nframes == 0 || ye < yb) ye = yb;
+    ResampleDesc& d = rd[i];
+    d.x[0] = sd.pcm[0]; d.x[1] = sd.pcm[1]; d.x_base = sd.pcm_base; d.x_end = sd.pcm_end;
+    d.y_base = yb; d.ny = ye - yb;
+    tot += d.ny * nch;
+    max_ny = d.ny > max_ny ? d.ny : max_ny;
+  }
+  int rc = ws.rs_desc.fit((size_t)S);
+  if (rc) return rc;
+  rc = ws.rs_y.fit((size_t)tot + 1);
+  if (rc) return rc;
+  long long off = 0;
+  for (int i = 0; i < S; i++) {
+    ResampleDesc& d = rd[i];
+    d.y[0] = ws.rs_y.p + off; d.y[1] = nch == 2 ? d.y[0] + d.ny : d.y[0];
+    off += d.ny * nch;
+    for (int c = 0; c < 2; c++) sds[i].pcm[c] = reinterpret_cast<const int16_t*>(d.y[c]);
+    sds[i].pcm_base = d.y_base; sds[i].pcm_end = d.y_base + d.ny;
+  }
+  cudaStream_t st = t_ctx.st;
+  CK(cudaEventRecord(t_ctx.ev_in, cudaStreamLegacy));      /* the input may come from the legacy default stream */
+  CK(cudaStreamWaitEvent(st, t_ctx.ev_in, 0));
+  CK(cudaMemcpyAsync(ws.rs_desc.p, rd.data(), sizeof(ResampleDesc) * S, cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(t_ctx.ev_rs[0], st));
+  if (max_ny > 0) {
+    dim3 grid((unsigned)((max_ny + RS_THREADS - 1) / RS_THREADS), nch, S);
+    k_resample<<<grid, RS_THREADS, 0, st>>>(ws.rs_desc.p, r, cfg->host.scale_applied, cfg->host.scale);
+    g_launches++;
+    DBG("k_resample");
+  }
+  CK(cudaEventRecord(t_ctx.ev_rs[1], st));
+  return 0;
+}
+
 /* Encodes the streams `sds` into d_out: the caller sets each descriptor's PCM, pcm_base / pcm_end, frame0, nframes,
  * out_base and carried state; this assigns unit_base / frame_base, grows the thread's workspace and runs the pipeline.
  * The stream index is a grid y / z coordinate of several kernels (CUDA limit 65535): a larger batch runs as consecutive
  * launches of at most MP3_MAX_LAUNCH_STREAMS streams on the thread's stream, the later ones behind every PCM upload.
- * Timings add up over the launches; the pass count is the largest any of them needed. */
+ * Timings add up over the launches; the pass count is the largest any of them needed.
+ * With resampling (cfg->rs.ratio > 1) the descriptors hold the caller's input as resample_streams describes; each launch
+ * first resamples it (timing slot 14). */
 int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, const LaunchOpts& o) {
   if (o.timings_ms) for (int i = 0; i < 16; i++) o.timings_ms[i] = 0.0f;
   const PcmArrival* arrival = o.arrival;
@@ -467,15 +568,25 @@ int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, co
     if (F == 0) continue;                     /* empty group: nothing to launch */
     int rc = t_ctx.ws.fit(n, cfg->host.nch, U, F);
     if (rc) return rc;
+    const bool resampled = cfg->rs.ratio > 1;
+    if (resampled) {
+      if (arrival)                              /* the resampler reads all of the input: wait for every slice */
+        for (int j = 0; j < arrival->chunks; j++) CK(cudaStreamWaitEvent(t_ctx.st, arrival->ready[j], 0));
+      arrival = nullptr;
+      rc = resample_streams(cfg, group, n);
+      if (rc) return rc;
+    }
     Timings tm;
     rc = run_pipeline(cfg, group, n, d_out, o, arrival, &tm);
     if (rc) return rc;
     arrival = nullptr;
+    float rs_ms = 0.0f;
+    if (resampled && o.timings_ms && o.sync) CK(cudaEventElapsedTime(&rs_ms, t_ctx.ev_rs[0], t_ctx.ev_rs[1]));
     if (o.committed)
       CK(cudaMemcpyAsync(o.committed + g0, t_ctx.ws.streams.p, sizeof(StreamDesc) * n, cudaMemcpyDeviceToHost, t_ctx.st));
     if (o.timings_ms) {
       const float t[16] = {tm.psy, tm.scan, tm.mask, tm.fb, tm.q1, tm.qn, tm.total, 0.0f,
-                           tm.q_prepare, tm.q_search, tm.q_outer, tm.q_finish, tm.q_pack, tm.q_mid, 0.0f, 0.0f};
+                           tm.q_prepare, tm.q_search, tm.q_outer, tm.q_finish, tm.q_pack, tm.q_mid, rs_ms, 0.0f};
       for (int i = 0; i < 16; i++) o.timings_ms[i] += t[i];
       if ((float)tm.passes > o.timings_ms[7]) o.timings_ms[7] = (float)tm.passes;
     }
@@ -509,14 +620,18 @@ int64_t mp3b200_stream_frames(int64_t nsamples) { return frames_for(nsamples, 2)
 
 namespace {
 /* the byte geometry of a configuration is three integers; building the full tables costs ~1 ms, so it is done once */
-ByteGeom byte_geom(int channels, int samplerate, int kbps) {
+ByteGeom byte_geom(int channels, int samplerate, int kbps, int flags = 0) {
+  flags = config_flags(channels, samplerate, kbps, flags);
+  if (flags < 0) return ByteGeom{-1, 0, 2, samplerate, 1};
   std::lock_guard<std::mutex> lk(g_mu);
-  auto key = std::make_tuple(channels, samplerate, kbps);
+  auto key = std::make_tuple(channels, samplerate, kbps, flags);
   auto it = g_byte_geom.find(key);
   if (it != g_byte_geom.end()) return it->second;
   Mp3Tables* t = new Mp3Tables();
-  const int rc = mp3_build_tables(channels, samplerate, kbps, t);
-  ByteGeom g = rc == 0 ? ByteGeom{t->frame_bytes_nopad, t->frac_SpF, t->mode_gr, t->samplerate} : ByteGeom{-1, 0, 2, samplerate};
+  Mp3Resample rs;
+  const int rc = mp3_build_tables(channels, samplerate, kbps, t, flags, &rs);
+  ByteGeom g = rc == 0 && rs.ratio <= RS_MAX_RATIO ? ByteGeom{t->frame_bytes_nopad, t->frac_SpF, t->mode_gr, t->samplerate, rs.ratio}
+                                                   : ByteGeom{-1, 0, 2, samplerate, 1};
   delete t;
   g_byte_geom[key] = g;
   return g;
@@ -524,9 +639,13 @@ ByteGeom byte_geom(int channels, int samplerate, int kbps) {
 }  // namespace
 
 int64_t mp3b200_stream_bytes(int channels, int samplerate, int kbps, int64_t nsamples) {
-  const ByteGeom g = byte_geom(channels, samplerate, kbps);
+  return mp3b200_stream_bytes_ex(channels, samplerate, kbps, 0, nsamples);
+}
+
+int64_t mp3b200_stream_bytes_ex(int channels, int samplerate, int kbps, int flags, int64_t nsamples) {
+  const ByteGeom g = byte_geom(channels, samplerate, kbps, flags);
   if (g.frame_bytes_nopad < 0 || nsamples < 0) return -1;
-  return bytes_of_frames(g, 0, frames_for(nsamples, g.mode_gr));
+  return bytes_of_frames(g, 0, frames_for(nsamples, g.mode_gr, g.ratio));
 }
 
 int64_t mp3b200_stream_frames_cfg(int channels, int samplerate, int kbps, int64_t nsamples) {
@@ -539,6 +658,8 @@ int mp3b200_granules_per_frame(int channels, int samplerate, int kbps) {
   const ByteGeom g = byte_geom(channels, samplerate, kbps);
   return g.frame_bytes_nopad < 0 ? -1 : g.mode_gr;
 }
+
+int mp3b200_out_samplerate(int channels, int samplerate, int kbps) { return mp3_out_samplerate(channels, samplerate, kbps); }
 
 }  // extern "C"
 
@@ -554,7 +675,7 @@ std::vector<StreamDesc> whole_streams(Config* cfg, int nstreams, const int16_t* 
     sd.pcm[0] = d_pcm + pcm_off[s];
     sd.pcm[1] = cfg->host.nch == 2 ? sd.pcm[0] + nsamples[s] : sd.pcm[0];
     sd.pcm_base = 0; sd.pcm_end = nsamples[s];
-    sd.frame0 = 0; sd.nframes = (int)frames_for(nsamples[s], cfg->host.mode_gr);
+    sd.frame0 = 0; sd.nframes = (int)frames_for(nsamples[s], cfg->host.mode_gr, cfg->rs.ratio);
     sd.out_base = out_off[s];
     init_stream_state(sd);
   }
@@ -576,7 +697,7 @@ int encode_host_streams(Config* cfg, int nstreams, const int16_t* const* left, c
     pcm_off[s] = tot_samples;
     tot_samples += nsamples[s] * nch;
     out_off[s] = tot_bytes;
-    audio[s] = bytes_of_frames(cfg->host, 0, frames_for(nsamples[s], cfg->host.mode_gr));
+    audio[s] = bytes_of_frames(cfg->host, 0, frames_for(nsamples[s], cfg->host.mode_gr, cfg->rs.ratio));
     if (cap[s] < audio[s] + extra) { g_err = "output buffer too small"; return MP3B200_ERR_BUFFER; }
     out_bytes[s] = audio[s] + extra;
     tot_bytes += audio[s];
@@ -619,9 +740,15 @@ extern "C" {
 int mp3b200_encode_streams_device(int channels, int samplerate, int kbps, int nstreams, const int16_t* d_pcm,
                                   const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
                                   const int64_t* out_off, float* timings_ms) {
+  return mp3b200_encode_streams_device_ex(channels, samplerate, kbps, 0, nstreams, d_pcm, pcm_off, nsamples, d_out, out_off, timings_ms);
+}
+
+int mp3b200_encode_streams_device_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
+                                     const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
+                                     const int64_t* out_off, float* timings_ms) {
   if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
   Config* cfg;
-  int rc = get_config(channels, samplerate, kbps, &cfg);
+  int rc = get_config(channels, samplerate, kbps, flags, &cfg);
   if (rc) return rc;
   rc = t_ctx.use(cfg->device);
   if (rc) return rc;
@@ -634,9 +761,15 @@ int mp3b200_encode_streams_device(int channels, int samplerate, int kbps, int ns
 int mp3b200_encode_streams(int channels, int samplerate, int kbps, int nstreams, const int16_t* const* left,
                            const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
                            const int64_t* cap, int64_t* out_bytes) {
+  return mp3b200_encode_streams_ex(channels, samplerate, kbps, 0, nstreams, left, right, nsamples, out, cap, out_bytes);
+}
+
+int mp3b200_encode_streams_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
+                              const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
+                              const int64_t* cap, int64_t* out_bytes) {
   if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
   Config* cfg;
-  int rc = get_config(channels, samplerate, kbps, &cfg);
+  int rc = get_config(channels, samplerate, kbps, flags, &cfg);
   if (rc) return rc;
   std::vector<int64_t> out_off;
   std::vector<long long> audio;
@@ -673,7 +806,7 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* tp) {
   uint8_t* bytes_out = tp->bytes_out;
   const int64_t bytes_cap = tp->bytes_cap;
   Config* cfg;
-  int rc = get_config(channels, tp->samplerate, tp->kbps, &cfg);
+  int rc = get_config(channels, tp->samplerate, tp->kbps, 0, &cfg);
   if (rc) return rc;
   rc = t_ctx.use(cfg->device);
   if (rc) return rc;
@@ -784,6 +917,41 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* tp) {
   return rc;
 }
 
+int mp3b200_debug_resample(int channels, int samplerate, int kbps, const int16_t* left, const int16_t* right, int64_t nsamples,
+                           float* y, int64_t ny) {
+  if (nsamples < 0 || ny < 0 || (nsamples > 0 && !left) || (ny > 0 && !y)) { g_err = "bad buffers"; return MP3B200_ERR_HANDLE; }
+  Config* cfg;
+  int rc = get_config(channels, samplerate, kbps, MP3B200_RESAMPLE, &cfg);
+  if (rc) return rc;
+  if (cfg->rs.ratio == 1) { g_err = "this configuration does not resample"; return MP3B200_ERR_CONFIG; }
+  rc = t_ctx.use(cfg->device);
+  if (rc) return rc;
+  if (ny == 0) return 0;
+  const int nch = cfg->host.nch;
+  rc = t_ctx.pcm.fit((size_t)(nsamples * nch + 8));
+  if (rc) return rc;
+  rc = t_ctx.ws.rs_desc.fit(1);
+  if (rc) return rc;
+  rc = t_ctx.ws.rs_y.fit((size_t)(ny * nch));
+  if (rc) return rc;
+  int16_t* d_pcm = t_ctx.pcm.p;
+  if (nsamples > 0) {
+    CK(cudaMemcpyAsync(d_pcm, left, sizeof(int16_t) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
+    if (nch == 2) CK(cudaMemcpyAsync(d_pcm + nsamples, right ? right : left, sizeof(int16_t) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
+  }
+  ResampleDesc d;
+  d.x[0] = d_pcm; d.x[1] = nch == 2 ? d_pcm + nsamples : d_pcm; d.x_base = 0; d.x_end = nsamples;
+  d.y[0] = t_ctx.ws.rs_y.p; d.y[1] = d.y[0] + (nch == 2 ? ny : 0); d.y_base = 0; d.ny = ny;
+  CK(cudaMemcpyAsync(t_ctx.ws.rs_desc.p, &d, sizeof d, cudaMemcpyHostToDevice, t_ctx.st));
+  k_resample<<<dim3((unsigned)((ny + RS_THREADS - 1) / RS_THREADS), nch, 1), RS_THREADS, 0, t_ctx.st>>>(
+      t_ctx.ws.rs_desc.p, cfg->rs.ratio, cfg->host.scale_applied, cfg->host.scale);
+  g_launches++;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(y, t_ctx.ws.rs_y.p, sizeof(float) * (size_t)(ny * nch), cudaMemcpyDeviceToHost, t_ctx.st));
+  CK(cudaStreamSynchronize(t_ctx.st));
+  return 0;
+}
+
 }  // extern "C"
 
 /* ---- container / metadata step (SURVEY.md 8(f3)): music CRC on the device, tag frames on the host ---- */
@@ -890,8 +1058,13 @@ int mp3b200_crc16_combine(int crc_a, int crc_b, int64_t len_b) {
 }
 
 int mp3b200_lametag_size(int channels, int samplerate, int kbps) {
+  return mp3b200_lametag_size_ex(channels, samplerate, kbps, 0);
+}
+
+int mp3b200_lametag_size_ex(int channels, int samplerate, int kbps, int flags) {
+  flags = config_flags(channels, samplerate, kbps, flags);
   Mp3TagParams p;
-  if (mp3_tag_params(channels, samplerate, kbps, &p) != 0) return MP3B200_ERR_CONFIG;
+  if (flags < 0 || mp3_tag_params(channels, samplerate, kbps, &p, flags) != 0) return MP3B200_ERR_CONFIG;
   return p.fits ? p.frame_bytes : 0;
 }
 
@@ -914,7 +1087,7 @@ int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int ns
                                   const int64_t* cap, int64_t* out_bytes) {
   if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
   Config* cfg;
-  int rc = get_config(channels, samplerate, kbps, &cfg);
+  int rc = get_config(channels, samplerate, kbps, 0, &cfg);
   if (rc) return rc;
   Mp3TagParams p;
   if (mp3_tag_params(channels, samplerate, kbps, &p) != 0) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }

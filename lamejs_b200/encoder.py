@@ -70,6 +70,14 @@ def lib():
     L.mp3b200_debug_music_crc.argtypes = [vp, vp, vp, c_int, vp, vp]
     L.mp3b200_debug_stages.argtypes = [c_int, c_int, c_int, vp, vp, c_i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, c_i64]
     L.mp3b200_debug_stages_ex.argtypes = [ctypes.POINTER(DebugTaps)]
+    L.mp3b200_create_ex.argtypes = [c_int, c_int, c_int, c_int, ctypes.POINTER(vp)]
+    L.mp3b200_out_samplerate.argtypes = [c_int, c_int, c_int]
+    L.mp3b200_stream_bytes_ex.restype = c_i64
+    L.mp3b200_stream_bytes_ex.argtypes = [c_int, c_int, c_int, c_int, c_i64]
+    L.mp3b200_encode_streams_ex.argtypes = [c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp]
+    L.mp3b200_encode_streams_device_ex.argtypes = [c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp]
+    L.mp3b200_lametag_size_ex.argtypes = [c_int, c_int, c_int, c_int]
+    L.mp3b200_debug_resample.argtypes = [c_int, c_int, c_int, vp, vp, c_i64, vp, c_i64]
     _lib = L
     return L
 
@@ -92,8 +100,20 @@ def granules_per_frame(channels, samplerate, kbps):
     return int(lib().mp3b200_granules_per_frame(channels, samplerate, kbps))
 
 
-def stream_bytes(channels, samplerate, kbps, nsamples):
+RESAMPLE = 1     # MP3B200_RESAMPLE
+
+
+def stream_bytes(channels, samplerate, kbps, nsamples, resample=False):
+    """Bytes encodeBuffer(nsamples) + flush() produce, -1 for a rejected configuration.  resample=True also accepts the
+    configurations lamejs resamples by an integer ratio (nsamples at the input rate)."""
+    if resample:
+        return int(lib().mp3b200_stream_bytes_ex(channels, samplerate, kbps, RESAMPLE, int(nsamples)))
     return int(lib().mp3b200_stream_bytes(channels, samplerate, kbps, int(nsamples)))
+
+
+def out_samplerate(channels, samplerate, kbps):
+    """The rate lamejs encodes (channels, samplerate, kbps) at (!= samplerate: it resamples); 0 for a bad channel count."""
+    return int(lib().mp3b200_out_samplerate(channels, samplerate, kbps))
 
 
 class WavHeader:
@@ -206,16 +226,19 @@ def lametag_build(channels, samplerate, kbps, nframes, music_bytes, music_crc, e
 class Mp3Encoder:
     """Drop-in for lamejs.Mp3Encoder(channels, samplerate, kbps) (src/js/index.js:66-136).  `write_vbr_tag=True` is
     gfp.bWriteVbrTag (index.js:107 sets it false): the stream then starts with a placeholder frame, and `lametag_frame()`
-    after flush() returns the finished Info / LAME tag frame to write over it."""
+    after flush() returns the finished Info / LAME tag frame to write over it.  `resample=True` also accepts the
+    configurations lamejs resamples by an integer ratio, e.g. Mp3Encoder(2, 48000, 64), which encodes at 24 kHz: samples
+    are fed at the input rate and resampled on the GPU (seek() is not supported then)."""
 
-    def __init__(self, channels=1, samplerate=44100, kbps=128, write_vbr_tag=False):
+    def __init__(self, channels=1, samplerate=44100, kbps=128, write_vbr_tag=False, resample=False):
         self._L = lib()
         self._h = ctypes.c_void_p()
         self.channels = channels
-        rc = self._L.mp3b200_create(channels, samplerate, kbps, ctypes.byref(self._h))
+        flags = RESAMPLE if resample else 0
+        rc = self._L.mp3b200_create_ex(channels, samplerate, kbps, flags, ctypes.byref(self._h))
         _check(rc)
         self.tag_on = bool(write_vbr_tag) and _check(self._L.mp3b200_set_write_vbr_tag(self._h, 1)) == 1
-        self._tag_room = lametag_size(channels, samplerate, kbps) if self.tag_on else 0
+        self._tag_room = _check(self._L.mp3b200_lametag_size_ex(channels, samplerate, kbps, flags)) if self.tag_on else 0
 
     def lametag_frame(self):
         buf = np.zeros(2880, dtype=np.uint8)
@@ -322,7 +345,7 @@ def flush_batch(encoders):
     return [o[: int(g)].tobytes() for o, g in zip(outs, got)]
 
 
-def _encode_host_streams(fn, channels, samplerate, kbps, lefts, rights, room):
+def _encode_host_streams(fn, channels, samplerate, kbps, lefts, rights, room, resample=False):
     """Marshalling of the whole-stream host calls: out[s] has room for the stream's bytes plus `room`."""
     S = len(lefts)
     if S == 0:
@@ -330,7 +353,7 @@ def _encode_host_streams(fn, channels, samplerate, kbps, lefts, rights, room):
     lefts = [np.ascontiguousarray(x, dtype=np.int16) for x in lefts]
     rights = lefts if (rights is None or channels == 1) else [np.ascontiguousarray(x, dtype=np.int16) for x in rights]
     ns = np.array([len(x) for x in lefts], dtype=np.int64)
-    nb = [stream_bytes(channels, samplerate, kbps, int(n)) for n in ns]
+    nb = [stream_bytes(channels, samplerate, kbps, int(n), resample) for n in ns]
     if any(b < 0 for b in nb):
         raise Mp3B200Error("unsupported configuration: channels=%d samplerate=%d kbps=%d (lame_init_params would resample)" % (channels, samplerate, kbps))
     nb = [b + room for b in nb]
@@ -344,9 +367,13 @@ def _encode_host_streams(fn, channels, samplerate, kbps, lefts, rights, room):
     return [o[: int(g)].tobytes() for o, g in zip(outs, got)]
 
 
-def encode_streams(channels, samplerate, kbps, lefts, rights=None):
+def encode_streams(channels, samplerate, kbps, lefts, rights=None, resample=False):
     """Batch extension: encodeBuffer(whole stream) + flush() for many independent streams in one launch sequence.
-    Host buffers in, list of bytes out."""
+    Host buffers in, list of bytes out.  resample=True: see Mp3Encoder."""
+    if resample:
+        def fn(ch, sr, kb, *args):
+            return lib().mp3b200_encode_streams_ex(ch, sr, kb, RESAMPLE, *args)
+        return _encode_host_streams(fn, channels, samplerate, kbps, lefts, rights, 0, True)
     return _encode_host_streams(lib().mp3b200_encode_streams, channels, samplerate, kbps, lefts, rights, 0)
 
 
@@ -367,16 +394,31 @@ def debug_music_crc(d_buf_ptr, offsets, lengths, timed=False):
     return ([int(c) for c in crc], float(ms.value)) if timed else [int(c) for c in crc]
 
 
-def encode_streams_device(channels, samplerate, kbps, d_pcm_ptr, pcm_off, nsamples, d_out_ptr, out_off):
-    """Device-resident batch (raw device pointers as ints).  Returns the 16 timing slots of include/mp3b200.h (ms)."""
+def encode_streams_device(channels, samplerate, kbps, d_pcm_ptr, pcm_off, nsamples, d_out_ptr, out_off, resample=False):
+    """Device-resident batch (raw device pointers as ints).  Returns the 16 timing slots of include/mp3b200.h (ms); with
+    resample=True slot 14 is the resampler's time."""
     L = lib()
     pcm_off = np.ascontiguousarray(pcm_off, dtype=np.int64)
     nsamples = np.ascontiguousarray(nsamples, dtype=np.int64)
     out_off = np.ascontiguousarray(out_off, dtype=np.int64)
     tm = np.zeros(16, dtype=np.float32)
-    _check(L.mp3b200_encode_streams_device(channels, samplerate, kbps, len(nsamples), d_pcm_ptr, pcm_off.ctypes.data,
-                                           nsamples.ctypes.data, d_out_ptr, out_off.ctypes.data, tm.ctypes.data))
+    _check(L.mp3b200_encode_streams_device_ex(channels, samplerate, kbps, RESAMPLE if resample else 0, len(nsamples), d_pcm_ptr,
+                                              pcm_off.ctypes.data, nsamples.ctypes.data, d_out_ptr, out_off.ctypes.data, tm.ctypes.data))
     return tm
+
+
+def debug_resample(channels, samplerate, kbps, left, right=None, ny=None):
+    """k_resample's output for an input extended with zeros on both sides: float32 array [nch][ny] (default ny: every output
+    the input reaches)."""
+    L = lib()
+    left = np.ascontiguousarray(left, dtype=np.int16)
+    right = left if (right is None or channels == 1) else np.ascontiguousarray(right, dtype=np.int16)
+    r = samplerate // out_samplerate(channels, samplerate, kbps)
+    if ny is None:
+        ny = (len(left) + 15) // r + 1
+    y = np.zeros((channels, ny), dtype=np.float32)
+    _check(L.mp3b200_debug_resample(channels, samplerate, kbps, left.ctypes.data, right.ctypes.data, len(left), y.ctypes.data, ny))
+    return y
 
 
 def debug_stages(channels, samplerate, kbps, left, right=None, force_blocktype=None, want=("xr",)):
