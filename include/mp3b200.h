@@ -115,6 +115,10 @@ int64_t mp3b200_stream_frames(int64_t nsamples);                 /* MPEG-1 confi
 int64_t mp3b200_stream_frames_cfg(int channels, int samplerate, int kbps, int64_t nsamples);
 /* granules per frame: 2 (MPEG-1: 32 / 44.1 / 48 kHz) or 1 (MPEG-2 / 2.5: 8 .. 24 kHz); -1 if rejected */
 int mp3b200_granules_per_frame(int channels, int samplerate, int kbps);
+/* the same two with flags (MP3B200_RESAMPLE: nsamples are input samples; the frames and granules are those of the output
+ * rate the configuration encodes at) */
+int64_t mp3b200_stream_frames_ex(int channels, int samplerate, int kbps, int flags, int64_t nsamples);
+int mp3b200_granules_per_frame_ex(int channels, int samplerate, int kbps, int flags);
 
 /* Host buffers.  left[s]/right[s]: nsamples[s] Int16 each; right ignored for mono; with stereo input, right == NULL or
  * right[s] == NULL encodes left[s] on both channels.  out[s] receives
@@ -248,8 +252,8 @@ int mp3b200_debug_stages(int channels, int samplerate, int kbps, const int16_t* 
                          int32_t* l3_enc, int32_t* ginfo, uint8_t* bytes_out, int64_t bytes_cap);
 
 /* The same taps, and the quantizer's state, through one struct (mp3b200_debug_stages is a thin wrapper of it).  `size` must
- * be sizeof(mp3b200_debug_taps).  Inputs and the first outputs are those of mp3b200_debug_stages; in addition ([G] granules
- * per frame):
+ * be sizeof(mp3b200_debug_taps): a caller built against an older, shorter struct (before `flags`) is refused with
+ * MP3B200_ERR_HANDLE.  Inputs and the first outputs are those of mp3b200_debug_stages; in addition ([G] granules per frame):
  *   scalefac       int32 [F][G][nch][39]  final scalefactors; gr1 bands that scfsi shares with gr0 hold -1 (as in lamejs)
  *   subblock_gain  int32 [F][G][nch][3]
  *   xmin           float [F][G][nch][39]  calc_xmin's output as the rate loop receives it: the psymax bands (21 long, 36 short),
@@ -261,6 +265,9 @@ int mp3b200_debug_stages(int channels, int samplerate, int kbps, const int16_t* 
  *                  These are the states the final bytes were encoded from: the last verification found every frame's start
  *                  state equal to its predecessor's end state, and a search result kept from an earlier, speculated start
  *                  was kept only because the search from this start landed on the same gain and granule info.
+ * `flags` selects the configuration like the _ex entry points (mp3b200_debug_stages: 0).  With MP3B200_RESAMPLE a
+ * configuration lamejs resamples is tapped after k_resample: left / right / nsamples are input samples, and every shape above
+ * is that of the output rate ([F] = mp3b200_stream_frames_ex(..., flags, nsamples), [G] = mp3b200_granules_per_frame_ex).
  * Any output pointer may be NULL. */
 typedef struct mp3b200_debug_taps {
   int32_t size, channels, samplerate, kbps;
@@ -271,6 +278,7 @@ typedef struct mp3b200_debug_taps {
   int32_t *l3_enc, *ginfo; uint8_t* bytes_out; int64_t bytes_cap;
   int32_t *scalefac, *subblock_gain; float* xmin; int32_t* max_nonzero_coeff; double* xrpow_max;
   int32_t *scfsi, *old_value, *cur_step;
+  int32_t flags;
 } mp3b200_debug_taps;
 int mp3b200_debug_stages_ex(const mp3b200_debug_taps* t);
 

@@ -649,13 +649,21 @@ int64_t mp3b200_stream_bytes_ex(int channels, int samplerate, int kbps, int flag
 }
 
 int64_t mp3b200_stream_frames_cfg(int channels, int samplerate, int kbps, int64_t nsamples) {
-  const ByteGeom g = byte_geom(channels, samplerate, kbps);
+  return mp3b200_stream_frames_ex(channels, samplerate, kbps, 0, nsamples);
+}
+
+int64_t mp3b200_stream_frames_ex(int channels, int samplerate, int kbps, int flags, int64_t nsamples) {
+  const ByteGeom g = byte_geom(channels, samplerate, kbps, flags);
   if (g.frame_bytes_nopad < 0 || nsamples < 0) return -1;
-  return frames_for(nsamples, g.mode_gr);
+  return frames_for(nsamples, g.mode_gr, g.ratio);
 }
 
 int mp3b200_granules_per_frame(int channels, int samplerate, int kbps) {
-  const ByteGeom g = byte_geom(channels, samplerate, kbps);
+  return mp3b200_granules_per_frame_ex(channels, samplerate, kbps, 0);
+}
+
+int mp3b200_granules_per_frame_ex(int channels, int samplerate, int kbps, int flags) {
+  const ByteGeom g = byte_geom(channels, samplerate, kbps, flags);
   return g.frame_bytes_nopad < 0 ? -1 : g.mode_gr;
 }
 
@@ -806,13 +814,14 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* tp) {
   uint8_t* bytes_out = tp->bytes_out;
   const int64_t bytes_cap = tp->bytes_cap;
   Config* cfg;
-  int rc = get_config(channels, tp->samplerate, tp->kbps, 0, &cfg);
+  int rc = get_config(channels, tp->samplerate, tp->kbps, tp->flags, &cfg);
   if (rc) return rc;
   rc = t_ctx.use(cfg->device);
   if (rc) return rc;
   const int nch = cfg->host.nch;
   const int G = cfg->host.mode_gr;
-  const long long F = frames_for(nsamples, G), U = G * F;
+  /* nsamples are the caller's (input) samples; frames and granules are those of the rate the configuration encodes at */
+  const long long F = frames_for(nsamples, G, cfg->rs.ratio), U = G * F;
   /* one whole stream, staged and encoded like a batch of host streams of one */
   const long long nbytes = bytes_of_frames(cfg->host, 0, F);
   rc = t_ctx.pcm.fit((size_t)(nsamples * nch + 8));

@@ -21,7 +21,7 @@ class DebugTaps(ctypes.Structure):
                 ("xr", _vp), ("blocktype", _vp), ("en_l", _vp), ("thm_l", _vp), ("en_s", _vp), ("thm_s", _vp), ("ath_adjust", _vp),
                 ("l3_enc", _vp), ("ginfo", _vp), ("bytes_out", _vp), ("bytes_cap", ctypes.c_int64),
                 ("scalefac", _vp), ("subblock_gain", _vp), ("xmin", _vp), ("max_nonzero_coeff", _vp), ("xrpow_max", _vp),
-                ("scfsi", _vp), ("old_value", _vp), ("cur_step", _vp)]
+                ("scfsi", _vp), ("old_value", _vp), ("cur_step", _vp), ("flags", ctypes.c_int32)]
 
 
 def lib():
@@ -56,6 +56,9 @@ def lib():
     L.mp3b200_stream_frames_cfg.restype = c_i64
     L.mp3b200_stream_frames_cfg.argtypes = [c_int, c_int, c_int, c_i64]
     L.mp3b200_granules_per_frame.argtypes = [c_int, c_int, c_int]
+    L.mp3b200_stream_frames_ex.restype = c_i64
+    L.mp3b200_stream_frames_ex.argtypes = [c_int, c_int, c_int, c_int, c_i64]
+    L.mp3b200_granules_per_frame_ex.argtypes = [c_int, c_int, c_int, c_int]
     L.mp3b200_encode_streams.argtypes = [c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp]
     L.mp3b200_encode_streams_device.argtypes = [c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp]
     L.mp3b200_set_write_vbr_tag.argtypes = [vp, c_int]
@@ -88,19 +91,21 @@ def _check(rc):
     return rc
 
 
-def stream_frames(nsamples, channels=None, samplerate=None, kbps=None):
-    """Frames encodeBuffer(nsamples) + flush() produce.  Without a configuration: MPEG-1 (1152-sample frames)."""
+RESAMPLE = 1     # MP3B200_RESAMPLE
+
+
+def stream_frames(nsamples, channels=None, samplerate=None, kbps=None, resample=False):
+    """Frames encodeBuffer(nsamples) + flush() produce, -1 for a rejected configuration.  Without a configuration: MPEG-1
+    (1152-sample frames).  resample=True: see stream_bytes."""
     if samplerate is None:
         return int(lib().mp3b200_stream_frames(int(nsamples)))
-    return int(lib().mp3b200_stream_frames_cfg(channels, samplerate, kbps, int(nsamples)))
+    return int(lib().mp3b200_stream_frames_ex(channels, samplerate, kbps, RESAMPLE if resample else 0, int(nsamples)))
 
 
-def granules_per_frame(channels, samplerate, kbps):
-    """2 for MPEG-1 (32/44.1/48 kHz), 1 for MPEG-2 / 2.5 (8..24 kHz); -1 for configurations the library rejects."""
-    return int(lib().mp3b200_granules_per_frame(channels, samplerate, kbps))
-
-
-RESAMPLE = 1     # MP3B200_RESAMPLE
+def granules_per_frame(channels, samplerate, kbps, resample=False):
+    """2 for MPEG-1 (32/44.1/48 kHz), 1 for MPEG-2 / 2.5 (8..24 kHz); -1 for configurations the library rejects.  With
+    resample=True a configuration lamejs resamples gets the value of the rate it encodes at."""
+    return int(lib().mp3b200_granules_per_frame_ex(channels, samplerate, kbps, RESAMPLE if resample else 0))
 
 
 def stream_bytes(channels, samplerate, kbps, nsamples, resample=False):
@@ -421,16 +426,18 @@ def debug_resample(channels, samplerate, kbps, left, right=None, ny=None):
     return y
 
 
-def debug_stages(channels, samplerate, kbps, left, right=None, force_blocktype=None, want=("xr",)):
+def debug_stages(channels, samplerate, kbps, left, right=None, force_blocktype=None, want=("xr",), resample=False):
     """Stage taps for parity tests: returns a dict of numpy arrays (see include/mp3b200.h).  `want` names any of xr,
     blocktype, en_l, thm_l, en_s, thm_s, ath_adjust, l3_enc, ginfo, bytes, scalefac, subblock_gain, xmin, max_nonzero_coeff,
-    xrpow_max, scfsi, old_value and cur_step (the last two [F][3][nch]: frame start, after gr0, frame end)."""
+    xrpow_max, scfsi, old_value and cur_step (the last two [F][3][nch]: frame start, after gr0, frame end).  resample=True
+    also accepts the configurations lamejs resamples by an integer ratio: left / right are input samples, the taps are
+    those of the output rate, after k_resample."""
     L = lib()
     left = np.ascontiguousarray(left, dtype=np.int16)
     right = left if (right is None or channels == 1) else np.ascontiguousarray(right, dtype=np.int16)
     n = len(left)
-    F = stream_frames(n, channels, samplerate, kbps)
-    G = granules_per_frame(channels, samplerate, kbps)
+    F = stream_frames(n, channels, samplerate, kbps, resample)
+    G = granules_per_frame(channels, samplerate, kbps, resample)
     if F < 0 or G < 0:
         raise Mp3B200Error("unsupported configuration: channels=%d samplerate=%d kbps=%d" % (channels, samplerate, kbps))
     nch = channels
@@ -455,7 +462,7 @@ def debug_stages(channels, samplerate, kbps, left, right=None, force_blocktype=N
     p_ath = alloc("ath_adjust", (F,), np.float64)
     p_l3 = alloc("l3_enc", (F, G, nch, 576), np.int32)
     p_gi = alloc("ginfo", (F, G, nch, 16), np.int32)
-    nb = stream_bytes(channels, samplerate, kbps, n)
+    nb = stream_bytes(channels, samplerate, kbps, n, resample)
     if nb < 0:
         raise Mp3B200Error("unsupported configuration: channels=%d samplerate=%d kbps=%d" % (channels, samplerate, kbps))
     p_by = alloc("bytes", (nb,), np.uint8)
@@ -466,6 +473,7 @@ def debug_stages(channels, samplerate, kbps, left, right=None, force_blocktype=N
                   scalefac=alloc("scalefac", (F, G, nch, 39), np.int32), subblock_gain=alloc("subblock_gain", (F, G, nch, 3), np.int32),
                   xmin=alloc("xmin", (F, G, nch, 39), np.float32), max_nonzero_coeff=alloc("max_nonzero_coeff", (F, G, nch), np.int32),
                   xrpow_max=alloc("xrpow_max", (F, G, nch), np.float64), scfsi=alloc("scfsi", (F, nch, 4), np.int32),
-                  old_value=alloc("old_value", (F, 3, nch), np.int32), cur_step=alloc("cur_step", (F, 3, nch), np.int32))
+                  old_value=alloc("old_value", (F, 3, nch), np.int32), cur_step=alloc("cur_step", (F, 3, nch), np.int32),
+                  flags=RESAMPLE if resample else 0)
     _check(L.mp3b200_debug_stages_ex(ctypes.byref(t)))
     return res

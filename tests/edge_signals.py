@@ -3,9 +3,14 @@
 tones near 20 kHz), and the configurations each one is encoded with.
 
 CASES drives tests/test_gpu_edges.py (every stage tap and the bytes against the oracle) and tests/test_edge_corpus_cpu.py
-(the oracle, built with coverage, reaches the branches the corpus is meant to reach)."""
+(the oracle, built with coverage, reaches the branches the corpus is meant to reach).  RESAMPLED_CASES are the same
+generators fed to configurations lamejs resamples by an integer ratio r (MP3B200_RESAMPLE): the signals are made at the
+input rate and sized and laid out in output samples times r, so the clicks still walk through every sub-block of the
+output granules.  tests/test_gpu_edges.py runs them through every stage tap too, and tests/test_resample_cpu.py checks what
+the resampler turns them into."""
 import numpy as np
 
+import oracle_lib
 from synth import white
 
 FULL = 32767
@@ -62,17 +67,19 @@ def fs_white(n, seed=3):
     return _noise(n, seed)
 
 
-def click_train(n, spacing, seed=4):
+def click_train(n, spacing, seed=4, ratio=1):
     """Full-scale clicks (a short noise burst of 16 samples) on a +-1 LSB floor, `spacing` granules apart; the offset of
     each click inside its granule walks through every sub-block quarter (48 samples), so that over the train the
-    attacks land in every sub-block of the attack detector, and across the 16-frame boundaries of the block-type scan."""
+    attacks land in every sub-block of the attack detector, and across the 16-frame boundaries of the block-type scan.
+    With `ratio` r (input samples per output sample of a resampled configuration) granules and offsets are r times longer:
+    they are those of the output."""
     a, b = _noise(n, seed)
     l = (a.astype(np.int32) % 3 - 1).astype(np.int16)
     r = (b.astype(np.int32) % 3 - 1).astype(np.int16)
     k = 0
-    pos = GRANULE // 2
+    pos = GRANULE * ratio // 2
     while True:
-        at = pos + (k * 48) % GRANULE
+        at = pos + (k * 48 * ratio) % (GRANULE * ratio)
         if at + 16 > n:
             break
         burst_l, burst_r = _noise(16, 100 + k)
@@ -80,23 +87,24 @@ def click_train(n, spacing, seed=4):
         if k % 3:                                  # every third click is left only
             r[at:at + 16] = np.where(burst_r >= 0, FULL, -FULL - 1)
         k += 1
-        pos += spacing * GRANULE
+        pos += spacing * GRANULE * ratio
     return l, r
 
 
-def click_pairs(n, seed=9):
+def click_pairs(n, seed=9, ratio=1):
     """Pairs of full-scale clicks one short block (192 samples) apart, every other granule, the pair's offset walking
     through the granule in 32-sample steps: the second click of a pair is an attack in the last sub-block of one granule
-    while the first one left lastAttacks set -- the case in which an attack in sub-block 0 is suppressed."""
+    while the first one left lastAttacks set -- the case in which an attack in sub-block 0 is suppressed.  `ratio`: as in
+    click_train."""
     a, b = _noise(n, seed)
     l = (a.astype(np.int32) % 3 - 1).astype(np.int16)
     r = (b.astype(np.int32) % 3 - 1).astype(np.int16)
     k = 0
     while True:
-        at = 2 * GRANULE * k + (32 * k) % GRANULE
-        if at + SUBBLOCK + 8 > n:
+        at = ratio * (2 * GRANULE * k + (32 * k) % GRANULE)
+        if at + SUBBLOCK * ratio + 8 > n:
             break
-        for x in (at, at + SUBBLOCK):
+        for x in (at, at + SUBBLOCK * ratio):
             l[x:x + 8] = FULL
             r[x:x + 8] = -FULL - 1
         k += 1
@@ -132,7 +140,9 @@ def hf_tone(n, sr, seed=8):
     return l.astype(np.int16), r.astype(np.int16)
 
 
-def make(kind, n, sr, framesize):
+def make(kind, n, sr, framesize, ratio=1):
+    """`n` samples of `kind` at `sr`; `framesize` and `ratio` are in input samples (a resampled configuration's output frame
+    and granule are `ratio` times longer at the input)."""
     if kind == "square":
         return square(n)
     if kind == "dc_max":
@@ -150,9 +160,9 @@ def make(kind, n, sr, framesize):
     if kind == "fs_white":
         return fs_white(n)
     if kind.startswith("clicks"):
-        return click_train(n, int(kind[6:]))
+        return click_train(n, int(kind[6:]), ratio=ratio)
     if kind == "click_pairs":
-        return click_pairs(n)
+        return click_pairs(n, ratio=ratio)
     if kind == "silent_right":
         return silent_right(n)
     if kind == "l_minus_r":
@@ -184,15 +194,46 @@ CASES = [
 ]
 
 
+# (kind, channels, input samplerate, kbps, output frames): configurations lamejs resamples by an integer ratio, all of them
+# MPEG-2 or MPEG-2.5 at the output and all with gfp.scale = 0.95 (scale_applied), spread over the ratios 2, 3, 4 and 6 and
+# mono / stereo.  After the filter these inputs are what Int16 input never is: full-scale squares, DC and click trains
+# overshoot +-32768, and +-1 LSB input becomes fractional samples.  nyquist puts all its energy where the filter removes
+# it, hf_tone above the output's Nyquist frequency.
+RESAMPLED_CASES = [
+    ("square", 2, 48000, 64, 40), ("square", 1, 48000, 8, 40),
+    ("dc_max", 1, 32000, 16, 30), ("dc_max", 2, 24000, 24, 30), ("dc_min", 1, 48000, 24, 30), ("dc_min", 2, 32000, 8, 30),
+    ("nyquist", 2, 24000, 16, 40), ("nyquist", 1, 48000, 40, 40),
+    ("hf_tone", 2, 48000, 64, 30), ("hf_tone", 1, 44100, 32, 40),
+    ("lsb_dither", 2, 48000, 56, 30), ("lsb_dither", 1, 16000, 8, 40), ("lsb_dither", 2, 32000, 16, 40),
+    ("lsb_clicks", 1, 48000, 40, 30), ("lsb_clicks", 2, 48000, 16, 40),
+    ("fs_white", 1, 48000, 8, 40), ("fs_white", 2, 24000, 8, 40),
+] + [("clicks%d" % s, 2, 48000, 64, 56) for s in range(1, 7)] + [("clicks%d" % s, 1, 48000, 16, 60) for s in (1, 2, 3, 5)] + [
+    ("click_pairs", 2, 44100, 48, 60), ("click_pairs", 1, 32000, 8, 80),
+    ("loud_silent", 2, 48000, 64, 60), ("loud_silent", 1, 24000, 8, 60),
+    ("silent_right", 2, 32000, 40, 40), ("silent_right", 2, 48000, 8, 40),
+    ("l_minus_r", 2, 16000, 24, 40), ("l_minus_r", 2, 48000, 32, 40),
+    ("clipped_sine", 2, 48000, 40, 40), ("clipped_sine", 1, 32000, 24, 40),
+]
+
+
 def case_id(c):
     kind, ch, sr, kbps, frames = c
     return "%s-%dch-%d-%dk" % (kind, ch, sr, kbps)
 
 
+def ratio(case):
+    """input samples per output sample of a case's configuration (1: lamejs encodes at the input rate)"""
+    _, ch, sr, kbps, _ = case
+    return sr // oracle_lib.out_samplerate(ch, sr, kbps)
+
+
 def signal(case):
-    """(left, right or None) of a case: `frames` frames of its configuration plus a ragged tail."""
+    """(left, right or None) of a case: `frames` frames of its configuration plus a ragged tail.  For a resampled case the
+    frames are output frames and the signal is r times as long (r = ratio(case)), its tail too."""
     kind, ch, sr, kbps, frames = case
-    framesize = 1152 if sr >= 32000 else 576
-    n = frames * framesize + 211
-    l, r = make(kind, n, sr, framesize)
-    return l, (r if ch == 2 else None)
+    r = ratio(case)
+    out_rate = sr // r
+    framesize = (1152 if out_rate >= 32000 else 576) * r
+    n = frames * framesize + 211 * r
+    l, rt = make(kind, n, sr, framesize, r)
+    return l, (rt if ch == 2 else None)

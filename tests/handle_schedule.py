@@ -9,6 +9,11 @@ Xing / Info tag.  The sizes of the calls are where the handle's bookkeeping turn
 once.  The signals (click trains, loud/silent alternation, bursts, ...) put call boundaries inside short-block runs and ATH
 decay.
 
+A configuration lamejs resamples by an integer ratio r (RESAMPLED_CONFIGS) runs on handles created with MP3B200_RESAMPLE.  Its
+calls are counted in input samples: the output granule / frame and first-frame edges times r, each +-1 and +-16 input
+samples (the filter's half-width: output m reads inputs up to r m + 16), and 1- and 2-sample calls that complete no output
+sample.  Its state blobs carry the 'M3R1' magic and the two rates in front of the halo.
+
 The expected bytes of every call come from one OracleEncoder per logical stream that replays that stream's calls in order,
 which is how include/mp3b200.h defines a batch call.  A call that fails for a too small buffer hands out nothing and keeps
 its frames: the stream's next call returns them in front of its own.  After every operation the runner also compares the
@@ -29,10 +34,34 @@ START, SHORT = 1, 2
 
 # the configurations of tests/test_gpu_handle_soak.py: MPEG-1 stereo / mono, MPEG-2 stereo, MPEG-2.5 mono
 CONFIGS = [(2, 44100, 128), (1, 48000, 320), (2, 22050, 64), (1, 8000, 16)]
+# and resampled ones: 48 -> 24 kHz stereo (r = 2, MPEG-2) and 48 -> 8 kHz mono (r = 6, MPEG-2.5)
+RESAMPLED_CONFIGS = [(2, 48000, 64), (1, 48000, 8)]
 
 SMALL_SIZES = [0, 1, 2, 575, 576, 577, 1151, 1152, 1153, 1328, 1329]
 EDGE_KINDS = ["clicks1", "clicks2", "clicks3", "clicks5", "click_pairs", "loud_silent", "square", "lsb_dither"]
 SYNTH_KINDS = ["burst", "noise", "sweep", "octave", "sine", "silence", "white"]
+RS_HALF = 16                # half-width of lamejs's resampling filter, in input samples
+RESAMPLE = 1                # MP3B200_RESAMPLE
+MAGIC_RESAMPLED = 0x3152334D    # 'M3R1'
+
+
+def ratio_of(cfg):
+    """input samples per output sample: 1 for a configuration lamejs encodes at its input rate"""
+    ch, sr, kbps = cfg
+    return sr // oracle_lib.out_samplerate(ch, sr, kbps)
+
+
+def small_sizes(cfg):
+    """the call sizes, in input samples, around which a handle's bookkeeping turns"""
+    r = ratio_of(cfg)
+    if r == 1:
+        return SMALL_SIZES
+    out_fs = framesize(cfg[1] // r)
+    # output edges: a granule, a frame, two frames, and the first frame (a fresh FIFO holds 528 samples; a frame is encoded
+    # once it holds framesize + 752)
+    edges = sorted({576, out_fs, 2 * out_fs, out_fs + 752 - 528, out_fs + 752})
+    return [0, 1, 2] + sorted({r * e + d for e in edges for d in (-RS_HALF, -1, 0, 1, RS_HALF, RS_HALF + 1)})
+
 
 # one entry of a call: logical stream s (None: a NULL handle), its samples [lo, hi) (encode only), and whether the call gets
 # a one-byte output buffer
@@ -46,7 +75,10 @@ def framesize(sr):
 class Schedule:
     def __init__(self, cfg, signals, kinds, tagged, ops):
         self.cfg, self.signals, self.kinds, self.tagged, self.ops = cfg, signals, kinds, tagged, ops
-        self.fs = framesize(cfg[1])
+        self.ratio = ratio_of(cfg)
+        self.resample = self.ratio > 1
+        self.G = 2 if cfg[1] // self.ratio >= 32000 else 1          # granules per frame at the output rate
+        self.fs = framesize(cfg[1] // self.ratio) * self.ratio       # a frame, in input samples
 
     @property
     def nstreams(self):
@@ -56,9 +88,11 @@ class Schedule:
 def make_schedule(cfg, nstreams, nops, seed, big=0.03, p_fail=0.06):
     """A seeded schedule of `nops` operations over `nstreams` logical streams, ended by a flush of every stream.  `big` is the
     share of calls that carry up to 200 frames at once; `p_fail` the share of calls on untagged streams given a one-byte
-    buffer."""
+    buffer.  Sizes are input samples; frames are output frames."""
     ch, sr, kbps = cfg
-    fs = framesize(sr)
+    r = ratio_of(cfg)
+    fs = framesize(sr // r) * r
+    smalls = small_sizes(cfg)
     rng = np.random.default_rng(seed)
     K = nstreams
     tagged = {s for s in range(K) if s % 8 == 5}
@@ -69,7 +103,7 @@ def make_schedule(cfg, nstreams, nops, seed, big=0.03, p_fail=0.06):
     def size():
         u = rng.random()
         if u < 0.5:
-            return int(rng.choice(SMALL_SIZES))
+            return int(rng.choice(smalls))
         if u < 1.0 - big:
             return fs * int(rng.integers(1, 17)) + int(rng.integers(-1, 2))
         return int(rng.integers(fs, 200 * fs + 1))
@@ -115,8 +149,8 @@ def make_schedule(cfg, nstreams, nops, seed, big=0.03, p_fail=0.06):
     for s in range(K):
         n = max(pos[s], 1)
         kind = (EDGE_KINDS + SYNTH_KINDS)[(s + seed) % (len(EDGE_KINDS) + len(SYNTH_KINDS))]
-        l, r = edge_signals.make(kind, n, sr, fs) if kind in EDGE_KINDS else make_signal(kind, n, sr, seed * 64 + s)
-        signals.append((np.ascontiguousarray(l), np.ascontiguousarray(r) if ch == 2 else None))
+        x, y = edge_signals.make(kind, n, sr, fs, r) if kind in EDGE_KINDS else make_signal(kind, n, sr, seed * 64 + s)
+        signals.append((np.ascontiguousarray(x), np.ascontiguousarray(y) if ch == 2 else None))
         kinds.append(kind)
     return Schedule(cfg, signals, kinds, tagged, ops)
 
@@ -132,7 +166,7 @@ class Expected:
 def replay(sched, trace=False):
     ch, sr, kbps = sched.cfg
     K = sched.nstreams
-    G = 2 if sr >= 32000 else 1
+    G = sched.G
     nflush = [0] * K
     for _, entries in sched.ops:
         for c in entries:
@@ -255,8 +289,9 @@ def blob_state_diff(blob, st, nch):
     """Names of the fields in which a handle's exported state blob differs from the oracle's state `st` (OracleEncoder.state())
     for the same stream after the same calls.  Floats are compared as bit patterns.  A handle whose last call failed still
     holds frames the oracle has encoded (frames_pending > 0): its fill level must agree, its sequential state is checked after
-    the call that delivers them."""
+    the call that delivers them.  A resampled handle's blob ('M3R1') has StateBlobRates (two int32) between header and halo."""
     h = np.frombuffer(bytes(blob[:BLOB_HEADER.itemsize]), dtype=BLOB_HEADER)[0]
+    halo_at = BLOB_HEADER.itemsize + (8 if h["magic"] == MAGIC_RESAMPLED else 0)
     bad = []
     if h["frames_done"] + h["frames_pending"] != st["frames_done"]:
         bad.append("frames_done")
@@ -274,7 +309,7 @@ def blob_state_diff(blob, st, nch):
     if h["frames_done"] > 0:
         if h["halo_floats"] != nch * 122:
             return bad + ["halo_floats"]
-        halo = np.frombuffer(bytes(blob[BLOB_HEADER.itemsize:BLOB_HEADER.itemsize + 4 * nch * 122]), dtype="<f4").reshape(nch, 122)
+        halo = np.frombuffer(bytes(blob[halo_at:halo_at + 4 * nch * 122]), dtype="<f4").reshape(nch, 122)
         want = np.concatenate([st["en_l"][:nch], st["thm_l"][:nch], st["en_s"][:nch].reshape(nch, 39),
                                st["thm_s"][:nch].reshape(nch, 39)], axis=1)
         if not np.array_equal(_bits(halo), _bits(want)):
@@ -319,7 +354,7 @@ def run(M, sched, ex):
 
     def create(s):
         h = vp()
-        assert L.mp3b200_create(ch, sr, kbps, ctypes.byref(h)) == 0
+        assert L.mp3b200_create_ex(ch, sr, kbps, RESAMPLE if sched.resample else 0, ctypes.byref(h)) == 0
         if s in sched.tagged:
             assert L.mp3b200_set_write_vbr_tag(h, 1) == int(ex.tags[s]["tag_on"])
         return h

@@ -17,16 +17,16 @@ import stage_taps  # noqa: E402
 from synth import make_signal, white  # noqa: E402
 
 
-def device_encode(M, torch, ch, sr, kbps, sigs):
+def device_encode(M, torch, ch, sr, kbps, sigs, resample=False):
     """encode_streams_device on a packed device copy of `sigs`: (list of bytes, quantizer passes)."""
     ns = [len(l) for l, _ in sigs]
     pcm = np.concatenate([np.concatenate([l, r]) if ch == 2 else l for l, r in sigs] + [np.zeros(8, np.int16)])
     pcm_off = np.cumsum([0] + [n * ch for n in ns])[:-1]
-    nb = [M.stream_bytes(ch, sr, kbps, n) for n in ns]
+    nb = [M.stream_bytes(ch, sr, kbps, n, resample) for n in ns]
     out_off = np.cumsum([0] + nb)[:-1]
     d_pcm = torch.from_numpy(pcm).cuda()
     d_out = torch.zeros(sum(nb) + 8, dtype=torch.uint8, device="cuda")
-    tm = M.encode_streams_device(ch, sr, kbps, d_pcm.data_ptr(), pcm_off, ns, d_out.data_ptr(), out_off)
+    tm = M.encode_streams_device(ch, sr, kbps, d_pcm.data_ptr(), pcm_off, ns, d_out.data_ptr(), out_off, resample=resample)
     out = d_out.cpu().numpy()
     return [out[o:o + b].tobytes() for o, b in zip(out_off, nb)], int(tm[7])
 
@@ -44,16 +44,16 @@ def main():
             if o != O.encode_stream(ch, sr, kbps, l, r if ch == 2 else None)[0]:
                 fail.append("%s stream %d (%d samples)" % (tag, i, len(l)))
 
-    def check_taps(tag, ch, sr, kbps, sigs):
+    def check_taps(tag, ch, sr, kbps, sigs, resample=False):
         """every stage tap of each stream, the quantizer's carried state included: where a stale speculated state would
         show although the bytes agree"""
-        G = M.granules_per_frame(ch, sr, kbps)
+        G = M.granules_per_frame(ch, sr, kbps, resample)
         for i, (l, r) in enumerate(sigs):
             r = r if ch == 2 else None
-            F = M.stream_frames(len(l), ch, sr, kbps)
+            F = M.stream_frames(len(l), ch, sr, kbps, resample)
             ref, _, tr = O.encode_stream(ch, sr, kbps, l, r, trace_frames=F + 2)
             try:
-                stage_taps.compare(M.debug_stages(ch, sr, kbps, l, r, want=stage_taps.ALL_TAPS), tr, ref, G, ch)
+                stage_taps.compare(M.debug_stages(ch, sr, kbps, l, r, want=stage_taps.ALL_TAPS, resample=resample), tr, ref, G, ch)
             except AssertionError as e:
                 fail.append("%s stream %d taps: %s" % (tag, i, str(e)[:300]))
 
@@ -70,6 +70,18 @@ def main():
         check(tag + " host", M.encode_streams(ch, sr, kbps, [s[0] for s in sigs], [s[1] for s in sigs] if ch == 2 else None),
               ch, sr, kbps, sigs)
         check_taps(tag, ch, sr, kbps, sigs)
+
+    # a resampled ragged batch (48 -> 24 kHz, MP3B200_RESAMPLE): lengths around the first output sample and the output frame
+    # edges, in input samples
+    ch, sr, kbps, r = 2, 48000, 64, 2
+    lens = [1, 17, r * 800 + 16, 5000, r * 576 * 31 + 5, r * 576 * 64, r * 576 * 150 + 3]
+    sigs = []
+    for i, n in enumerate(lens):
+        l, rt = white(n, 0x5EED0040 + i) if i % 3 == 0 else make_signal(("burst", "noise", "sweep")[i % 3], n, sr, 70 + i)
+        sigs.append((l, np.roll(rt, 7)))
+    got, passes["resampled"] = device_encode(M, torch, ch, sr, kbps, sigs, resample=True)
+    check("resampled", got, ch, sr, kbps, sigs)
+    check_taps("resampled", ch, sr, kbps, sigs, resample=True)
 
     # live handles fed 5000-sample calls: several frames per call, so the handle path speculates too
     for ch, sr, kbps in ((2, 44100, 128), (1, 24000, 48)):
@@ -106,6 +118,19 @@ def main():
         check("edge %d/%d/%d" % (ch, sr, kbps), got, ch, sr, kbps, sigs)
         check_taps("edge %d/%d/%d" % (ch, sr, kbps), ch, sr, kbps, sigs)
     passes["edge"] = edge_passes
+
+    # the resampled edge corpus, one batch per configuration
+    by_cfg = {}
+    for c in edge_signals.RESAMPLED_CASES:
+        by_cfg.setdefault(c[1:4], []).append(edge_signals.signal(c))
+    edge_passes = 0
+    for (ch, sr, kbps), sigs in by_cfg.items():
+        sigs = [(l, r if ch == 2 else l) for l, r in sigs]
+        got, p = device_encode(M, torch, ch, sr, kbps, sigs, resample=True)
+        edge_passes = max(edge_passes, p)
+        check("resampled edge %d/%d/%d" % (ch, sr, kbps), got, ch, sr, kbps, sigs)
+        check_taps("resampled edge %d/%d/%d" % (ch, sr, kbps), ch, sr, kbps, sigs, resample=True)
+    passes["resampled_edge"] = edge_passes
     print(json.dumps({"fail": fail, "passes": passes}))
 
 

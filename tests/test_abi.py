@@ -52,19 +52,20 @@ def test_stream_geometry_sweep_matches_oracle(M, oracle, samplerate, kbps):
 
 DEBUG_TAPS_FIELDS = ["size", "channels", "samplerate", "kbps", "left", "right", "nsamples", "force_blocktype", "xr", "blocktype",
                      "en_l", "thm_l", "en_s", "thm_s", "ath_adjust", "l3_enc", "ginfo", "bytes_out", "bytes_cap", "scalefac",
-                     "subblock_gain", "xmin", "max_nonzero_coeff", "xrpow_max", "scfsi", "old_value", "cur_step"]
+                     "subblock_gain", "xmin", "max_nonzero_coeff", "xrpow_max", "scfsi", "old_value", "cur_step", "flags"]
 
 
-def test_debug_taps_layout(M, tmp_path):
+def test_debug_taps_layout_with_flags(M, tmp_path):
     """mp3b200_debug_taps: the Python binding's ctypes struct has the C header's field order, offsets and size, and both are
-    pinned (16 bytes of int32 header, then 8-byte pointers / int64; 200 bytes on LP64)."""
+    pinned (16 bytes of int32 header, then 8-byte pointers / int64, then the int32 flags; 208 bytes on LP64)."""
     from lamejs_b200.encoder import DebugTaps
 
     assert [f[0] for f in DebugTaps._fields_] == DEBUG_TAPS_FIELDS
     want = {n: 4 * i for i, n in enumerate(DEBUG_TAPS_FIELDS[:4])}
     want.update({n: 16 + 8 * i for i, n in enumerate(DEBUG_TAPS_FIELDS[4:])})
+    assert want["flags"] == 200
     assert {n: getattr(DebugTaps, n).offset for n in DEBUG_TAPS_FIELDS} == want
-    assert ctypes.sizeof(DebugTaps) == 200
+    assert ctypes.sizeof(DebugTaps) == 208
     src = tmp_path / "layout.c"
     src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "mp3b200.h"\nint main(void) {\n' +
                    "".join('  printf("%%s %%zu\\n", "%s", offsetof(mp3b200_debug_taps, %s));\n' % (n, n) for n in DEBUG_TAPS_FIELDS) +
@@ -72,15 +73,33 @@ def test_debug_taps_layout(M, tmp_path):
     exe = tmp_path / "layout"
     subprocess.check_call(["cc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
     got = dict(line.split() for line in subprocess.check_output([str(exe)], text=True).splitlines())
-    assert {n: int(got[n]) for n in DEBUG_TAPS_FIELDS} == want and int(got["sizeof"]) == 200
+    assert {n: int(got[n]) for n in DEBUG_TAPS_FIELDS} == want and int(got["sizeof"]) == 208
 
 
 def test_debug_taps_size_is_checked(M):
-    """A struct of another size is refused before any device work (no GPU needed)."""
+    """A struct of another size is refused before any device work (no GPU needed); so is a caller built against the struct
+    before `flags` was added (200 bytes)."""
     from lamejs_b200.encoder import DebugTaps
 
-    t = DebugTaps(size=ctypes.sizeof(DebugTaps) - 8)
-    assert M.lib().mp3b200_debug_stages_ex(ctypes.byref(t)) == -3
+    for size in (ctypes.sizeof(DebugTaps) - 8, 200, 0):
+        t = DebugTaps(size=size)
+        assert M.lib().mp3b200_debug_stages_ex(ctypes.byref(t)) == -3, size
+
+
+def test_resampled_stream_geometry(M, oracle):
+    """mp3b200_stream_frames_ex / _granules_per_frame_ex, which size the stage taps of a resampled configuration: the frames
+    and granules of the output rate, counted from input samples, equal the oracle's; without the flag the configuration
+    stays rejected (-1), and a native configuration answers the same with and without it."""
+    for ch, sr, kb, gr in ((2, 48000, 64, 1), (1, 48000, 8, 1), (2, 44100, 48, 1), (1, 32000, 24, 1)):
+        assert M.granules_per_frame(ch, sr, kb) == -1 and M.stream_frames(5000, ch, sr, kb) == -1
+        assert M.granules_per_frame(ch, sr, kb, resample=True) == gr
+        r = sr // M.out_samplerate(ch, sr, kb)
+        for n in (0, 1, 16, 17, r * 576 + 16, r * (576 + 752 - 528) + 16, r * (576 + 752 - 528) + 17, 30011):
+            _, _, tr = oracle.encode_stream(ch, sr, kb, np.zeros(n, dtype=np.int16), None, trace_frames=64)
+            assert M.stream_frames(n, ch, sr, kb, resample=True) == len(tr), (ch, sr, kb, n)
+    for ch, sr, kb in ((2, 44100, 128), (1, 22050, 32)):
+        assert M.granules_per_frame(ch, sr, kb, resample=True) == M.granules_per_frame(ch, sr, kb)
+        assert M.stream_frames(12345, ch, sr, kb, resample=True) == M.stream_frames(12345, ch, sr, kb)
 
 
 def test_config_errors(M):

@@ -1,6 +1,8 @@
 """The product's per-configuration constant block (lamejs_b200/csrc/mp3_config.cpp -> Mp3Tables, what every kernel reads)
 against the oracle's lame_init_params / psymodel_init / iteration_init restatement, for every sample rate x bitrate x
-channel count: scalefactor bands, psy partitions, spreading rows, ATH, filter gains, windows -- bit for bit, on CPU.
+channel count: scalefactor bands, psy partitions, spreading rows, ATH, filter gains, windows, masking adjustment -- bit for bit,
+on CPU.  The product's tables are built with MP3B200_RESAMPLE, so the 29 configurations lamejs resamples by an integer ratio
+are compared with the oracle's output-rate tables too (their filter taps are pinned by tests/test_resample_cpu.py).
 (The oracle's tables are pinned to real lamejs through the byte fixtures of test_lamejs_pin.py.)"""
 import os
 import subprocess
@@ -17,3 +19,4 @@ def test_product_tables_equal_oracle_tables():
     p = subprocess.run([exe], capture_output=True, text=True)
     assert p.returncode == 0, p.stdout[-3000:]
     assert "342 configurations, 0 with mismatches" in p.stdout
+    assert "29 resampled configurations compared" in p.stdout, p.stdout[-3000:]

@@ -2,7 +2,8 @@
 call's bytes and byte count, and the tag of the tagged streams, equal what one lamejs encoder per stream would hand out for
 the same calls (the oracle); after every operation, the state each named handle carries into its next call (its exported
 blob's header and halo: ATH adjust, block-type state, OldValue / CurrentStep, frame count, FIFO fill, the masking handed to
-the next granule) equals that stream's OracleEncoder.state(), through hand-overs and flush-then-reuse.  The directed tests
+the next granule) equals that stream's OracleEncoder.state(), through hand-overs and flush-then-reuse; the same on resampled
+handles (MP3B200_RESAMPLE, 48 -> 24 and 48 -> 8 kHz).  The directed tests
 cover a handle listed twice in one batch call, a failed handle inside a batch,
 NULL handles, a handle of another configuration, state blobs of different chunkings, and blobs whose bookkeeping was
 tampered with."""
@@ -26,8 +27,9 @@ def M():
     return lamejs_b200
 
 
-@pytest.mark.parametrize("cfg,K,nops,seed", [(cfg, 32, 300, 100 + i) for i, cfg in enumerate(HS.CONFIGS)],
-                         ids=["%d-%d-%d" % c for c in HS.CONFIGS])
+@pytest.mark.parametrize("cfg,K,nops,seed", [(cfg, 32, 300, 100 + i) for i, cfg in enumerate(HS.CONFIGS)] +
+                         [(cfg, 32, 300, 200 + i) for i, cfg in enumerate(HS.RESAMPLED_CONFIGS)],
+                         ids=["%d-%d-%d" % c for c in HS.CONFIGS] + ["%d-%d-%d-rs" % c for c in HS.RESAMPLED_CONFIGS])
 def test_handle_soak(M, oracle, cfg, K, nops, seed):
     s = HS.make_schedule(cfg, K, nops, seed)           # the schedules tests/test_handle_schedule_cpu.py checks
     ex = HS.replay(s)

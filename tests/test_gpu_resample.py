@@ -1,5 +1,6 @@
-"""Integer-ratio resampling on the GPU (MP3B200_RESAMPLE): k_resample against the oracle's resampler, the bytes of every
-entry point against the oracle and real lamejs, the handle API on resampled handles, and that nothing else moved."""
+"""Integer-ratio resampling on the GPU (MP3B200_RESAMPLE): k_resample against the oracle's resampler, every stage tap behind
+it against the oracle's traces, the bytes of every entry point against the oracle and real lamejs, the handle API on
+resampled handles, and that nothing else moved."""
 import hashlib
 import json
 import os
@@ -89,6 +90,44 @@ def test_resampler_tap_equals_oracle(M, cfg):
     got = M.debug_resample(ch, sr, kb, l, r, ny=y.shape[1])
     assert got.shape == y.shape
     assert np.array_equal(got.view(np.uint32), y.view(np.uint32))
+
+
+@pytest.mark.parametrize("cfg", INT, ids=IDS)
+def test_stage_parity(M, oracle, cfg):
+    """Every stage tap after k_resample -- MDCT spectrum, block types, masking, ATH adjust, quantized lines, side info,
+    scalefactors, xmin, and the OldValue / CurrentStep chain -- bit-equal to the oracle's frame and quantizer traces, for two
+    signals of about 20 output frames plus a ragged tail (L != R)."""
+    import stage_taps
+
+    ch, sr, kb = cfg
+    r = sr // M.out_samplerate(ch, sr, kb)
+    G = M.granules_per_frame(ch, sr, kb, resample=True)
+    n = r * (20 * 576 * G + 211) + 5
+    for kind, seed in (("burst", 21), ("noise", 22)):
+        l, rt = stereo(kind, n, sr, seed)
+        rr = rt if ch == 2 else None
+        F = M.stream_frames(n, ch, sr, kb, resample=True)
+        ref, _, tr = oracle.encode_stream(ch, sr, kb, l, rr, trace_frames=F + 2)
+        assert len(tr) == F and F >= 20
+        g = M.debug_stages(ch, sr, kb, l, rr, want=stage_taps.ALL_TAPS, resample=True)
+        stage_taps.compare(g, tr, ref, G, ch, "%s %d/%d/%d" % (kind, ch, sr, kb))
+
+
+def test_stage_taps_flag_on_native_configurations(M):
+    """debug_stages(..., resample=True) on configurations that encode at their input rate returns the unflagged taps; without
+    the flag a resampled configuration is refused."""
+    import stage_taps
+
+    l, r = stereo("burst", 9 * 1152 + 300, 44100, 31)
+    for ch, sr, kb in ((2, 44100, 128), (1, 22050, 32), (2, 8000, 16)):
+        rr = r if ch == 2 else None
+        plain = M.debug_stages(ch, sr, kb, l, rr, want=stage_taps.ALL_TAPS)
+        flagged = M.debug_stages(ch, sr, kb, l, rr, want=stage_taps.ALL_TAPS, resample=True)
+        assert plain.keys() == flagged.keys()
+        for k in plain:
+            assert plain[k].shape == flagged[k].shape and plain[k].tobytes() == flagged[k].tobytes(), (ch, sr, kb, k)
+    with pytest.raises(M.Mp3B200Error):
+        M.debug_stages(2, 48000, 64, l, r, want=("xr",))
 
 
 @pytest.mark.parametrize("cfg", INT, ids=IDS)

@@ -3,8 +3,9 @@ speed, never the bytes.  The library is rebuilt with deliberately bad guesses --
 step (Q_SPEC_START, Q_SPEC_STEP), the start step handed to gr1 (Q_SPEC_GR1_STEP), the in-state of the block-type / ATH scan
 chunks (SCAN_GUESS_LA, SCAN_GUESS_BT, SCAN_GUESS_ATH) -- and with the re-validation folded into the first pass switched off
 (Q_SPEC_FOLD=0), so that every wrong guess is repaired by the fixed-point loop.  Each variant encodes ragged MPEG-1 and LSF
-batches, live handles fed 5000-sample calls, one MPEG-1 and one LSF handle call schedule (tests/handle_schedule.py) with many
-calls of up to 200 frames, and the edge corpus, all byte-equal to the oracle (tests/speculation_worker.py,
+batches, a ragged batch resampled from 48 to 24 kHz, live handles fed 5000-sample calls, one MPEG-1 and one LSF handle call
+schedule (tests/handle_schedule.py) with many calls of up to 200 frames, and the edge corpus, native and resampled, all
+byte-equal to the oracle (tests/speculation_worker.py,
 one subprocess per library because the library is loaded once per process).  The streams of the ragged batches and the
 edge corpus also go through every stage tap, and the schedules compare each handle's state blob after every call: a
 repaired frame that kept a state from its speculated start would show there even where the bytes agree."""

@@ -2,14 +2,15 @@
 split every stream into calls without losing or repeating a sample, the expected results hand out every byte exactly once,
 and the schedules reach the call patterns they exist for -- calls that complete 0, 1 and 16 or more frames, call boundaries
 right after a START and after a SHORT granule, flush then reuse, hand-overs, repeated handles, NULL handles and failed calls.
-A schedule that silently stopped reaching them would leave the GPU soak green for the wrong reason."""
+The resampled schedules (48 -> 24 and 48 -> 8 kHz) must reach the same minimum counts.  A schedule that silently stopped
+reaching them would leave the GPU soak green for the wrong reason."""
 import pytest
 
 import handle_schedule as HS
 import oracle_lib
 
-# seeds and sizes of the GPU soak; the totals below are asserted over all four configurations
-SOAK = [(cfg, 32, 300, 100 + i) for i, cfg in enumerate(HS.CONFIGS)]
+# seeds and sizes of the GPU soak; the totals below are asserted over all of its configurations, native and resampled
+SOAK = [(cfg, 32, 300, 100 + i) for i, cfg in enumerate(HS.CONFIGS)] + [(cfg, 32, 300, 200 + i) for i, cfg in enumerate(HS.RESAMPLED_CONFIGS)]
 
 MIN_PER_CONFIG = {"calls_0_frames": 50, "calls_1_frame": 50, "calls_16plus_frames": 20, "after_start": 10, "after_short": 20,
                   "handovers": 10, "repeated_batches": 20, "null_entries": 5, "injected_failures": 10, "flush_then_reuse": 20}
@@ -59,7 +60,8 @@ def test_schedules_reach_what_they_exist_for(soaks):
         print(s.cfg, r)
         for k, v in MIN_PER_CONFIG.items():
             assert r[k] >= v, (s.cfg, k, r[k])
-        assert any(t["tag_on"] for t in ex.tags) or s.cfg == (1, 8000, 16), s.cfg   # 16 kbps at 8 kHz: the tag does not fit
+        # 16 kbps at 8 kHz, and 8 kbps resampled to 8 kHz: the tag does not fit
+        assert any(t["tag_on"] for t in ex.tags) or s.cfg in ((1, 8000, 16), (1, 48000, 8)), s.cfg
         for k, v in r.items():
             total[k] = total.get(k, 0) + v
     print("all configurations:", total)

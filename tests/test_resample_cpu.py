@@ -134,3 +134,63 @@ def test_stream_bytes_sweep_matches_oracle(M, cfg):
     for n in _sweep_lengths(r, 1 if SWEEP_FULL[r] == cfg else 37):
         data, _, _ = O.encode_stream(ch, sr, kb, np.zeros(n, dtype=np.int16), None)
         assert M.stream_bytes(ch, sr, kb, n, resample=True) == len(data), n
+
+
+@pytest.fixture(scope="module")
+def resampled_corpus():
+    """per case of edge_signals.RESAMPLED_CASES: (what the oracle's resampler wrote, gfp.scale, the oracle's frame trace)"""
+    import edge_signals as E
+
+    out = []
+    for c in E.RESAMPLED_CASES:
+        kind, ch, sr, kb, frames = c
+        l, r = E.signal(c)
+        y, _, scale, data = T.record(ch, sr, kb, l, r)
+        ref, _, tr = O.encode_stream(ch, sr, kb, l, r, trace_frames=frames + 8)
+        assert ref == data
+        out.append((c, y, scale, tr))
+    return out
+
+
+def test_resampled_edge_corpus_spread():
+    """The resampled edge cases are integer-ratio configurations over the ratios 2, 3, 4 and 6, mono and stereo, MPEG-2 and
+    MPEG-2.5 output; they are sized in output frames times the ratio; the native corpus stays native."""
+    import edge_signals as E
+
+    assert all(E.ratio(c) == 1 for c in E.CASES)
+    assert all(c[1:4] in INT for c in E.RESAMPLED_CASES)
+    assert {E.ratio(c) for c in E.RESAMPLED_CASES} == {2, 3, 4, 6}
+    assert {c[1] for c in E.RESAMPLED_CASES} == {1, 2}
+    outs = {O.out_samplerate(*c[1:4]) for c in E.RESAMPLED_CASES}
+    assert 8000 in outs and outs & {16000, 22050, 24000}
+    for c in E.RESAMPLED_CASES:
+        r = E.ratio(c)
+        assert len(E.signal(c)[0]) == r * (576 * c[4] + 211), c
+
+
+def test_resampled_edge_corpus_reaches_what_int16_never_is(resampled_corpus):
+    """What the resampler makes of the corpus: the filter's overshoot takes squares, DC, clicks and clipped sines past the
+    Int16 range on many cases (beyond 43,000 for the click trains); +-1 LSB input becomes fractional samples (the shares
+    measured when the corpus was made: about 91 % for dither, 10 % for sparse clicks, with no sample above 1.5); the
+    input-rate Nyquist tone and the tone above the output's Nyquist frequency are mostly filtered out; and over the list
+    the encoder takes all four block types.  Keeps the corpus from silently going tame."""
+    over, peak_all, blocktypes = [], 0.0, set()
+    for c, y, scale, tr in resampled_corpus:
+        kind, ch = c[0], c[1]
+        peak = float(np.abs(y).max())
+        peak_all = max(peak_all, peak)
+        frac = float(np.mean(y != np.round(y)))
+        assert scale == np.float64(0.95), c                          # every integer-ratio preset scales its input
+        if peak > 32768:
+            over.append(c)
+        if kind == "lsb_dither":
+            assert frac >= 0.90 and peak <= 1.5, (c, frac, peak)
+        if kind == "lsb_clicks":
+            assert frac >= 0.09 and peak <= 1.5, (c, frac, peak)
+        if kind in ("nyquist", "hf_tone"):
+            assert peak < 9000, (c, peak)                              # measured: 2,466 .. 7,783 of 32,767 in
+        blocktypes |= set(np.unique(tr["blocktype"][:, :1, :ch]).tolist())
+    assert len(over) >= 15, over
+    assert {c[0] for c in over} >= {"square", "dc_max", "dc_min", "clicks1", "click_pairs", "clipped_sine"}
+    assert peak_all >= 43000, peak_all
+    assert blocktypes == {0, 1, 2, 3}, blocktypes
