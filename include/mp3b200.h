@@ -183,6 +183,48 @@ int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int ns
                                   const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
                                   const int64_t* cap, int64_t* out_bytes);
 
+/* ---- ReplayGain (lamejs gfp.findReplayGain, GainAnalysis.js; LAME writes it by default) --------------------------------
+ * With MP3B200_REPLAYGAIN, mp3b200_encode_streams_tagged_ex also runs lamejs's ReplayGain analysis on every stream, on the
+ * GPU beside the encoder (lamejs_b200/csrc/k_replaygain.cuh), and fills the tag's Radio Replay Gain field as lamejs does
+ * with findReplayGain on and decode_on_the_fly off: the analysis sees what lamejs puts into mfbuf (the scaled input, or the
+ * resampler's output), in the pieces lamejs analyses it in, flush zeros included, and every sum and histogram bin equals
+ * lamejs's.  title_db[s] (optional) receives GetTitleGain of stream s in dB, album_db (optional) GetAlbumGain over the batch
+ * (analyzeResult of the summed histograms); -24601 (GAIN_NOT_ENOUGH_SAMPLES) when a stream holds less than one RMS window
+ * (the tag then carries -51.0 dB, the clamp) or when the tag does not fit the frame (lamejs analyses only with the tag on;
+ * the streams are then written without either).  The peak amplitude field stays 0: lamejs finds it only by decoding.
+ * Flags MP3B200_RESAMPLE and MP3B200_REPLAYGAIN may be combined; flags = 0 is mp3b200_encode_streams_tagged.  A batch with
+ * MP3B200_REPLAYGAIN holds at most 65535 streams.
+ * Streaming handles:
+ *   set_find_replay_gain  gfp.findReplayGain, before the first sample and after mp3b200_set_write_vbr_tag (which switches it
+ *                         off again).  Returns 1 (on), 0 (off: asked to, or the tag is off: lamejs analyses only with the tag
+ *                         on, Lame.js:911-916), negative on error.  Every sample a call feeds, flush zeros included, is analysed
+ *                         in the pieces lamejs analyses it in; each flush ends a title (GetTitleGain in flush_bitstream) and a
+ *                         handle that goes on after a flush starts a new one.  The tag frame carries the last title's gain.
+ *   get_replay_gain       after a flush: 1 and the last title's gain in dB (-24601: less than one RMS window) and gfc.RadioGain;
+ *                         0 before the first flush or with the analysis off.
+ *   album_gain            GetAlbumGain over the titles the handles ended (analyzeResult of their summed B histograms).
+ * mp3b200_export_state, mp3b200_import_state and mp3b200_seek return -2 on a handle that analyses ReplayGain: a state blob
+ * does not carry the analysis. */
+#define MP3B200_REPLAYGAIN 2
+int mp3b200_encode_streams_tagged_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
+                                     const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
+                                     const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db);
+/* mp3b200_lametag_build with flags (MP3B200_RESAMPLE) and the Radio Replay Gain field of an analysed stream: radio_gain is
+ * gfc.RadioGain = floor(title_db * 10 + 0.5), clamped to +-51.0 dB like lamejs; for segment callers that analyse the whole
+ * stream themselves (ReplayGain is not combined across segments). */
+int mp3b200_set_find_replay_gain(mp3b200_encoder* h, int on);
+int mp3b200_get_replay_gain(mp3b200_encoder* h, double* title_db, int* radio_gain);
+int mp3b200_album_gain(mp3b200_encoder* const* handles, int n, double* album_db);
+int mp3b200_lametag_build_ex(int channels, int samplerate, int kbps, int flags, int64_t nframes, int64_t music_bytes, int music_crc,
+                             int encoder_padding, int radio_gain, uint8_t* buf, int cap);
+/* Test tap: one whole stream through mp3b200_encode_streams_tagged_ex with MP3B200_REPLAYGAIN (flags: MP3B200_RESAMPLE).
+ * win_sums [w][2] = lsum, rsum of RMS window w (bit-exact), win_idx[w] its histogram index, for w < nwin_cap; hist (12000
+ * bins), title_db; stats[0] windows, [1] repair passes, [2] chunks run again, [3] the analysis time in ms (a float's bits).
+ * Any output pointer may be NULL. */
+int mp3b200_debug_replaygain(int channels, int samplerate, int kbps, int flags, const int16_t* left, const int16_t* right,
+                             int64_t nsamples, double* win_sums, int32_t* win_idx, int64_t nwin_cap, int32_t* hist,
+                             double* title_db, int32_t* stats);
+
 /* The rest of VBRTag.js's surface:
  *   put_vbr_tag     putVbrTag (VBRTag.js:937-965) on a stream held in memory: writes the finished frame over the placeholder,
  *                   behind an ID3v2 tag if the stream starts with one (skipId3v2; the port's inverted test is not reproduced).

@@ -26,6 +26,9 @@ const lib = ffi.Library(process.env.MP3B200_LIB || 'libmp3b200', {
   mp3b200_seek: ['int', [voidPtr, 'int64', 'pointer', 'pointer', 'int']],
   mp3b200_set_write_vbr_tag: ['int', [voidPtr, 'int']],
   mp3b200_get_lametag_frame: ['int', [voidPtr, 'pointer', 'int']],
+  mp3b200_set_find_replay_gain: ['int', [voidPtr, 'int']],
+  mp3b200_get_replay_gain: ['int', [voidPtr, 'pointer', 'pointer']],
+  mp3b200_album_gain: ['int', ['pointer', 'int', 'pointer']],
   mp3b200_lametag_size: ['int', ['int', 'int', 'int']],
   mp3b200_wav_read_header: ['int', ['pointer', 'int64', 'pointer']],
   mp3b200_last_error: ['string', []],
@@ -51,7 +54,13 @@ function Mp3Encoder(channels, samplerate, kbps, options) {
     const on = lib.mp3b200_set_write_vbr_tag(h, 1);          // 0: the frame is too small for the tag (InitVbrTag refuses)
     if (on < 0) throw new Error('mp3b200_set_write_vbr_tag failed (' + on + '): ' + lib.mp3b200_last_error());
     if (on === 1) tagRoom = lib.mp3b200_lametag_size(channels, samplerate, kbps);
+    // options.findReplayGain: gfp.findReplayGain (needs the tag): each flush() ends a title; replayGain() reads it
+    if (options.findReplayGain) {
+      const rg = lib.mp3b200_set_find_replay_gain(h, 1);
+      if (rg < 0) throw new Error('mp3b200_set_find_replay_gain failed (' + rg + '): ' + lib.mp3b200_last_error());
+    }
   }
+  this._handle = h;
   let maxSamples = 1152;
   let buf = Buffer.alloc((0 | (1.25 * maxSamples + 7200)) + tagRoom);   // index.js:113-114
 
@@ -101,6 +110,13 @@ function Mp3Encoder(channels, samplerate, kbps, options) {
     if (rc !== 0) throw new Error('mp3b200_seek failed (' + rc + '): ' + lib.mp3b200_last_error());
   };
 
+  /** {titleDb, radioGain} of the title the last flush() ended, or null (before it, or without options.findReplayGain) */
+  this.replayGain = function () {
+    const db = ref.alloc('double'), radio = ref.alloc('int');
+    const rc = lib.mp3b200_get_replay_gain(h, db, radio);
+    if (rc < 0) throw new Error('mp3b200_get_replay_gain failed (' + rc + '): ' + lib.mp3b200_last_error());
+    return rc === 1 ? { titleDb: db.deref(), radioGain: radio.deref() } : null;
+  };
   this.close = function () { lib.mp3b200_destroy(h); };
 }
 
@@ -119,6 +135,16 @@ WavHeader.readHeader = function (dataView) {
   w.dataOffset = Number(out.readBigInt64LE(0)); w.dataLen = Number(out.readBigInt64LE(8));
   w.channels = out.readInt32LE(16); w.sampleRate = out.readUInt32LE(20);
   return w;
+};
+
+/** GetAlbumGain over the titles the encoders (options.findReplayGain) have ended with flush() */
+Mp3Encoder.albumGain = function (encoders) {
+  const hs = Buffer.alloc(8 * Math.max(encoders.length, 1));
+  encoders.forEach((e, i) => ref.writePointer(hs, i * 8, e._handle));
+  const out = ref.alloc('double');
+  const rc = lib.mp3b200_album_gain(hs, encoders.length, out);
+  if (rc < 0) throw new Error('mp3b200_album_gain failed (' + rc + '): ' + lib.mp3b200_last_error());
+  return out.deref();
 };
 
 module.exports = { Mp3Encoder, WavHeader };

@@ -26,6 +26,7 @@
 #include "k_quant.cuh"
 #include "k_tag.cuh"
 #include "k_resample.cuh"
+#include "k_replaygain.cuh"
 #include "mp3_tag.h"
 
 namespace {
@@ -74,6 +75,8 @@ int ensure_device(int dev) {
     CK(cudaMemcpyToSymbol(c_enwindow, MP3_ENWINDOW, sizeof(double) * 285));
     CK(cudaMemcpyToSymbol(c_mdct_win, MP3_MDCT_WIN, sizeof(double) * 144));
     CK(cudaMemcpyToSymbol(c_sb_order, MP3_SB_ORDER, sizeof(int) * 32));
+    CK(cudaMemcpyToSymbol(c_rg_yule, RG_YULE, sizeof RG_YULE));
+    CK(cudaMemcpyToSymbol(c_rg_butter, RG_BUTTER, sizeof RG_BUTTER));
     int rc = psy_upload_constants();
     if (rc) return rc;
     rc = quant_upload_constants();
@@ -120,6 +123,8 @@ struct LameFifo {
   long long framesize, mf_size = 576 - 48, mf_samples_to_encode = ENC_POST_DELAY;
   int ratio = 1;
   long long in_fed = 0;                   /* input samples fed so far (resampling only) */
+  std::vector<long long>* pieces = nullptr;   /* when set: the sizes of the pieces AnalyzeSamples sees (ReplayGain), the
+                                                 n_out of every fill_buffer step: up to framesize outputs each */
   explicit LameFifo(int mode_gr, int r = 1) : framesize(576LL * mode_gr), ratio(r) {}
   long long outputs(long long p) const {
     if (ratio == 1) return p;
@@ -131,6 +136,8 @@ struct LameFifo {
     if (n <= 0) return 0;
     const long long k = outputs(in_fed + n) - outputs(in_fed);
     in_fed += n;
+    if (pieces)
+      for (long long i = 0; i < k; i += framesize) pieces->push_back(k - i < framesize ? k - i : framesize);
     const long long need = framesize + 752;
     const long long frames = mf_size + k >= need ? (mf_size + k - need) / framesize + 1 : 0;
     if (mf_samples_to_encode < 1) mf_samples_to_encode = ENC_POST_DELAY;
@@ -258,10 +265,23 @@ struct ThreadCtx {
   Buf<uint8_t, true> pin;                 /* pinned host staging */
   Buf<long long> crc_ranges;              /* music CRC: [2][R] offsets / lengths */
   Buf<unsigned> crc;                      /* music CRC: [R] results */
+  cudaStream_t rg_st = nullptr;           /* ReplayGain analysis, beside the encoder */
+  cudaEvent_t ev_rg[3] = {};              /* fork, start, end */
+  Buf<RgTitle> rg_titles;
+  Buf<long long> rg_piece;
+  Buf<double> rg_sum, rg_gain;
+  Buf<RgState> rg_wstate, rg_cstart;
+  Buf<RgEnd> rg_end_a, rg_end_b;
+  Buf<RgCarry> rg_carry;
+  Buf<int> rg_idx, rg_hist, rg_count;
   void release() {
     if (device < 0) return;
     cudaSetDevice(device);
     ws.release(); pcm.release(); out.release(); pin.release(); crc_ranges.release(); crc.release();
+    rg_titles.release(); rg_piece.release(); rg_sum.release(); rg_gain.release(); rg_wstate.release(); rg_cstart.release();
+    rg_end_a.release(); rg_end_b.release(); rg_carry.release(); rg_idx.release(); rg_hist.release(); rg_count.release();
+    for (auto& e : ev_rg) if (e) { cudaEventDestroy(e); e = nullptr; }
+    if (rg_st) { cudaStreamDestroy(rg_st); rg_st = nullptr; }
     for (auto& e : ev) if (e) { cudaEventDestroy(e); e = nullptr; }
     for (auto& e : evq) if (e) { cudaEventDestroy(e); e = nullptr; }
     for (auto& e : ready) if (e) { cudaEventDestroy(e); e = nullptr; }
@@ -281,6 +301,8 @@ struct ThreadCtx {
     release();
     CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&up_st, cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(&rg_st, cudaStreamNonBlocking));
+    for (auto& e : ev_rg) CK(cudaEventCreate(&e));
     for (auto& e : ev) CK(cudaEventCreate(&e));
     for (auto& e : evq) CK(cudaEventCreate(&e));
     for (auto& e : ready) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -326,6 +348,7 @@ struct LaunchOpts {
   bool sync = true;                      /* false: return with the work queued on t_ctx.st (no timings) */
   StreamDesc* committed = nullptr;       /* host: each stream's descriptor as the pipeline left it (the carried state),
                                             valid once t_ctx.st has drained */
+  struct RgJob* rg = nullptr;            /* ReplayGain of every stream, beside the encoder (one launch group only) */
 };
 
 /* One pipeline launch for the streams sds[0 .. S) (at most MP3_MAX_LAUNCH_STREAMS, unit / frame bases set, the workspace
@@ -546,6 +569,191 @@ int resample_streams(Config* cfg, StreamDesc* sds, int S) {
   return 0;
 }
 
+/* ---- ReplayGain (lamejs findReplayGain; k_replaygain.cuh) ----
+ * A launch analyses, for each stream listed in the job, the samples [g0, g0 + sum(pieces)) of its current title (which
+ * started at t0), reading the PCM its descriptor points at once the launch has resampled it (stream sample indices: Int16 as
+ * mfbuf holds it, or the resampler's Float32 rows); `pieces` are the AnalyzeSamples calls lamejs makes for them. */
+struct RgSpec {
+  int stream = 0;                                /* index in the launch */
+  std::vector<long long> pieces;                 /* piece sizes (LameFifo::pieces) */
+  long long t0 = 0, g0 = 0;
+  RgCarry* carry = nullptr;                      /* device; NULL: a fresh title in launch workspace */
+  int* hist = nullptr;                           /* device A; NULL: launch workspace */
+  int* hist_b = nullptr;                         /* device B of a handle (GetTitleGain moves A into it); NULL: none */
+  int title_end = 1;
+};
+struct RgJob {
+  std::vector<RgSpec> specs;
+  /* results */
+  std::vector<double> title_db;                  /* per spec (RG_NOT_ENOUGH_SAMPLES where the title does not end) */
+  double album_db = 0;                           /* analyzeResult of the specs' summed A */
+  int passes = 0, reruns = 0;
+  float ms = 0;                                  /* CUDA-event time of the analysis on its stream */
+  /* debug: spec 0's windows */
+  bool want_windows = false;
+  std::vector<double> win_sum;                   /* [windows][2] */
+  std::vector<int> win_idx;
+  std::vector<int> hist0;
+  /* filled by rg_queue */
+  long long chunk_rows = 0;
+  int max_chunks = 0, max_win = 0, nwin0 = 0;
+  RgParams prm;
+};
+
+int rg_req_index(int sr) {
+  static const int rates[9] = {48000, 44100, 32000, 24000, 22050, 16000, 12000, 11025, 8000};
+  for (int i = 0; i < 9; i++) if (rates[i] == sr) return i;
+  return -1;
+}
+
+/* queues pass 1 and the first RG_QUEUED_PASSES repair passes on t_ctx.rg_st, after the PCM (the upload slices in `arrival`,
+ * or everything queued on t_ctx.st so far: uploads and the resampler) */
+int rg_queue(Config* cfg, const StreamDesc* sds, RgJob& job, const PcmArrival* arrival) {
+  ThreadCtx& c = t_ctx;
+  const int sr = cfg->host.samplerate, W = (sr + 19) / 20, nch = cfg->host.nch, req = rg_req_index(sr);
+  if (req < 0) { g_err = "no ReplayGain filter for this rate"; return MP3B200_ERR_CONFIG; }
+  const int T = (int)job.specs.size();
+  std::vector<RgTitle> t((size_t)T);
+  long long npiece = 0, nwin = 0, nchunk = 0;
+  for (const RgSpec& sp : job.specs) npiece += (long long)sp.pieces.size();
+  int rc = 0;
+  if ((rc = c.rg_piece.fit((size_t)npiece + 1)) || (rc = c.rg_carry.fit((size_t)T + 1)) || (rc = c.rg_hist.fit((size_t)(T + 1) * RG_HIST)))
+    return rc;
+  std::vector<long long> starts((size_t)npiece + 1);
+  long long po = 0;
+  job.max_chunks = job.max_win = 0;
+  for (int i = 0; i < T; i++) {
+    const RgSpec& sp = job.specs[i];
+    const StreamDesc& sd = sds[sp.stream];
+    RgTitle& ti = t[i];
+    ti.x[0] = sd.pcm[0]; ti.x[1] = sd.pcm[1];
+    ti.x_base = sd.pcm_base; ti.x_end = sd.pcm_end;
+    long long at = sp.g0;
+    ti.piece = c.rg_piece.p + po;
+    for (long long k : sp.pieces) { starts[po++] = at; at += k; }
+    ti.npieces = (int)sp.pieces.size();
+    ti.t0 = sp.t0; ti.g0 = sp.g0; ti.g1 = at;
+    ti.wa = (int)((sp.g0 - sp.t0) / W);
+    ti.nwin = (int)((at - sp.t0) / W) - ti.wa;
+    const int pseudo = ti.nwin + (at > sp.t0 + (long long)(ti.wa + ti.nwin) * W ? 1 : 0);   /* + the partial window at g1 */
+    ti.win0 = (int)nwin;
+    ti.nchunks = (pseudo + RG_CHUNK_WINDOWS - 1) / RG_CHUNK_WINDOWS;
+    ti.chunk0 = (int)nchunk;
+    ti.carry = sp.carry ? sp.carry : c.rg_carry.p + i;
+    ti.hist = sp.hist ? sp.hist : c.rg_hist.p + (size_t)i * RG_HIST;
+    ti.hist_b = sp.hist_b;
+    ti.title_end = sp.title_end;
+    nwin += ti.nwin; nchunk += ti.nchunks;
+    job.max_chunks = ti.nchunks > job.max_chunks ? ti.nchunks : job.max_chunks;
+    job.max_win = ti.nwin > job.max_win ? ti.nwin : job.max_win;
+  }
+  job.nwin0 = T > 0 ? t[0].nwin : 0;
+  job.chunk_rows = nchunk * nch;
+  const int max_passes = job.max_chunks + RG_QUEUED_PASSES + 2;
+  if ((rc = c.rg_titles.fit((size_t)T + 1)) || (rc = c.rg_sum.fit((size_t)nwin * 2 + 2)) || (rc = c.rg_wstate.fit((size_t)nwin * nch + 1)) ||
+      (rc = c.rg_cstart.fit((size_t)job.chunk_rows + 1)) || (rc = c.rg_end_a.fit((size_t)job.chunk_rows + 1)) ||
+      (rc = c.rg_end_b.fit((size_t)job.chunk_rows + 1)) || (rc = c.rg_idx.fit((size_t)nwin + 1)) ||
+      (rc = c.rg_count.fit((size_t)max_passes + 2)) || (rc = c.rg_gain.fit((size_t)T + 1)))
+    return rc;
+  cudaStream_t st = c.rg_st;
+  if (arrival) for (int j = 0; j < arrival->chunks; j++) CK(cudaStreamWaitEvent(st, arrival->ready[j], 0));
+  CK(cudaEventRecord(c.ev_rg[0], c.st));
+  CK(cudaStreamWaitEvent(st, c.ev_rg[0], 0));
+  CK(cudaEventRecord(c.ev_rg[1], st));
+  CK(cudaMemcpyAsync(c.rg_piece.p, starts.data(), sizeof(long long) * (size_t)(npiece + 1), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(c.rg_titles.p, t.data(), sizeof(RgTitle) * (size_t)T, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(c.rg_count.p, 0, sizeof(int) * (size_t)(max_passes + 2), st));
+  CK(cudaMemsetAsync(c.rg_hist.p, 0, sizeof(int) * (size_t)(T + 1) * RG_HIST, st));
+  CK(cudaMemsetAsync(c.rg_carry.p, 0, sizeof(RgCarry) * (size_t)(T + 1), st));
+  RgParams& p = job.prm;
+  p.titles = c.rg_titles.p; p.nch = nch; p.W = W; p.req = req; p.f32 = cfg->rs.ratio > 1;
+  p.scale_applied = cfg->rs.ratio > 1 ? 0 : cfg->host.scale_applied;   /* k_resample already scaled its input */
+  p.scale = cfg->host.scale;
+  p.win_sum = c.rg_sum.p; p.win_state = c.rg_wstate.p; p.chunk_start = c.rg_cstart.p; p.end_in = c.rg_end_a.p; p.end_out = c.rg_end_b.p;
+  p.done = c.rg_count.p; p.reruns = c.rg_count.p + 1; p.pass_changed = c.rg_count.p + 2;
+  job.passes = 0;
+  if (job.max_chunks > 0) {
+    dim3 grid((unsigned)((job.max_chunks * nch + RG_THREADS - 1) / RG_THREADS), (unsigned)T);
+    k_rg_pass1<<<grid, RG_THREADS, 0, st>>>(p);
+    g_launches++;
+    for (int q = 0; q < RG_QUEUED_PASSES; q++) {
+      k_rg_repair<<<grid, RG_THREADS, 0, st>>>(p, job.passes);
+      k_rg_check<<<(unsigned)((job.chunk_rows + 255) / 256), 256, 0, st>>>(p, job.passes, job.chunk_rows);
+      job.passes++;
+      g_launches += 2;
+    }
+  }
+  CK(cudaGetLastError());
+  return 0;
+}
+
+/* after the encoder has been queued: runs repair passes until one changes nothing, then the histograms, the gains of the
+ * titles that end and the carries; reads the results.  Returns with t_ctx.rg_st drained. */
+int rg_finish(Config* cfg, RgJob& job) {
+  ThreadCtx& c = t_ctx;
+  cudaStream_t st = c.rg_st;
+  RgParams& p = job.prm;
+  const int nch = cfg->host.nch, T = (int)job.specs.size();
+  if (job.max_chunks > 0) {
+    dim3 grid((unsigned)((job.max_chunks * nch + RG_THREADS - 1) / RG_THREADS), (unsigned)T);
+    for (;;) {
+      int done = 0;
+      CK(cudaMemcpyAsync(&done, p.done, sizeof(int), cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      if (done) break;
+      if (job.passes >= job.max_chunks + RG_QUEUED_PASSES + 1) { g_err = "ReplayGain repair did not converge"; return MP3B200_ERR_CUDA; }
+      k_rg_repair<<<grid, RG_THREADS, 0, st>>>(p, job.passes);
+      k_rg_check<<<(unsigned)((job.chunk_rows + 255) / 256), 256, 0, st>>>(p, job.passes, job.chunk_rows);
+      job.passes++;
+      g_launches += 2;
+    }
+    CK(cudaMemcpyAsync(&job.reruns, p.reruns, sizeof(int), cudaMemcpyDeviceToHost, st));
+    /* the pass that found nothing to change: the first with pass_changed == 0 (later queued ones returned at once) */
+    std::vector<int> pc((size_t)job.passes);
+    CK(cudaMemcpyAsync(pc.data(), p.pass_changed, sizeof(int) * (size_t)job.passes, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    int used = 0;
+    while (used < job.passes && pc[used] != 0) used++;
+    job.passes = used + 1;
+  }
+  if (job.max_win > 0) {
+    k_rg_hist<<<dim3((unsigned)((job.max_win + 255) / 256), (unsigned)T), 256, 0, st>>>(p.titles, p.W, p.win_sum, c.rg_idx.p);
+    g_launches++;
+  }
+  int* album = c.rg_hist.p + (size_t)T * RG_HIST;
+  k_rg_album<<<(RG_HIST + 255) / 256, 256, 0, st>>>(p.titles, T, album);
+  CK(cudaMemsetAsync(c.rg_gain.p, 0, sizeof(double) * (size_t)(T + 1), st));
+  k_rg_result<<<T + 1, 256, 0, st>>>(p.titles, T, album, c.rg_gain.p);
+  std::vector<int> hist0;
+  if (job.want_windows && T > 0) {
+    job.hist0.assign(RG_HIST, 0);
+    RgTitle t0;
+    CK(cudaMemcpyAsync(&t0, p.titles, sizeof t0, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpyAsync(job.hist0.data(), t0.hist, sizeof(int) * RG_HIST, cudaMemcpyDeviceToHost, st));
+  }
+  k_rg_finish<<<T, 256, 0, st>>>(p.titles, p.end_in, nch);
+  g_launches += 3;
+  CK(cudaEventRecord(c.ev_rg[2], st));
+  std::vector<double> g((size_t)T + 1);
+  CK(cudaMemcpyAsync(g.data(), c.rg_gain.p, sizeof(double) * (size_t)(T + 1), cudaMemcpyDeviceToHost, st));
+  if (job.want_windows) {
+    job.win_sum.assign((size_t)job.nwin0 * 2, 0.0);
+    job.win_idx.assign((size_t)job.nwin0, 0);
+    if (job.nwin0 > 0) {
+      CK(cudaMemcpyAsync(job.win_sum.data(), c.rg_sum.p, sizeof(double) * 2 * (size_t)job.nwin0, cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(job.win_idx.data(), c.rg_idx.p, sizeof(int) * (size_t)job.nwin0, cudaMemcpyDeviceToHost, st));
+    }
+  }
+  CK(cudaStreamSynchronize(st));
+  CK(cudaGetLastError());
+  CK(cudaEventElapsedTime(&job.ms, c.ev_rg[1], c.ev_rg[2]));
+  job.title_db.assign((size_t)T, (double)RG_NOT_ENOUGH_SAMPLES);
+  for (int i = 0; i < T; i++) if (job.specs[i].title_end) job.title_db[i] = g[i];
+  job.album_db = g[T];
+  return 0;
+}
+
 /* Encodes the streams `sds` into d_out: the caller sets each descriptor's PCM, pcm_base / pcm_end, frame0, nframes,
  * out_base and carried state; this assigns unit_base / frame_base, grows the thread's workspace and runs the pipeline.
  * The stream index is a grid y / z coordinate of several kernels (CUDA limit 65535): a larger batch runs as consecutive
@@ -557,6 +765,7 @@ int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, co
   if (o.timings_ms) for (int i = 0; i < 16; i++) o.timings_ms[i] = 0.0f;
   const PcmArrival* arrival = o.arrival;
   const int nstreams = (int)sds.size();
+  if (o.rg && nstreams > MP3_MAX_LAUNCH_STREAMS) { g_err = "ReplayGain batches hold at most 65535 streams"; return MP3B200_ERR_HANDLE; }
   for (int g0 = 0; g0 < nstreams; g0 += MP3_MAX_LAUNCH_STREAMS) {
     const int n = nstreams - g0 < MP3_MAX_LAUNCH_STREAMS ? nstreams - g0 : MP3_MAX_LAUNCH_STREAMS;
     StreamDesc* group = sds.data() + g0;
@@ -576,9 +785,17 @@ int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, co
       rc = resample_streams(cfg, group, n);
       if (rc) return rc;
     }
+    if (o.rg) {
+      rc = rg_queue(cfg, group, *o.rg, arrival);
+      if (rc) return rc;
+    }
     Timings tm;
     rc = run_pipeline(cfg, group, n, d_out, o, arrival, &tm);
     if (rc) return rc;
+    if (o.rg) {
+      rc = rg_finish(cfg, *o.rg);
+      if (rc) return rc;
+    }
     arrival = nullptr;
     float rs_ms = 0.0f;
     if (resampled && o.timings_ms && o.sync) CK(cudaEventElapsedTime(&rs_ms, t_ctx.ev_rs[0], t_ctx.ev_rs[1]));
@@ -695,7 +912,7 @@ std::vector<StreamDesc> whole_streams(Config* cfg, int nstreams, const int16_t* 
  * out_off[s].  Stereo input with right == NULL or right[s] == NULL encodes left[s] on both channels. */
 int encode_host_streams(Config* cfg, int nstreams, const int16_t* const* left, const int16_t* const* right,
                         const int64_t* nsamples, const int64_t* cap, int extra, int64_t* out_bytes,
-                        std::vector<int64_t>& out_off, std::vector<long long>& audio) {
+                        std::vector<int64_t>& out_off, std::vector<long long>& audio, RgJob* rg = nullptr) {
   const int nch = cfg->host.nch;
   std::vector<int64_t> pcm_off(nstreams);
   out_off.assign(nstreams, 0);
@@ -738,6 +955,7 @@ int encode_host_streams(Config* cfg, int nstreams, const int16_t* const* left, c
   std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off.data(), nsamples, out_off.data());
   LaunchOpts o;
   o.arrival = &arr;
+  o.rg = rg;
   return launch_streams(cfg, sds, t_ctx.out.p, o);
 }
 
@@ -1094,16 +1312,39 @@ int mp3b200_lametag_build(int channels, int samplerate, int kbps, int64_t nframe
 int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int nstreams, const int16_t* const* left,
                                   const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
                                   const int64_t* cap, int64_t* out_bytes) {
+  return mp3b200_encode_streams_tagged_ex(channels, samplerate, kbps, 0, nstreams, left, right, nsamples, out, cap, out_bytes,
+                                          nullptr, nullptr);
+}
+
+}  // extern "C"
+
+namespace {
+/* encode_streams_tagged_ex; `rg` (flags & MP3B200_REPLAYGAIN) receives the analysis */
+int encode_tagged(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
+                  const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out, const int64_t* cap,
+                  int64_t* out_bytes, RgJob* rg) {
   if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
+  if (flags & ~(MP3B200_RESAMPLE | MP3B200_REPLAYGAIN)) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
   Config* cfg;
-  int rc = get_config(channels, samplerate, kbps, 0, &cfg);
+  int rc = get_config(channels, samplerate, kbps, flags & MP3B200_RESAMPLE, &cfg);
   if (rc) return rc;
   Mp3TagParams p;
-  if (mp3_tag_params(channels, samplerate, kbps, &p) != 0) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
+  if (mp3_tag_params(channels, samplerate, kbps, &p, cfg->flags) != 0) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
   const int tfs = p.fits ? p.frame_bytes : 0;
+  if (rg && tfs == 0) rg = nullptr;               /* lamejs analyses only when the tag is written (Lame.js:911-916) */
+  if (rg) {
+    rg->specs.assign((size_t)nstreams, RgSpec());
+    for (int s = 0; s < nstreams; s++) {
+      rg->specs[s].stream = s;
+      LameFifo fifo(cfg->host.mode_gr, cfg->rs.ratio);
+      fifo.pieces = &rg->specs[s].pieces;
+      fifo.feed(nsamples[s]);
+      fifo.flush();
+    }
+  }
   std::vector<int64_t> out_off;
   std::vector<long long> audio;
-  rc = encode_host_streams(cfg, nstreams, left, right, nsamples, cap, tfs, out_bytes, out_off, audio);
+  rc = encode_host_streams(cfg, nstreams, left, right, nsamples, cap, tfs, out_bytes, out_off, audio, rg);
   if (rc || nstreams == 0) return rc;
   /* the music CRC of every stream, where the bytes are */
   std::vector<long long> off(out_off.begin(), out_off.end());
@@ -1113,13 +1354,14 @@ int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int ns
   Mp3SeekBag* bag = new Mp3SeekBag();
   for (int s = 0; s < nstreams; s++) {
     int wrote = 0;
-    LameFifo fifo(cfg->host.mode_gr);
+    LameFifo fifo(cfg->host.mode_gr, cfg->rs.ratio);
     const long long frames = fifo.feed(nsamples[s]);
     const FifoFlush fl = fifo.flush();
     if (tfs > 0 && frames + fl.frames > 0) {
       bag->reset();
       bag->add_frames(frames + fl.frames, p.kbps);
-      wrote = mp3_tag_frame(p, *bag, audio[s], crc[s], (int)fl.end_padding, out[s]);
+      const int field = rg ? mp3_radio_gain_field(mp3_radio_gain(rg->title_db[s])) : 0;
+      wrote = mp3_tag_frame(p, *bag, audio[s], crc[s], (int)fl.end_padding, out[s], field);
     }
     out_bytes[s] = audio[s] + wrote;
     if (audio[s] > 0 && cudaMemcpyAsync(out[s] + wrote, t_ctx.out.p + out_off[s], (size_t)audio[s], cudaMemcpyDeviceToHost, t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
@@ -1127,6 +1369,66 @@ int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int ns
   delete bag;
   if (cudaStreamSynchronize(t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
   return rc;
+}
+}  // namespace
+
+extern "C" {
+
+int mp3b200_encode_streams_tagged_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
+                                     const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
+                                     const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db) {
+  RgJob job;
+  const bool want = (flags & MP3B200_REPLAYGAIN) != 0;
+  const int rc = encode_tagged(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, want ? &job : nullptr);
+  if (rc) return rc;
+  const bool ran = want && (int)job.title_db.size() == nstreams && nstreams > 0;
+  for (int s = 0; title_db && s < nstreams; s++) title_db[s] = ran ? job.title_db[s] : RG_NOT_ENOUGH_SAMPLES;
+  if (album_db) *album_db = ran ? job.album_db : RG_NOT_ENOUGH_SAMPLES;
+  return 0;
+}
+
+int mp3b200_lametag_build_ex(int channels, int samplerate, int kbps, int flags, int64_t nframes, int64_t music_bytes, int music_crc,
+                             int encoder_padding, int radio_gain, uint8_t* buf, int cap) {
+  flags = config_flags(channels, samplerate, kbps, flags);
+  Mp3TagParams p;
+  if (flags < 0 || mp3_tag_params(channels, samplerate, kbps, &p, flags) != 0) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
+  if (!p.fits || nframes <= 0) return 0;
+  if (!buf || cap < p.frame_bytes) return p.frame_bytes;
+  Mp3SeekBag* bag = new Mp3SeekBag();
+  bag->reset();
+  bag->add_frames(nframes, p.kbps);
+  const int n = mp3_tag_frame(p, *bag, music_bytes, (unsigned)music_crc, encoder_padding, buf, mp3_radio_gain_field(radio_gain));
+  delete bag;
+  return n;
+}
+
+int mp3b200_debug_replaygain(int channels, int samplerate, int kbps, int flags, const int16_t* left, const int16_t* right,
+                             int64_t nsamples, double* win_sums, int32_t* win_idx, int64_t nwin_cap, int32_t* hist,
+                             double* title_db, int32_t* stats) {
+  if (nsamples < 0 || !left) return MP3B200_ERR_HANDLE;
+  RgJob job;
+  job.want_windows = true;
+  const int64_t bytes = mp3b200_stream_bytes_ex(channels, samplerate, kbps, flags & MP3B200_RESAMPLE, nsamples);
+  const int tsz = mp3b200_lametag_size_ex(channels, samplerate, kbps, flags & MP3B200_RESAMPLE);
+  if (bytes < 0 || tsz < 0) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
+  if (tsz == 0) { g_err = "the tag does not fit: no ReplayGain"; return MP3B200_ERR_CONFIG; }
+  std::vector<uint8_t> out((size_t)(bytes + tsz));
+  uint8_t* outp = out.data();
+  const int16_t* r = right ? right : left;
+  const int64_t cap = bytes + tsz;
+  int64_t ob = 0;
+  const int rc = encode_tagged(channels, samplerate, kbps, (flags & MP3B200_RESAMPLE) | MP3B200_REPLAYGAIN, 1, &left, &r, &nsamples,
+                               &outp, &cap, &ob, &job);
+  if (rc) return rc;
+  const long long n = (long long)job.win_idx.size();
+  for (long long w = 0; w < n && w < nwin_cap; w++) {
+    if (win_sums) { win_sums[2 * w] = job.win_sum[2 * w]; win_sums[2 * w + 1] = job.win_sum[2 * w + 1]; }
+    if (win_idx) win_idx[w] = job.win_idx[w];
+  }
+  if (hist && !job.hist0.empty()) memcpy(hist, job.hist0.data(), sizeof(int32_t) * RG_HIST);
+  if (title_db) *title_db = job.title_db[0];
+  if (stats) { stats[0] = (int32_t)n; stats[1] = job.passes; stats[2] = job.reruns; memcpy(stats + 3, &job.ms, sizeof(float)); }
+  return 0;
 }
 
 }  // extern "C"

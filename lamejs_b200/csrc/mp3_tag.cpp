@@ -62,7 +62,16 @@ int mp3_tag_placeholder(const Mp3TagParams& p, uint8_t* out) {
   return p.frame_bytes;
 }
 
-int mp3_tag_frame(const Mp3TagParams& p, const Mp3SeekBag& bag, long long music_bytes, unsigned music_crc, int encoder_padding, uint8_t* out) {
+int mp3_radio_gain(double title_db) { return (int)floor(title_db * 10.0 + 0.5); }
+
+int mp3_radio_gain_field(int radio_gain) {
+  if (radio_gain > 0x1FE) radio_gain = 0x1FE;
+  if (radio_gain < -0x1FE) radio_gain = -0x1FE;
+  return radio_gain >= 0 ? (0x2000 | 0xC00 | radio_gain) : (0x2000 | 0xC00 | 0x200 | -radio_gain);
+}
+
+int mp3_tag_frame(const Mp3TagParams& p, const Mp3SeekBag& bag, long long music_bytes, unsigned music_crc, int encoder_padding, uint8_t* out,
+                  int radio_gain_field) {
   if (!p.fits || bag.pos <= 0) return 0;
   memset(out, 0, (size_t)p.frame_bytes);
   mp3_tag_header(p, 0 /* MPG_MD_LR_LR: what every encoded frame leaves in gfc.mode_ext */, out);
@@ -85,7 +94,9 @@ int mp3_tag_frame(const Mp3TagParams& p, const Mp3SeekBag& bag, long long music_
   memcpy(q + 4, "LAME3.98r", 9);                             /* Version.js:56-59 */
   q[13] = 1;                                                 /* tag revision 0, method 1 = CBR */
   q[14] = (uint8_t)p.lowpass_byte;
-  /* q[15..18] peak amplitude, q[19..22] replay gains: not analysed by Mp3Encoder, zero */
+  /* q[15..18] peak amplitude: zero (it needs the decoder); q[19..20] Radio Replay Gain when analysed (0 otherwise),
+   * q[21..22] Audiophile Replay Gain: zero (lamejs never sets it) */
+  put_be(q + 19, 2, radio_gain_field);
   q[23] = (uint8_t)p.flags_byte;
   q[24] = (uint8_t)(p.kbps >= 255 ? 255 : p.kbps);
   const int delay = 576;                                     /* Encoder.ENCDELAY */

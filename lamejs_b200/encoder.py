@@ -69,6 +69,12 @@ def lib():
     L.mp3b200_lametag_size.argtypes = [c_int, c_int, c_int]
     L.mp3b200_lametag_build.argtypes = [c_int, c_int, c_int, c_i64, c_i64, c_int, c_int, vp, c_int]
     L.mp3b200_encode_streams_tagged.argtypes = [c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp]
+    L.mp3b200_encode_streams_tagged_ex.argtypes = [c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.mp3b200_lametag_build_ex.argtypes = [c_int, c_int, c_int, c_int, c_i64, c_i64, c_int, c_int, c_int, vp, c_int]
+    L.mp3b200_set_find_replay_gain.argtypes = [vp, c_int]
+    L.mp3b200_get_replay_gain.argtypes = [vp, vp, vp]
+    L.mp3b200_album_gain.argtypes = [vp, c_int, vp]
+    L.mp3b200_debug_replaygain.argtypes = [c_int, c_int, c_int, c_int, vp, vp, c_i64, vp, vp, c_i64, vp, vp, vp]
     L.mp3b200_wav_read_header.argtypes = [vp, c_i64, vp]
     L.mp3b200_debug_music_crc.argtypes = [vp, vp, vp, c_int, vp, vp]
     L.mp3b200_debug_stages.argtypes = [c_int, c_int, c_int, vp, vp, c_i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, c_i64]
@@ -92,6 +98,7 @@ def _check(rc):
 
 
 RESAMPLE = 1     # MP3B200_RESAMPLE
+REPLAYGAIN = 2   # MP3B200_REPLAYGAIN
 
 
 def stream_frames(nsamples, channels=None, samplerate=None, kbps=None, resample=False):
@@ -233,9 +240,13 @@ class Mp3Encoder:
     gfp.bWriteVbrTag (index.js:107 sets it false): the stream then starts with a placeholder frame, and `lametag_frame()`
     after flush() returns the finished Info / LAME tag frame to write over it.  `resample=True` also accepts the
     configurations lamejs resamples by an integer ratio, e.g. Mp3Encoder(2, 48000, 64), which encodes at 24 kHz: samples
-    are fed at the input rate and resampled on the GPU (seek() is not supported then)."""
+    are fed at the input rate and resampled on the GPU (seek() is not supported then).  `find_replay_gain=True` is
+    gfp.findReplayGain (it needs the tag: without write_vbr_tag, or where the tag does not fit, it stays off): every
+    sample is analysed on the GPU, each flush() ends a title, `replay_gain` is then the last title's (gain in dB,
+    gfc.RadioGain) and the tag carries it; album_gain(encoders) combines titles.  State export / import and seek() are not
+    supported then."""
 
-    def __init__(self, channels=1, samplerate=44100, kbps=128, write_vbr_tag=False, resample=False):
+    def __init__(self, channels=1, samplerate=44100, kbps=128, write_vbr_tag=False, resample=False, find_replay_gain=False):
         self._L = lib()
         self._h = ctypes.c_void_p()
         self.channels = channels
@@ -244,6 +255,15 @@ class Mp3Encoder:
         _check(rc)
         self.tag_on = bool(write_vbr_tag) and _check(self._L.mp3b200_set_write_vbr_tag(self._h, 1)) == 1
         self._tag_room = _check(self._L.mp3b200_lametag_size_ex(channels, samplerate, kbps, flags)) if self.tag_on else 0
+        self.replay_gain_on = bool(find_replay_gain) and _check(self._L.mp3b200_set_find_replay_gain(self._h, 1)) == 1
+
+    @property
+    def replay_gain(self):
+        """(title gain in dB, gfc.RadioGain) of the title the last flush() ended; None before it or with the analysis off"""
+        db, radio = ctypes.c_double(0.0), ctypes.c_int(0)
+        if _check(self._L.mp3b200_get_replay_gain(self._h, ctypes.byref(db), ctypes.byref(radio))) != 1:
+            return None
+        return float(db.value), int(radio.value)
 
     def lametag_frame(self):
         buf = np.zeros(2880, dtype=np.uint8)
@@ -382,11 +402,76 @@ def encode_streams(channels, samplerate, kbps, lefts, rights=None, resample=Fals
     return _encode_host_streams(lib().mp3b200_encode_streams, channels, samplerate, kbps, lefts, rights, 0)
 
 
-def encode_streams_tagged(channels, samplerate, kbps, lefts, rights=None):
+def encode_streams_tagged(channels, samplerate, kbps, lefts, rights=None, resample=False):
     """encode_streams with gfp.bWriteVbrTag on: every returned stream starts with its finished Info / LAME tag frame (frame
-    and byte counts, seek table, encoder delay / padding, CRC-16 of the audio bytes computed on the GPU)."""
-    return _encode_host_streams(lib().mp3b200_encode_streams_tagged, channels, samplerate, kbps, lefts, rights,
-                                lametag_size(channels, samplerate, kbps))
+    and byte counts, seek table, encoder delay / padding, CRC-16 of the audio bytes computed on the GPU).  resample=True:
+    see Mp3Encoder."""
+    if not resample:
+        return _encode_host_streams(lib().mp3b200_encode_streams_tagged, channels, samplerate, kbps, lefts, rights,
+                                    lametag_size(channels, samplerate, kbps))
+    return encode_streams_replaygain(channels, samplerate, kbps, lefts, rights, resample=True, find_replay_gain=False)[0]
+
+
+def encode_streams_replaygain(channels, samplerate, kbps, lefts, rights=None, resample=False, find_replay_gain=True):
+    """encode_streams_tagged with gfp.findReplayGain: every stream's ReplayGain is analysed on the GPU and written into its
+    tag, as lamejs does.  Returns (streams, title_db, album_db): the list of bytes, GetTitleGain of each stream in dB and
+    GetAlbumGain of the batch (-24601: less than one RMS window, or the tag does not fit and nothing was analysed)."""
+    flags = (REPLAYGAIN if find_replay_gain else 0) | (RESAMPLE if resample else 0)
+    title = np.zeros(max(len(lefts), 1), dtype=np.float64)
+    album = ctypes.c_double(0.0)
+
+    def fn(ch, sr, kb, *args):
+        return lib().mp3b200_encode_streams_tagged_ex(ch, sr, kb, flags, *args, title.ctypes.data, ctypes.byref(album))
+    room = lib().mp3b200_lametag_size_ex(channels, samplerate, kbps, RESAMPLE if resample else 0)
+    out = _encode_host_streams(fn, channels, samplerate, kbps, lefts, rights, max(room, 0), resample)
+    return out, [float(t) for t in title[:len(lefts)]], float(album.value) if lefts else float(GAIN_NOT_ENOUGH_SAMPLES)
+
+
+def album_gain(encoders):
+    """GetAlbumGain over the titles the Mp3Encoders (find_replay_gain=True) have ended with flush()"""
+    hs = (ctypes.c_void_p * max(len(encoders), 1))(*[e._h.value for e in encoders])
+    out = ctypes.c_double(0.0)
+    _check(lib().mp3b200_album_gain(hs, len(encoders), ctypes.byref(out)))
+    return float(out.value)
+
+
+GAIN_NOT_ENOUGH_SAMPLES = -24601
+
+
+def radio_gain(title_db):
+    """gfc.RadioGain, the value the tag stores (tenths of a dB): Math.floor(title_db * 10 + 0.5)"""
+    return int(np.floor(title_db * 10.0 + 0.5))
+
+
+def lametag_build_ex(channels, samplerate, kbps, nframes, music_bytes, music_crc, encoder_padding, radio_gain, resample=False):
+    """mp3b200_lametag_build with the Radio Replay Gain field (gfc.RadioGain of a stream the caller analysed)"""
+    buf = np.zeros(2880, dtype=np.uint8)
+    n = lib().mp3b200_lametag_build_ex(channels, samplerate, kbps, RESAMPLE if resample else 0, nframes, music_bytes, music_crc,
+                                       encoder_padding, radio_gain, buf.ctypes.data, len(buf))
+    _check(min(n, 0))
+    return buf[:n].tobytes()
+
+
+def debug_replaygain(channels, samplerate, kbps, left, right=None, resample=False):
+    """The ReplayGain analysis of one whole stream (encodeBuffer(all) + flush()) as the GPU ran it: dict with `sums`
+    (float64 [windows][2]: lsum, rsum), `idx` (int32 [windows]), `hist` (int32 [12000]), `title_db`, `passes` (repair
+    passes), `reruns` (chunks run again) and `ms` (the analysis's CUDA-event time)."""
+    L = lib()
+    left = np.ascontiguousarray(left, dtype=np.int16)
+    right = left if (right is None or channels == 1) else np.ascontiguousarray(right, dtype=np.int16)
+    cap = len(left) // 400 + 64
+    sums = np.zeros((cap, 2), dtype=np.float64)
+    idx = np.zeros(cap, dtype=np.int32)
+    hist = np.zeros(12000, dtype=np.int32)
+    title = ctypes.c_double(0.0)
+    stats = np.zeros(4, dtype=np.int32)
+    _check(L.mp3b200_debug_replaygain(channels, samplerate, kbps, RESAMPLE if resample else 0, left.ctypes.data, right.ctypes.data,
+                                      len(left), sums.ctypes.data, idx.ctypes.data, cap, hist.ctypes.data, ctypes.byref(title),
+                                      stats.ctypes.data))
+    n = int(stats[0])
+    assert n <= cap
+    return {"sums": sums[:n].copy(), "idx": idx[:n].copy(), "hist": hist, "title_db": float(title.value), "passes": int(stats[1]),
+            "reruns": int(stats[2]), "ms": float(stats[3:4].view(np.float32)[0])}
 
 
 def debug_music_crc(d_buf_ptr, offsets, lengths, timed=False):
