@@ -330,6 +330,44 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* t);
 int mp3b200_debug_resample(int channels, int samplerate, int kbps, const int16_t* left, const int16_t* right, int64_t nsamples,
                            float* y, int64_t ny);
 
+/* ---- Float32 input (lamejs encodeBuffer with a Float32Array or a plain Array, Lame.js:1500-1510,1554-1560) -------------
+ * lamejs stores every value the caller passes into a Float32Array, x = Float32(v), and scales it in place,
+ * x = Float32((double)x * scale), when the preset's scale is not 1; the encoder works on those values.  The _f32 twins below
+ * take such Float32 samples (a caller with doubles rounds them to Float32 once, as that store does) and encode them exactly
+ * as lamejs does; an integer-valued sample in Int16 range encodes exactly like that Int16 sample through the Int16 calls.
+ * Samples that are not finite (before or after the scale) are refused with MP3B200_ERR_CONFIG: the host calls refuse them
+ * before anything runs and leave a handle untouched; mp3b200_encode_streams_device_f32 finds them on the device, and its
+ * output buffer is then unspecified.  lamejs would carry NaN through its psy model and rate loop.
+ * Streaming handles: a handle switches to Float32 mode at its first Float32 call (encode_f32, encode_batch_f32, seek_f32)
+ * and stays there; its retained samples are converted exactly, and the samples of later Int16 calls are converted too, so
+ * any mix of Int16 and Float32 calls encodes as the same mix of Int16Array / Float32Array calls does in lamejs.  A batch may
+ * mix handles of both modes.  A Float32-mode handle exports a blob with its own magic ('M3F1', resampled 'M3G1') that carries
+ * Float32 samples; importing a blob sets the handle's mode.  flush, the tag and the ReplayGain calls are unchanged.
+ * The whole-stream calls take the flags of their Int16 twins: encode_streams_f32 those of _ex, encode_streams_tagged_f32
+ * those of _tagged_ex, encode_streams_device_f32 those of _device_ex (d_pcm: one device allocation of Float32 samples laid
+ * out like d_pcm there; timings included). */
+int mp3b200_encode_f32(mp3b200_encoder* h, const float* left, const float* right, int nsamples, uint8_t* out, int cap);
+int mp3b200_encode_batch_f32(mp3b200_encoder* const* handles, const float* const* left, const float* const* right,
+                             const int* nsamples, uint8_t* const* out, const int* cap, int nstreams, int* out_bytes);
+int mp3b200_seek_f32(mp3b200_encoder* h, int64_t frame, const float* left_hist, const float* right_hist, int nhist);
+int mp3b200_encode_streams_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* const* left,
+                               const float* const* right, const int64_t* nsamples, uint8_t* const* out,
+                               const int64_t* cap, int64_t* out_bytes);
+int mp3b200_encode_streams_tagged_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* const* left,
+                                      const float* const* right, const int64_t* nsamples, uint8_t* const* out,
+                                      const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db);
+int mp3b200_encode_streams_device_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* d_pcm,
+                                      const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
+                                      const int64_t* out_off, float* timings_ms);
+/* Test taps: mp3b200_debug_stages_ex with the input `left` / `right` (right NULL: left) instead of t->left / t->right, and
+ * mp3b200_debug_resample / mp3b200_debug_replaygain with Float32 input. */
+int mp3b200_debug_stages_f32(const mp3b200_debug_taps* t, const float* left, const float* right);
+int mp3b200_debug_resample_f32(int channels, int samplerate, int kbps, const float* left, const float* right, int64_t nsamples,
+                               float* y, int64_t ny);
+int mp3b200_debug_replaygain_f32(int channels, int samplerate, int kbps, int flags, const float* left, const float* right,
+                                 int64_t nsamples, double* win_sums, int32_t* win_idx, int64_t nwin_cap, int32_t* hist,
+                                 double* title_db, int32_t* stats);
+
 const char* mp3b200_last_error(void);
 /* total number of kernel launches issued by this library since load (bench.py "gpu_launches") */
 int64_t mp3b200_launch_count(void);

@@ -4,7 +4,8 @@
  *
  *   const lamejs = require('mp3b200');            // instead of require('lamejs')
  *   const enc = new lamejs.Mp3Encoder(2, 44100, 128);
- *   const mp3 = enc.encodeBuffer(left, right);    // Int16Array in, Int8Array out (frames completed by this call)
+ *   const mp3 = enc.encodeBuffer(left, right);    // Int16Array (or, as in lamejs, Float32Array / Array of numbers) in,
+ *                                                 // Int8Array out (frames completed by this call)
  *   const tail = enc.flush();
  *
  * Same constructor / encodeBuffer / flush surface and return types as zhuker/lamejs src/js/index.js:66-136.
@@ -24,6 +25,8 @@ const lib = ffi.Library(process.env.MP3B200_LIB || 'libmp3b200', {
   mp3b200_export_state: ['int', [voidPtr, 'pointer', 'int']],
   mp3b200_import_state: ['int', [voidPtr, 'pointer', 'int']],
   mp3b200_seek: ['int', [voidPtr, 'int64', 'pointer', 'pointer', 'int']],
+  mp3b200_encode_f32: ['int', [voidPtr, 'pointer', 'pointer', 'int', 'pointer', 'int']],
+  mp3b200_seek_f32: ['int', [voidPtr, 'int64', 'pointer', 'pointer', 'int']],
   mp3b200_set_write_vbr_tag: ['int', [voidPtr, 'int']],
   mp3b200_get_lametag_frame: ['int', [voidPtr, 'pointer', 'int']],
   mp3b200_set_find_replay_gain: ['int', [voidPtr, 'int']],
@@ -65,6 +68,10 @@ function Mp3Encoder(channels, samplerate, kbps, options) {
   let buf = Buffer.alloc((0 | (1.25 * maxSamples + 7200)) + tagRoom);   // index.js:113-114
 
   const asBuf = (a) => Buffer.from(a.buffer, a.byteOffset, a.byteLength);
+  // lamejs copies whatever it is given into Float32Arrays (Lame.js:1500-1510): an Int16Array pair keeps the Int16 entry
+  // point, anything else (Float32Array, Float64Array, a plain Array of numbers) is stored into a Float32Array the same way
+  const isInt16 = (a) => a instanceof Int16Array;
+  const asF32 = (a) => (a instanceof Float32Array ? a : Float32Array.from(a));
 
   this.encodeBuffer = function (left, right) {
     if (channels === 1) right = left;
@@ -72,7 +79,9 @@ function Mp3Encoder(channels, samplerate, kbps, options) {
       maxSamples = left.length;
       buf = Buffer.alloc((0 | (1.25 * maxSamples + 7200)) + tagRoom);
     }
-    const n = lib.mp3b200_encode(h, asBuf(left), asBuf(right), left.length, buf, buf.length);
+    const n = isInt16(left) && isInt16(right)
+      ? lib.mp3b200_encode(h, asBuf(left), asBuf(right), left.length, buf, buf.length)
+      : lib.mp3b200_encode_f32(h, asBuf(asF32(left)), asBuf(asF32(right)), left.length, buf, buf.length);
     if (n < 0) throw new Error('mp3b200_encode failed (' + n + '): ' + lib.mp3b200_last_error());
     return new Int8Array(buf.subarray(0, n));                // a fresh copy, like index.js:129
   };
@@ -106,7 +115,9 @@ function Mp3Encoder(channels, samplerate, kbps, options) {
   };
   this.seek = function (frame, leftHist, rightHist) {
     if (channels === 1 || !rightHist) rightHist = leftHist;
-    const rc = lib.mp3b200_seek(h, frame, asBuf(leftHist), asBuf(rightHist), leftHist.length);
+    const rc = isInt16(leftHist) && isInt16(rightHist)
+      ? lib.mp3b200_seek(h, frame, asBuf(leftHist), asBuf(rightHist), leftHist.length)
+      : lib.mp3b200_seek_f32(h, frame, asBuf(asF32(leftHist)), asBuf(asF32(rightHist)), leftHist.length);
     if (rc !== 0) throw new Error('mp3b200_seek failed (' + rc + '): ' + lib.mp3b200_last_error());
   };
 

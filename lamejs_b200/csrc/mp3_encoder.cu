@@ -230,6 +230,9 @@ struct Workspace {
   Buf<ScanChunk> scan;                    /* [F / SCAN_FRAMES + S] */
   Buf<ResampleDesc> rs_desc;              /* resampled batches: [S] */
   Buf<float> rs_y;                        /* resampled batches: the resampler's output rows, the PCM the pipeline reads */
+  Buf<StageDesc> st_desc;                 /* Float32 input: [S] */
+  Buf<float> st_y;                        /* Float32 input: the staged (scaled) rows */
+  Buf<int> nonfinite;                     /* Float32 input: set by k_stage_f32 when a sample is not finite */
   int fit(int S, int nch, long long U, long long F) {
     const size_t gc = (size_t)U * nch, rows = (size_t)(U + S) * nch, f = (size_t)F + 1;
     const bool failed = streams.fit(S) || bt_final.fit((size_t)U * 2 + 16) || bt_prev.fit((size_t)U * 2 + 16) ||
@@ -243,7 +246,7 @@ struct Workspace {
     streams.release(); bt_final.release(); bt_prev.release(); xr.release(); slab.release(); psy.release(); scan_in.release();
     ratio.release(); ath_psy.release(); ath_q.release(); qstate.release(); ginfo.release(); l3enc.release(); xrq.release();
     xrpow.release(); neg.release(); prep.release(); dirty.release(); counter.release(); scan.release();
-    rs_desc.release(); rs_y.release();
+    rs_desc.release(); rs_y.release(); st_desc.release(); st_y.release(); nonfinite.release();
   }
 };
 
@@ -261,6 +264,7 @@ struct ThreadCtx {
   Workspace ws;
   int evq_pred[QE_COUNT] = {};
   Buf<int16_t> pcm;                       /* staged PCM of host callers */
+  Buf<float> pcmf;                        /* the same for Float32 input */
   Buf<uint8_t> out;                       /* encoded bytes of host callers */
   Buf<uint8_t, true> pin;                 /* pinned host staging */
   Buf<long long> crc_ranges;              /* music CRC: [2][R] offsets / lengths */
@@ -277,7 +281,7 @@ struct ThreadCtx {
   void release() {
     if (device < 0) return;
     cudaSetDevice(device);
-    ws.release(); pcm.release(); out.release(); pin.release(); crc_ranges.release(); crc.release();
+    ws.release(); pcm.release(); pcmf.release(); out.release(); pin.release(); crc_ranges.release(); crc.release();
     rg_titles.release(); rg_piece.release(); rg_sum.release(); rg_gain.release(); rg_wstate.release(); rg_cstart.release();
     rg_end_a.release(); rg_end_b.release(); rg_carry.release(); rg_idx.release(); rg_hist.release(); rg_count.release();
     for (auto& e : ev_rg) if (e) { cudaEventDestroy(e); e = nullptr; }
@@ -349,6 +353,8 @@ struct LaunchOpts {
   StreamDesc* committed = nullptr;       /* host: each stream's descriptor as the pipeline left it (the carried state),
                                             valid once t_ctx.st has drained */
   struct RgJob* rg = nullptr;            /* ReplayGain of every stream, beside the encoder (one launch group only) */
+  bool f32_in = false;                   /* the descriptors point at the caller's Float32 rows (k_stage_f32 stages them); with
+                                            sync, a non-finite sample makes the launch return MP3B200_ERR_CONFIG */
 };
 
 /* One pipeline launch for the streams sds[0 .. S) (at most MP3_MAX_LAUNCH_STREAMS, unit / frame bases set, the workspace
@@ -362,7 +368,7 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
   Workspace& ws = t_ctx.ws;
 
   const int nch = cfg->host.nch;
-  const bool f32_pcm = cfg->rs.ratio > 1;   /* the streams read the resampler's Float32 output */
+  const bool f32_pcm = cfg->rs.ratio > 1 || o.f32_in;   /* the streams read Float32 rows: the resampler's or the staged input */
   int max_frames = 0;
   long long total_frames = 0;          /* rows actually used this launch (the workspace may be larger) */
   int scan_rows = 0;
@@ -519,12 +525,51 @@ long long hist_base_at(int mode_gr, long long frame) {
   return b > 0 ? b : 0;
 }
 
-/* Resampled launches: the descriptors sds[0 .. S) hold the caller's input (Int16 at rs.in_rate; pcm_base / pcm_end count
+/* Float32 input: the descriptors sds[0 .. S) point at the caller's Float32 rows.  Queues k_stage_f32, which writes them
+ * scaled into the workspace (ws.nonfinite flags a non-finite sample), and points the descriptors at the staged rows; the
+ * sample indices stay as they were. */
+int stage_streams(Config* cfg, StreamDesc* sds, int S) {
+  const int nch = cfg->host.nch;
+  Workspace& ws = t_ctx.ws;
+  std::vector<StageDesc> d((size_t)S);
+  long long tot = 0, max_n = 0;
+  for (int i = 0; i < S; i++) {
+    const long long n = sds[i].pcm_end > sds[i].pcm_base ? sds[i].pcm_end - sds[i].pcm_base : 0;
+    for (int c = 0; c < 2; c++) d[i].x[c] = reinterpret_cast<const float*>(sds[i].pcm[c]);
+    d[i].n = n;
+    tot += n * nch;
+    max_n = n > max_n ? n : max_n;
+  }
+  int rc = ws.st_desc.fit((size_t)S);
+  if (rc) return rc;
+  rc = ws.st_y.fit((size_t)tot + 1);
+  if (rc) return rc;
+  long long off = 0;
+  for (int i = 0; i < S; i++) {
+    d[i].y[0] = ws.st_y.p + off; d[i].y[1] = nch == 2 ? d[i].y[0] + d[i].n : d[i].y[0];
+    off += d[i].n * nch;
+    for (int c = 0; c < 2; c++) sds[i].pcm[c] = reinterpret_cast<const int16_t*>(d[i].y[c]);
+  }
+  cudaStream_t st = t_ctx.st;
+  CK(cudaEventRecord(t_ctx.ev_in, cudaStreamLegacy));      /* the input may come from the legacy default stream */
+  CK(cudaStreamWaitEvent(st, t_ctx.ev_in, 0));
+  CK(cudaMemcpyAsync(ws.st_desc.p, d.data(), sizeof(StageDesc) * S, cudaMemcpyHostToDevice, st));
+  if (max_n > 0) {
+    const long long per = (long long)STAGE_THREADS * STAGE_PER_THREAD;
+    dim3 grid((unsigned)((max_n + per - 1) / per), nch, S);
+    k_stage_f32<<<grid, STAGE_THREADS, 0, st>>>(ws.st_desc.p, cfg->host.scale_applied, cfg->host.scale, ws.nonfinite.p);
+    g_launches++;
+    DBG("k_stage_f32");
+  }
+  return 0;
+}
+
+/* Resampled launches: the descriptors sds[0 .. S) hold the caller's input (Int16 at rs.in_rate, or staged Float32 rows; pcm_base / pcm_end count
  * input samples, and pcm_base is at most max(0, r * hist_base_at(frame0) - 16), the first input the outputs below read).
  * Queues k_resample for the outputs the streams' frames read -- from hist_base_at(frame0) up to the last output the input
  * reaches; later outputs are 0 -- into the workspace, and points the descriptors at them: from then on pcm_base / pcm_end
  * count outputs, and the stream reads like PCM at the output rate. */
-int resample_streams(Config* cfg, StreamDesc* sds, int S) {
+int resample_streams(Config* cfg, StreamDesc* sds, int S, bool f32_in) {
   const int r = cfg->rs.ratio, nch = cfg->host.nch;
   Workspace& ws = t_ctx.ws;
   std::vector<ResampleDesc> rd((size_t)S);
@@ -561,7 +606,8 @@ int resample_streams(Config* cfg, StreamDesc* sds, int S) {
   CK(cudaEventRecord(t_ctx.ev_rs[0], st));
   if (max_ny > 0) {
     dim3 grid((unsigned)((max_ny + RS_THREADS - 1) / RS_THREADS), nch, S);
-    k_resample<<<grid, RS_THREADS, 0, st>>>(ws.rs_desc.p, r, cfg->host.scale_applied, cfg->host.scale);
+    if (f32_in) k_resample<float><<<grid, RS_THREADS, 0, st>>>(ws.rs_desc.p, r, 0, cfg->host.scale);   /* staged: scaled */
+    else k_resample<int16_t><<<grid, RS_THREADS, 0, st>>>(ws.rs_desc.p, r, cfg->host.scale_applied, cfg->host.scale);
     g_launches++;
     DBG("k_resample");
   }
@@ -608,7 +654,7 @@ int rg_req_index(int sr) {
 
 /* queues pass 1 and the first RG_QUEUED_PASSES repair passes on t_ctx.rg_st, after the PCM (the upload slices in `arrival`,
  * or everything queued on t_ctx.st so far: uploads and the resampler) */
-int rg_queue(Config* cfg, const StreamDesc* sds, RgJob& job, const PcmArrival* arrival) {
+int rg_queue(Config* cfg, const StreamDesc* sds, RgJob& job, const PcmArrival* arrival, bool f32_in) {
   ThreadCtx& c = t_ctx;
   const int sr = cfg->host.samplerate, W = (sr + 19) / 20, nch = cfg->host.nch, req = rg_req_index(sr);
   if (req < 0) { g_err = "no ReplayGain filter for this rate"; return MP3B200_ERR_CONFIG; }
@@ -666,8 +712,8 @@ int rg_queue(Config* cfg, const StreamDesc* sds, RgJob& job, const PcmArrival* a
   CK(cudaMemsetAsync(c.rg_hist.p, 0, sizeof(int) * (size_t)(T + 1) * RG_HIST, st));
   CK(cudaMemsetAsync(c.rg_carry.p, 0, sizeof(RgCarry) * (size_t)(T + 1), st));
   RgParams& p = job.prm;
-  p.titles = c.rg_titles.p; p.nch = nch; p.W = W; p.req = req; p.f32 = cfg->rs.ratio > 1;
-  p.scale_applied = cfg->rs.ratio > 1 ? 0 : cfg->host.scale_applied;   /* k_resample already scaled its input */
+  p.titles = c.rg_titles.p; p.nch = nch; p.W = W; p.req = req; p.f32 = cfg->rs.ratio > 1 || f32_in;
+  p.scale_applied = p.f32 ? 0 : cfg->host.scale_applied;   /* k_resample / k_stage_f32 already scaled their input */
   p.scale = cfg->host.scale;
   p.win_sum = c.rg_sum.p; p.win_state = c.rg_wstate.p; p.chunk_start = c.rg_cstart.p; p.end_in = c.rg_end_a.p; p.end_out = c.rg_end_b.p;
   p.done = c.rg_count.p; p.reruns = c.rg_count.p + 1; p.pass_changed = c.rg_count.p + 2;
@@ -766,6 +812,11 @@ int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, co
   const PcmArrival* arrival = o.arrival;
   const int nstreams = (int)sds.size();
   if (o.rg && nstreams > MP3_MAX_LAUNCH_STREAMS) { g_err = "ReplayGain batches hold at most 65535 streams"; return MP3B200_ERR_HANDLE; }
+  if (o.f32_in) {
+    int rc = t_ctx.ws.nonfinite.fit(1);
+    if (rc) return rc;
+    CK(cudaMemsetAsync(t_ctx.ws.nonfinite.p, 0, sizeof(int), t_ctx.st));
+  }
   for (int g0 = 0; g0 < nstreams; g0 += MP3_MAX_LAUNCH_STREAMS) {
     const int n = nstreams - g0 < MP3_MAX_LAUNCH_STREAMS ? nstreams - g0 : MP3_MAX_LAUNCH_STREAMS;
     StreamDesc* group = sds.data() + g0;
@@ -778,15 +829,21 @@ int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, co
     int rc = t_ctx.ws.fit(n, cfg->host.nch, U, F);
     if (rc) return rc;
     const bool resampled = cfg->rs.ratio > 1;
-    if (resampled) {
-      if (arrival)                              /* the resampler reads all of the input: wait for every slice */
+    if (resampled || o.f32_in) {
+      if (arrival)                              /* the resampler / stager reads all of the input: wait for every slice */
         for (int j = 0; j < arrival->chunks; j++) CK(cudaStreamWaitEvent(t_ctx.st, arrival->ready[j], 0));
       arrival = nullptr;
-      rc = resample_streams(cfg, group, n);
+    }
+    if (o.f32_in) {
+      rc = stage_streams(cfg, group, n);
+      if (rc) return rc;
+    }
+    if (resampled) {
+      rc = resample_streams(cfg, group, n, o.f32_in);
       if (rc) return rc;
     }
     if (o.rg) {
-      rc = rg_queue(cfg, group, *o.rg, arrival);
+      rc = rg_queue(cfg, group, *o.rg, arrival, o.f32_in);
       if (rc) return rc;
     }
     Timings tm;
@@ -807,6 +864,12 @@ int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, co
       for (int i = 0; i < 16; i++) o.timings_ms[i] += t[i];
       if ((float)tm.passes > o.timings_ms[7]) o.timings_ms[7] = (float)tm.passes;
     }
+  }
+  if (o.f32_in && o.sync) {
+    int bad = 0;
+    CK(cudaMemcpyAsync(&bad, t_ctx.ws.nonfinite.p, sizeof(int), cudaMemcpyDeviceToHost, t_ctx.st));
+    CK(cudaStreamSynchronize(t_ctx.st));
+    if (bad) { g_err = "non-finite input sample"; return MP3B200_ERR_CONFIG; }
   }
   return 0;
 }
@@ -891,14 +954,16 @@ int mp3b200_out_samplerate(int channels, int samplerate, int kbps) { return mp3_
 namespace {
 /* Whole streams (encodeBuffer(everything) + flush() on fresh encoders): stream s reads nsamples[s] samples per channel at
  * d_pcm + pcm_off[s] (stereo: the right channel follows the left) and writes its bytes at out_off[s]. */
-std::vector<StreamDesc> whole_streams(Config* cfg, int nstreams, const int16_t* d_pcm, const int64_t* pcm_off,
+template <class T>     /* int16_t, or float (the launch stages the rows: LaunchOpts::f32_in) */
+std::vector<StreamDesc> whole_streams(Config* cfg, int nstreams, const T* d_pcm, const int64_t* pcm_off,
                                       const int64_t* nsamples, const int64_t* out_off) {
   std::vector<StreamDesc> sds(nstreams);
   for (int s = 0; s < nstreams; s++) {
     StreamDesc& sd = sds[s];
     memset(&sd, 0, sizeof sd);
-    sd.pcm[0] = d_pcm + pcm_off[s];
-    sd.pcm[1] = cfg->host.nch == 2 ? sd.pcm[0] + nsamples[s] : sd.pcm[0];
+    const T* x = d_pcm + pcm_off[s];
+    sd.pcm[0] = reinterpret_cast<const int16_t*>(x);
+    sd.pcm[1] = reinterpret_cast<const int16_t*>(cfg->host.nch == 2 ? x + nsamples[s] : x);
     sd.pcm_base = 0; sd.pcm_end = nsamples[s];
     sd.frame0 = 0; sd.nframes = (int)frames_for(nsamples[s], cfg->host.mode_gr, cfg->rs.ratio);
     sd.out_base = out_off[s];
@@ -907,10 +972,34 @@ std::vector<StreamDesc> whole_streams(Config* cfg, int nstreams, const int16_t* 
   return sds;
 }
 
+/* the thread's device buffer for host PCM of sample type T */
+template <class T> Buf<T>& staging_pcm();
+template <> Buf<int16_t>& staging_pcm<int16_t>() { return t_ctx.pcm; }
+template <> Buf<float>& staging_pcm<float>() { return t_ctx.pcmf; }
+
+/* Float32 input (lamejs's store and scale): true when every sample is finite, and stays finite once scaled like
+ * k_stage_f32 scales it.  The host entry points refuse other input with MP3B200_ERR_CONFIG before anything runs. */
+bool finite_after_scale(const Mp3Tables& T, const float* x, long long n) {
+  for (long long i = 0; i < n; i++) {
+    float v = x[i];
+    if (T.scale_applied) v = (float)((double)v * T.scale);
+    if (!std::isfinite(v)) return false;
+  }
+  return true;
+}
+bool streams_finite(const Config* cfg, int nstreams, const float* const* left, const float* const* right, const int64_t* nsamples) {
+  for (int s = 0; s < nstreams; s++) {
+    if (!finite_after_scale(cfg->host, left[s], nsamples[s])) return false;
+    if (cfg->host.nch == 2 && right && right[s] && !finite_after_scale(cfg->host, right[s], nsamples[s])) return false;
+  }
+  return true;
+}
+
 /* Whole streams from host buffers: checks that out[s] has room for the stream's audio[s] bytes plus `extra`
- * (out_bytes[s] = their sum), stages the PCM in the thread's buffers and encodes the batch into t_ctx.out, stream s at
- * out_off[s].  Stereo input with right == NULL or right[s] == NULL encodes left[s] on both channels. */
-int encode_host_streams(Config* cfg, int nstreams, const int16_t* const* left, const int16_t* const* right,
+ * (out_bytes[s] = their sum), stages the PCM (Int16 or Float32) in the thread's buffers and encodes the batch into t_ctx.out,
+ * stream s at out_off[s].  Stereo input with right == NULL or right[s] == NULL encodes left[s] on both channels. */
+template <class T>
+int encode_host_streams(Config* cfg, int nstreams, const T* const* left, const T* const* right,
                         const int64_t* nsamples, const int64_t* cap, int extra, int64_t* out_bytes,
                         std::vector<int64_t>& out_off, std::vector<long long>& audio, RgJob* rg = nullptr) {
   const int nch = cfg->host.nch;
@@ -930,11 +1019,11 @@ int encode_host_streams(Config* cfg, int nstreams, const int16_t* const* left, c
   if (nstreams == 0) return MP3B200_OK;
   int rc = t_ctx.use(cfg->device);
   if (rc) return rc;
-  rc = t_ctx.pcm.fit((size_t)tot_samples + 8);
+  rc = staging_pcm<T>().fit((size_t)tot_samples + 8);
   if (rc) return rc;
   rc = t_ctx.out.fit((size_t)tot_bytes + 8);
   if (rc) return rc;
-  int16_t* d_pcm = t_ctx.pcm.p;
+  T* d_pcm = staging_pcm<T>().p;
   /* Upload in time slices on a copy stream; the psy analysis of a slice starts when it has landed, so only the first
    * slice's transfer is exposed.  Many small streams are uploaded whole (one slice): per-copy overhead would win. */
   PcmArrival arr;
@@ -944,10 +1033,10 @@ int encode_host_streams(Config* cfg, int nstreams, const int16_t* const* left, c
     for (int s = 0; s < nstreams; s++) {
       const int64_t lo = nsamples[s] * j / arr.chunks, hi = nsamples[s] * (j + 1) / arr.chunks;
       if (hi <= lo) continue;
-      CK(cudaMemcpyAsync(d_pcm + pcm_off[s] + lo, left[s] + lo, sizeof(int16_t) * (hi - lo), cudaMemcpyHostToDevice, t_ctx.up_st));
+      CK(cudaMemcpyAsync(d_pcm + pcm_off[s] + lo, left[s] + lo, sizeof(T) * (hi - lo), cudaMemcpyHostToDevice, t_ctx.up_st));
       if (nch == 2) {
-        const int16_t* r = (right && right[s]) ? right[s] : left[s];
-        CK(cudaMemcpyAsync(d_pcm + pcm_off[s] + nsamples[s] + lo, r + lo, sizeof(int16_t) * (hi - lo), cudaMemcpyHostToDevice, t_ctx.up_st));
+        const T* r = (right && right[s]) ? right[s] : left[s];
+        CK(cudaMemcpyAsync(d_pcm + pcm_off[s] + nsamples[s] + lo, r + lo, sizeof(T) * (hi - lo), cudaMemcpyHostToDevice, t_ctx.up_st));
       }
     }
     CK(cudaEventRecord(t_ctx.ready[j], t_ctx.up_st));
@@ -956,6 +1045,7 @@ int encode_host_streams(Config* cfg, int nstreams, const int16_t* const* left, c
   LaunchOpts o;
   o.arrival = &arr;
   o.rg = rg;
+  o.f32_in = sizeof(T) == sizeof(float);
   return launch_streams(cfg, sds, t_ctx.out.p, o);
 }
 
@@ -969,9 +1059,12 @@ int mp3b200_encode_streams_device(int channels, int samplerate, int kbps, int ns
   return mp3b200_encode_streams_device_ex(channels, samplerate, kbps, 0, nstreams, d_pcm, pcm_off, nsamples, d_out, out_off, timings_ms);
 }
 
-int mp3b200_encode_streams_device_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
-                                     const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
-                                     const int64_t* out_off, float* timings_ms) {
+}  // extern "C"
+
+namespace {
+template <class T>
+int encode_device(int channels, int samplerate, int kbps, int flags, int nstreams, const T* d_pcm, const int64_t* pcm_off,
+                  const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off, float* timings_ms) {
   if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
   Config* cfg;
   int rc = get_config(channels, samplerate, kbps, flags, &cfg);
@@ -981,7 +1074,42 @@ int mp3b200_encode_streams_device_ex(int channels, int samplerate, int kbps, int
   std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off, nsamples, out_off);
   LaunchOpts o;
   o.timings_ms = timings_ms;
+  o.f32_in = sizeof(T) == sizeof(float);
   return launch_streams(cfg, sds, d_out, o);
+}
+
+template <class T>
+int encode_host(int channels, int samplerate, int kbps, int flags, int nstreams, const T* const* left, const T* const* right,
+                const int64_t* nsamples, uint8_t* const* out, const int64_t* cap, int64_t* out_bytes) {
+  if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
+  Config* cfg;
+  int rc = get_config(channels, samplerate, kbps, flags, &cfg);
+  if (rc) return rc;
+  if constexpr (sizeof(T) == sizeof(float))
+    if (!streams_finite(cfg, nstreams, left, right, nsamples)) { g_err = "non-finite input sample"; return MP3B200_ERR_CONFIG; }
+  std::vector<int64_t> out_off;
+  std::vector<long long> audio;
+  rc = encode_host_streams(cfg, nstreams, left, right, nsamples, cap, 0, out_bytes, out_off, audio);
+  if (rc || nstreams == 0) return rc;
+  for (int s = 0; s < nstreams; s++)
+    if (cudaMemcpyAsync(out[s], t_ctx.out.p + out_off[s], (size_t)audio[s], cudaMemcpyDeviceToHost, t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
+  if (cudaStreamSynchronize(t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
+  return rc;
+}
+}  // namespace
+
+extern "C" {
+
+int mp3b200_encode_streams_device_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
+                                     const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
+                                     const int64_t* out_off, float* timings_ms) {
+  return encode_device(channels, samplerate, kbps, flags, nstreams, d_pcm, pcm_off, nsamples, d_out, out_off, timings_ms);
+}
+
+int mp3b200_encode_streams_device_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* d_pcm,
+                                      const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
+                                      const int64_t* out_off, float* timings_ms) {
+  return encode_device(channels, samplerate, kbps, flags, nstreams, d_pcm, pcm_off, nsamples, d_out, out_off, timings_ms);
 }
 
 int mp3b200_encode_streams(int channels, int samplerate, int kbps, int nstreams, const int16_t* const* left,
@@ -993,18 +1121,13 @@ int mp3b200_encode_streams(int channels, int samplerate, int kbps, int nstreams,
 int mp3b200_encode_streams_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
                               const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
                               const int64_t* cap, int64_t* out_bytes) {
-  if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
-  Config* cfg;
-  int rc = get_config(channels, samplerate, kbps, flags, &cfg);
-  if (rc) return rc;
-  std::vector<int64_t> out_off;
-  std::vector<long long> audio;
-  rc = encode_host_streams(cfg, nstreams, left, right, nsamples, cap, 0, out_bytes, out_off, audio);
-  if (rc || nstreams == 0) return rc;
-  for (int s = 0; s < nstreams; s++)
-    if (cudaMemcpyAsync(out[s], t_ctx.out.p + out_off[s], (size_t)audio[s], cudaMemcpyDeviceToHost, t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
-  if (cudaStreamSynchronize(t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
-  return rc;
+  return encode_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes);
+}
+
+int mp3b200_encode_streams_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* const* left,
+                               const float* const* right, const int64_t* nsamples, uint8_t* const* out,
+                               const int64_t* cap, int64_t* out_bytes) {
+  return encode_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes);
 }
 
 int mp3b200_debug_stages(int channels, int samplerate, int kbps, const int16_t* left, const int16_t* right,
@@ -1020,10 +1143,14 @@ int mp3b200_debug_stages(int channels, int samplerate, int kbps, const int16_t* 
   return mp3b200_debug_stages_ex(&t);
 }
 
-int mp3b200_debug_stages_ex(const mp3b200_debug_taps* tp) {
+}  // extern "C"
+
+namespace {
+/* mp3b200_debug_stages_ex with the input `left` / `right` (Int16 or Float32) instead of the struct's */
+template <class T>
+int debug_stages(const mp3b200_debug_taps* tp, const T* left, const T* right) {
   if (!tp || tp->size != (int32_t)sizeof(mp3b200_debug_taps)) { g_err = "mp3b200_debug_taps: size must be sizeof(mp3b200_debug_taps)"; return MP3B200_ERR_HANDLE; }
   const int channels = tp->channels;
-  const int16_t *left = tp->left, *right = tp->right;
   const int64_t nsamples = tp->nsamples;
   const int32_t* force_blocktype = tp->force_blocktype;
   float *xr = tp->xr, *en_l = tp->en_l, *thm_l = tp->thm_l, *en_s = tp->en_s, *thm_s = tp->thm_s;
@@ -1034,6 +1161,10 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* tp) {
   Config* cfg;
   int rc = get_config(channels, tp->samplerate, tp->kbps, tp->flags, &cfg);
   if (rc) return rc;
+  if constexpr (sizeof(T) == sizeof(float)) {
+    if (!right) right = left;
+    if (!streams_finite(cfg, 1, &left, &right, &nsamples)) { g_err = "non-finite input sample"; return MP3B200_ERR_CONFIG; }
+  }
   rc = t_ctx.use(cfg->device);
   if (rc) return rc;
   const int nch = cfg->host.nch;
@@ -1042,20 +1173,21 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* tp) {
   const long long F = frames_for(nsamples, G, cfg->rs.ratio), U = G * F;
   /* one whole stream, staged and encoded like a batch of host streams of one */
   const long long nbytes = bytes_of_frames(cfg->host, 0, F);
-  rc = t_ctx.pcm.fit((size_t)(nsamples * nch + 8));
+  rc = staging_pcm<T>().fit((size_t)(nsamples * nch + 8));
   if (rc) return rc;
   rc = t_ctx.out.fit((size_t)nbytes + 8);
   if (rc) return rc;
-  int16_t* d_pcm = t_ctx.pcm.p;
+  T* d_pcm = staging_pcm<T>().p;
   uint8_t* d_out = t_ctx.out.p;
-  CK(cudaMemcpyAsync(d_pcm, left, sizeof(int16_t) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
-  if (nch == 2) CK(cudaMemcpyAsync(d_pcm + nsamples, right, sizeof(int16_t) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
+  CK(cudaMemcpyAsync(d_pcm, left, sizeof(T) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
+  if (nch == 2) CK(cudaMemcpyAsync(d_pcm + nsamples, right, sizeof(T) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
   const int64_t zero = 0;
   std::vector<StreamDesc> sds = whole_streams(cfg, 1, d_pcm, &zero, &nsamples, &zero);
   const bool want_gi = ginfo || tp->scalefac || tp->subblock_gain;
   const bool want_prep = tp->xmin || tp->max_nonzero_coeff || tp->xrpow_max;
   const bool want_q = tp->scfsi || tp->old_value || tp->cur_step;
   LaunchOpts opts;
+  opts.f32_in = sizeof(T) == sizeof(float);
   opts.force_bt = force_blocktype;
   opts.stop_after_mdct = !(l3_enc || bytes_out || want_gi || want_prep || want_q);
   rc = launch_streams(cfg, sds, d_out, opts);
@@ -1144,39 +1276,71 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* tp) {
   return rc;
 }
 
-int mp3b200_debug_resample(int channels, int samplerate, int kbps, const int16_t* left, const int16_t* right, int64_t nsamples,
-                           float* y, int64_t ny) {
+template <class T>
+int debug_resample(int channels, int samplerate, int kbps, const T* left, const T* right, int64_t nsamples, float* y, int64_t ny) {
   if (nsamples < 0 || ny < 0 || (nsamples > 0 && !left) || (ny > 0 && !y)) { g_err = "bad buffers"; return MP3B200_ERR_HANDLE; }
   Config* cfg;
   int rc = get_config(channels, samplerate, kbps, MP3B200_RESAMPLE, &cfg);
   if (rc) return rc;
   if (cfg->rs.ratio == 1) { g_err = "this configuration does not resample"; return MP3B200_ERR_CONFIG; }
+  if (!right) right = left;
+  if constexpr (sizeof(T) == sizeof(float))
+    if (!streams_finite(cfg, 1, &left, &right, &nsamples)) { g_err = "non-finite input sample"; return MP3B200_ERR_CONFIG; }
   rc = t_ctx.use(cfg->device);
   if (rc) return rc;
   if (ny == 0) return 0;
   const int nch = cfg->host.nch;
-  rc = t_ctx.pcm.fit((size_t)(nsamples * nch + 8));
+  rc = staging_pcm<T>().fit((size_t)(nsamples * nch + 8));
   if (rc) return rc;
   rc = t_ctx.ws.rs_desc.fit(1);
   if (rc) return rc;
   rc = t_ctx.ws.rs_y.fit((size_t)(ny * nch));
   if (rc) return rc;
-  int16_t* d_pcm = t_ctx.pcm.p;
+  T* d_pcm = staging_pcm<T>().p;
   if (nsamples > 0) {
-    CK(cudaMemcpyAsync(d_pcm, left, sizeof(int16_t) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
-    if (nch == 2) CK(cudaMemcpyAsync(d_pcm + nsamples, right ? right : left, sizeof(int16_t) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
+    CK(cudaMemcpyAsync(d_pcm, left, sizeof(T) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
+    if (nch == 2) CK(cudaMemcpyAsync(d_pcm + nsamples, right, sizeof(T) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
+  }
+  StreamDesc sd;
+  memset(&sd, 0, sizeof sd);
+  sd.pcm[0] = reinterpret_cast<const int16_t*>(d_pcm);
+  sd.pcm[1] = reinterpret_cast<const int16_t*>(nch == 2 ? d_pcm + nsamples : d_pcm);
+  sd.pcm_end = nsamples;
+  if constexpr (sizeof(T) == sizeof(float)) {       /* the launch path's staging: Float32(x * scale) rows */
+    rc = t_ctx.ws.nonfinite.fit(1);
+    if (rc) return rc;
+    rc = stage_streams(cfg, &sd, 1);
+    if (rc) return rc;
   }
   ResampleDesc d;
-  d.x[0] = d_pcm; d.x[1] = nch == 2 ? d_pcm + nsamples : d_pcm; d.x_base = 0; d.x_end = nsamples;
+  d.x[0] = sd.pcm[0]; d.x[1] = sd.pcm[1]; d.x_base = 0; d.x_end = nsamples;
   d.y[0] = t_ctx.ws.rs_y.p; d.y[1] = d.y[0] + (nch == 2 ? ny : 0); d.y_base = 0; d.ny = ny;
   CK(cudaMemcpyAsync(t_ctx.ws.rs_desc.p, &d, sizeof d, cudaMemcpyHostToDevice, t_ctx.st));
-  k_resample<<<dim3((unsigned)((ny + RS_THREADS - 1) / RS_THREADS), nch, 1), RS_THREADS, 0, t_ctx.st>>>(
-      t_ctx.ws.rs_desc.p, cfg->rs.ratio, cfg->host.scale_applied, cfg->host.scale);
+  const dim3 grid((unsigned)((ny + RS_THREADS - 1) / RS_THREADS), nch, 1);
+  if constexpr (sizeof(T) == sizeof(float))
+    k_resample<float><<<grid, RS_THREADS, 0, t_ctx.st>>>(t_ctx.ws.rs_desc.p, cfg->rs.ratio, 0, cfg->host.scale);
+  else
+    k_resample<int16_t><<<grid, RS_THREADS, 0, t_ctx.st>>>(t_ctx.ws.rs_desc.p, cfg->rs.ratio, cfg->host.scale_applied, cfg->host.scale);
   g_launches++;
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(y, t_ctx.ws.rs_y.p, sizeof(float) * (size_t)(ny * nch), cudaMemcpyDeviceToHost, t_ctx.st));
   CK(cudaStreamSynchronize(t_ctx.st));
   return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int mp3b200_debug_stages_ex(const mp3b200_debug_taps* tp) { return debug_stages(tp, tp ? tp->left : nullptr, tp ? tp->right : nullptr); }
+int mp3b200_debug_stages_f32(const mp3b200_debug_taps* tp, const float* left, const float* right) { return debug_stages(tp, left, right); }
+
+int mp3b200_debug_resample(int channels, int samplerate, int kbps, const int16_t* left, const int16_t* right, int64_t nsamples,
+                           float* y, int64_t ny) {
+  return debug_resample(channels, samplerate, kbps, left, right, nsamples, y, ny);
+}
+int mp3b200_debug_resample_f32(int channels, int samplerate, int kbps, const float* left, const float* right, int64_t nsamples,
+                               float* y, int64_t ny) {
+  return debug_resample(channels, samplerate, kbps, left, right, nsamples, y, ny);
 }
 
 }  // extern "C"
@@ -1319,15 +1483,18 @@ int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int ns
 }  // extern "C"
 
 namespace {
-/* encode_streams_tagged_ex; `rg` (flags & MP3B200_REPLAYGAIN) receives the analysis */
-int encode_tagged(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
-                  const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out, const int64_t* cap,
+/* encode_streams_tagged_ex / _f32; `rg` (flags & MP3B200_REPLAYGAIN) receives the analysis */
+template <class T>
+int encode_tagged(int channels, int samplerate, int kbps, int flags, int nstreams, const T* const* left,
+                  const T* const* right, const int64_t* nsamples, uint8_t* const* out, const int64_t* cap,
                   int64_t* out_bytes, RgJob* rg) {
   if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
   if (flags & ~(MP3B200_RESAMPLE | MP3B200_REPLAYGAIN)) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
   Config* cfg;
   int rc = get_config(channels, samplerate, kbps, flags & MP3B200_RESAMPLE, &cfg);
   if (rc) return rc;
+  if constexpr (sizeof(T) == sizeof(float))
+    if (!streams_finite(cfg, nstreams, left, right, nsamples)) { g_err = "non-finite input sample"; return MP3B200_ERR_CONFIG; }
   Mp3TagParams p;
   if (mp3_tag_params(channels, samplerate, kbps, &p, cfg->flags) != 0) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
   const int tfs = p.fits ? p.frame_bytes : 0;
@@ -1374,9 +1541,13 @@ int encode_tagged(int channels, int samplerate, int kbps, int flags, int nstream
 
 extern "C" {
 
-int mp3b200_encode_streams_tagged_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
-                                     const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
-                                     const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db) {
+}  // extern "C"
+
+namespace {
+template <class T>
+int encode_tagged_rg(int channels, int samplerate, int kbps, int flags, int nstreams, const T* const* left, const T* const* right,
+                     const int64_t* nsamples, uint8_t* const* out, const int64_t* cap, int64_t* out_bytes, double* title_db,
+                     double* album_db) {
   RgJob job;
   const bool want = (flags & MP3B200_REPLAYGAIN) != 0;
   const int rc = encode_tagged(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, want ? &job : nullptr);
@@ -1385,6 +1556,20 @@ int mp3b200_encode_streams_tagged_ex(int channels, int samplerate, int kbps, int
   for (int s = 0; title_db && s < nstreams; s++) title_db[s] = ran ? job.title_db[s] : RG_NOT_ENOUGH_SAMPLES;
   if (album_db) *album_db = ran ? job.album_db : RG_NOT_ENOUGH_SAMPLES;
   return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int mp3b200_encode_streams_tagged_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
+                                     const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
+                                     const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db) {
+  return encode_tagged_rg(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, title_db, album_db);
+}
+int mp3b200_encode_streams_tagged_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* const* left,
+                                      const float* const* right, const int64_t* nsamples, uint8_t* const* out,
+                                      const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db) {
+  return encode_tagged_rg(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, title_db, album_db);
 }
 
 int mp3b200_lametag_build_ex(int channels, int samplerate, int kbps, int flags, int64_t nframes, int64_t music_bytes, int music_crc,
@@ -1402,9 +1587,12 @@ int mp3b200_lametag_build_ex(int channels, int samplerate, int kbps, int flags, 
   return n;
 }
 
-int mp3b200_debug_replaygain(int channels, int samplerate, int kbps, int flags, const int16_t* left, const int16_t* right,
-                             int64_t nsamples, double* win_sums, int32_t* win_idx, int64_t nwin_cap, int32_t* hist,
-                             double* title_db, int32_t* stats) {
+}  // extern "C"
+
+namespace {
+template <class T>
+int debug_replaygain(int channels, int samplerate, int kbps, int flags, const T* left, const T* right, int64_t nsamples,
+                     double* win_sums, int32_t* win_idx, int64_t nwin_cap, int32_t* hist, double* title_db, int32_t* stats) {
   if (nsamples < 0 || !left) return MP3B200_ERR_HANDLE;
   RgJob job;
   job.want_windows = true;
@@ -1414,7 +1602,7 @@ int mp3b200_debug_replaygain(int channels, int samplerate, int kbps, int flags, 
   if (tsz == 0) { g_err = "the tag does not fit: no ReplayGain"; return MP3B200_ERR_CONFIG; }
   std::vector<uint8_t> out((size_t)(bytes + tsz));
   uint8_t* outp = out.data();
-  const int16_t* r = right ? right : left;
+  const T* r = right ? right : left;
   const int64_t cap = bytes + tsz;
   int64_t ob = 0;
   const int rc = encode_tagged(channels, samplerate, kbps, (flags & MP3B200_RESAMPLE) | MP3B200_REPLAYGAIN, 1, &left, &r, &nsamples,
@@ -1429,6 +1617,20 @@ int mp3b200_debug_replaygain(int channels, int samplerate, int kbps, int flags, 
   if (title_db) *title_db = job.title_db[0];
   if (stats) { stats[0] = (int32_t)n; stats[1] = job.passes; stats[2] = job.reruns; memcpy(stats + 3, &job.ms, sizeof(float)); }
   return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int mp3b200_debug_replaygain(int channels, int samplerate, int kbps, int flags, const int16_t* left, const int16_t* right,
+                             int64_t nsamples, double* win_sums, int32_t* win_idx, int64_t nwin_cap, int32_t* hist,
+                             double* title_db, int32_t* stats) {
+  return debug_replaygain(channels, samplerate, kbps, flags, left, right, nsamples, win_sums, win_idx, nwin_cap, hist, title_db, stats);
+}
+int mp3b200_debug_replaygain_f32(int channels, int samplerate, int kbps, int flags, const float* left, const float* right,
+                                 int64_t nsamples, double* win_sums, int32_t* win_idx, int64_t nwin_cap, int32_t* hist,
+                                 double* title_db, int32_t* stats) {
+  return debug_replaygain(channels, samplerate, kbps, flags, left, right, nsamples, win_sums, win_idx, nwin_cap, hist, title_db, stats);
 }
 
 }  // extern "C"
