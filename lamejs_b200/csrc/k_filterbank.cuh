@@ -333,46 +333,25 @@ k_subband_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict
   const int scale_applied = T->scale_applied;
   const double scale = T->scale;
   const int span = 576 * (scount - 1) + 1055;
-  if constexpr (F32_PCM) {
-    const float* __restrict__ pbuf = reinterpret_cast<const float*>(sd.pcm[ch]);
-    const long long pbase = sd.pcm_base, pend = sd.pcm_end;
-#pragma unroll 1
-    for (int j0 = tid; j0 < span; j0 += FB_THREADS * 8) {
-      float v[8];
-#pragma unroll
-      for (int k = 0; k < 8; k++) {
-        const int j = j0 + k * FB_THREADS;
-        const long long i = lo + j;
-        v[k] = (j < span && i >= 0 && i < pend) ? __ldg(&pbuf[i - pbase]) : 0.0f;
-      }
-#pragma unroll
-      for (int k = 0; k < 8; k++) {
-        const int j = j0 + k * FB_THREADS;
-        if (j < span) pcm[fb_pad(j)] = (double)v[k];
-      }
-    }
-  } else {
-    /* 8 independent Int16 loads per thread in flight (one dependent load per iteration left this phase, a third of the
+  {
+    /* 8 independent loads per thread in flight (one dependent load per iteration left this phase, a third of the
      * kernel's samples in the round-2 profile, waiting for HBM latency) */
-    const int16_t* __restrict__ pbuf = sd.pcm[ch];
+    using Sample = pcm_sample_t<F32_PCM>;
+    const Sample* __restrict__ pbuf = static_cast<const Sample*>(sd.pcm[ch]);
     const long long pbase = sd.pcm_base, pend = sd.pcm_end;
 #pragma unroll 1
     for (int j0 = tid; j0 < span; j0 += FB_THREADS * 8) {
-      short v[8];
+      Sample v[8];
 #pragma unroll
       for (int k = 0; k < 8; k++) {
         const int j = j0 + k * FB_THREADS;
         const long long i = lo + j;
-        v[k] = (j < span && i >= 0 && i < pend) ? __ldg(&pbuf[i - pbase]) : (short)0;
+        v[k] = (j < span && i >= 0 && i < pend) ? __ldg(&pbuf[i - pbase]) : (Sample)0;
       }
 #pragma unroll
       for (int k = 0; k < 8; k++) {
         const int j = j0 + k * FB_THREADS;
-        if (j < span) {
-          double d = (double)(int)v[k];                /* load_pcm: Float32(Int16 * scale); unscaled: one conversion */
-          if (scale_applied) d = (double)(float)(d * scale);
-          pcm[fb_pad(j)] = d;
-        }
+        if (j < span) pcm[fb_pad(j)] = pcm_value(v[k], scale_applied, scale);
       }
     }
   }

@@ -227,44 +227,23 @@ k_psy_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ s
   const int scale_applied = T->scale_applied;
   const double scale = T->scale;
   const long long x0 = 576 * c - 224;                /* stream sample of bufPos */
-  if constexpr (F32_PCM) {
-    /* the resampler's Float32 output: scaled before the filter, widened without scaling */
-    const float* __restrict__ pbuf = reinterpret_cast<const float*>(sd.pcm[ch]);
+  {
+    /* all of a thread's loads in flight at once (they were one dependent HBM round trip per iteration) */
+    using Sample = pcm_sample_t<F32_PCM>;
+    const Sample* __restrict__ pbuf = static_cast<const Sample*>(sd.pcm[ch]);
     const long long pbase = sd.pcm_base, pend = sd.pcm_end;
     constexpr int NB = (1024 + PSY_THREADS - 1) / PSY_THREADS;
-    float v[NB];
+    Sample v[NB];
 #pragma unroll
     for (int k = 0; k < NB; k++) {
       const int j = tid + k * PSY_THREADS;
       const long long i = x0 + j;
-      v[k] = (j < 1024 && i >= 0 && i < pend) ? __ldg(&pbuf[i - pbase]) : 0.0f;
+      v[k] = (j < 1024 && i >= 0 && i < pend) ? __ldg(&pbuf[i - pbase]) : (Sample)0;
     }
 #pragma unroll
     for (int k = 0; k < NB; k++) {
       const int j = tid + k * PSY_THREADS;
-      if (j < 1024) xs[j] = (double)v[k];
-    }
-  } else {
-    /* all of a thread's Int16 loads in flight at once (they were one dependent HBM round trip per iteration) */
-    const int16_t* __restrict__ pbuf = sd.pcm[ch];
-    const long long pbase = sd.pcm_base, pend = sd.pcm_end;
-    constexpr int NB = (1024 + PSY_THREADS - 1) / PSY_THREADS;
-    short v[NB];
-#pragma unroll
-    for (int k = 0; k < NB; k++) {
-      const int j = tid + k * PSY_THREADS;
-      const long long i = x0 + j;
-      v[k] = (j < 1024 && i >= 0 && i < pend) ? __ldg(&pbuf[i - pbase]) : (short)0;
-    }
-#pragma unroll
-    for (int k = 0; k < NB; k++) {
-      const int j = tid + k * PSY_THREADS;
-      if (j < 1024) {
-        /* load_pcm: Float32(Int16 * scale); without a scale the Int16 widens to double in one conversion */
-        double d = (double)(int)v[k];
-        if (scale_applied) d = (double)(float)(d * scale);
-        xs[j] = d;
-      }
+      if (j < 1024) xs[j] = pcm_value(v[k], scale_applied, scale);
     }
   }
   __syncthreads();

@@ -8,6 +8,7 @@
 #define MP3B200_DEVICE_CUH
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 #include "mp3_config.h"
 #include "mp3_math.cuh"
 
@@ -33,7 +34,7 @@ enum { BT_NORM = 0, BT_START = 1, BT_SHORT = 2, BT_STOP = 3 };
 
 /* One stream (= one lamejs Mp3Encoder instance) inside a batch. */
 struct StreamDesc {
-  const int16_t* pcm[2];   /* device pointers to sample index `pcm_base` of each channel */
+  const void* pcm[2];      /* device pointers to sample index `pcm_base` of each channel (pcm_sample_t of the launch) */
   long long pcm_base;      /* stream sample index of pcm[ch][0] (history kept by streaming handles) */
   long long pcm_end;       /* samples with index >= pcm_end (and < 0) read as 0: lead-in and flush padding */
   int frame0;              /* first frame of this launch (absolute index within the stream) */
@@ -53,12 +54,16 @@ struct StreamDesc {
   int old_value[2], current_step[2];
 };
 
-/* scaled PCM sample exactly as lamejs holds it in mfbuf: Float32( Int16 * scale ) (Lame.js:1506-1560) */
-__device__ __forceinline__ float load_pcm(const StreamDesc& sd, int ch, long long i, int scale_applied, double scale) {
-  if (i < 0 || i >= sd.pcm_end) return 0.0f;
-  const float v = (float)sd.pcm[ch][i - sd.pcm_base];
-  return scale_applied ? (float)((double)v * scale) : v;
+/* The rows a launch's descriptors point at: the caller's Int16 samples, scale still to apply, or Float32 rows already
+ * scaled (k_stage_f32 / k_resample).  pcm_value gives the sample as lamejs holds it in mfbuf, Float32( Int16 * scale )
+ * (Lame.js:1506-1560), widened to double; unscaled Int16 widens in one conversion. */
+template <bool F32> using pcm_sample_t = std::conditional_t<F32, float, int16_t>;
+__device__ __forceinline__ double pcm_value(int16_t v, int scale_applied, double scale) {
+  double d = (double)(int)v;
+  if (scale_applied) d = (double)(float)(d * scale);
+  return d;
 }
+__device__ __forceinline__ double pcm_value(float v, int, double) { return (double)v; }
 
 /* padding bits: number of padded frames among frames 0..k  (Encoder.js:442-446 in closed form) */
 __device__ __host__ __forceinline__ long long pad_count(long long k, int frac, int sr) {

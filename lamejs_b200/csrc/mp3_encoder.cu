@@ -263,8 +263,7 @@ struct ThreadCtx {
   cudaEvent_t ev_rs[2] = {};              /* around k_resample */
   Workspace ws;
   int evq_pred[QE_COUNT] = {};
-  Buf<int16_t> pcm;                       /* staged PCM of host callers */
-  Buf<float> pcmf;                        /* the same for Float32 input */
+  Buf<uint8_t> pcm;                       /* staged PCM of host callers (Int16 or Float32 rows) */
   Buf<uint8_t> out;                       /* encoded bytes of host callers */
   Buf<uint8_t, true> pin;                 /* pinned host staging */
   Buf<long long> crc_ranges;              /* music CRC: [2][R] offsets / lengths */
@@ -281,7 +280,7 @@ struct ThreadCtx {
   void release() {
     if (device < 0) return;
     cudaSetDevice(device);
-    ws.release(); pcm.release(); pcmf.release(); out.release(); pin.release(); crc_ranges.release(); crc.release();
+    ws.release(); pcm.release(); out.release(); pin.release(); crc_ranges.release(); crc.release();
     rg_titles.release(); rg_piece.release(); rg_sum.release(); rg_gain.release(); rg_wstate.release(); rg_cstart.release();
     rg_end_a.release(); rg_end_b.release(); rg_carry.release(); rg_idx.release(); rg_hist.release(); rg_count.release();
     for (auto& e : ev_rg) if (e) { cudaEventDestroy(e); e = nullptr; }
@@ -357,18 +356,23 @@ struct LaunchOpts {
                                             sync, a non-finite sample makes the launch return MP3B200_ERR_CONFIG */
 };
 
+/* The rows the descriptors of a launch point at: the caller's Int16 samples, {false, host.scale_applied}, or Float32 rows
+ * already scaled by k_stage_f32 or k_resample, SCALED_F32.  The kernels that read them are instantiated for `f32`. */
+struct Rows { bool f32; int scale_applied; };
+constexpr Rows SCALED_F32 = {true, 0};
+
 /* One pipeline launch for the streams sds[0 .. S) (at most MP3_MAX_LAUNCH_STREAMS, unit / frame bases set, the workspace
  * large enough).  All launches go to the calling thread's stream (t_ctx.st), which first waits for whatever the caller
  * queued on the legacy default stream (torch and plain CUDA callers produce their device buffers there); with o.sync the
  * call returns after the stream has drained, so the results are visible to any stream afterwards. */
 int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, const LaunchOpts& o, const PcmArrival* arrival,
-                 Timings* tm) {
+                 Rows rows, Timings* tm) {
   cudaStream_t st = t_ctx.st;
   cudaEvent_t* ev = t_ctx.ev;
   Workspace& ws = t_ctx.ws;
 
   const int nch = cfg->host.nch;
-  const bool f32_pcm = cfg->rs.ratio > 1 || o.f32_in;   /* the streams read Float32 rows: the resampler's or the staged input */
+  const bool f32_pcm = rows.f32;
   int max_frames = 0;
   long long total_frames = 0;          /* rows actually used this launch (the workspace may be larger) */
   int scan_rows = 0;
@@ -535,7 +539,7 @@ int stage_streams(Config* cfg, StreamDesc* sds, int S) {
   long long tot = 0, max_n = 0;
   for (int i = 0; i < S; i++) {
     const long long n = sds[i].pcm_end > sds[i].pcm_base ? sds[i].pcm_end - sds[i].pcm_base : 0;
-    for (int c = 0; c < 2; c++) d[i].x[c] = reinterpret_cast<const float*>(sds[i].pcm[c]);
+    for (int c = 0; c < 2; c++) d[i].x[c] = static_cast<const float*>(sds[i].pcm[c]);
     d[i].n = n;
     tot += n * nch;
     max_n = n > max_n ? n : max_n;
@@ -548,7 +552,7 @@ int stage_streams(Config* cfg, StreamDesc* sds, int S) {
   for (int i = 0; i < S; i++) {
     d[i].y[0] = ws.st_y.p + off; d[i].y[1] = nch == 2 ? d[i].y[0] + d[i].n : d[i].y[0];
     off += d[i].n * nch;
-    for (int c = 0; c < 2; c++) sds[i].pcm[c] = reinterpret_cast<const int16_t*>(d[i].y[c]);
+    for (int c = 0; c < 2; c++) sds[i].pcm[c] = d[i].y[c];
   }
   cudaStream_t st = t_ctx.st;
   CK(cudaEventRecord(t_ctx.ev_in, cudaStreamLegacy));      /* the input may come from the legacy default stream */
@@ -564,12 +568,32 @@ int stage_streams(Config* cfg, StreamDesc* sds, int S) {
   return 0;
 }
 
-/* Resampled launches: the descriptors sds[0 .. S) hold the caller's input (Int16 at rs.in_rate, or staged Float32 rows; pcm_base / pcm_end count
+/* Queues k_resample for the S descriptors rd (uploaded here), whose input rows `in` describes; ev_rs[0 / 1] bracket the
+ * kernel (timing slot 14). */
+int queue_resample(const Config* cfg, const ResampleDesc* rd, int S, long long max_ny, Rows in) {
+  Workspace& ws = t_ctx.ws;
+  cudaStream_t st = t_ctx.st;
+  int rc = ws.rs_desc.fit((size_t)S);
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(ws.rs_desc.p, rd, sizeof(ResampleDesc) * S, cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(t_ctx.ev_rs[0], st));
+  if (max_ny > 0) {
+    dim3 grid((unsigned)((max_ny + RS_THREADS - 1) / RS_THREADS), cfg->host.nch, S);
+    if (in.f32) k_resample<float><<<grid, RS_THREADS, 0, st>>>(ws.rs_desc.p, cfg->rs.ratio, in.scale_applied, cfg->host.scale);
+    else k_resample<int16_t><<<grid, RS_THREADS, 0, st>>>(ws.rs_desc.p, cfg->rs.ratio, in.scale_applied, cfg->host.scale);
+    g_launches++;
+    DBG("k_resample");
+  }
+  CK(cudaEventRecord(t_ctx.ev_rs[1], st));
+  return 0;
+}
+
+/* Resampled launches: the descriptors sds[0 .. S) hold the caller's input as `in` describes (pcm_base / pcm_end count
  * input samples, and pcm_base is at most max(0, r * hist_base_at(frame0) - 16), the first input the outputs below read).
  * Queues k_resample for the outputs the streams' frames read -- from hist_base_at(frame0) up to the last output the input
  * reaches; later outputs are 0 -- into the workspace, and points the descriptors at them: from then on pcm_base / pcm_end
  * count outputs, and the stream reads like PCM at the output rate. */
-int resample_streams(Config* cfg, StreamDesc* sds, int S, bool f32_in) {
+int resample_streams(Config* cfg, StreamDesc* sds, int S, Rows in) {
   const int r = cfg->rs.ratio, nch = cfg->host.nch;
   Workspace& ws = t_ctx.ws;
   std::vector<ResampleDesc> rd((size_t)S);
@@ -587,32 +611,19 @@ int resample_streams(Config* cfg, StreamDesc* sds, int S, bool f32_in) {
     tot += d.ny * nch;
     max_ny = d.ny > max_ny ? d.ny : max_ny;
   }
-  int rc = ws.rs_desc.fit((size_t)S);
-  if (rc) return rc;
-  rc = ws.rs_y.fit((size_t)tot + 1);
+  int rc = ws.rs_y.fit((size_t)tot + 1);
   if (rc) return rc;
   long long off = 0;
   for (int i = 0; i < S; i++) {
     ResampleDesc& d = rd[i];
     d.y[0] = ws.rs_y.p + off; d.y[1] = nch == 2 ? d.y[0] + d.ny : d.y[0];
     off += d.ny * nch;
-    for (int c = 0; c < 2; c++) sds[i].pcm[c] = reinterpret_cast<const int16_t*>(d.y[c]);
+    for (int c = 0; c < 2; c++) sds[i].pcm[c] = d.y[c];
     sds[i].pcm_base = d.y_base; sds[i].pcm_end = d.y_base + d.ny;
   }
-  cudaStream_t st = t_ctx.st;
   CK(cudaEventRecord(t_ctx.ev_in, cudaStreamLegacy));      /* the input may come from the legacy default stream */
-  CK(cudaStreamWaitEvent(st, t_ctx.ev_in, 0));
-  CK(cudaMemcpyAsync(ws.rs_desc.p, rd.data(), sizeof(ResampleDesc) * S, cudaMemcpyHostToDevice, st));
-  CK(cudaEventRecord(t_ctx.ev_rs[0], st));
-  if (max_ny > 0) {
-    dim3 grid((unsigned)((max_ny + RS_THREADS - 1) / RS_THREADS), nch, S);
-    if (f32_in) k_resample<float><<<grid, RS_THREADS, 0, st>>>(ws.rs_desc.p, r, 0, cfg->host.scale);   /* staged: scaled */
-    else k_resample<int16_t><<<grid, RS_THREADS, 0, st>>>(ws.rs_desc.p, r, cfg->host.scale_applied, cfg->host.scale);
-    g_launches++;
-    DBG("k_resample");
-  }
-  CK(cudaEventRecord(t_ctx.ev_rs[1], st));
-  return 0;
+  CK(cudaStreamWaitEvent(t_ctx.st, t_ctx.ev_in, 0));
+  return queue_resample(cfg, rd.data(), S, max_ny, in);
 }
 
 /* ---- ReplayGain (lamejs findReplayGain; k_replaygain.cuh) ----
@@ -654,7 +665,7 @@ int rg_req_index(int sr) {
 
 /* queues pass 1 and the first RG_QUEUED_PASSES repair passes on t_ctx.rg_st, after the PCM (the upload slices in `arrival`,
  * or everything queued on t_ctx.st so far: uploads and the resampler) */
-int rg_queue(Config* cfg, const StreamDesc* sds, RgJob& job, const PcmArrival* arrival, bool f32_in) {
+int rg_queue(Config* cfg, const StreamDesc* sds, RgJob& job, const PcmArrival* arrival, Rows rows) {
   ThreadCtx& c = t_ctx;
   const int sr = cfg->host.samplerate, W = (sr + 19) / 20, nch = cfg->host.nch, req = rg_req_index(sr);
   if (req < 0) { g_err = "no ReplayGain filter for this rate"; return MP3B200_ERR_CONFIG; }
@@ -712,8 +723,8 @@ int rg_queue(Config* cfg, const StreamDesc* sds, RgJob& job, const PcmArrival* a
   CK(cudaMemsetAsync(c.rg_hist.p, 0, sizeof(int) * (size_t)(T + 1) * RG_HIST, st));
   CK(cudaMemsetAsync(c.rg_carry.p, 0, sizeof(RgCarry) * (size_t)(T + 1), st));
   RgParams& p = job.prm;
-  p.titles = c.rg_titles.p; p.nch = nch; p.W = W; p.req = req; p.f32 = cfg->rs.ratio > 1 || f32_in;
-  p.scale_applied = p.f32 ? 0 : cfg->host.scale_applied;   /* k_resample / k_stage_f32 already scaled their input */
+  p.titles = c.rg_titles.p; p.nch = nch; p.W = W; p.req = req; p.f32 = rows.f32;
+  p.scale_applied = rows.scale_applied;
   p.scale = cfg->host.scale;
   p.win_sum = c.rg_sum.p; p.win_state = c.rg_wstate.p; p.chunk_start = c.rg_cstart.p; p.end_in = c.rg_end_a.p; p.end_out = c.rg_end_b.p;
   p.done = c.rg_count.p; p.reruns = c.rg_count.p + 1; p.pass_changed = c.rg_count.p + 2;
@@ -834,20 +845,23 @@ int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, co
         for (int j = 0; j < arrival->chunks; j++) CK(cudaStreamWaitEvent(t_ctx.st, arrival->ready[j], 0));
       arrival = nullptr;
     }
+    Rows rows = {false, cfg->host.scale_applied};
     if (o.f32_in) {
       rc = stage_streams(cfg, group, n);
       if (rc) return rc;
+      rows = SCALED_F32;
     }
     if (resampled) {
-      rc = resample_streams(cfg, group, n, o.f32_in);
+      rc = resample_streams(cfg, group, n, rows);
       if (rc) return rc;
+      rows = SCALED_F32;
     }
     if (o.rg) {
-      rc = rg_queue(cfg, group, *o.rg, arrival, o.f32_in);
+      rc = rg_queue(cfg, group, *o.rg, arrival, rows);
       if (rc) return rc;
     }
     Timings tm;
-    rc = run_pipeline(cfg, group, n, d_out, o, arrival, &tm);
+    rc = run_pipeline(cfg, group, n, d_out, o, arrival, rows, &tm);
     if (rc) return rc;
     if (o.rg) {
       rc = rg_finish(cfg, *o.rg);
@@ -962,8 +976,8 @@ std::vector<StreamDesc> whole_streams(Config* cfg, int nstreams, const T* d_pcm,
     StreamDesc& sd = sds[s];
     memset(&sd, 0, sizeof sd);
     const T* x = d_pcm + pcm_off[s];
-    sd.pcm[0] = reinterpret_cast<const int16_t*>(x);
-    sd.pcm[1] = reinterpret_cast<const int16_t*>(cfg->host.nch == 2 ? x + nsamples[s] : x);
+    sd.pcm[0] = x;
+    sd.pcm[1] = cfg->host.nch == 2 ? x + nsamples[s] : x;
     sd.pcm_base = 0; sd.pcm_end = nsamples[s];
     sd.frame0 = 0; sd.nframes = (int)frames_for(nsamples[s], cfg->host.mode_gr, cfg->rs.ratio);
     sd.out_base = out_off[s];
@@ -972,13 +986,14 @@ std::vector<StreamDesc> whole_streams(Config* cfg, int nstreams, const T* d_pcm,
   return sds;
 }
 
-/* the thread's device buffer for host PCM of sample type T */
-template <class T> Buf<T>& staging_pcm();
-template <> Buf<int16_t>& staging_pcm<int16_t>() { return t_ctx.pcm; }
-template <> Buf<float>& staging_pcm<float>() { return t_ctx.pcmf; }
+/* the thread's device buffer for n samples of host PCM of type T; NULL (g_err set) when it cannot grow */
+template <class T> T* staging_pcm(size_t n) { return t_ctx.pcm.fit(sizeof(T) * n) ? nullptr : reinterpret_cast<T*>(t_ctx.pcm.p); }
+
+/* the right row of stream s: stereo input with right == NULL or right[s] == NULL encodes left[s] on both channels */
+template <class T> const T* right_row(const T* const* left, const T* const* right, int s) { return right && right[s] ? right[s] : left[s]; }
 
 /* Float32 input (lamejs's store and scale): true when every sample is finite, and stays finite once scaled like
- * k_stage_f32 scales it.  The host entry points refuse other input with MP3B200_ERR_CONFIG before anything runs. */
+ * k_stage_f32 scales it */
 bool finite_after_scale(const Mp3Tables& T, const float* x, long long n) {
   for (long long i = 0; i < n; i++) {
     float v = x[i];
@@ -987,12 +1002,17 @@ bool finite_after_scale(const Mp3Tables& T, const float* x, long long n) {
   }
   return true;
 }
-bool streams_finite(const Config* cfg, int nstreams, const float* const* left, const float* const* right, const int64_t* nsamples) {
-  for (int s = 0; s < nstreams; s++) {
-    if (!finite_after_scale(cfg->host, left[s], nsamples[s])) return false;
-    if (cfg->host.nch == 2 && right && right[s] && !finite_after_scale(cfg->host, right[s], nsamples[s])) return false;
-  }
-  return true;
+
+/* The input gate of the host entry points: the caller's rows are checked before anything runs, and refused with
+ * MP3B200_ERR_CONFIG.  Int16 rows always pass; Float32 rows must stay finite through lamejs's store and scale. */
+int check_input(const Config*, int, const int16_t* const*, const int16_t* const*, const int64_t*) { return MP3B200_OK; }
+int check_input(const Config* cfg, int nstreams, const float* const* left, const float* const* right, const int64_t* nsamples) {
+  for (int s = 0; s < nstreams; s++)
+    if (!finite_after_scale(cfg->host, left[s], nsamples[s]) ||
+        (cfg->host.nch == 2 && !finite_after_scale(cfg->host, right_row(left, right, s), nsamples[s]))) {
+      g_err = "non-finite input sample"; return MP3B200_ERR_CONFIG;
+    }
+  return MP3B200_OK;
 }
 
 /* Whole streams from host buffers: checks that out[s] has room for the stream's audio[s] bytes plus `extra`
@@ -1019,11 +1039,10 @@ int encode_host_streams(Config* cfg, int nstreams, const T* const* left, const T
   if (nstreams == 0) return MP3B200_OK;
   int rc = t_ctx.use(cfg->device);
   if (rc) return rc;
-  rc = staging_pcm<T>().fit((size_t)tot_samples + 8);
-  if (rc) return rc;
+  T* d_pcm = staging_pcm<T>((size_t)tot_samples + 8);
+  if (!d_pcm) return MP3B200_ERR_CUDA;
   rc = t_ctx.out.fit((size_t)tot_bytes + 8);
   if (rc) return rc;
-  T* d_pcm = staging_pcm<T>().p;
   /* Upload in time slices on a copy stream; the psy analysis of a slice starts when it has landed, so only the first
    * slice's transfer is exposed.  Many small streams are uploaded whole (one slice): per-copy overhead would win. */
   PcmArrival arr;
@@ -1034,10 +1053,9 @@ int encode_host_streams(Config* cfg, int nstreams, const T* const* left, const T
       const int64_t lo = nsamples[s] * j / arr.chunks, hi = nsamples[s] * (j + 1) / arr.chunks;
       if (hi <= lo) continue;
       CK(cudaMemcpyAsync(d_pcm + pcm_off[s] + lo, left[s] + lo, sizeof(T) * (hi - lo), cudaMemcpyHostToDevice, t_ctx.up_st));
-      if (nch == 2) {
-        const T* r = (right && right[s]) ? right[s] : left[s];
-        CK(cudaMemcpyAsync(d_pcm + pcm_off[s] + nsamples[s] + lo, r + lo, sizeof(T) * (hi - lo), cudaMemcpyHostToDevice, t_ctx.up_st));
-      }
+      if (nch == 2)
+        CK(cudaMemcpyAsync(d_pcm + pcm_off[s] + nsamples[s] + lo, right_row(left, right, s) + lo, sizeof(T) * (hi - lo),
+                           cudaMemcpyHostToDevice, t_ctx.up_st));
     }
     CK(cudaEventRecord(t_ctx.ready[j], t_ctx.up_st));
   }
@@ -1045,7 +1063,7 @@ int encode_host_streams(Config* cfg, int nstreams, const T* const* left, const T
   LaunchOpts o;
   o.arrival = &arr;
   o.rg = rg;
-  o.f32_in = sizeof(T) == sizeof(float);
+  o.f32_in = std::is_same_v<T, float>;
   return launch_streams(cfg, sds, t_ctx.out.p, o);
 }
 
@@ -1074,7 +1092,7 @@ int encode_device(int channels, int samplerate, int kbps, int flags, int nstream
   std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off, nsamples, out_off);
   LaunchOpts o;
   o.timings_ms = timings_ms;
-  o.f32_in = sizeof(T) == sizeof(float);
+  o.f32_in = std::is_same_v<T, float>;
   return launch_streams(cfg, sds, d_out, o);
 }
 
@@ -1084,9 +1102,7 @@ int encode_host(int channels, int samplerate, int kbps, int flags, int nstreams,
   if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
   Config* cfg;
   int rc = get_config(channels, samplerate, kbps, flags, &cfg);
-  if (rc) return rc;
-  if constexpr (sizeof(T) == sizeof(float))
-    if (!streams_finite(cfg, nstreams, left, right, nsamples)) { g_err = "non-finite input sample"; return MP3B200_ERR_CONFIG; }
+  if (rc || (rc = check_input(cfg, nstreams, left, right, nsamples))) return rc;
   std::vector<int64_t> out_off;
   std::vector<long long> audio;
   rc = encode_host_streams(cfg, nstreams, left, right, nsamples, cap, 0, out_bytes, out_off, audio);
@@ -1160,11 +1176,8 @@ int debug_stages(const mp3b200_debug_taps* tp, const T* left, const T* right) {
   const int64_t bytes_cap = tp->bytes_cap;
   Config* cfg;
   int rc = get_config(channels, tp->samplerate, tp->kbps, tp->flags, &cfg);
-  if (rc) return rc;
-  if constexpr (sizeof(T) == sizeof(float)) {
-    if (!right) right = left;
-    if (!streams_finite(cfg, 1, &left, &right, &nsamples)) { g_err = "non-finite input sample"; return MP3B200_ERR_CONFIG; }
-  }
+  if (rc || (rc = check_input(cfg, 1, &left, &right, &nsamples))) return rc;
+  if (!right) right = left;
   rc = t_ctx.use(cfg->device);
   if (rc) return rc;
   const int nch = cfg->host.nch;
@@ -1173,11 +1186,10 @@ int debug_stages(const mp3b200_debug_taps* tp, const T* left, const T* right) {
   const long long F = frames_for(nsamples, G, cfg->rs.ratio), U = G * F;
   /* one whole stream, staged and encoded like a batch of host streams of one */
   const long long nbytes = bytes_of_frames(cfg->host, 0, F);
-  rc = staging_pcm<T>().fit((size_t)(nsamples * nch + 8));
-  if (rc) return rc;
+  T* d_pcm = staging_pcm<T>((size_t)(nsamples * nch + 8));
+  if (!d_pcm) return MP3B200_ERR_CUDA;
   rc = t_ctx.out.fit((size_t)nbytes + 8);
   if (rc) return rc;
-  T* d_pcm = staging_pcm<T>().p;
   uint8_t* d_out = t_ctx.out.p;
   CK(cudaMemcpyAsync(d_pcm, left, sizeof(T) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
   if (nch == 2) CK(cudaMemcpyAsync(d_pcm + nsamples, right, sizeof(T) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
@@ -1187,7 +1199,7 @@ int debug_stages(const mp3b200_debug_taps* tp, const T* left, const T* right) {
   const bool want_prep = tp->xmin || tp->max_nonzero_coeff || tp->xrpow_max;
   const bool want_q = tp->scfsi || tp->old_value || tp->cur_step;
   LaunchOpts opts;
-  opts.f32_in = sizeof(T) == sizeof(float);
+  opts.f32_in = std::is_same_v<T, float>;
   opts.force_bt = force_blocktype;
   opts.stop_after_mdct = !(l3_enc || bytes_out || want_gi || want_prep || want_q);
   rc = launch_streams(cfg, sds, d_out, opts);
@@ -1283,45 +1295,38 @@ int debug_resample(int channels, int samplerate, int kbps, const T* left, const 
   int rc = get_config(channels, samplerate, kbps, MP3B200_RESAMPLE, &cfg);
   if (rc) return rc;
   if (cfg->rs.ratio == 1) { g_err = "this configuration does not resample"; return MP3B200_ERR_CONFIG; }
+  if ((rc = check_input(cfg, 1, &left, &right, &nsamples))) return rc;
   if (!right) right = left;
-  if constexpr (sizeof(T) == sizeof(float))
-    if (!streams_finite(cfg, 1, &left, &right, &nsamples)) { g_err = "non-finite input sample"; return MP3B200_ERR_CONFIG; }
   rc = t_ctx.use(cfg->device);
   if (rc) return rc;
   if (ny == 0) return 0;
   const int nch = cfg->host.nch;
-  rc = staging_pcm<T>().fit((size_t)(nsamples * nch + 8));
-  if (rc) return rc;
-  rc = t_ctx.ws.rs_desc.fit(1);
-  if (rc) return rc;
+  T* d_pcm = staging_pcm<T>((size_t)(nsamples * nch + 8));
+  if (!d_pcm) return MP3B200_ERR_CUDA;
   rc = t_ctx.ws.rs_y.fit((size_t)(ny * nch));
   if (rc) return rc;
-  T* d_pcm = staging_pcm<T>().p;
   if (nsamples > 0) {
     CK(cudaMemcpyAsync(d_pcm, left, sizeof(T) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
     if (nch == 2) CK(cudaMemcpyAsync(d_pcm + nsamples, right, sizeof(T) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
   }
   StreamDesc sd;
   memset(&sd, 0, sizeof sd);
-  sd.pcm[0] = reinterpret_cast<const int16_t*>(d_pcm);
-  sd.pcm[1] = reinterpret_cast<const int16_t*>(nch == 2 ? d_pcm + nsamples : d_pcm);
+  sd.pcm[0] = d_pcm;
+  sd.pcm[1] = nch == 2 ? d_pcm + nsamples : d_pcm;
   sd.pcm_end = nsamples;
-  if constexpr (sizeof(T) == sizeof(float)) {       /* the launch path's staging: Float32(x * scale) rows */
+  Rows rows = {false, cfg->host.scale_applied};
+  if (std::is_same_v<T, float>) {                   /* the launch path's staging: Float32(x * scale) rows */
     rc = t_ctx.ws.nonfinite.fit(1);
     if (rc) return rc;
     rc = stage_streams(cfg, &sd, 1);
     if (rc) return rc;
+    rows = SCALED_F32;
   }
   ResampleDesc d;
   d.x[0] = sd.pcm[0]; d.x[1] = sd.pcm[1]; d.x_base = 0; d.x_end = nsamples;
   d.y[0] = t_ctx.ws.rs_y.p; d.y[1] = d.y[0] + (nch == 2 ? ny : 0); d.y_base = 0; d.ny = ny;
-  CK(cudaMemcpyAsync(t_ctx.ws.rs_desc.p, &d, sizeof d, cudaMemcpyHostToDevice, t_ctx.st));
-  const dim3 grid((unsigned)((ny + RS_THREADS - 1) / RS_THREADS), nch, 1);
-  if constexpr (sizeof(T) == sizeof(float))
-    k_resample<float><<<grid, RS_THREADS, 0, t_ctx.st>>>(t_ctx.ws.rs_desc.p, cfg->rs.ratio, 0, cfg->host.scale);
-  else
-    k_resample<int16_t><<<grid, RS_THREADS, 0, t_ctx.st>>>(t_ctx.ws.rs_desc.p, cfg->rs.ratio, cfg->host.scale_applied, cfg->host.scale);
-  g_launches++;
+  rc = queue_resample(cfg, &d, 1, ny, rows);
+  if (rc) return rc;
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(y, t_ctx.ws.rs_y.p, sizeof(float) * (size_t)(ny * nch), cudaMemcpyDeviceToHost, t_ctx.st));
   CK(cudaStreamSynchronize(t_ctx.st));
@@ -1492,9 +1497,7 @@ int encode_tagged(int channels, int samplerate, int kbps, int flags, int nstream
   if (flags & ~(MP3B200_RESAMPLE | MP3B200_REPLAYGAIN)) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
   Config* cfg;
   int rc = get_config(channels, samplerate, kbps, flags & MP3B200_RESAMPLE, &cfg);
-  if (rc) return rc;
-  if constexpr (sizeof(T) == sizeof(float))
-    if (!streams_finite(cfg, nstreams, left, right, nsamples)) { g_err = "non-finite input sample"; return MP3B200_ERR_CONFIG; }
+  if (rc || (rc = check_input(cfg, nstreams, left, right, nsamples))) return rc;
   Mp3TagParams p;
   if (mp3_tag_params(channels, samplerate, kbps, &p, cfg->flags) != 0) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
   const int tfs = p.fits ? p.frame_bytes : 0;
@@ -1537,13 +1540,6 @@ int encode_tagged(int channels, int samplerate, int kbps, int flags, int nstream
   if (cudaStreamSynchronize(t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
   return rc;
 }
-}  // namespace
-
-extern "C" {
-
-}  // extern "C"
-
-namespace {
 template <class T>
 int encode_tagged_rg(int channels, int samplerate, int kbps, int flags, int nstreams, const T* const* left, const T* const* right,
                      const int64_t* nsamples, uint8_t* const* out, const int64_t* cap, int64_t* out_bytes, double* title_db,
@@ -1602,10 +1598,9 @@ int debug_replaygain(int channels, int samplerate, int kbps, int flags, const T*
   if (tsz == 0) { g_err = "the tag does not fit: no ReplayGain"; return MP3B200_ERR_CONFIG; }
   std::vector<uint8_t> out((size_t)(bytes + tsz));
   uint8_t* outp = out.data();
-  const T* r = right ? right : left;
   const int64_t cap = bytes + tsz;
   int64_t ob = 0;
-  const int rc = encode_tagged(channels, samplerate, kbps, (flags & MP3B200_RESAMPLE) | MP3B200_REPLAYGAIN, 1, &left, &r, &nsamples,
+  const int rc = encode_tagged(channels, samplerate, kbps, (flags & MP3B200_RESAMPLE) | MP3B200_REPLAYGAIN, 1, &left, &right, &nsamples,
                                &outp, &cap, &ob, &job);
   if (rc) return rc;
   const long long n = (long long)job.win_idx.size();

@@ -100,15 +100,34 @@ def lib():
     return L
 
 
-def _is_float(*arrays):
-    """True when any of the sample arrays holds floating-point values: they then go to the _f32 entry points, which take
-    them as lamejs's Float32Array store does (integer dtypes keep the Int16 path)"""
-    return any(a is not None and np.asarray(a).dtype.kind in "fc" for a in arrays)
+def _rows(lefts, rights=None):
+    """One call's sample rows as the C entry points take them: (lefts, rights, f32).  When any row holds floating-point
+    values all become Float32, rounded once from the caller's values (Math.fround), for the _f32 entry points, which take
+    them as lamejs's Float32Array store does; otherwise contiguous Int16.  A missing right row (rights None, or an entry
+    None) is its left row."""
+    rights = [None] * len(lefts) if rights is None else list(rights)
+    f32 = any(a is not None and np.asarray(a).dtype.kind in "fc" for a in (*lefts, *rights))
+    dt = np.float32 if f32 else np.int16
+    lefts = [np.ascontiguousarray(x, dtype=dt) for x in lefts]
+    return lefts, [l if r is None else np.ascontiguousarray(r, dtype=dt) for l, r in zip(lefts, rights)], f32
 
 
-def _samples(x, f32):
-    """contiguous Int16, or Float32 rounded once from the caller's values (Math.fround: round to nearest even)"""
-    return np.ascontiguousarray(x, dtype=np.float32 if f32 else np.int16)
+# each Int16 entry point and its Float32 twin, which takes the same arguments with Float32 rows
+_F32_TWIN = {
+    "mp3b200_encode": "mp3b200_encode_f32",
+    "mp3b200_encode_batch": "mp3b200_encode_batch_f32",
+    "mp3b200_seek": "mp3b200_seek_f32",
+    "mp3b200_encode_streams_ex": "mp3b200_encode_streams_f32",
+    "mp3b200_encode_streams_tagged_ex": "mp3b200_encode_streams_tagged_f32",
+    "mp3b200_encode_streams_device_ex": "mp3b200_encode_streams_device_f32",
+    "mp3b200_debug_resample": "mp3b200_debug_resample_f32",
+    "mp3b200_debug_replaygain": "mp3b200_debug_replaygain_f32",
+}
+
+
+def _entry(name, f32):
+    """the entry point `name`, or its Float32 twin"""
+    return getattr(lib(), _F32_TWIN[name] if f32 else name)
 
 
 def _check(rc):
@@ -306,15 +325,11 @@ class Mp3Encoder:
     def encodeBuffer(self, left, right=None):
         """Int16 samples, or floating-point samples (Float32Array / plain Array in lamejs: rounded to Float32 once and
         scaled like lamejs scales them; non-finite values are refused)"""
-        if self.channels == 1 or right is None:
-            right = left
-        f32 = _is_float(left, right)
-        left, right = _samples(left, f32), _samples(right, f32)
+        (left,), (right,), f32 = _rows([left], [None if self.channels == 1 else right])
         assert len(left) == len(right)
         cap = int(1.25 * len(left) + 7200) + self._tag_room     # index.js:114,124
         buf = np.empty(cap, dtype=np.uint8)
-        fn = self._L.mp3b200_encode_f32 if f32 else self._L.mp3b200_encode
-        n = _check(fn(self._h, left.ctypes.data, right.ctypes.data, len(left), buf.ctypes.data, cap))
+        n = _check(_entry("mp3b200_encode", f32)(self._h, left.ctypes.data, right.ctypes.data, len(left), buf.ctypes.data, cap))
         return buf[:n].tobytes()
 
     def flush(self):
@@ -340,12 +355,8 @@ class Mp3Encoder:
     def seek(self, frame, left_hist, right_hist=None):
         """fresh encoder -> frame `frame` of a stream with start-of-stream sequential state; *_hist = samples
         [max(0, frame*framesize-1104), frame*framesize+224)"""
-        if self.channels == 1 or right_hist is None:
-            right_hist = left_hist
-        f32 = _is_float(left_hist, right_hist)
-        left_hist, right_hist = _samples(left_hist, f32), _samples(right_hist, f32)
-        fn = self._L.mp3b200_seek_f32 if f32 else self._L.mp3b200_seek
-        _check(fn(self._h, int(frame), left_hist.ctypes.data, right_hist.ctypes.data, len(left_hist)))
+        (left_hist,), (right_hist,), f32 = _rows([left_hist], [None if self.channels == 1 else right_hist])
+        _check(_entry("mp3b200_seek", f32)(self._h, int(frame), left_hist.ctypes.data, right_hist.ctypes.data, len(left_hist)))
 
     def close(self):
         if self._h:
@@ -362,11 +373,8 @@ class Mp3Encoder:
 def encode_batch(encoders, lefts, rights=None):
     """encodeBuffer on many live Mp3Encoder objects of one configuration in ONE pipeline launch (SURVEY 8(b) batch row):
     returns [enc.encodeBuffer(l, r) for ...] byte strings."""
-    L = lib()
     S = len(encoders)
-    f32 = _is_float(*lefts, *(rights or []))
-    lefts = [_samples(x, f32) for x in lefts]
-    rights = lefts if rights is None else [_samples(x if x is not None else l, f32) for x, l in zip(rights, lefts)]
+    lefts, rights, f32 = _rows(lefts, rights)
     ns = np.array([len(x) for x in lefts], dtype=np.int32)
     caps = np.array([int(1.25 * n + 7200) for n in ns], dtype=np.int32)
     outs = [np.empty(int(c), dtype=np.uint8) for c in caps]
@@ -375,8 +383,7 @@ def encode_batch(encoders, lefts, rights=None):
     rp = (ctypes.c_void_p * S)(*[x.ctypes.data for x in rights])
     op = (ctypes.c_void_p * S)(*[x.ctypes.data for x in outs])
     got = np.zeros(S, dtype=np.int32)
-    fn = L.mp3b200_encode_batch_f32 if f32 else L.mp3b200_encode_batch
-    _check(fn(hp, lp, rp, ns.ctypes.data, op, caps.ctypes.data, S, got.ctypes.data))
+    _check(_entry("mp3b200_encode_batch", f32)(hp, lp, rp, ns.ctypes.data, op, caps.ctypes.data, S, got.ctypes.data))
     for g in got:
         _check(int(g))
     return [o[: int(g)].tobytes() for o, g in zip(outs, got)]
@@ -398,17 +405,13 @@ def flush_batch(encoders):
     return [o[: int(g)].tobytes() for o, g in zip(outs, got)]
 
 
-def _encode_host_streams(fn, channels, samplerate, kbps, lefts, rights, room, resample=False, fn_f32=None):
-    """Marshalling of the whole-stream host calls: out[s] has room for the stream's bytes plus `room`.  Floating-point
-    samples go to fn_f32 (the _f32 twin of fn, flags bound like fn's)."""
+def _encode_host_streams(name, flags, channels, samplerate, kbps, lefts, rights, room, resample, *tail):
+    """Marshalling of the whole-stream host calls `name` (an _ex entry point) and its Float32 twin: out[s] has room for
+    the stream's bytes plus `room`; `tail` are the arguments after out_bytes."""
     S = len(lefts)
     if S == 0:
         return []
-    f32 = _is_float(*lefts, *(rights if rights is not None and channels == 2 else []))
-    if f32:
-        fn = fn_f32
-    lefts = [_samples(x, f32) for x in lefts]
-    rights = lefts if (rights is None or channels == 1) else [_samples(x, f32) for x in rights]
+    lefts, rights, f32 = _rows(lefts, None if channels == 1 else rights)
     ns = np.array([len(x) for x in lefts], dtype=np.int64)
     nb = [stream_bytes(channels, samplerate, kbps, int(n), resample) for n in ns]
     if any(b < 0 for b in nb):
@@ -420,23 +423,16 @@ def _encode_host_streams(fn, channels, samplerate, kbps, lefts, rights, room, re
     op = (ctypes.c_void_p * S)(*[x.ctypes.data for x in outs])
     caps = np.array(nb, dtype=np.int64)
     got = np.zeros(S, dtype=np.int64)
-    _check(fn(channels, samplerate, kbps, S, lp, rp, ns.ctypes.data, op, caps.ctypes.data, got.ctypes.data))
+    _check(_entry(name, f32)(channels, samplerate, kbps, flags, S, lp, rp, ns.ctypes.data, op, caps.ctypes.data, got.ctypes.data,
+                             *tail))
     return [o[: int(g)].tobytes() for o, g in zip(outs, got)]
 
 
 def encode_streams(channels, samplerate, kbps, lefts, rights=None, resample=False):
     """Batch extension: encodeBuffer(whole stream) + flush() for many independent streams in one launch sequence.
     Host buffers in, list of bytes out.  resample=True: see Mp3Encoder."""
-    flags = RESAMPLE if resample else 0
-
-    def fn(ch, sr, kb, *args):
-        return lib().mp3b200_encode_streams_ex(ch, sr, kb, flags, *args)
-
-    def fn_f32(ch, sr, kb, *args):
-        return lib().mp3b200_encode_streams_f32(ch, sr, kb, flags, *args)
-    if resample:
-        return _encode_host_streams(fn, channels, samplerate, kbps, lefts, rights, 0, True, fn_f32)
-    return _encode_host_streams(lib().mp3b200_encode_streams, channels, samplerate, kbps, lefts, rights, 0, fn_f32=fn_f32)
+    return _encode_host_streams("mp3b200_encode_streams_ex", RESAMPLE if resample else 0, channels, samplerate, kbps, lefts,
+                                rights, 0, resample)
 
 
 def encode_streams_tagged(channels, samplerate, kbps, lefts, rights=None, resample=False):
@@ -444,10 +440,8 @@ def encode_streams_tagged(channels, samplerate, kbps, lefts, rights=None, resamp
     and byte counts, seek table, encoder delay / padding, CRC-16 of the audio bytes computed on the GPU).  resample=True:
     see Mp3Encoder."""
     if not resample:
-        def fn_f32(ch, sr, kb, *args):
-            return lib().mp3b200_encode_streams_tagged_f32(ch, sr, kb, 0, *args, None, None)
-        return _encode_host_streams(lib().mp3b200_encode_streams_tagged, channels, samplerate, kbps, lefts, rights,
-                                    lametag_size(channels, samplerate, kbps), fn_f32=fn_f32)
+        return _encode_host_streams("mp3b200_encode_streams_tagged_ex", 0, channels, samplerate, kbps, lefts, rights,
+                                    lametag_size(channels, samplerate, kbps), False, None, None)
     return encode_streams_replaygain(channels, samplerate, kbps, lefts, rights, resample=True, find_replay_gain=False)[0]
 
 
@@ -458,14 +452,9 @@ def encode_streams_replaygain(channels, samplerate, kbps, lefts, rights=None, re
     flags = (REPLAYGAIN if find_replay_gain else 0) | (RESAMPLE if resample else 0)
     title = np.zeros(max(len(lefts), 1), dtype=np.float64)
     album = ctypes.c_double(0.0)
-
-    def fn(ch, sr, kb, *args):
-        return lib().mp3b200_encode_streams_tagged_ex(ch, sr, kb, flags, *args, title.ctypes.data, ctypes.byref(album))
-
-    def fn_f32(ch, sr, kb, *args):
-        return lib().mp3b200_encode_streams_tagged_f32(ch, sr, kb, flags, *args, title.ctypes.data, ctypes.byref(album))
     room = lib().mp3b200_lametag_size_ex(channels, samplerate, kbps, RESAMPLE if resample else 0)
-    out = _encode_host_streams(fn, channels, samplerate, kbps, lefts, rights, max(room, 0), resample, fn_f32)
+    out = _encode_host_streams("mp3b200_encode_streams_tagged_ex", flags, channels, samplerate, kbps, lefts, rights, max(room, 0),
+                               resample, title.ctypes.data, ctypes.byref(album))
     return out, [float(t) for t in title[:len(lefts)]], float(album.value) if lefts else float(GAIN_NOT_ENOUGH_SAMPLES)
 
 
@@ -498,19 +487,16 @@ def debug_replaygain(channels, samplerate, kbps, left, right=None, resample=Fals
     """The ReplayGain analysis of one whole stream (encodeBuffer(all) + flush()) as the GPU ran it: dict with `sums`
     (float64 [windows][2]: lsum, rsum), `idx` (int32 [windows]), `hist` (int32 [12000]), `title_db`, `passes` (repair
     passes), `reruns` (chunks run again) and `ms` (the analysis's CUDA-event time)."""
-    L = lib()
-    right = left if (right is None or channels == 1) else right
-    f32 = _is_float(left, right)
-    left, right = _samples(left, f32), _samples(right, f32)
+    (left,), (right,), f32 = _rows([left], [None if channels == 1 else right])
     cap = len(left) // 400 + 64
     sums = np.zeros((cap, 2), dtype=np.float64)
     idx = np.zeros(cap, dtype=np.int32)
     hist = np.zeros(12000, dtype=np.int32)
     title = ctypes.c_double(0.0)
     stats = np.zeros(4, dtype=np.int32)
-    fn = L.mp3b200_debug_replaygain_f32 if f32 else L.mp3b200_debug_replaygain
-    _check(fn(channels, samplerate, kbps, RESAMPLE if resample else 0, left.ctypes.data, right.ctypes.data,
-              len(left), sums.ctypes.data, idx.ctypes.data, cap, hist.ctypes.data, ctypes.byref(title), stats.ctypes.data))
+    _check(_entry("mp3b200_debug_replaygain", f32)(channels, samplerate, kbps, RESAMPLE if resample else 0, left.ctypes.data,
+                                                   right.ctypes.data, len(left), sums.ctypes.data, idx.ctypes.data, cap,
+                                                   hist.ctypes.data, ctypes.byref(title), stats.ctypes.data))
     n = int(stats[0])
     assert n <= cap
     return {"sums": sums[:n].copy(), "idx": idx[:n].copy(), "hist": hist, "title_db": float(title.value), "passes": int(stats[1]),
@@ -531,30 +517,26 @@ def encode_streams_device(channels, samplerate, kbps, d_pcm_ptr, pcm_off, nsampl
     """Device-resident batch (raw device pointers as ints).  Returns the 16 timing slots of include/mp3b200.h (ms); with
     resample=True slot 14 is the resampler's time.  float32=True: d_pcm holds Float32 samples (a float32 torch tensor),
     encoded as lamejs encodes a Float32Array; a non-finite sample raises Mp3B200Error."""
-    L = lib()
     pcm_off = np.ascontiguousarray(pcm_off, dtype=np.int64)
     nsamples = np.ascontiguousarray(nsamples, dtype=np.int64)
     out_off = np.ascontiguousarray(out_off, dtype=np.int64)
     tm = np.zeros(16, dtype=np.float32)
-    fn = L.mp3b200_encode_streams_device_f32 if float32 else L.mp3b200_encode_streams_device_ex
-    _check(fn(channels, samplerate, kbps, RESAMPLE if resample else 0, len(nsamples), d_pcm_ptr,
-              pcm_off.ctypes.data, nsamples.ctypes.data, d_out_ptr, out_off.ctypes.data, tm.ctypes.data))
+    _check(_entry("mp3b200_encode_streams_device_ex", float32)(channels, samplerate, kbps, RESAMPLE if resample else 0, len(nsamples),
+                                                                d_pcm_ptr, pcm_off.ctypes.data, nsamples.ctypes.data, d_out_ptr,
+                                                                out_off.ctypes.data, tm.ctypes.data))
     return tm
 
 
 def debug_resample(channels, samplerate, kbps, left, right=None, ny=None):
     """k_resample's output for an input extended with zeros on both sides: float32 array [nch][ny] (default ny: every output
     the input reaches)."""
-    L = lib()
-    right = left if (right is None or channels == 1) else right
-    f32 = _is_float(left, right)
-    left, right = _samples(left, f32), _samples(right, f32)
+    (left,), (right,), f32 = _rows([left], [None if channels == 1 else right])
     r = samplerate // out_samplerate(channels, samplerate, kbps)
     if ny is None:
         ny = (len(left) + 15) // r + 1
     y = np.zeros((channels, ny), dtype=np.float32)
-    fn = L.mp3b200_debug_resample_f32 if f32 else L.mp3b200_debug_resample
-    _check(fn(channels, samplerate, kbps, left.ctypes.data, right.ctypes.data, len(left), y.ctypes.data, ny))
+    _check(_entry("mp3b200_debug_resample", f32)(channels, samplerate, kbps, left.ctypes.data, right.ctypes.data, len(left),
+                                                 y.ctypes.data, ny))
     return y
 
 
@@ -565,9 +547,7 @@ def debug_stages(channels, samplerate, kbps, left, right=None, force_blocktype=N
     also accepts the configurations lamejs resamples by an integer ratio: left / right are input samples, the taps are
     those of the output rate, after k_resample."""
     L = lib()
-    right = left if (right is None or channels == 1) else right
-    f32 = _is_float(left, right)
-    left, right = _samples(left, f32), _samples(right, f32)
+    (left,), (right,), f32 = _rows([left], [None if channels == 1 else right])
     n = len(left)
     F = stream_frames(n, channels, samplerate, kbps, resample)
     G = granules_per_frame(channels, samplerate, kbps, resample)
