@@ -222,37 +222,43 @@ void rs_filter(double resample_ratio, float* h) {
   for (int i = 0; i < MP3_RS_TAPS; i++) h[i] = (float)((double)h[i] / sum);
 }
 
-}  // namespace
-
-int mp3_out_samplerate(int channels, int samplerate, int kbps) {
-  if (channels != 1 && channels != 2) return 0;
+/* the low-pass optimum_bandwidth picks (Lame.js:838-885), before the output rate is known: it sees the UNSNAPPED kbps and the
+ * INPUT rate */
+double input_lowpass(int channels, int samplerate, int kbps) {
   double lowpass = kLowpassHz[ladder_index(kbps)];
   if (channels == 1) lowpass *= 1.5;
   double lp = (double)to_i32(lowpass);
   if (2 * lp > samplerate) lp = samplerate / 2.0;
-  return suggested_out_rate(to_i32(lp), samplerate);
+  return lp;
 }
 
-int mp3_build_tables(int channels, int samplerate, int kbps, Mp3Tables* t, int flags, Mp3Resample* rs) {
+}  // namespace
+
+int mp3_out_samplerate(int channels, int samplerate, int kbps) {
+  if (channels != 1 && channels != 2) return 0;
+  return suggested_out_rate(to_i32(input_lowpass(channels, samplerate, kbps)), samplerate);
+}
+
+int mp3_build_config(int channels, int samplerate, int kbps, int flags, Mp3Tables* t, Mp3Resample* rs, Mp3TagParams* tag) {
   memset(t, 0, sizeof *t);
-  if (rs) { memset(rs, 0, sizeof *rs); rs->in_rate = samplerate; rs->ratio = 1; }
+  memset(rs, 0, sizeof *rs);
+  memset(tag, 0, sizeof *tag);
+  rs->in_rate = samplerate;
+  rs->ratio = 1;
   if (channels != 1 && channels != 2) return -1;
   t->nch = channels;
   t->mono = channels == 1;
 
   /* ---- rate / bandwidth decisions (Lame.js:838-896, 1044-1061) ---- */
-  const int ladder_raw = ladder_index(kbps);          /* optimum_bandwidth sees the UNSNAPPED kbps and the INPUT rate */
-  double lowpass = kLowpassHz[ladder_raw];
-  if (t->mono) lowpass *= 1.5;
-  double lp = (double)to_i32(lowpass);
-  if (2 * lp > samplerate) lp = samplerate / 2.0;
+  double lp = input_lowpass(channels, samplerate, kbps);
   const int out_rate = suggested_out_rate(to_i32(lp), samplerate);
   lp = dmin(20500, lp);
   lp = dmin(out_rate / 2.0, lp);
   if (out_rate != samplerate) {                        /* fill_buffer_resample */
     const double ratio = (double)samplerate / out_rate;
     if (!(flags & 1) || !(fabs(ratio - floor(.5 + ratio)) < .0001)) return -1;   /* intratio (Lame.js:1735) */
-    if (rs) { rs->ratio = samplerate / out_rate; rs_filter(ratio, rs->h); }
+    rs->ratio = samplerate / out_rate;
+    rs_filter(ratio, rs->h);
     samplerate = out_rate;                             /* everything below is at the rate lamejs encodes at */
   }
   switch (samplerate) {                                /* SmpFrqIndex (Lame.js:369-402) */
@@ -531,37 +537,23 @@ int mp3_build_tables(int channels, int samplerate, int kbps, Mp3Tables* t, int f
     }
     t->tw_off[4] = off;
   }
-  return 0;
-}
 
-/* The tag's view of a configuration: lowpassfreq as lame_init_params leaves it (Lame.js:838-896), the preset's safejoint
- * bit (Presets.js:262-263), and the "non optimal settings" rule of putLameVBR (VBRTag.js:722-731), which for Mp3Encoder
- * reduces to: reservoir disabled below 320 kbps, or a source rate of 32 kHz and below. */
-int mp3_tag_params(int channels, int samplerate, int kbps, Mp3TagParams* p, int flags) {
-  memset(p, 0, sizeof *p);
-  Mp3Tables* t = new Mp3Tables();
-  const int rc = mp3_build_tables(channels, samplerate, kbps, t, flags);
-  if (rc == 0) {
-    /* with resampling, the low-pass and the source-rate fields see the input rate, the rest the output rate */
-    p->version = t->version; p->mpeg25 = t->mpeg25; p->samplerate = t->samplerate; p->kbps = t->kbps; p->mono = t->mono;
-    p->bitrate_index = t->bitrate_index; p->samplerate_index = t->samplerate_index; p->sideinfo_len = t->sideinfo_len;
-    p->frame_bytes = t->frame_bytes_nopad;
-    p->fits = p->frame_bytes >= p->sideinfo_len + 156 && p->frame_bytes <= 2880;
-    double lowpass = kLowpassHz[ladder_index(kbps)];            /* the unsnapped rate, like mp3_build_tables */
-    if (t->mono) lowpass *= 1.5;
-    double lp = (double)to_i32(lowpass);
-    if (2 * lp > samplerate) lp = samplerate / 2.0;
-    lp = dmin(20500, lp);
-    lp = dmin(t->samplerate / 2.0, lp);
-    const double lb = lp / 100.0 + .5;
-    p->lowpass_byte = to_i32(lb > 255 ? 255 : lb);
-    p->quality_byte = 100 - 10 * 4 - 3;
-    const Preset& ps = kPresets[ladder_index(t->kbps)];
-    p->flags_byte = 4 + (1 << 4) + ((ps.safejoint ? 1 : 0) << 5);
-    const int source_class = samplerate <= 32000 ? 0 : samplerate == 48000 ? 2 : samplerate > 48000 ? 3 : 1;
-    const int non_optimal = (t->kbps < 320 || samplerate <= 32000) ? 1 : 0;
-    p->misc_byte = t->noise_shaping + ((t->mono ? 0 : 1) << 2) + (non_optimal << 5) + (source_class << 6);
-  }
-  delete t;
-  return rc;
+  /* ---- the tag's fields (VBRTag.js:281-364, 558-802) ----
+   * lowpassfreq as lame_init_params leaves it, the preset's safejoint bit (Presets.js:262-263), and the "non optimal
+   * settings" rule of putLameVBR (VBRTag.js:722-731), which for Mp3Encoder reduces to: reservoir disabled below 320 kbps, or
+   * a source rate of 32 kHz and below.  With resampling, the low-pass and the source-rate fields see the input rate, the
+   * rest the output rate. */
+  tag->version = t->version; tag->mpeg25 = t->mpeg25; tag->samplerate = t->samplerate; tag->kbps = t->kbps; tag->mono = t->mono;
+  tag->bitrate_index = t->bitrate_index; tag->samplerate_index = t->samplerate_index; tag->sideinfo_len = t->sideinfo_len;
+  tag->frame_bytes = t->frame_bytes_nopad;
+  tag->fits = tag->frame_bytes >= tag->sideinfo_len + 156 && tag->frame_bytes <= 2880;
+  const double lb = lp / 100.0 + .5;
+  tag->lowpass_byte = to_i32(lb > 255 ? 255 : lb);
+  tag->quality_byte = 100 - 10 * 4 - 3;
+  tag->flags_byte = 4 + (1 << 4) + ((ps.safejoint ? 1 : 0) << 5);
+  const int in_rate = rs->in_rate;
+  const int source_class = in_rate <= 32000 ? 0 : in_rate == 48000 ? 2 : in_rate > 48000 ? 3 : 1;
+  const int non_optimal = (t->kbps < 320 || in_rate <= 32000) ? 1 : 0;
+  tag->misc_byte = t->noise_shaping + ((t->mono ? 0 : 1) << 2) + (non_optimal << 5) + (source_class << 6);
+  return 0;
 }

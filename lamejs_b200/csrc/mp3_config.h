@@ -105,7 +105,6 @@ struct Mp3TagParams {
   int flags_byte;                 /* ATHtype | nspsytune << 4 | safejoint << 5 */
   int misc_byte;                  /* noise_shaping | stereo mode << 2 | non-optimal << 5 | source rate class << 6 */
 };
-int mp3_tag_params(int channels, int samplerate, int kbps, Mp3TagParams* p, int flags = 0);
 
 /* lamejs's resampler for an integer rate ratio r = in / out (fill_buffer_resample, Lame.js:1719-1843): one 33-tap filter,
  * output m = Float32(sum_i (double)h[i] * x[r m - 16 + i]) over the (scaled) input x, zero before 0 and past the end. */
@@ -120,9 +119,10 @@ struct Mp3Resample {
 /* the output rate lame_init_params picks (Lame.js:285-364), or 0 for a channel count lamejs cannot take */
 int mp3_out_samplerate(int channels, int samplerate, int kbps);
 
-/* returns 0, or -1 when lamejs itself would fail or would resample (out_samplerate != samplerate).  With flags &
+/* Derives everything about the caller's (channels, samplerate, kbps) in one pass: the tables, the resampler and the tag's
+ * fields.  Returns 0, or -1 when lamejs itself would fail or would resample (out_samplerate != samplerate).  With flags &
  * MP3B200_RESAMPLE a configuration whose output rate divides the input rate (|ratio - round(ratio)| < 1e-4, lamejs's own
- * test) is also accepted: the tables are then those of the output rate and `rs` (if given) receives the filter. */
-int mp3_build_tables(int channels, int samplerate, int kbps, Mp3Tables* t, int flags = 0, Mp3Resample* rs = nullptr);
+ * test) is also accepted: the tables are then those of the output rate and `rs` holds the filter. */
+int mp3_build_config(int channels, int samplerate, int kbps, int flags, Mp3Tables* t, Mp3Resample* rs, Mp3TagParams* tag);
 
 #endif

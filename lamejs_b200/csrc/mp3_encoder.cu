@@ -50,18 +50,46 @@ bool g_fb_attr_done[MP3_MAX_DEVICES][2] = {};   /* k_subband_analysis<false / tr
     }                                                                                             \
   } while (0)
 
-/* host.samplerate is the rate lamejs encodes at; with resampling (rs.ratio > 1) the caller's samples arrive at rs.in_rate
- * and k_resample turns them into samples at host.samplerate on the device */
-struct Config { Mp3Tables host; Mp3Tables* dev; int device; int flags, kbps_asked; Mp3Resample rs; };
-std::map<std::tuple<int, int, int, int, int>, Config*> g_configs;   /* (device, ch, sr, kbps, flags) */
-struct ByteGeom { int frame_bytes_nopad, frac_SpF, mode_gr, samplerate, ratio; };
-std::map<std::tuple<int, int, int, int>, ByteGeom> g_byte_geom;   /* (ch, sr, kbps, flags) -> byte geometry; frame_bytes_nopad < 0: unsupported */
+/* One configuration as mp3_build_config derives it from the caller's (channels, samplerate, kbps, flags), built once on the
+ * host.  host.samplerate is the rate lamejs encodes at; with resampling (rs.ratio > 1) the caller's samples arrive at
+ * rs.in_rate and k_resample turns them into samples at host.samplerate on the device.  dev[d] is the tables' copy on device
+ * d, uploaded by get_config on first use there. */
+struct Config {
+  Mp3Tables host;
+  Mp3Resample rs;
+  Mp3TagParams tag;
+  bool encodable;                         /* rs.ratio <= RS_MAX_RATIO; the tag entry points describe the others too */
+  Mp3Tables* dev[MP3_MAX_DEVICES];
+};
+std::map<std::tuple<int, int, int, int>, Config*> g_configs;   /* (ch, sr, kbps, flags) -> NULL: lamejs cannot encode it */
 
-/* the flags that select a configuration: MP3B200_RESAMPLE only matters where lamejs resamples, so a flagged configuration
- * that encodes at its input rate is the unflagged one.  -1: unknown flag bits. */
-int config_flags(int ch, int sr, int kbps, int flags) {
-  if (flags & ~MP3B200_RESAMPLE) return -1;
-  return (flags & MP3B200_RESAMPLE) && mp3_out_samplerate(ch, sr, kbps) != sr ? MP3B200_RESAMPLE : 0;
+/* g_mu held.  The configuration, built on first use, or NULL (g_err set) when lamejs cannot encode it.  MP3B200_RESAMPLE only
+ * matters where lamejs resamples, so a flagged configuration that encodes at its input rate is the unflagged one. */
+Config* find_config(int ch, int sr, int kbps, int flags) {
+  if (flags & ~MP3B200_RESAMPLE) { g_err = "unknown flags"; return nullptr; }
+  if (flags && mp3_out_samplerate(ch, sr, kbps) == sr) flags = 0;
+  const auto key = std::make_tuple(ch, sr, kbps, flags);
+  auto it = g_configs.find(key);
+  if (it == g_configs.end()) {
+    Config* c = new Config();
+    if (mp3_build_config(ch, sr, kbps, flags, &c->host, &c->rs, &c->tag) == 0) c->encodable = c->rs.ratio <= RS_MAX_RATIO;
+    else { delete c; c = nullptr; }
+    it = g_configs.emplace(key, c).first;
+  }
+  if (!it->second) g_err = "unsupported configuration";
+  return it->second;
+}
+
+/* find_config for the entry points that need no device */
+const Config* host_config(int ch, int sr, int kbps, int flags) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return find_config(ch, sr, kbps, flags);
+}
+
+/* the same for the entry points that size an encode: NULL also where k_resample cannot take the ratio */
+const Config* encodable_config(int ch, int sr, int kbps, int flags) {
+  const Config* c = host_config(ch, sr, kbps, flags);
+  return c && c->encodable ? c : nullptr;
 }
 
 /* g_mu held.  Makes `dev` current for the calling thread and uploads the constant tables once per device. */
@@ -83,30 +111,6 @@ int ensure_device(int dev) {
     if (rc) return rc;
     g_consts_ready[dev] = true;
   }
-  return 0;
-}
-
-int get_config(int ch, int sr, int kbps, int flags, Config** out) {
-  flags = config_flags(ch, sr, kbps, flags);
-  if (flags < 0) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
-  std::lock_guard<std::mutex> lk(g_mu);
-  const int dev = g_device;
-  int rc = ensure_device(dev);
-  if (rc) return rc;
-  auto key = std::make_tuple(dev, ch, sr, kbps, flags);
-  auto it = g_configs.find(key);
-  if (it != g_configs.end()) { *out = it->second; return 0; }
-  Config* c = new Config();
-  if (mp3_build_tables(ch, sr, kbps, &c->host, flags, &c->rs) != 0 || c->rs.ratio > RS_MAX_RATIO) {
-    delete c; g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG;
-  }
-  c->device = dev; c->flags = flags; c->kbps_asked = kbps;
-  if (c->rs.ratio > 1)     /* the ratio's filter row (the same taps for every configuration of that ratio) */
-    CK(cudaMemcpyToSymbol(c_rs_h, c->rs.h, sizeof(float) * MP3_RS_TAPS, sizeof(float) * MP3_RS_TAPS * c->rs.ratio));
-  CK(cudaMalloc(&c->dev, sizeof(Mp3Tables)));
-  CK(cudaMemcpy(c->dev, &c->host, sizeof(Mp3Tables), cudaMemcpyHostToDevice));
-  g_configs[key] = c;
-  *out = c;
   return 0;
 }
 
@@ -181,8 +185,8 @@ long long frames_for(long long n, int mode_gr, int ratio = 1) {
   return fed + f.flush().frames;
 }
 
-/* bytes of frames k0 .. k0 + n - 1 of a stream (g: Mp3Tables or ByteGeom): frame k is padded when pad_count steps at k */
-template <class Geom> long long bytes_of_frames(const Geom& g, long long k0, long long n) {
+/* bytes of frames k0 .. k0 + n - 1 of a stream: frame k is padded when pad_count steps at k */
+long long bytes_of_frames(const Mp3Tables& g, long long k0, long long n) {
   return n * g.frame_bytes_nopad + pad_count(k0 + n - 1, g.frac_SpF, g.samplerate) - pad_count(k0 - 1, g.frac_SpF, g.samplerate);
 }
 
@@ -324,6 +328,31 @@ struct ThreadCtx {
 };
 thread_local ThreadCtx t_ctx;
 
+/* The configuration for a launch on the current device (g_device): uploads its tables there on first use and binds the
+ * calling thread's context (t_ctx) to that device, so cfg->dev[t_ctx.device] holds them. */
+int get_config(int ch, int sr, int kbps, int flags, Config** out) {
+  if (flags & ~MP3B200_RESAMPLE) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
+  int dev = 0;
+  {
+    std::lock_guard<std::mutex> lk(g_mu);
+    dev = g_device;
+    int rc = ensure_device(dev);
+    if (rc) return rc;
+    Config* c = find_config(ch, sr, kbps, flags);
+    if (!c || !c->encodable) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
+    if (!c->dev[dev]) {
+      if (c->rs.ratio > 1)     /* the ratio's filter row (the same taps for every configuration of that ratio) */
+        CK(cudaMemcpyToSymbol(c_rs_h, c->rs.h, sizeof(float) * MP3_RS_TAPS, sizeof(float) * MP3_RS_TAPS * c->rs.ratio));
+      Mp3Tables* d = nullptr;
+      CK(cudaMalloc(&d, sizeof(Mp3Tables)));
+      CK(cudaMemcpy(d, &c->host, sizeof(Mp3Tables), cudaMemcpyHostToDevice));
+      c->dev[dev] = d;
+    }
+    *out = c;
+  }
+  return t_ctx.use(dev);
+}
+
 /* MP3B200_DEBUG_SYNC=1: synchronise after every launch and name the failing kernel */
 bool debug_sync() { static int v = -1; if (v < 0) { const char* e = getenv("MP3B200_DEBUG_SYNC"); v = (e && e[0] == '1') ? 1 : 0; } return v == 1; }
 #define DBG(name)                                                                           \
@@ -371,6 +400,7 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
   cudaEvent_t* ev = t_ctx.ev;
   Workspace& ws = t_ctx.ws;
 
+  const Mp3Tables* const tab = cfg->dev[t_ctx.device];
   const int nch = cfg->host.nch;
   const bool f32_pcm = rows.f32;
   int max_frames = 0;
@@ -416,8 +446,8 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
       if (arrival) CK(cudaStreamWaitEvent(st, arrival->ready[j], 0));
       if (u_hi[j] <= u_lo[j]) continue;
       dim3 gridj(u_hi[j] - u_lo[j], nch, S);
-      if (f32_pcm) k_psy_analysis<true><<<gridj, PSY_THREADS, 0, st>>>(cfg->dev, ws.streams.p, ws.psy.p, j, nchunks, u_lo[j]);
-      else k_psy_analysis<false><<<gridj, PSY_THREADS, 0, st>>>(cfg->dev, ws.streams.p, ws.psy.p, j, nchunks, u_lo[j]);
+      if (f32_pcm) k_psy_analysis<true><<<gridj, PSY_THREADS, 0, st>>>(tab, ws.streams.p, ws.psy.p, j, nchunks, u_lo[j]);
+      else k_psy_analysis<false><<<gridj, PSY_THREADS, 0, st>>>(tab, ws.streams.p, ws.psy.p, j, nchunks, u_lo[j]);
       g_launches++;
       DBG("k_psy_analysis");
     }
@@ -426,9 +456,9 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
   /* K3a: attack pre-pass (parallel) + sequential per-stream scans */
   {
     dim3 grid((cfg->host.mode_gr * max_frames + 127) / 128, 1, S);
-    k_attack_prepass<<<grid, 128, 0, st>>>(cfg->dev, ws.streams.p, ws.psy.p, ws.scan_in.p);
+    k_attack_prepass<<<grid, 128, 0, st>>>(tab, ws.streams.p, ws.psy.p, ws.scan_in.p);
     DBG("k_attack_prepass");
-    k_stream_scan<<<S, SCAN_THREADS, 0, st>>>(cfg->dev, ws.streams.p, S, ws.scan_in.p, ws.bt_final.p, ws.bt_prev.p, ws.ath_psy.p, ws.ath_q.p, ws.scan.p);
+    k_stream_scan<<<S, SCAN_THREADS, 0, st>>>(tab, ws.streams.p, S, ws.scan_in.p, ws.bt_final.p, ws.bt_prev.p, ws.ath_psy.p, ws.ath_q.p, ws.scan.p);
     g_launches += 2;
     DBG("k_stream_scan");
     /* K1a: subband analysis, programmatic dependent of the scan (reads nothing the scan writes; see k_stream_scan) */
@@ -438,7 +468,7 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
       void (*const k_fb)(const Mp3Tables*, const StreamDesc*, float*) = f32_pcm ? k_subband_analysis<true> : k_subband_analysis<false>;
       {
         std::lock_guard<std::mutex> lk(g_mu);   /* the attribute is per device */
-        if (!g_fb_attr_done[cfg->device][f32_pcm]) { CK(cudaFuncSetAttribute(k_fb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); g_fb_attr_done[cfg->device][f32_pcm] = true; }
+        if (!g_fb_attr_done[t_ctx.device][f32_pcm]) { CK(cudaFuncSetAttribute(k_fb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); g_fb_attr_done[t_ctx.device][f32_pcm] = true; }
       }
       cudaLaunchConfig_t lc = {};
       lc.gridDim = dim3((G * max_frames + 1 + FB_SLABS - 1) / FB_SLABS, nch, S);
@@ -447,7 +477,7 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
       at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
       at[0].val.programmaticStreamSerializationAllowed = 1;
       lc.attrs = at; lc.numAttrs = 1;
-      CK(cudaLaunchKernelEx(&lc, k_fb, (const Mp3Tables*)cfg->dev, (const StreamDesc*)ws.streams.p, ws.slab.p));
+      CK(cudaLaunchKernelEx(&lc, k_fb, tab, (const StreamDesc*)ws.streams.p, ws.slab.p));
       g_launches++;
       DBG("k_subband_analysis");
     }
@@ -464,7 +494,7 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
   /* K3b: masking thresholds */
   {
     dim3 grid(cfg->host.mode_gr * max_frames + 1, 1, S);
-    k_psy_masking<<<grid, MASK_THREADS, 0, st>>>(cfg->dev, ws.streams.p, ws.psy.p, ws.bt_prev.p, ws.ath_psy.p, ws.ratio.p);
+    k_psy_masking<<<grid, MASK_THREADS, 0, st>>>(tab, ws.streams.p, ws.psy.p, ws.bt_prev.p, ws.ath_psy.p, ws.ratio.p);
     g_launches++;
     DBG("k_psy_masking");
   }
@@ -473,7 +503,7 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
    * it saves only a few microseconds for the pair -- not worth losing the per-kernel times.) */
   {
     dim3 grid((cfg->host.mode_gr * max_frames + FB_G - 1) / FB_G, nch, S);
-    k_mdct<<<grid, FB_G * 32, 0, st>>>(cfg->dev, ws.streams.p, ws.slab.p, ws.bt_final.p, ws.xr.p);
+    k_mdct<<<grid, FB_G * 32, 0, st>>>(tab, ws.streams.p, ws.slab.p, ws.bt_final.p, ws.xr.p);
     g_launches++;
     DBG("k_mdct");
   }
@@ -483,7 +513,7 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
     QuantBuffers qb;
     qb.xr = ws.xr.p; qb.ratio = ws.ratio.p; qb.bt = ws.bt_final.p; qb.ath_q = ws.ath_q.p; qb.qs = ws.qstate.p; qb.ginfo = ws.ginfo.p;
     qb.l3enc = ws.l3enc.p; qb.xrq = ws.xrq.p; qb.xrpow = ws.xrpow.p; qb.neg = ws.neg.p; qb.prep = ws.prep.p; qb.list = ws.dirty.p; qb.counter = ws.counter.p;
-    int rc = quant_run(cfg->dev, cfg->host, ws.streams.p, S, streams_with_frames, max_frames, total_frames, qb, d_out, st, t_ctx.aux_st, t_ctx.ev_fork, t_ctx.ev_join, ev[5], t_ctx.evq, t_ctx.evq_pred, &passes, &g_launches);
+    int rc = quant_run(tab, cfg->host, ws.streams.p, S, streams_with_frames, max_frames, total_frames, qb, d_out, st, t_ctx.aux_st, t_ctx.ev_fork, t_ctx.ev_join, ev[5], t_ctx.evq, t_ctx.evq_pred, &passes, &g_launches);
     if (rc) { g_err = "quantizer stage failed: " + std::string(cudaGetErrorString(cudaGetLastError())); return rc; }
   } else {
     CK(cudaEventRecord(ev[5], st));
@@ -912,34 +942,14 @@ int mp3b200_set_device(int device) {
 
 int64_t mp3b200_stream_frames(int64_t nsamples) { return frames_for(nsamples, 2); }
 
-namespace {
-/* the byte geometry of a configuration is three integers; building the full tables costs ~1 ms, so it is done once */
-ByteGeom byte_geom(int channels, int samplerate, int kbps, int flags = 0) {
-  flags = config_flags(channels, samplerate, kbps, flags);
-  if (flags < 0) return ByteGeom{-1, 0, 2, samplerate, 1};
-  std::lock_guard<std::mutex> lk(g_mu);
-  auto key = std::make_tuple(channels, samplerate, kbps, flags);
-  auto it = g_byte_geom.find(key);
-  if (it != g_byte_geom.end()) return it->second;
-  Mp3Tables* t = new Mp3Tables();
-  Mp3Resample rs;
-  const int rc = mp3_build_tables(channels, samplerate, kbps, t, flags, &rs);
-  ByteGeom g = rc == 0 && rs.ratio <= RS_MAX_RATIO ? ByteGeom{t->frame_bytes_nopad, t->frac_SpF, t->mode_gr, t->samplerate, rs.ratio}
-                                                   : ByteGeom{-1, 0, 2, samplerate, 1};
-  delete t;
-  g_byte_geom[key] = g;
-  return g;
-}
-}  // namespace
-
 int64_t mp3b200_stream_bytes(int channels, int samplerate, int kbps, int64_t nsamples) {
   return mp3b200_stream_bytes_ex(channels, samplerate, kbps, 0, nsamples);
 }
 
 int64_t mp3b200_stream_bytes_ex(int channels, int samplerate, int kbps, int flags, int64_t nsamples) {
-  const ByteGeom g = byte_geom(channels, samplerate, kbps, flags);
-  if (g.frame_bytes_nopad < 0 || nsamples < 0) return -1;
-  return bytes_of_frames(g, 0, frames_for(nsamples, g.mode_gr, g.ratio));
+  const Config* c = encodable_config(channels, samplerate, kbps, flags);
+  if (!c || nsamples < 0) return -1;
+  return bytes_of_frames(c->host, 0, frames_for(nsamples, c->host.mode_gr, c->rs.ratio));
 }
 
 int64_t mp3b200_stream_frames_cfg(int channels, int samplerate, int kbps, int64_t nsamples) {
@@ -947,9 +957,9 @@ int64_t mp3b200_stream_frames_cfg(int channels, int samplerate, int kbps, int64_
 }
 
 int64_t mp3b200_stream_frames_ex(int channels, int samplerate, int kbps, int flags, int64_t nsamples) {
-  const ByteGeom g = byte_geom(channels, samplerate, kbps, flags);
-  if (g.frame_bytes_nopad < 0 || nsamples < 0) return -1;
-  return frames_for(nsamples, g.mode_gr, g.ratio);
+  const Config* c = encodable_config(channels, samplerate, kbps, flags);
+  if (!c || nsamples < 0) return -1;
+  return frames_for(nsamples, c->host.mode_gr, c->rs.ratio);
 }
 
 int mp3b200_granules_per_frame(int channels, int samplerate, int kbps) {
@@ -957,8 +967,8 @@ int mp3b200_granules_per_frame(int channels, int samplerate, int kbps) {
 }
 
 int mp3b200_granules_per_frame_ex(int channels, int samplerate, int kbps, int flags) {
-  const ByteGeom g = byte_geom(channels, samplerate, kbps, flags);
-  return g.frame_bytes_nopad < 0 ? -1 : g.mode_gr;
+  const Config* c = encodable_config(channels, samplerate, kbps, flags);
+  return c ? c->host.mode_gr : -1;
 }
 
 int mp3b200_out_samplerate(int channels, int samplerate, int kbps) { return mp3_out_samplerate(channels, samplerate, kbps); }
@@ -1037,11 +1047,9 @@ int encode_host_streams(Config* cfg, int nstreams, const T* const* left, const T
     tot_bytes += audio[s];
   }
   if (nstreams == 0) return MP3B200_OK;
-  int rc = t_ctx.use(cfg->device);
-  if (rc) return rc;
   T* d_pcm = staging_pcm<T>((size_t)tot_samples + 8);
   if (!d_pcm) return MP3B200_ERR_CUDA;
-  rc = t_ctx.out.fit((size_t)tot_bytes + 8);
+  int rc = t_ctx.out.fit((size_t)tot_bytes + 8);
   if (rc) return rc;
   /* Upload in time slices on a copy stream; the psy analysis of a slice starts when it has landed, so only the first
    * slice's transfer is exposed.  Many small streams are uploaded whole (one slice): per-copy overhead would win. */
@@ -1085,9 +1093,7 @@ int encode_device(int channels, int samplerate, int kbps, int flags, int nstream
                   const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off, float* timings_ms) {
   if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
   Config* cfg;
-  int rc = get_config(channels, samplerate, kbps, flags, &cfg);
-  if (rc) return rc;
-  rc = t_ctx.use(cfg->device);
+  const int rc = get_config(channels, samplerate, kbps, flags, &cfg);
   if (rc) return rc;
   std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off, nsamples, out_off);
   LaunchOpts o;
@@ -1178,8 +1184,6 @@ int debug_stages(const mp3b200_debug_taps* tp, const T* left, const T* right) {
   int rc = get_config(channels, tp->samplerate, tp->kbps, tp->flags, &cfg);
   if (rc || (rc = check_input(cfg, 1, &left, &right, &nsamples))) return rc;
   if (!right) right = left;
-  rc = t_ctx.use(cfg->device);
-  if (rc) return rc;
   const int nch = cfg->host.nch;
   const int G = cfg->host.mode_gr;
   /* nsamples are the caller's (input) samples; frames and granules are those of the rate the configuration encodes at */
@@ -1297,8 +1301,6 @@ int debug_resample(int channels, int samplerate, int kbps, const T* left, const 
   if (cfg->rs.ratio == 1) { g_err = "this configuration does not resample"; return MP3B200_ERR_CONFIG; }
   if ((rc = check_input(cfg, 1, &left, &right, &nsamples))) return rc;
   if (!right) right = left;
-  rc = t_ctx.use(cfg->device);
-  if (rc) return rc;
   if (ny == 0) return 0;
   const int nch = cfg->host.nch;
   T* d_pcm = staging_pcm<T>((size_t)(nsamples * nch + 8));
@@ -1400,6 +1402,22 @@ int music_crc_ranges(int device, const uint8_t* d_buf, const std::vector<long lo
   CK(cudaGetLastError());
   return 0;
 }
+
+/* mp3b200_lametag_build(_ex): `field` is the tag's Radio Replay Gain field, 0 for a stream nobody analysed */
+int build_lametag(int channels, int samplerate, int kbps, int flags, int64_t nframes, int64_t music_bytes, int music_crc,
+                  int encoder_padding, int field, uint8_t* buf, int cap) {
+  const Config* c = host_config(channels, samplerate, kbps, flags);
+  if (!c) return MP3B200_ERR_CONFIG;
+  const Mp3TagParams& p = c->tag;
+  if (!p.fits || nframes <= 0) return 0;
+  if (!buf || cap < p.frame_bytes) return p.frame_bytes;              /* like getLameTagFrame: the size it needs */
+  Mp3SeekBag* bag = new Mp3SeekBag();
+  bag->reset();
+  bag->add_frames(nframes, p.kbps);
+  const int n = mp3_tag_frame(p, *bag, music_bytes, (unsigned)music_crc, encoder_padding, buf, field);
+  delete bag;
+  return n;
+}
 }  // namespace
 
 extern "C" {
@@ -1458,24 +1476,14 @@ int mp3b200_lametag_size(int channels, int samplerate, int kbps) {
 }
 
 int mp3b200_lametag_size_ex(int channels, int samplerate, int kbps, int flags) {
-  flags = config_flags(channels, samplerate, kbps, flags);
-  Mp3TagParams p;
-  if (flags < 0 || mp3_tag_params(channels, samplerate, kbps, &p, flags) != 0) return MP3B200_ERR_CONFIG;
-  return p.fits ? p.frame_bytes : 0;
+  const Config* c = host_config(channels, samplerate, kbps, flags);
+  if (!c) return MP3B200_ERR_CONFIG;
+  return c->tag.fits ? c->tag.frame_bytes : 0;
 }
 
 int mp3b200_lametag_build(int channels, int samplerate, int kbps, int64_t nframes, int64_t music_bytes, int music_crc, int encoder_padding,
                           uint8_t* buf, int cap) {
-  Mp3TagParams p;
-  if (mp3_tag_params(channels, samplerate, kbps, &p) != 0) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
-  if (!p.fits || nframes <= 0) return 0;
-  if (!buf || cap < p.frame_bytes) return p.frame_bytes;              /* like getLameTagFrame: the size it needs */
-  Mp3SeekBag* bag = new Mp3SeekBag();
-  bag->reset();
-  bag->add_frames(nframes, p.kbps);
-  const int n = mp3_tag_frame(p, *bag, music_bytes, (unsigned)music_crc, encoder_padding, buf);
-  delete bag;
-  return n;
+  return build_lametag(channels, samplerate, kbps, 0, nframes, music_bytes, music_crc, encoder_padding, 0, buf, cap);
 }
 
 int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int nstreams, const int16_t* const* left,
@@ -1498,8 +1506,7 @@ int encode_tagged(int channels, int samplerate, int kbps, int flags, int nstream
   Config* cfg;
   int rc = get_config(channels, samplerate, kbps, flags & MP3B200_RESAMPLE, &cfg);
   if (rc || (rc = check_input(cfg, nstreams, left, right, nsamples))) return rc;
-  Mp3TagParams p;
-  if (mp3_tag_params(channels, samplerate, kbps, &p, cfg->flags) != 0) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
+  const Mp3TagParams& p = cfg->tag;
   const int tfs = p.fits ? p.frame_bytes : 0;
   if (rg && tfs == 0) rg = nullptr;               /* lamejs analyses only when the tag is written (Lame.js:911-916) */
   if (rg) {
@@ -1519,7 +1526,7 @@ int encode_tagged(int channels, int samplerate, int kbps, int flags, int nstream
   /* the music CRC of every stream, where the bytes are */
   std::vector<long long> off(out_off.begin(), out_off.end());
   std::vector<unsigned> crc;
-  rc = music_crc_ranges(cfg->device, t_ctx.out.p, off, audio, crc);
+  rc = music_crc_ranges(t_ctx.device, t_ctx.out.p, off, audio, crc);
   if (rc) return rc;
   Mp3SeekBag* bag = new Mp3SeekBag();
   for (int s = 0; s < nstreams; s++) {
@@ -1570,17 +1577,8 @@ int mp3b200_encode_streams_tagged_f32(int channels, int samplerate, int kbps, in
 
 int mp3b200_lametag_build_ex(int channels, int samplerate, int kbps, int flags, int64_t nframes, int64_t music_bytes, int music_crc,
                              int encoder_padding, int radio_gain, uint8_t* buf, int cap) {
-  flags = config_flags(channels, samplerate, kbps, flags);
-  Mp3TagParams p;
-  if (flags < 0 || mp3_tag_params(channels, samplerate, kbps, &p, flags) != 0) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
-  if (!p.fits || nframes <= 0) return 0;
-  if (!buf || cap < p.frame_bytes) return p.frame_bytes;
-  Mp3SeekBag* bag = new Mp3SeekBag();
-  bag->reset();
-  bag->add_frames(nframes, p.kbps);
-  const int n = mp3_tag_frame(p, *bag, music_bytes, (unsigned)music_crc, encoder_padding, buf, mp3_radio_gain_field(radio_gain));
-  delete bag;
-  return n;
+  return build_lametag(channels, samplerate, kbps, flags, nframes, music_bytes, music_crc, encoder_padding,
+                       mp3_radio_gain_field(radio_gain), buf, cap);
 }
 
 }  // extern "C"
@@ -1592,13 +1590,12 @@ int debug_replaygain(int channels, int samplerate, int kbps, int flags, const T*
   if (nsamples < 0 || !left) return MP3B200_ERR_HANDLE;
   RgJob job;
   job.want_windows = true;
-  const int64_t bytes = mp3b200_stream_bytes_ex(channels, samplerate, kbps, flags & MP3B200_RESAMPLE, nsamples);
-  const int tsz = mp3b200_lametag_size_ex(channels, samplerate, kbps, flags & MP3B200_RESAMPLE);
-  if (bytes < 0 || tsz < 0) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
-  if (tsz == 0) { g_err = "the tag does not fit: no ReplayGain"; return MP3B200_ERR_CONFIG; }
-  std::vector<uint8_t> out((size_t)(bytes + tsz));
+  const Config* c = encodable_config(channels, samplerate, kbps, flags & MP3B200_RESAMPLE);
+  if (!c) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
+  if (!c->tag.fits) { g_err = "the tag does not fit: no ReplayGain"; return MP3B200_ERR_CONFIG; }
+  const int64_t cap = bytes_of_frames(c->host, 0, frames_for(nsamples, c->host.mode_gr, c->rs.ratio)) + c->tag.frame_bytes;
+  std::vector<uint8_t> out((size_t)cap);
   uint8_t* outp = out.data();
-  const int64_t cap = bytes + tsz;
   int64_t ob = 0;
   const int rc = encode_tagged(channels, samplerate, kbps, (flags & MP3B200_RESAMPLE) | MP3B200_REPLAYGAIN, 1, &left, &right, &nsamples,
                                &outp, &cap, &ob, &job);

@@ -183,7 +183,8 @@ def test_entry_points_reject_bad_arguments_without_a_device():
     assert L.mp3b200_music_crc(None) == -1 and L.mp3b200_bytes_written(None) == -1
 
 
-@pytest.mark.parametrize("ch,sr,kbps", [(2, 44100, 130), (2, 44100, 120), (1, 44100, 100), (2, 48000, 300), (1, 32000, 70), (2, 24000, 50), (1, 16000, 60), (2, 48000, 1000)])
+@pytest.mark.parametrize("ch,sr,kbps", [(2, 44100, 130), (2, 44100, 120), (1, 44100, 100), (2, 48000, 300), (1, 32000, 70), (2, 24000, 50), (1, 16000, 60), (2, 48000, 1000),
+                                        (1, 44100, 72), (1, 32000, 52), (2, 12000, 36), (2, 8000, 28), (2, 44100, 104)])
 def test_tag_frame_with_bitrates_off_the_ladder(oracle, ch, sr, kbps):
     """kbps is snapped like FindNearestBitrate, but the low-pass (a tag field) comes from the rate as given (Lame.js:838-885 runs
     before :1053): the tag must follow both"""

@@ -43,7 +43,10 @@ def test_crc_kernel_on_device_buffers(M, oracle, torch_cuda):
 
 @pytest.mark.parametrize("kind,ch,sr,kbps,frames,chunk", [
     ("noise", 2, 44100, 128, 40, 1152), ("burst", 2, 48000, 320, 30, 0), ("octave", 1, 32000, 64, 25, 777),
-    ("noise", 2, 24000, 64, 50, 1152), ("noise", 1, 8000, 24, 40, 576), ("sweep", 2, 44100, 192, 450, 5000)])
+    ("noise", 2, 24000, 64, 50, 1152), ("noise", 1, 8000, 24, 40, 576), ("sweep", 2, 44100, 192, 450, 5000),
+    # off the bitrate ladder: the tag's low-pass comes from the rate as given, the frames from the snapped one
+    ("noise", 1, 44100, 72, 30, 1152), ("octave", 1, 32000, 52, 25, 777), ("noise", 2, 12000, 36, 40, 576),
+    ("sweep", 2, 8000, 28, 40, 0), ("burst", 2, 44100, 104, 30, 5000)])
 def test_tagged_handle_matches_oracle(M, oracle, kind, ch, sr, kbps, frames, chunk):
     fs = 1152 if sr >= 32000 else 576
     l, r = make_signal(kind, frames * fs + 77, sr, seed=9)
@@ -74,12 +77,14 @@ def test_tagged_handle_matches_oracle(M, oracle, kind, ch, sr, kbps, frames, chu
 
 
 def test_tag_refused_and_tag_off(M, oracle):
-    l, _ = make_signal("noise", 20 * 576, 8000, seed=4)
-    enc = M.Mp3Encoder(1, 8000, 8, write_vbr_tag=True)            # 72-byte frames: InitVbrTag switches the tag off
-    assert not enc.tag_on
-    got = enc.encodeBuffer(l) + enc.flush()
-    assert got == oracle.encode_stream(1, 8000, 8, l, None)[0] and enc.lametag_frame() == b"" and enc.music_crc() == -1
-    enc.close()
+    # 72- and 52-byte frames: InitVbrTag switches the tag off (at 12 kbps the snapped 8 kbps alone would make lamejs resample)
+    for sr, kbps in ((8000, 8), (11025, 12)):
+        l, _ = make_signal("noise", 20 * 576, sr, seed=4)
+        enc = M.Mp3Encoder(1, sr, kbps, write_vbr_tag=True)
+        assert not enc.tag_on
+        got = enc.encodeBuffer(l) + enc.flush()
+        assert got == oracle.encode_stream(1, sr, kbps, l, None)[0] and enc.lametag_frame() == b"" and enc.music_crc() == -1
+        enc.close()
     e2 = M.Mp3Encoder(2, 44100, 128)                              # ordinary encoder: accumulators idle, nothing prefixed
     l, r = make_signal("noise", 5 * 1152, 44100, seed=5)
     assert e2.encodeBuffer(l, r) + e2.flush() == oracle.encode_stream(2, 44100, 128, l, r)[0]

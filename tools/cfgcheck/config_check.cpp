@@ -20,7 +20,8 @@ static bool deq(double a, double b) { return memcmp(&a, &b, 8) == 0; }
 static int check(int ch, int sr, int kbps) {
   Mp3Tables* t = (Mp3Tables*)malloc(sizeof(Mp3Tables));
   Mp3Resample rs;
-  const int rc = mp3_build_tables(ch, sr, kbps, t, 1 /* MP3B200_RESAMPLE */, &rs);
+  Mp3TagParams tag;
+  const int rc = mp3_build_config(ch, sr, kbps, 1 /* MP3B200_RESAMPLE */, t, &rs, &tag);
   LjEnc* e = lj_create(ch, sr, kbps);
   /* the flagged product takes what lamejs encodes at the input rate and what it resamples by an integer ratio (lamejs's own
    * test, |in / out - round(in / out)| < 1e-4) */
