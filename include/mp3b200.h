@@ -338,6 +338,11 @@ int mp3b200_debug_resample(int channels, int samplerate, int kbps, const int16_t
  * Samples that are not finite (before or after the scale) are refused with MP3B200_ERR_CONFIG: the host calls refuse them
  * before anything runs and leave a handle untouched; mp3b200_encode_streams_device_f32 finds them on the device, and its
  * output buffer is then unspecified.  lamejs would carry NaN through its psy model and rate loop.
+ * Samples beyond 2^35 (2^20 x full scale) once scaled are refused the same way: the library is compared with lamejs up to
+ * there (DESIGN.md 12).  Below that, a frame whose bits do not fit its slot even at
+ * global_gain 255 (from about 2e5 x full scale, depending on signal and bitrate) is refused with MP3B200_ERR_CONFIG by the
+ * call that encodes it, the call in which lamejs throws; it is never packed.  Every handle of a refused call is left exactly
+ * as it was before the call (samples, pending frames, ReplayGain analysis), so quieter input continues.
  * Streaming handles: a handle switches to Float32 mode at its first Float32 call (encode_f32, encode_batch_f32, seek_f32)
  * and stays there; its retained samples are converted exactly, and the samples of later Int16 calls are converted too, so
  * any mix of Int16 and Float32 calls encodes as the same mix of Int16Array / Float32Array calls does in lamejs.  A batch may

@@ -1967,7 +1967,7 @@ __global__ void __launch_bounds__(Q_THREADS)
 k_q_pack(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ streams, QuantFrameState* __restrict__ qs,
          const GranuleInfoDev* __restrict__ ginfo, const short* __restrict__ l3enc, const unsigned* __restrict__ neg_g,
          const int* __restrict__ list, const int* __restrict__ count_ptr, int count_direct, int revalidate,
-         int* __restrict__ counter, uint8_t* __restrict__ out) {
+         int* __restrict__ counter, uint8_t* __restrict__ out, int* __restrict__ over_budget) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   PackShared* ps = reinterpret_cast<PackShared*>(smem_raw) + (threadIdx.x >> 5);
   const int lane = LANE, nch = T->nch;
@@ -1981,6 +1981,15 @@ k_q_pack(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ streams
     const FrameGeom fg = frame_geom(T, streams, q);
     const StreamDesc& sd = streams[fg.z];
     const size_t g0 = ((size_t)sd.unit_base + T->mode_gr * fg.f) * nch;   /* first of the frame's mode_gr * nch granule-channels */
+    /* A frame whose granules do not fit its slot is not packed (nothing is written past ps->bits): lamejs throws there
+     * (format_bitstream's consistency check, BitStream.js:856-885).  *over_budget counts the frames whose latest pack was
+     * refused (q->valid == 2), so a frame a re-validation pass repacks within budget takes its count back. */
+    int used = 0;
+#pragma unroll 1
+    for (int k = 0; k < T->mode_gr * nch; k++) used += ginfo[g0 + k].part2_3_length + ginfo[g0 + k].part2_length;
+    const bool over = used > 8 * (fg.frame_bytes - T->sideinfo_len);
+    if (lane == 0 && over != (q->valid == 2)) atomicAdd(over_budget, over ? 1 : -1);
+    if (over) { if (lane == 0) q->valid = 2; continue; }
     __syncwarp();
 #pragma unroll 1
     for (int i = lane; i < 368; i += 32) ps->bits[i] = 0;
@@ -2082,6 +2091,7 @@ __global__ void k_qstate_commit(StreamDesc* __restrict__ streams, int nstreams, 
 struct QuantBuffers {
   const float* xr; const PsyRatioDev* ratio; const signed char* bt; const double* ath_q;
   QuantFrameState* qs; GranuleInfoDev* ginfo; short* l3enc; float* xrq; float* xrpow; unsigned* neg; GcPrep* prep;
+  int* over_budget;               /* frames over their bit budget (k_q_pack), [1] */
   int* list; int* counter;        /* list: 2 x (frames + 1) entries (verify list, short list); counter[0..1]: their lengths;
                                      counter[2..Q_NCOUNTERS): task counters, one per launch */
 };
@@ -2168,7 +2178,7 @@ static int quant_run(const Mp3Tables* dT, const Mp3Tables& hT, StreamDesc* d_str
     finish(gr, nullptr, nullptr, count, reval); mark(slot_f);
   };
   auto pack = [&](const int* list, const int* cptr, long long count, int reval) {
-    k_q_pack<<<grid_for(count, 9), Q_THREADS, smem_pack, st>>>(dT, d_streams, B.qs, B.ginfo, B.l3enc, B.neg, list, cptr, (int)count, reval, fresh_counter(), d_out);
+    k_q_pack<<<grid_for(count, 9), Q_THREADS, smem_pack, st>>>(dT, d_streams, B.qs, B.ginfo, B.l3enc, B.neg, list, cptr, (int)count, reval, fresh_counter(), d_out, B.over_budget);
     (*launches)++;
   };
   auto verify = [&](int predict_step = 0) {

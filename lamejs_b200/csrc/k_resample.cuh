@@ -66,8 +66,14 @@ k_resample(const ResampleDesc* __restrict__ descs, int ratio, int scale_applied,
  * encodeBuffer stores each caller value into a Float32Array, x = Float32(v) (the caller's float rows hold that already), and
  * scales it in place, x = Float32((double)x * scale), when the preset's scale is not 1.  k_stage_f32 writes those rows,
  * where the <true> instantiations of the psy analysis and the filterbank, k_resample<float> and the ReplayGain analysis read
- * them.  A non-finite value (before or after the scale) sets *nonfinite and is staged as 0, so that nothing downstream sees it:
- * such a call is refused, and its output is not used. */
+ * them.  A non-finite value (before or after the scale), or one beyond MP3_F32_MAX_SAMPLE after it, sets refused[0] and is
+ * staged as 0, so that nothing downstream sees it: such a call is refused, and its output is not used.
+ * MP3_F32_MAX_SAMPLE (2^35, 2^20 x full scale) is the loudest input the library has been compared with lamejs at, stage by
+ * stage and byte for byte (tests/golden/lamejs_loud_golden.json).  Louder rungs the fixtures hold, up to 3.3e7 x full scale,
+ * still encode in lamejs on some signals but not yet byte-identically here; from 1e15 x full scale lamejs's own masking
+ * energies overflow Float32, from 1e30 its MDCT lines, and it encodes (when it does not throw) from infinities and NaNs
+ * (DESIGN.md 12). */
+#define MP3_F32_MAX_SAMPLE 34359738368.0f
 #define STAGE_THREADS 256
 #define STAGE_PER_THREAD 4
 struct StageDesc {
@@ -78,7 +84,7 @@ struct StageDesc {
 
 /* grid (ceil(max n / (STAGE_THREADS * STAGE_PER_THREAD)), nch, nstreams) */
 __global__ void __launch_bounds__(STAGE_THREADS)
-k_stage_f32(const StageDesc* __restrict__ descs, int scale_applied, double scale, int* __restrict__ nonfinite) {
+k_stage_f32(const StageDesc* __restrict__ descs, int scale_applied, double scale, int* __restrict__ refused) {
   const StageDesc& d = descs[blockIdx.z];
   const int ch = blockIdx.y;
   const float* __restrict__ x = d.x[ch];
@@ -91,10 +97,10 @@ k_stage_f32(const StageDesc* __restrict__ descs, int scale_applied, double scale
     if (i >= d.n) break;
     float v = __ldg(&x[i]);
     if (scale_applied) v = (float)((double)v * scale);
-    if (!isfinite(v)) { bad = true; v = 0.0f; }
+    if (!(fabsf(v) <= MP3_F32_MAX_SAMPLE)) { bad = true; v = 0.0f; }
     y[i] = v;
   }
-  if (bad) atomicOr(nonfinite, 1);
+  if (bad) atomicOr(refused, 1);
 }
 
 #endif

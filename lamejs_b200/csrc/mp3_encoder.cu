@@ -236,7 +236,8 @@ struct Workspace {
   Buf<float> rs_y;                        /* resampled batches: the resampler's output rows, the PCM the pipeline reads */
   Buf<StageDesc> st_desc;                 /* Float32 input: [S] */
   Buf<float> st_y;                        /* Float32 input: the staged (scaled) rows */
-  Buf<int> nonfinite;                     /* Float32 input: set by k_stage_f32 when a sample is not finite */
+  Buf<int> refusals;                      /* [2]: [0] set by k_stage_f32 when a Float32 sample is refused (non-finite or beyond
+                                             MP3_F32_MAX_SAMPLE), [1] frames whose bits do not fit their slot (k_q_pack) */
   int fit(int S, int nch, long long U, long long F) {
     const size_t gc = (size_t)U * nch, rows = (size_t)(U + S) * nch, f = (size_t)F + 1;
     const bool failed = streams.fit(S) || bt_final.fit((size_t)U * 2 + 16) || bt_prev.fit((size_t)U * 2 + 16) ||
@@ -250,7 +251,7 @@ struct Workspace {
     streams.release(); bt_final.release(); bt_prev.release(); xr.release(); slab.release(); psy.release(); scan_in.release();
     ratio.release(); ath_psy.release(); ath_q.release(); qstate.release(); ginfo.release(); l3enc.release(); xrq.release();
     xrpow.release(); neg.release(); prep.release(); dirty.release(); counter.release(); scan.release();
-    rs_desc.release(); rs_y.release(); st_desc.release(); st_y.release(); nonfinite.release();
+    rs_desc.release(); rs_y.release(); st_desc.release(); st_y.release(); refusals.release();
   }
 };
 
@@ -370,6 +371,22 @@ struct Timings { float psy = 0, scan = 0, mask = 0, fb = 0, q1 = 0, qn = 0, tota
 /* chunks > 1: the caller uploads each stream's PCM in that many time slices on another stream and records ready[j] after
  * slice j; the psy analysis of slice j starts as soon as it has landed. */
 struct PcmArrival { int chunks = 1; cudaEvent_t* ready = nullptr; };
+
+/* set by check_refusals when it refuses a launch for a frame over its bit budget (the one refusal a handle call can only
+ * find after its launch, and then undoes: handles_call) */
+thread_local bool t_over_budget = false;
+
+/* After a launch has drained, one read-back of ws.refusals: MP3B200_ERR_CONFIG when k_stage_f32 refused a Float32 sample,
+ * or when a frame's bits did not fit its slot (k_q_pack left it unpacked), where lamejs throws out of the call
+ * (BitStream.js:856-885).  The call's output must not be used. */
+int check_refusals() {
+  int r[2] = {0, 0};
+  CK(cudaMemcpyAsync(r, t_ctx.ws.refusals.p, sizeof r, cudaMemcpyDeviceToHost, t_ctx.st));
+  CK(cudaStreamSynchronize(t_ctx.st));
+  if (r[0]) { g_err = "non-finite input sample (or one beyond 2^35 once scaled)"; return MP3B200_ERR_CONFIG; }
+  if (r[1]) { g_err = "frame over its bit budget (input too loud to encode)"; t_over_budget = true; return MP3B200_ERR_CONFIG; }
+  return 0;
+}
 
 /* Options of launch_streams */
 struct LaunchOpts {
@@ -513,6 +530,7 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
     QuantBuffers qb;
     qb.xr = ws.xr.p; qb.ratio = ws.ratio.p; qb.bt = ws.bt_final.p; qb.ath_q = ws.ath_q.p; qb.qs = ws.qstate.p; qb.ginfo = ws.ginfo.p;
     qb.l3enc = ws.l3enc.p; qb.xrq = ws.xrq.p; qb.xrpow = ws.xrpow.p; qb.neg = ws.neg.p; qb.prep = ws.prep.p; qb.list = ws.dirty.p; qb.counter = ws.counter.p;
+    qb.over_budget = ws.refusals.p + 1;
     int rc = quant_run(tab, cfg->host, ws.streams.p, S, streams_with_frames, max_frames, total_frames, qb, d_out, st, t_ctx.aux_st, t_ctx.ev_fork, t_ctx.ev_join, ev[5], t_ctx.evq, t_ctx.evq_pred, &passes, &g_launches);
     if (rc) { g_err = "quantizer stage failed: " + std::string(cudaGetErrorString(cudaGetLastError())); return rc; }
   } else {
@@ -560,7 +578,7 @@ long long hist_base_at(int mode_gr, long long frame) {
 }
 
 /* Float32 input: the descriptors sds[0 .. S) point at the caller's Float32 rows.  Queues k_stage_f32, which writes them
- * scaled into the workspace (ws.nonfinite flags a non-finite sample), and points the descriptors at the staged rows; the
+ * scaled into the workspace (ws.refusals[0] flags a refused sample), and points the descriptors at the staged rows; the
  * sample indices stay as they were. */
 int stage_streams(Config* cfg, StreamDesc* sds, int S) {
   const int nch = cfg->host.nch;
@@ -591,7 +609,7 @@ int stage_streams(Config* cfg, StreamDesc* sds, int S) {
   if (max_n > 0) {
     const long long per = (long long)STAGE_THREADS * STAGE_PER_THREAD;
     dim3 grid((unsigned)((max_n + per - 1) / per), nch, S);
-    k_stage_f32<<<grid, STAGE_THREADS, 0, st>>>(ws.st_desc.p, cfg->host.scale_applied, cfg->host.scale, ws.nonfinite.p);
+    k_stage_f32<<<grid, STAGE_THREADS, 0, st>>>(ws.st_desc.p, cfg->host.scale_applied, cfg->host.scale, ws.refusals.p);
     g_launches++;
     DBG("k_stage_f32");
   }
@@ -853,10 +871,10 @@ int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, co
   const PcmArrival* arrival = o.arrival;
   const int nstreams = (int)sds.size();
   if (o.rg && nstreams > MP3_MAX_LAUNCH_STREAMS) { g_err = "ReplayGain batches hold at most 65535 streams"; return MP3B200_ERR_HANDLE; }
-  if (o.f32_in) {
-    int rc = t_ctx.ws.nonfinite.fit(1);
+  {
+    int rc = t_ctx.ws.refusals.fit(2);
     if (rc) return rc;
-    CK(cudaMemsetAsync(t_ctx.ws.nonfinite.p, 0, sizeof(int), t_ctx.st));
+    CK(cudaMemsetAsync(t_ctx.ws.refusals.p, 0, 2 * sizeof(int), t_ctx.st));
   }
   for (int g0 = 0; g0 < nstreams; g0 += MP3_MAX_LAUNCH_STREAMS) {
     const int n = nstreams - g0 < MP3_MAX_LAUNCH_STREAMS ? nstreams - g0 : MP3_MAX_LAUNCH_STREAMS;
@@ -909,13 +927,7 @@ int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, co
       if ((float)tm.passes > o.timings_ms[7]) o.timings_ms[7] = (float)tm.passes;
     }
   }
-  if (o.f32_in && o.sync) {
-    int bad = 0;
-    CK(cudaMemcpyAsync(&bad, t_ctx.ws.nonfinite.p, sizeof(int), cudaMemcpyDeviceToHost, t_ctx.st));
-    CK(cudaStreamSynchronize(t_ctx.st));
-    if (bad) { g_err = "non-finite input sample"; return MP3B200_ERR_CONFIG; }
-  }
-  return 0;
+  return o.sync && (o.f32_in || !o.stop_after_mdct) ? check_refusals() : 0;
 }
 
 }  // namespace
@@ -1002,13 +1014,13 @@ template <class T> T* staging_pcm(size_t n) { return t_ctx.pcm.fit(sizeof(T) * n
 /* the right row of stream s: stereo input with right == NULL or right[s] == NULL encodes left[s] on both channels */
 template <class T> const T* right_row(const T* const* left, const T* const* right, int s) { return right && right[s] ? right[s] : left[s]; }
 
-/* Float32 input (lamejs's store and scale): true when every sample is finite, and stays finite once scaled like
- * k_stage_f32 scales it */
+/* Float32 input (lamejs's store and scale): true when every sample, scaled like k_stage_f32 scales it, is finite and
+ * within MP3_F32_MAX_SAMPLE */
 bool finite_after_scale(const Mp3Tables& T, const float* x, long long n) {
   for (long long i = 0; i < n; i++) {
     float v = x[i];
     if (T.scale_applied) v = (float)((double)v * T.scale);
-    if (!std::isfinite(v)) return false;
+    if (!(std::fabs(v) <= MP3_F32_MAX_SAMPLE)) return false;   /* also false for NaN */
   }
   return true;
 }
@@ -1020,7 +1032,7 @@ int check_input(const Config* cfg, int nstreams, const float* const* left, const
   for (int s = 0; s < nstreams; s++)
     if (!finite_after_scale(cfg->host, left[s], nsamples[s]) ||
         (cfg->host.nch == 2 && !finite_after_scale(cfg->host, right_row(left, right, s), nsamples[s]))) {
-      g_err = "non-finite input sample"; return MP3B200_ERR_CONFIG;
+      g_err = "non-finite input sample (or one beyond 2^35 once scaled)"; return MP3B200_ERR_CONFIG;
     }
   return MP3B200_OK;
 }
@@ -1318,7 +1330,7 @@ int debug_resample(int channels, int samplerate, int kbps, const T* left, const 
   sd.pcm_end = nsamples;
   Rows rows = {false, cfg->host.scale_applied};
   if (std::is_same_v<T, float>) {                   /* the launch path's staging: Float32(x * scale) rows */
-    rc = t_ctx.ws.nonfinite.fit(1);
+    rc = t_ctx.ws.refusals.fit(2);
     if (rc) return rc;
     rc = stage_streams(cfg, &sd, 1);
     if (rc) return rc;

@@ -332,8 +332,16 @@ void lj_format_bitstream(LjEnc* e) {
   drain_into_ancillary(e, e->resvDrain_post);
   bits += e->resvDrain_post;
   e->main_data_begin += (bitsPerFrame - bits) / 8;
-  /* BitStream.js:851-884: consistency checks; on a mismatch the reference prints and re-bases ResvSize */
-  if ((e->main_data_begin * 8) != e->ResvSize) e->ResvSize = e->main_data_begin * 8;
+  /* BitStream.js:851-884: consistency checks.  Both report through System.err, which lamejs's common.js does not define:
+   * a failing check throws a TypeError out of lame_encode_buffer / lame_encode_flush.  That happens when a frame's bits
+   * do not fit its slot (loud Float32 input), and the encoder is left unusable.  Java's LAME prints and re-bases ResvSize;
+   * the integer-quotient reservoir switch (not lamejs either) keeps that. */
+  if (e->java_int_div) {
+    if ((e->main_data_begin * 8) != e->ResvSize) e->ResvSize = e->main_data_begin * 8;
+  } else if (compute_flushbits(e) != e->ResvSize || (e->main_data_begin * 8) != e->ResvSize) {
+    e->bs_fatal = 1;
+    return;
+  }
   if (e->bs_totbit > 1000000000) {
     for (int i = 0; i < 256; ++i) e->header[i].write_timing -= e->bs_totbit;
     e->bs_totbit = 0;

@@ -111,8 +111,13 @@ struct LjEnc {
   int disable_reservoir, mode_joint;
   int java_int_div;                /* test switch: integer byte counts where Java (and LAME) divide integers, see lj_quant.cpp ResvFrameEnd */
   int encoder_padding;             /* gfp.encoder_padding, set by lame_encode_flush (Lame.js:1412) */
+  int gain_clamps;                 /* times bin_search_StepSize clamped global_gain > 255 (coverage of loud input) */
+  int bs_fatal;                    /* format_bitstream's consistency check failed: lamejs threw (LJ_ERR_BITSTREAM) */
   double lowpass_final;            /* gfp.lowpassfreq after lame_init_params (Lame.js:884-896) */
 };
+
+/* returned by lj_encode / lj_encode_f32 / lj_flush for the call in which lamejs throws, and for every later call */
+#define LJ_ERR_BITSTREAM (-10)
 
 /* lj_init.cpp */
 int  lj_init_params(LjEnc* e, int channels, int samplerate, int kbps);

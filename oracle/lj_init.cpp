@@ -427,8 +427,9 @@ static int encode_mp3_frame(LjEnc* e, uint8_t* mp3buf, int mp3buf_size) {
   lj_iteration_loop(e, pe_use, ms_ener_ratio, masking);
   e->qtrace_cur = NULL;
   lj_format_bitstream(e);
-  int mp3count = lj_copy_buffer(e, mp3buf, mp3buf_size, 1);
-  lj_add_vbr_frame(e);             /* Encoder.js:640-641 */
+  /* the frame lamejs throws on is traced (frame_bytes = LJ_ERR_BITSTREAM) but not handed out */
+  int mp3count = e->bs_fatal ? LJ_ERR_BITSTREAM : lj_copy_buffer(e, mp3buf, mp3buf_size, 1);
+  if (!e->bs_fatal) lj_add_vbr_frame(e);             /* Encoder.js:640-641 */
   if (tracing) {
     for (int gr = 0; gr < 2; gr++) for (int ch = 0; ch < e->channels_out; ch++) {
       const GrInfo& gi = e->tt[gr][ch];
@@ -647,6 +648,7 @@ void lj_destroy(LjEnc* e) { if (e) { free(e->s3_ll); free(e->s3_ss); free(e->bla
 /* index.js:117-130 + Lame.js:1490-1514.  Returns bytes written or a negative lame error. */
 int lj_encode(LjEnc* e, const int16_t* left, const int16_t* right, int n, uint8_t* out, int cap) {
   if (!e) return -3;
+  if (e->bs_fatal) return LJ_ERR_BITSTREAM;
   if (n == 0) return 0;
   if (e->channels_out == 1 || e->num_channels == 1) right = left;
   return encode_buffer(e, left, right, n, (double)n, out, cap);
@@ -655,6 +657,7 @@ int lj_encode(LjEnc* e, const int16_t* left, const int16_t* right, int n, uint8_
 /* index.js:132-135 + Lame.js:1381-1488; sample counts are JS numbers (fractional when resampling) */
 int lj_flush(LjEnc* e, uint8_t* out, int cap) {
   if (!e) return -3;
+  if (e->bs_fatal) return LJ_ERR_BITSTREAM;
   static const int16_t zeros[1152] = {0};
   int imp3 = 0, mp3count = 0;
   double samples_to_encode = e->mf_samples_to_encode - POSTDELAY;
@@ -689,6 +692,9 @@ int lj_flush(LjEnc* e, uint8_t* out, int cap) {
   return mp3count;
 }
 
+/* gfp.scale after lame_init_params: what lamejs multiplies every input sample by (the preset's, 1 when unset) */
+double lj_get_scale(const LjEnc* e) { return e->scale; }
+int lj_gain_clamps(const LjEnc* e) { return e->gain_clamps; }
 void lj_set_trace(LjEnc* e, LjFrameTrace* buf, int cap) { e->trace = buf; e->trace_cap = cap; e->trace_n = 0; }
 /* quantizer rows next to the frame trace: row k is filled together with lj_set_trace's row k (call it after lj_set_trace) */
 void lj_set_quant_trace(LjEnc* e, LjQuantTrace* buf, int cap) { e->qtrace = buf; e->qtrace_cap = cap; }

@@ -1063,7 +1063,7 @@ static int bin_search_StepSize(LjEnc* e, GrInfo* cod_info, int desired_rate, int
     }
     cod_info->global_gain += step;
     if (cod_info->global_gain < 0) { cod_info->global_gain = 0; flagGoneOver = true; }
-    if (cod_info->global_gain > 255) { cod_info->global_gain = 255; flagGoneOver = true; }
+    if (cod_info->global_gain > 255) { cod_info->global_gain = 255; flagGoneOver = true; e->gain_clamps++; }
   }
   while (nBits > desired_rate && cod_info->global_gain < 255) {
     cod_info->global_gain++;

@@ -37,6 +37,85 @@ def make(kind, n, sr, seed):
     return x[0].copy(), x[1].copy()
 
 
+# Loud input (tests/golden/make_lamejs_loud_golden.py): a unit-peak signal times magnitude x 32768, where the magnitude
+# is a number or "max", the largest Float32 that stays finite once scaled by the configuration's `scale`.
+LOUD_KINDS = ("burst", "noise", "nyquist", "impulse", "dcstep")
+LOUD_MAGNITUDES = (16, 256, 4096, 65536, 2 ** 18, 2 ** 20, 2 ** 22, 2 ** 24, 3.3e7, 1e9, 1e15, 1e20, 1e30, "max")
+# across the magnitude at which lamejs's frames stop fitting their slots (between 2e5 and 1e6 x full scale)
+LOUD_FINE = (3e5, 4e5, 5e5, 6e5, 7e5, 8e5)
+
+
+def _unit(kind, n, sr, seed):
+    """(left, right) float64 in [-1, 1]"""
+    if kind in ("burst", "noise"):
+        l, r = make_signal(kind, n, sr, seed=seed)
+        return l / 32768.0, r / 32768.0
+    t = np.arange(n)
+    if kind == "nyquist":
+        w = 2 * np.pi * 0.49 * t
+        return np.sin(w), np.cos(w * 0.995)
+    l, r = np.zeros(n), np.zeros(n)
+    if kind == "impulse":
+        l[n // 3] = 1.0
+        r[n // 2] = -1.0
+    elif kind == "dcstep":
+        l[n // 3:] = 1.0
+        r[n // 2:] = -1.0
+    else:
+        raise ValueError(kind)
+    return l, r
+
+
+def max_finite(scale):
+    """the largest Float32 v with Float32(v * scale) finite (lamejs's scale of a Float32Array, k_stage_f32)"""
+    top = np.float32(np.finfo(np.float32).max)
+    v = np.float32(min(float(top), float(top) / scale))
+
+    def ok(x):
+        with np.errstate(over="ignore"):
+            return np.isfinite(np.float32(float(x) * scale))
+    while not ok(v):
+        v = np.nextafter(v, np.float32(0))
+    while v < top and ok(np.nextafter(v, top)):
+        v = np.nextafter(v, top)
+    return float(v)
+
+
+def loud(kind, magnitude, n, sr, seed, scale):
+    """(left, right): float64 holding Float32 values"""
+    l, r = _unit(kind, n, sr, seed)
+    if magnitude == "max":
+        vmax = max_finite(scale)
+        a = vmax / max(np.abs(l).max(), np.abs(r).max())
+        x = np.clip(np.stack([l, r]) * a, -vmax, vmax)
+    else:
+        x = np.stack([l, r]) * (float(magnitude) * 32768.0)
+    with np.errstate(over="ignore"):
+        x = x.astype(np.float32).astype(np.float64)
+    assert np.isfinite(x).all()
+    return x[0].copy(), x[1].copy()
+
+
+def loud_case_signal(c):
+    """case_signal for a loud fixture case (its "scale" is the configuration's)"""
+    l, r = loud(c["kind"], c["magnitude"], c["samples"], c["samplerate"], c["seed"], c["scale"])
+    calls, pos = [], 0
+    for step in c["schedule"]:
+        if step[0] < 0:
+            calls.append(None)
+            continue
+        k = step[0]
+        calls.append((l[pos:pos + k].astype(np.float32), r[pos:pos + k].astype(np.float32) if c["channels"] == 2 else None))
+        pos += k
+    return l, (r if c["channels"] == 2 else None), calls
+
+
+def loud_peak(c):
+    """the largest sample of a loud fixture case once lamejs has scaled it (what the library's input limit compares)"""
+    l, r = loud(c["kind"], c["magnitude"], c["samples"], c["samplerate"], c["seed"], c["scale"])
+    return max(np.abs(l).max(), np.abs(r).max() if c["channels"] == 2 else 0.0) * c["scale"]
+
+
 def schedule(kind, n, ragged, seed):
     """encodeBuffer calls [size, type] (type "f": Float32Array, "i": Int16Array, "a": plain Array) and [-1] for flush()"""
     typ = "a" if kind == "array" else "f"

@@ -72,7 +72,8 @@ def _hex64(a):
     return np.ascontiguousarray(a, dtype="<f8").tobytes().hex()
 
 
-def lamejs_float(channels, samplerate, kbps, left, right, schedule, rg):
+def lamejs_float(channels, samplerate, kbps, left, right, schedule, rg, driver=None):
+    """runs lamejs on one case; `driver` (default _driver) makes the driver's source from `rg`"""
     import ref_lamejs as R
     src = R.modules_loader_source(hooks=False)
     for old, new in (RGM._JAVA_DIVISION, (RGM._WINDOW_HOOK[0], RGM._WINDOW_HOOK[1] + RGM._WINDOW_HOOK[0])):
@@ -85,7 +86,7 @@ def lamejs_float(channels, samplerate, kbps, left, right, schedule, rg):
         with open(d, "w") as f:
             f.write('var __HEXL="%s"; var __HEXR="%s"; var __CH=%d, __SR=%d, __KBPS=%d, __CHUNK=0, __SCHED=%s;\n'
                     % (_hex64(left), _hex64(right), channels, samplerate, kbps, json.dumps(schedule)))
-            f.write(_driver(rg))
+            f.write((driver or _driver)(rg))
         o = json.loads(R.run_js([p, d]))
     o["bytes"] = bytes.fromhex(o.pop("hex"))
     o["tag"] = bytes.fromhex(o["tag"])

@@ -9,6 +9,7 @@ extern "C" {
 /* lj_encode with the store `in_buffer[i] = left[i]` of Float32 values (the caller's values rounded to Float32 once) */
 int lj_encode_f32(LjEnc* e, const float* left, const float* right, int n, uint8_t* out, int cap) {
   if (!e) return -3;
+  if (e->bs_fatal) return LJ_ERR_BITSTREAM;
   if (n == 0) return 0;
   if (e->channels_out == 1 || e->num_channels == 1) right = left;
   const double nsamples = (double)n;

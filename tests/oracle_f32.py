@@ -59,6 +59,9 @@ def lib():
     L.lj_trace_count.argtypes = [vp]
     L.lj_enable_vbr_tag.argtypes = [vp]
     L.lj_get_lametag_frame.argtypes = [vp, vp, ci]
+    L.lj_get_scale.argtypes = [vp]
+    L.lj_gain_clamps.argtypes = [vp]
+    L.lj_get_scale.restype = ctypes.c_double
     assert L.lj_trace_size() == oracle_lib.TRACE_DTYPE.itemsize
     _lib = L
     return L
@@ -95,17 +98,13 @@ class Encoder:
         cap = int(1.25 * len(left) + 7200) + 2880
         buf = np.empty(cap, dtype=np.uint8)
         fn = self.L.lj_encode_f32 if f32 else self.L.lj_encode
-        k = fn(self.h, left.ctypes.data, right.ctypes.data, len(left), buf.ctypes.data, cap)
-        if k < 0:
-            raise RuntimeError("lj_encode error %d" % k)
+        k = oracle_lib.check(fn(self.h, left.ctypes.data, right.ctypes.data, len(left), buf.ctypes.data, cap), "lj_encode")
         return buf[:k].tobytes()
 
     def flush(self):
         cap = 7200 + 4 * 1440 + 2880
         buf = np.empty(cap, dtype=np.uint8)
-        k = self.L.lj_flush(self.h, buf.ctypes.data, cap)
-        if k < 0:
-            raise RuntimeError("lj_flush error %d" % k)
+        k = oracle_lib.check(self.L.lj_flush(self.h, buf.ctypes.data, cap), "lj_flush")
         return buf[:k].tobytes()
 
     def lametag_frame(self):

@@ -130,6 +130,23 @@ def lib():
     return _lib
 
 
+ERR_BITSTREAM = -10          # LJ_ERR_BITSTREAM (oracle/lj_encoder.h)
+
+
+class LamejsThrows(RuntimeError):
+    """The call in which lamejs throws, and every later one: format_bitstream's consistency check failed because a frame's
+    bits do not fit its slot (BitStream.js:856-885 reports through System.err, which lamejs does not define)."""
+
+
+def check(k, what):
+    """k from lj_encode / lj_encode_f32 / lj_flush: raises on an error, else returns k"""
+    if k == ERR_BITSTREAM:
+        raise LamejsThrows("%s: frame over its bit budget (lamejs throws)" % what)
+    if k < 0:
+        raise RuntimeError("%s error %d" % (what, k))
+    return k
+
+
 def out_samplerate(channels, samplerate, kbps):
     """Output sample rate lame_init_params picks (Lame.js:285-364): != samplerate means lamejs resamples."""
     return lib().lj_query_out_samplerate(channels, samplerate, kbps)
@@ -164,17 +181,13 @@ class OracleEncoder:
         assert len(left) == len(right)
         cap = int(1.25 * len(left) + 7200)
         buf = np.empty(cap, dtype=np.uint8)
-        k = self.L.lj_encode(self.h, left.ctypes.data, right.ctypes.data, len(left), buf.ctypes.data, cap)
-        if k < 0:
-            raise RuntimeError("lj_encode error %d" % k)
+        k = check(self.L.lj_encode(self.h, left.ctypes.data, right.ctypes.data, len(left), buf.ctypes.data, cap), "lj_encode")
         return buf[:k].tobytes()
 
     def flush(self):
         cap = 7200 + 4 * 1440
         buf = np.empty(cap, dtype=np.uint8)
-        k = self.L.lj_flush(self.h, buf.ctypes.data, cap)
-        if k < 0:
-            raise RuntimeError("lj_flush error %d" % k)
+        k = check(self.L.lj_flush(self.h, buf.ctypes.data, cap), "lj_flush")
         return buf[:k].tobytes()
 
     def traces(self):
