@@ -209,6 +209,36 @@ int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int ns
 int mp3b200_encode_streams_tagged_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
                                      const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
                                      const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db);
+/* Tagged whole streams on device buffers: mp3b200_encode_streams_tagged_ex for PCM that is already on the GPU, written as
+ * finished files into a device buffer.  The output is byte-identical to what mp3b200_encode_streams_tagged_ex (or _f32)
+ * returns for the same samples, and title_db / album_db (optional) receive the same gains.
+ *   d_pcm, pcm_off, nsamples   as for mp3b200_encode_streams_device_ex: one device allocation, per stream s nsamples[s]
+ *                              samples of the left channel at pcm_off[s] and (stereo) the right channel behind them.
+ *   flags                      MP3B200_RESAMPLE | MP3B200_REPLAYGAIN, meaning what they mean for _tagged_ex; any other bit
+ *                              returns MP3B200_ERR_CONFIG.
+ *   d_out, out_off             stream s is written as one file at d_out + out_off[s]: its tag frame, then its audio frames.
+ *                              A stream gets a tag frame where _tagged_ex writes one: the tag fits the configuration
+ *                              (mp3b200_lametag_size_ex > 0) and the stream has at least one frame (every stream has: flush()
+ *                              always encodes one).  The room stream s needs is mp3b200_stream_bytes_ex + mp3b200_lametag_size_ex
+ *                              for such a stream, mp3b200_stream_bytes_ex otherwise.  Nothing outside
+ *                              [out_off[s], out_off[s] + out_bytes[s]) is written.
+ *   out_bytes                  host array: out_bytes[s] receives the length of stream s's file.
+ *   title_db, album_db         as for _tagged_ex, including -24601 when a stream holds less than one RMS window, or when the
+ *                              tag does not fit and nothing is analysed.
+ * A batch with MP3B200_REPLAYGAIN holds at most 65535 streams (MP3B200_ERR_HANDLE, as for _tagged_ex); without it larger
+ * batches run as consecutive launches, as mp3b200_encode_streams_device does.  The call runs on a stream of its own that
+ * first waits for work already queued on the legacy default stream (where torch / plain CUDA callers produced d_pcm and
+ * d_out) and returns after that stream has drained.  The packer writes each stream's audio straight behind the room of its
+ * tag frame; the frames are built on the host, uploaded in one copy and put in place by one kernel (k_tag_scatter).
+ * _device_f32 takes Float32 samples, laid out the same way, as mp3b200_encode_streams_device_f32 does; a sample that is not
+ * finite, or beyond 2^35 once scaled, returns MP3B200_ERR_CONFIG, and no tag frame is placed (the audio bytes in d_out are
+ * then unspecified). */
+int mp3b200_encode_streams_tagged_device(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
+                                         const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off,
+                                         int64_t* out_bytes, double* title_db, double* album_db);
+int mp3b200_encode_streams_tagged_device_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* d_pcm,
+                                             const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off,
+                                             int64_t* out_bytes, double* title_db, double* album_db);
 /* mp3b200_lametag_build with flags (MP3B200_RESAMPLE) and the Radio Replay Gain field of an analysed stream: radio_gain is
  * gfc.RadioGain = floor(title_db * 10 + 0.5), clamped to +-51.0 dB like lamejs; for segment callers that analyse the whole
  * stream themselves (ReplayGain is not combined across segments). */

@@ -1,4 +1,5 @@
-/* k_tag.cuh -- the music CRC of the Xing / LAME tag on the GPU (SURVEY.md 8(f3)).
+/* k_tag.cuh -- the music CRC of the Xing / LAME tag on the GPU (SURVEY.md 8(f3)), and the placement of the tag frames of
+ * device-resident streams (k_tag_scatter).
  *
  * lamejs keeps gfc.nMusicCRC by pushing every byte copy_buffer hands out through a table-driven CRC-16 (polynomial
  * x^16 + x^15 + x^2 + 1, reflected, start 0; reference src/js/VBRTag.js:547-556, BitStream.js:924-928): one dependent table
@@ -123,6 +124,17 @@ k_music_crc(const uint8_t* __restrict__ buf, const long long* __restrict__ off, 
   c ^= __shfl_xor_sync(0xffffffffu, c, 2);
   c ^= __shfl_xor_sync(0xffffffffu, c, 1);
   if (lane == 0) atomicXor(&crc_out[r], crc_shift(c, (unsigned long long)p.after_piece, s_t.pow));
+}
+
+/* The tag frames of a batch of device-resident streams, built on the host (mp3_tag_frame) and uploaded in one copy, put in
+ * front of their streams: grid (frames), frame i is frame_bytes bytes at frames + i * frame_bytes and goes to out + dst[i].
+ * One block per frame, so a batch of any size is one launch. */
+enum { TAG_SCATTER_THREADS = 128 };
+__global__ void __launch_bounds__(TAG_SCATTER_THREADS)
+k_tag_scatter(const long long* __restrict__ dst, const uint8_t* __restrict__ frames, int frame_bytes, uint8_t* __restrict__ out) {
+  const uint8_t* src = frames + (size_t)blockIdx.x * frame_bytes;
+  uint8_t* d = out + dst[blockIdx.x];
+  for (int i = threadIdx.x; i < frame_bytes; i += TAG_SCATTER_THREADS) d[i] = src[i];
 }
 #endif
 

@@ -273,6 +273,7 @@ struct ThreadCtx {
   Buf<uint8_t, true> pin;                 /* pinned host staging */
   Buf<long long> crc_ranges;              /* music CRC: [2][R] offsets / lengths */
   Buf<unsigned> crc;                      /* music CRC: [R] results */
+  Buf<uint8_t> tags;                      /* tagged device streams: the uploaded tag frames and their offsets (k_tag_scatter) */
   cudaStream_t rg_st = nullptr;           /* ReplayGain analysis, beside the encoder */
   cudaEvent_t ev_rg[3] = {};              /* fork, start, end */
   Buf<RgTitle> rg_titles;
@@ -285,7 +286,7 @@ struct ThreadCtx {
   void release() {
     if (device < 0) return;
     cudaSetDevice(device);
-    ws.release(); pcm.release(); out.release(); pin.release(); crc_ranges.release(); crc.release();
+    ws.release(); pcm.release(); out.release(); pin.release(); crc_ranges.release(); crc.release(); tags.release();
     rg_titles.release(); rg_piece.release(); rg_sum.release(); rg_gain.release(); rg_wstate.release(); rg_cstart.release();
     rg_end_a.release(); rg_end_b.release(); rg_carry.release(); rg_idx.release(); rg_hist.release(); rg_count.release();
     for (auto& e : ev_rg) if (e) { cudaEventDestroy(e); e = nullptr; }
@@ -876,6 +877,11 @@ int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, co
     if (rc) return rc;
     CK(cudaMemsetAsync(t_ctx.ws.refusals.p, 0, 2 * sizeof(int), t_ctx.st));
   }
+  /* Before anything reads the descriptors' rows: the caller's device rows may come from the legacy default stream, and
+   * rg_queue forks the analysis stream from t_ctx.st ahead of run_pipeline's own wait (Int16 rows that are neither staged
+   * nor resampled are read by k_rg_pass1 where the caller left them). */
+  CK(cudaEventRecord(t_ctx.ev_in, cudaStreamLegacy));
+  CK(cudaStreamWaitEvent(t_ctx.st, t_ctx.ev_in, 0));
   for (int g0 = 0; g0 < nstreams; g0 += MP3_MAX_LAUNCH_STREAMS) {
     const int n = nstreams - g0 < MP3_MAX_LAUNCH_STREAMS ? nstreams - g0 : MP3_MAX_LAUNCH_STREAMS;
     StreamDesc* group = sds.data() + g0;
@@ -1508,69 +1514,172 @@ int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int ns
 }  // extern "C"
 
 namespace {
-/* encode_streams_tagged_ex / _f32; `rg` (flags & MP3B200_REPLAYGAIN) receives the analysis */
-template <class T>
-int encode_tagged(int channels, int samplerate, int kbps, int flags, int nstreams, const T* const* left,
-                  const T* const* right, const int64_t* nsamples, uint8_t* const* out, const int64_t* cap,
-                  int64_t* out_bytes, RgJob* rg) {
+/* The tagged whole streams (encodeBuffer(everything) + flush() on fresh encoders with the tag on) of both kinds of buffers.
+ * `io` says where the PCM comes from and where the files go (HostTagged, DeviceTagged):
+ *   io.check_input(cfg)                      the input gate of the host entry points (device rows: k_stage_f32)
+ *   io.launch(cfg, tfs, tag, rg, audio, at)  encodes the batch, with the analysis `rg` when set; stream s's audio[s] bytes
+ *                                            then lie at io.buf() + at[s].  tag[s] is the size of stream s's tag frame
+ *                                            (tfs, or 0: no frame)
+ *   io.frame(s)                              host memory for stream s's tag frame, once the launch has succeeded
+ *   io.finish(tag, audio, at)                puts the frames and the audio where they belong, and drains t_ctx.st
+ * out_bytes[s] receives the file's length; `rg` (flags & MP3B200_REPLAYGAIN) receives the analysis. */
+template <class Io>
+int encode_tagged(int channels, int samplerate, int kbps, int flags, int nstreams, const int64_t* nsamples, int64_t* out_bytes,
+                  RgJob* rg, Io& io) {
   if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
   if (flags & ~(MP3B200_RESAMPLE | MP3B200_REPLAYGAIN)) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
   Config* cfg;
   int rc = get_config(channels, samplerate, kbps, flags & MP3B200_RESAMPLE, &cfg);
-  if (rc || (rc = check_input(cfg, nstreams, left, right, nsamples))) return rc;
+  if (rc || (rc = io.check_input(cfg))) return rc;
   const Mp3TagParams& p = cfg->tag;
   const int tfs = p.fits ? p.frame_bytes : 0;
   if (rg && tfs == 0) rg = nullptr;               /* lamejs analyses only when the tag is written (Lame.js:911-916) */
-  if (rg) {
-    rg->specs.assign((size_t)nstreams, RgSpec());
-    for (int s = 0; s < nstreams; s++) {
-      rg->specs[s].stream = s;
-      LameFifo fifo(cfg->host.mode_gr, cfg->rs.ratio);
-      fifo.pieces = &rg->specs[s].pieces;
-      fifo.feed(nsamples[s]);
-      fifo.flush();
-    }
+  if (rg) rg->specs.assign((size_t)nstreams, RgSpec());
+  /* each stream's frames and end padding, and the pieces the analysis sees: closed form, before anything runs */
+  std::vector<long long> frames((size_t)nstreams);
+  std::vector<int> padding((size_t)nstreams), tag((size_t)nstreams);
+  for (int s = 0; s < nstreams; s++) {
+    LameFifo fifo(cfg->host.mode_gr, cfg->rs.ratio);
+    if (rg) { rg->specs[s].stream = s; fifo.pieces = &rg->specs[s].pieces; }
+    const long long fed = fifo.feed(nsamples[s]);
+    const FifoFlush fl = fifo.flush();
+    frames[s] = fed + fl.frames;
+    padding[s] = fl.end_padding;
+    tag[s] = tfs > 0 && frames[s] > 0 ? tfs : 0;
   }
-  std::vector<int64_t> out_off;
-  std::vector<long long> audio;
-  rc = encode_host_streams(cfg, nstreams, left, right, nsamples, cap, tfs, out_bytes, out_off, audio, rg);
+  std::vector<long long> audio, at;
+  rc = io.launch(cfg, tfs, tag, rg, audio, at);
   if (rc || nstreams == 0) return rc;
   /* the music CRC of every stream, where the bytes are */
-  std::vector<long long> off(out_off.begin(), out_off.end());
   std::vector<unsigned> crc;
-  rc = music_crc_ranges(t_ctx.device, t_ctx.out.p, off, audio, crc);
+  rc = music_crc_ranges(t_ctx.device, io.buf(), at, audio, crc);
   if (rc) return rc;
   Mp3SeekBag* bag = new Mp3SeekBag();
   for (int s = 0; s < nstreams; s++) {
-    int wrote = 0;
-    LameFifo fifo(cfg->host.mode_gr, cfg->rs.ratio);
-    const long long frames = fifo.feed(nsamples[s]);
-    const FifoFlush fl = fifo.flush();
-    if (tfs > 0 && frames + fl.frames > 0) {
+    if (tag[s]) {
       bag->reset();
-      bag->add_frames(frames + fl.frames, p.kbps);
+      bag->add_frames(frames[s], p.kbps);
       const int field = rg ? mp3_radio_gain_field(mp3_radio_gain(rg->title_db[s])) : 0;
-      wrote = mp3_tag_frame(p, *bag, audio[s], crc[s], (int)fl.end_padding, out[s], field);
+      mp3_tag_frame(p, *bag, audio[s], crc[s], padding[s], io.frame(s), field);
     }
-    out_bytes[s] = audio[s] + wrote;
-    if (audio[s] > 0 && cudaMemcpyAsync(out[s] + wrote, t_ctx.out.p + out_off[s], (size_t)audio[s], cudaMemcpyDeviceToHost, t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
+    out_bytes[s] = audio[s] + tag[s];
   }
   delete bag;
-  if (cudaStreamSynchronize(t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
-  return rc;
+  return io.finish(tag, audio, at);
 }
+
+/* Host rows in, host files out: the PCM is uploaded like mp3b200_encode_streams uploads it, out[s] (cap[s] bytes) receives
+ * the tag frame and then the audio, read back from t_ctx.out. */
 template <class T>
-int encode_tagged_rg(int channels, int samplerate, int kbps, int flags, int nstreams, const T* const* left, const T* const* right,
-                     const int64_t* nsamples, uint8_t* const* out, const int64_t* cap, int64_t* out_bytes, double* title_db,
-                     double* album_db) {
+struct HostTagged {
+  int nstreams;
+  const T* const* left;
+  const T* const* right;
+  const int64_t* nsamples;
+  uint8_t* const* out;
+  const int64_t* cap;
+  int64_t* out_bytes;
+  int check_input(const Config* cfg) const { return ::check_input(cfg, nstreams, left, right, nsamples); }
+  int launch(Config* cfg, int tfs, const std::vector<int>&, RgJob* rg, std::vector<long long>& audio, std::vector<long long>& at) {
+    std::vector<int64_t> out_off;
+    const int rc = encode_host_streams(cfg, nstreams, left, right, nsamples, cap, tfs, out_bytes, out_off, audio, rg);
+    at.assign(out_off.begin(), out_off.end());
+    return rc;
+  }
+  const uint8_t* buf() const { return t_ctx.out.p; }
+  uint8_t* frame(int s) { return out[s]; }
+  int finish(const std::vector<int>& tag, const std::vector<long long>& audio, const std::vector<long long>& at) {
+    int rc = 0;
+    for (int s = 0; s < nstreams; s++)
+      if (audio[s] > 0 && cudaMemcpyAsync(out[s] + tag[s], t_ctx.out.p + at[s], (size_t)audio[s], cudaMemcpyDeviceToHost, t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
+    if (cudaStreamSynchronize(t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
+    return rc;
+  }
+};
+
+/* Device rows in (laid out as mp3b200_encode_streams_device reads them), device files out: stream s's file starts at
+ * d_out + out_off[s].  The packer writes the audio straight behind the room of its tag frame; the frames are built on the
+ * host into one pinned buffer (t_ctx.pin: [k] destination offsets, then the k frames), uploaded with one copy and put in
+ * place by k_tag_scatter. */
+template <class T>
+struct DeviceTagged {
+  int nstreams;
+  const T* d_pcm;
+  const int64_t* pcm_off;
+  const int64_t* nsamples;
+  uint8_t* d_out;
+  const int64_t* out_off;
+  std::vector<int> slot;                  /* stream s's frame is frame slot[s] of the staging buffer */
+  int ntags = 0, tfs = 0;            /* tag frames of the batch, and their size */
+  int check_input(const Config*) const { return MP3B200_OK; }
+  int launch(Config* cfg, int tfs_, const std::vector<int>& tag, RgJob* rg, std::vector<long long>& audio, std::vector<long long>& at) {
+    tfs = tfs_;
+    std::vector<int64_t> audio_off((size_t)nstreams);
+    for (int s = 0; s < nstreams; s++) audio_off[s] = out_off[s] + tag[s];
+    std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off, nsamples, audio_off.data());
+    audio.assign((size_t)nstreams, 0);
+    at.assign(audio_off.begin(), audio_off.end());
+    slot.assign((size_t)nstreams, -1);
+    for (int s = 0; s < nstreams; s++) {
+      audio[s] = bytes_of_frames(cfg->host, 0, sds[s].nframes);
+      if (tag[s]) slot[s] = ntags++;
+    }
+    LaunchOpts o;
+    o.rg = rg;
+    o.f32_in = std::is_same_v<T, float>;
+    int rc = launch_streams(cfg, sds, d_out, o);
+    if (rc || ntags == 0) return rc;
+    rc = t_ctx.pin.fit(staging_bytes());
+    if (rc) return rc;
+    long long* dst = reinterpret_cast<long long*>(t_ctx.pin.p);
+    for (int s = 0; s < nstreams; s++) if (slot[s] >= 0) dst[slot[s]] = out_off[s];
+    return 0;
+  }
+  size_t staging_bytes() const { return (sizeof(long long) + (size_t)tfs) * (size_t)ntags; }
+  const uint8_t* buf() const { return d_out; }
+  uint8_t* frame(int s) { return t_ctx.pin.p + sizeof(long long) * (size_t)ntags + (size_t)tfs * (size_t)slot[s]; }
+  int finish(const std::vector<int>&, const std::vector<long long>&, const std::vector<long long>&) {
+    if (ntags == 0) return 0;
+    int rc = t_ctx.tags.fit(staging_bytes());
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(t_ctx.tags.p, t_ctx.pin.p, staging_bytes(), cudaMemcpyHostToDevice, t_ctx.st));
+    k_tag_scatter<<<ntags, TAG_SCATTER_THREADS, 0, t_ctx.st>>>(reinterpret_cast<const long long*>(t_ctx.tags.p),
+                                                               t_ctx.tags.p + sizeof(long long) * (size_t)ntags, tfs, d_out);
+    g_launches++;
+    CK(cudaStreamSynchronize(t_ctx.st));
+    CK(cudaGetLastError());
+    return 0;
+  }
+};
+
+/* encode_tagged with the gains handed out: title_db[s] / album_db (optional), RG_NOT_ENOUGH_SAMPLES where nothing ran */
+template <class Io>
+int encode_tagged_rg(int channels, int samplerate, int kbps, int flags, int nstreams, const int64_t* nsamples, int64_t* out_bytes,
+                     double* title_db, double* album_db, Io& io) {
   RgJob job;
   const bool want = (flags & MP3B200_REPLAYGAIN) != 0;
-  const int rc = encode_tagged(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, want ? &job : nullptr);
+  const int rc = encode_tagged(channels, samplerate, kbps, flags, nstreams, nsamples, out_bytes, want ? &job : nullptr, io);
   if (rc) return rc;
   const bool ran = want && (int)job.title_db.size() == nstreams && nstreams > 0;
   for (int s = 0; title_db && s < nstreams; s++) title_db[s] = ran ? job.title_db[s] : RG_NOT_ENOUGH_SAMPLES;
   if (album_db) *album_db = ran ? job.album_db : RG_NOT_ENOUGH_SAMPLES;
   return 0;
+}
+
+template <class T>
+int encode_tagged_host(int channels, int samplerate, int kbps, int flags, int nstreams, const T* const* left, const T* const* right,
+                       const int64_t* nsamples, uint8_t* const* out, const int64_t* cap, int64_t* out_bytes, double* title_db,
+                       double* album_db) {
+  HostTagged<T> io{nstreams, left, right, nsamples, out, cap, out_bytes};
+  return encode_tagged_rg(channels, samplerate, kbps, flags, nstreams, nsamples, out_bytes, title_db, album_db, io);
+}
+
+template <class T>
+int encode_tagged_device(int channels, int samplerate, int kbps, int flags, int nstreams, const T* d_pcm, const int64_t* pcm_off,
+                         const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off, int64_t* out_bytes, double* title_db,
+                         double* album_db) {
+  DeviceTagged<T> io{nstreams, d_pcm, pcm_off, nsamples, d_out, out_off};
+  return encode_tagged_rg(channels, samplerate, kbps, flags, nstreams, nsamples, out_bytes, title_db, album_db, io);
 }
 }  // namespace
 
@@ -1579,12 +1688,25 @@ extern "C" {
 int mp3b200_encode_streams_tagged_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
                                      const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
                                      const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db) {
-  return encode_tagged_rg(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, title_db, album_db);
+  return encode_tagged_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, title_db, album_db);
 }
 int mp3b200_encode_streams_tagged_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* const* left,
                                       const float* const* right, const int64_t* nsamples, uint8_t* const* out,
                                       const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db) {
-  return encode_tagged_rg(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, title_db, album_db);
+  return encode_tagged_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, title_db, album_db);
+}
+
+int mp3b200_encode_streams_tagged_device(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
+                                         const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off,
+                                         int64_t* out_bytes, double* title_db, double* album_db) {
+  return encode_tagged_device(channels, samplerate, kbps, flags, nstreams, d_pcm, pcm_off, nsamples, d_out, out_off, out_bytes,
+                              title_db, album_db);
+}
+int mp3b200_encode_streams_tagged_device_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* d_pcm,
+                                             const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off,
+                                             int64_t* out_bytes, double* title_db, double* album_db) {
+  return encode_tagged_device(channels, samplerate, kbps, flags, nstreams, d_pcm, pcm_off, nsamples, d_out, out_off, out_bytes,
+                              title_db, album_db);
 }
 
 int mp3b200_lametag_build_ex(int channels, int samplerate, int kbps, int flags, int64_t nframes, int64_t music_bytes, int music_crc,
@@ -1609,8 +1731,8 @@ int debug_replaygain(int channels, int samplerate, int kbps, int flags, const T*
   std::vector<uint8_t> out((size_t)cap);
   uint8_t* outp = out.data();
   int64_t ob = 0;
-  const int rc = encode_tagged(channels, samplerate, kbps, (flags & MP3B200_RESAMPLE) | MP3B200_REPLAYGAIN, 1, &left, &right, &nsamples,
-                               &outp, &cap, &ob, &job);
+  HostTagged<T> io{1, &left, &right, &nsamples, &outp, &cap, &ob};
+  const int rc = encode_tagged(channels, samplerate, kbps, (flags & MP3B200_RESAMPLE) | MP3B200_REPLAYGAIN, 1, &nsamples, &ob, &job, io);
   if (rc) return rc;
   const long long n = (long long)job.win_idx.size();
   for (long long w = 0; w < n && w < nwin_cap; w++) {

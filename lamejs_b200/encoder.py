@@ -93,6 +93,8 @@ def lib():
     L.mp3b200_encode_streams_f32.argtypes = [c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp]
     L.mp3b200_encode_streams_tagged_f32.argtypes = [c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mp3b200_encode_streams_device_f32.argtypes = [c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp]
+    L.mp3b200_encode_streams_tagged_device.argtypes = [c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.mp3b200_encode_streams_tagged_device_f32.argtypes = [c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mp3b200_debug_stages_f32.argtypes = [ctypes.POINTER(DebugTaps), vp, vp]
     L.mp3b200_debug_resample_f32.argtypes = [c_int, c_int, c_int, vp, vp, c_i64, vp, c_i64]
     L.mp3b200_debug_replaygain_f32.argtypes = [c_int, c_int, c_int, c_int, vp, vp, c_i64, vp, vp, c_i64, vp, vp, vp]
@@ -120,6 +122,7 @@ _F32_TWIN = {
     "mp3b200_encode_streams_ex": "mp3b200_encode_streams_f32",
     "mp3b200_encode_streams_tagged_ex": "mp3b200_encode_streams_tagged_f32",
     "mp3b200_encode_streams_device_ex": "mp3b200_encode_streams_device_f32",
+    "mp3b200_encode_streams_tagged_device": "mp3b200_encode_streams_tagged_device_f32",
     "mp3b200_debug_resample": "mp3b200_debug_resample_f32",
     "mp3b200_debug_replaygain": "mp3b200_debug_replaygain_f32",
 }
@@ -261,9 +264,10 @@ def crc16_combine(crc_a, crc_b, len_b):
     return _check(L.mp3b200_crc16_combine(int(crc_a), int(crc_b), int(len_b)))
 
 
-def lametag_size(channels, samplerate, kbps):
-    """Size of the Xing / Info / LAME tag frame of a configuration (0: InitVbrTag would switch the tag off)."""
-    return _check(lib().mp3b200_lametag_size(channels, samplerate, kbps))
+def lametag_size(channels, samplerate, kbps, resample=False):
+    """Size of the Xing / Info / LAME tag frame of a configuration (0: InitVbrTag would switch the tag off).  resample=True:
+    see Mp3Encoder."""
+    return _check(lib().mp3b200_lametag_size_ex(channels, samplerate, kbps, RESAMPLE if resample else 0))
 
 
 def lametag_build(channels, samplerate, kbps, nframes, music_bytes, music_crc, encoder_padding):
@@ -525,6 +529,29 @@ def encode_streams_device(channels, samplerate, kbps, d_pcm_ptr, pcm_off, nsampl
                                                                 d_pcm_ptr, pcm_off.ctypes.data, nsamples.ctypes.data, d_out_ptr,
                                                                 out_off.ctypes.data, tm.ctypes.data))
     return tm
+
+
+def encode_streams_device_tagged(channels, samplerate, kbps, d_pcm_ptr, pcm_off, nsamples, d_out_ptr, out_off, resample=False,
+                                 float32=False, find_replay_gain=False):
+    """encode_streams_device with the tag on (and, with find_replay_gain=True, the ReplayGain analysis): stream s is written
+    as one finished file at d_out + out_off[s], its Info / LAME tag frame followed by its audio, byte-identical to what
+    encode_streams_replaygain returns for the same samples.  Stream s needs stream_bytes(...) + lametag_size(...) bytes of
+    room (with the same `resample`).  Returns (out_bytes, title_db, album_db): the
+    length of each file, GetTitleGain of each stream in dB and GetAlbumGain of the batch (-24601: less than one RMS window,
+    or nothing was analysed)."""
+    pcm_off = np.ascontiguousarray(pcm_off, dtype=np.int64)
+    nsamples = np.ascontiguousarray(nsamples, dtype=np.int64)
+    out_off = np.ascontiguousarray(out_off, dtype=np.int64)
+    S = len(nsamples)
+    got = np.zeros(max(S, 1), dtype=np.int64)
+    title = np.zeros(max(S, 1), dtype=np.float64)
+    album = ctypes.c_double(0.0)
+    flags = (REPLAYGAIN if find_replay_gain else 0) | (RESAMPLE if resample else 0)
+    _check(_entry("mp3b200_encode_streams_tagged_device", float32)(channels, samplerate, kbps, flags, S, d_pcm_ptr, pcm_off.ctypes.data,
+                                                                    nsamples.ctypes.data, d_out_ptr, out_off.ctypes.data,
+                                                                    got.ctypes.data, title.ctypes.data, ctypes.byref(album)))
+    return ([int(g) for g in got[:S]], [float(t) for t in title[:S]],
+            float(album.value) if S else float(GAIN_NOT_ENOUGH_SAMPLES))
 
 
 def debug_resample(channels, samplerate, kbps, left, right=None, ny=None):
