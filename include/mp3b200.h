@@ -231,7 +231,7 @@ int mp3b200_encode_streams_tagged_ex(int channels, int samplerate, int kbps, int
  * d_out) and returns after that stream has drained.  The packer writes each stream's audio straight behind the room of its
  * tag frame; the frames are built on the host, uploaded in one copy and put in place by one kernel (k_tag_scatter).
  * _device_f32 takes Float32 samples, laid out the same way, as mp3b200_encode_streams_device_f32 does; a sample that is not
- * finite, or beyond 2^35 once scaled, returns MP3B200_ERR_CONFIG, and no tag frame is placed (the audio bytes in d_out are
+ * finite, or beyond 2^40 once scaled, returns MP3B200_ERR_CONFIG, and no tag frame is placed (the audio bytes in d_out are
  * then unspecified). */
 int mp3b200_encode_streams_tagged_device(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
                                          const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off,
@@ -368,7 +368,7 @@ int mp3b200_debug_resample(int channels, int samplerate, int kbps, const int16_t
  * Samples that are not finite (before or after the scale) are refused with MP3B200_ERR_CONFIG: the host calls refuse them
  * before anything runs and leave a handle untouched; mp3b200_encode_streams_device_f32 finds them on the device, and its
  * output buffer is then unspecified.  lamejs would carry NaN through its psy model and rate loop.
- * Samples beyond 2^35 (2^20 x full scale) once scaled are refused the same way: the library is compared with lamejs up to
+ * Samples beyond 2^40 (2^25 x full scale) once scaled are refused the same way: the library is compared with lamejs up to
  * there (DESIGN.md 12).  Below that, a frame whose bits do not fit its slot even at
  * global_gain 255 (from about 2e5 x full scale, depending on signal and bitrate) is refused with MP3B200_ERR_CONFIG by the
  * call that encodes it, the call in which lamejs throws; it is never packed.  Every handle of a refused call is left exactly

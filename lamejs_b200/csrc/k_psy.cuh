@@ -378,7 +378,7 @@ k_psy_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ s
     if (a > 0.0) {
       const double cnt = (double)(hi - lo + 1);
       a = 20.0 * (m * cnt - a) / (a * (lines - 1));
-      k = js_trunc(a);
+      k = js_trunc<DOM_TRUNC_MASK_IDX>(a);
       if (k > 8) k = 8;
     }
     o->mask_idx[b] = (unsigned char)k;
@@ -609,7 +609,8 @@ k_stream_scan(const Mp3Tables* __restrict__ T, StreamDesc* __restrict__ streams,
 __device__ __noinline__ double psy_log10(double x) { return m3_log10(x); }
 /* 0 | (log10(ratio) * 16) for 1 <= ratio < 10^1.5, from the threshold table when the host validated it (mp3_config.h) */
 __device__ __forceinline__ int log10_times16_trunc(const Mp3Tables* T, double ratio) {
-  if (!T->l16_ok) return js_trunc(psy_log10(ratio) * 16.0);
+  if (!T->l16_ok) return js_trunc<DOM_TRUNC_LOG16>(psy_log10(ratio) * 16.0);
+  DOMAIN_MISS(DOM_LOG16_TABLE, !(ratio >= 1.0 && ratio < 31.622776601683793));
   int i = 0;
 #pragma unroll
   for (int k = 1; k <= 24; k++) i += ratio >= T->l16_thr[k] ? 1 : 0;

@@ -243,6 +243,7 @@ __device__ __forceinline__ unsigned pair_bits(unsigned w, int cat, unsigned lin)
 }
 /* table and bits of a region from the warp totals (a, b, c) of its three packed sums */
 __device__ Q_HELPER int region_pick(int mx, const RegionClass& rc, int a, int b, int c, int* bits) {
+  DOMAIN_MISS(DOM_REGION_MX, mx > Q_IXMAX);
   if (mx > Q_IXMAX) { *bits = Q_LARGE_BITS; return -1; }
   if (mx == 0) return 0;
   int t = rc.t1;
@@ -274,6 +275,16 @@ Q_UNROLL(Q_RT_UNROLL)
 Q_UNROLL(Q_RT_UNROLL)
     for (int p = p0; p < p1; p += 32) { const unsigned w = w32[p]; s += __ldg(&tab[((w & 0xfu) << 4) | (w >> 16)]); }
   }
+#ifdef MP3_DOMAIN_CHECK
+  {   /* the same sums field by field, unpacked: a field that carried into its neighbour differs */
+    unsigned fa = 0, fb = 0, fc = 0;
+    for (int p = p0; p < p1; p += 32) {
+      const unsigned v = rc.cat == 6 ? pair_bits(w32[p], 6, rc.lin) : __ldg(&g_cat_tab[rc.cat][((w32[p] & 0xfu) << 4) | (w32[p] >> 16)]);
+      fa += v & 0x7ffu; fb += (v >> 11) & 0x7ffu; fc += v >> 22;
+    }
+    DOMAIN_MISS(DOM_BITSUM_FIELD, fa > 0x7ffu || fb > 0x7ffu || fc > 0x3ffu || wsumu(fa) > 0xffffu || wsumu(fb) > 0xffffu);
+  }
+#endif
   /* warp totals need up to 14 bits: reduce (a, b) as two 16-bit fields, c alone */
   const unsigned ab = wsumu((s & 0x7ffu) | (((s >> 11) & 0x7ffu) << 16));
   const int c = wsum((int)(s >> 22));
@@ -392,9 +403,10 @@ Q_UNROLL(Q_CB_UNROLL)
       if (2 * p < qend) {
         const float2 xp = *reinterpret_cast<const float2*>(&wk->xrpow[2 * p]);
         double x0 = (double)xp.x * istep, x1 = (double)xp.y * istep;
-        x0 += (double)__ldg(&T->adj43[js_trunc(x0)]);
-        x1 += (double)__ldg(&T->adj43[js_trunc(x1)]);
-        v = (unsigned)js_trunc(x0) | ((unsigned)js_trunc(x1) << 16);
+        x0 += (double)__ldg(&T->adj43[js_trunc<DOM_TRUNC_QUANT>(x0)]);
+        x1 += (double)__ldg(&T->adj43[js_trunc<DOM_TRUNC_QUANT>(x1)]);
+        v = (unsigned)js_trunc<DOM_TRUNC_QUANT>(x0) | ((unsigned)js_trunc<DOM_TRUNC_QUANT>(x1) << 16);
+        DOMAIN_MISS(DOM_PACK_SEARCH, x0 >= 32768.0 || x1 >= 32768.0);
         if (v != 0 && p < i0h) top = 2 * p + 2;
       }
       iw32[p] = v;
@@ -454,9 +466,10 @@ Q_UNROLL(Q_CB_UNROLL)
         if (md == 2) { v0 = (compare01 > (double)xp.x) ? 0u : 1u; v1 = (compare01 > (double)xp.y) ? 0u : 1u; }
         else {
           double x0 = (double)xp.x * istep, x1 = (double)xp.y * istep;
-          x0 += (double)__ldg(&T->adj43[js_trunc(x0)]);
-          x1 += (double)__ldg(&T->adj43[js_trunc(x1)]);
-          v0 = (unsigned)js_trunc(x0); v1 = (unsigned)js_trunc(x1);
+          x0 += (double)__ldg(&T->adj43[js_trunc<DOM_TRUNC_QUANT>(x0)]);
+          x1 += (double)__ldg(&T->adj43[js_trunc<DOM_TRUNC_QUANT>(x1)]);
+          v0 = (unsigned)js_trunc<DOM_TRUNC_QUANT>(x0); v1 = (unsigned)js_trunc<DOM_TRUNC_QUANT>(x1);
+          DOMAIN_MISS(DOM_PACK_OUTER, x0 >= 32768.0 || x1 >= 32768.0);
         }
         if (z1) v1 = 0;
         v = v0 | (v1 << 16);
@@ -536,7 +549,7 @@ Q_UNROLL(Q_CN_UNROLL)
         { f32s t; t = noise; wk->pn_noise_log[sfb] = t.v; }
       }
       if (noise > 0.0) {
-        int tmp = js_trunc(noise * 10 + .5);
+        int tmp = js_trunc<DOM_TRUNC_NOISE>(noise * 10 + .5);
         if (tmp < 1) tmp = 1;
         ssd += tmp * tmp;
         over++;
@@ -1305,6 +1318,7 @@ __device__ __noinline__ int band_stats_w(const Mp3Tables* T, const short* ix, in
       const unsigned v = __ldg(&tab[min(w & 0xffffu, 15u) * 16 + min(w >> 16, 15u)]);
       sa += v & 0x7ffu; sb += (v >> 11) & 0x7ffu; sc += v >> 22;
     }
+    DOMAIN_MISS(DOM_BITSUM_FIELD, sa > 0xffffu || sb > 0xffffu || sc > 0xffffu);
     ds->ab[b][c] = sa | (sb << 16);
     ds->cc[b][c] = (unsigned short)sc;
   }
@@ -1598,12 +1612,27 @@ __device__ __noinline__ void pack_gc_w(const Mp3Tables* T, unsigned int* buf, co
   __syncwarp();
 }
 
+/* writeheader (BitStream.js:218-229): n bits of val at bit pos, byte by byte, each byte OR-ed with ((val >> j) << shift)
+ * truncated to 8 bits -- val is not masked to n bits, so a value that does not fit its field (part2_3_length + part2_length
+ * above 4095 in a 12-bit field, which an LSF granule of loud input can reach) sets bits of the fields before it in the same
+ * byte, as lamejs's bytes show */
+__device__ __forceinline__ void put_header_bits(unsigned int* buf, int pos, int val, int n) {
+  while (n > 0) {
+    const int k = min(n, 8 - (pos & 7));
+    n -= k;
+    const unsigned byte = ((unsigned)(val >> n) << (8 - (pos & 7) - k)) & 0xffu;
+    const int b = pos >> 3;
+    atomicOr(&buf[b >> 2], byte << (24 - 8 * (b & 3)));
+    pos += k;
+  }
+}
+
 /* header + side info (encodeSideInfo2, BitStream.js:259-426, MPEG-1) by one thread */
 /* fin: the frame's four (two) finished GranuleInfoDev in HBM, [gr * nch + ch]; scfsi: [ch][4] */
 __device__ __noinline__ void pack_sideinfo(const Mp3Tables* T, unsigned int* buf, const GranuleInfoDev* __restrict__ fin,
                                            const int* scfsi, int padding) {
   int p = 0;
-#define WH(v, n) do { put_bits(buf, p, (unsigned)(v), (n)); p += (n); } while (0)
+#define WH(v, n) do { put_header_bits(buf, p, (int)(v), (n)); p += (n); } while (0)
   const int nch = T->nch;
   WH(T->mpeg25 ? 0xffe : 0xfff, 12); WH(T->version, 1); WH(4 - 3, 2); WH(1, 1);
   WH(T->bitrate_index, 4); WH(T->samplerate_index, 2); WH(padding, 1); WH(0, 1);

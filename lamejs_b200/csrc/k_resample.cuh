@@ -68,12 +68,15 @@ k_resample(const ResampleDesc* __restrict__ descs, int ratio, int scale_applied,
  * where the <true> instantiations of the psy analysis and the filterbank, k_resample<float> and the ReplayGain analysis read
  * them.  A non-finite value (before or after the scale), or one beyond MP3_F32_MAX_SAMPLE after it, sets refused[0] and is
  * staged as 0, so that nothing downstream sees it: such a call is refused, and its output is not used.
- * MP3_F32_MAX_SAMPLE (2^35, 2^20 x full scale) is the loudest input the library has been compared with lamejs at, stage by
- * stage and byte for byte (tests/golden/lamejs_loud_golden.json).  Louder rungs the fixtures hold, up to 3.3e7 x full scale,
- * still encode in lamejs on some signals but not yet byte-identically here; from 1e15 x full scale lamejs's own masking
- * energies overflow Float32, from 1e30 its MDCT lines, and it encodes (when it does not throw) from infinities and NaNs
- * (DESIGN.md 12). */
-#define MP3_F32_MAX_SAMPLE 34359738368.0f
+ * MP3_F32_MAX_SAMPLE (2^40, 2^25 x full scale) lies just above the rung 3.3e7 x full scale of
+ * tests/golden/lamejs_loud_golden.json, the loudest at which the library equals lamejs stage by stage and byte for byte with
+ * every domain counter (mp3_device.cuh) at zero.  At 1e9 x full scale a Float32 store overflows; from 1e15 lamejs's own
+ * masking energies overflow Float32, from 1e30 its MDCT lines, and it encodes (when it does not throw) from infinities and
+ * NaNs (DESIGN.md 12).  A test build may set another limit with
+ * -DMP3_F32_MAX_SAMPLE=...; non-finite samples stay refused. */
+#ifndef MP3_F32_MAX_SAMPLE
+#define MP3_F32_MAX_SAMPLE 1099511627776.0f
+#endif
 #define STAGE_THREADS 256
 #define STAGE_PER_THREAD 4
 struct StageDesc {

@@ -384,7 +384,7 @@ int check_refusals() {
   int r[2] = {0, 0};
   CK(cudaMemcpyAsync(r, t_ctx.ws.refusals.p, sizeof r, cudaMemcpyDeviceToHost, t_ctx.st));
   CK(cudaStreamSynchronize(t_ctx.st));
-  if (r[0]) { g_err = "non-finite input sample (or one beyond 2^35 once scaled)"; return MP3B200_ERR_CONFIG; }
+  if (r[0]) { g_err = "non-finite input sample (or one beyond 2^40 once scaled)"; return MP3B200_ERR_CONFIG; }
   if (r[1]) { g_err = "frame over its bit budget (input too loud to encode)"; t_over_budget = true; return MP3B200_ERR_CONFIG; }
   return 0;
 }
@@ -1038,7 +1038,7 @@ int check_input(const Config* cfg, int nstreams, const float* const* left, const
   for (int s = 0; s < nstreams; s++)
     if (!finite_after_scale(cfg->host, left[s], nsamples[s]) ||
         (cfg->host.nch == 2 && !finite_after_scale(cfg->host, right_row(left, right, s), nsamples[s]))) {
-      g_err = "non-finite input sample (or one beyond 2^35 once scaled)"; return MP3B200_ERR_CONFIG;
+      g_err = "non-finite input sample (or one beyond 2^40 once scaled)"; return MP3B200_ERR_CONFIG;
     }
   return MP3B200_OK;
 }
@@ -1767,5 +1767,17 @@ int mp3b200_debug_replaygain_f32(int channels, int samplerate, int kbps, int fla
 extern "C" int mp3b200_debug_taskstat(int* out, int rows) {
   if (rows > (1 << 16)) rows = 1 << 16;
   return cudaMemcpyFromSymbol(out, g_taskstat, sizeof(int) * 8 * (size_t)rows) == cudaSuccess ? 0 : -1;
+}
+#endif
+
+#ifdef MP3_DOMAIN_CHECK
+/* the out-of-domain counters of every DomainSite (mp3_device.cuh) on the current device, cleared after reading; returns the
+ * number of sites (out needs that many slots) */
+extern "C" int mp3b200_debug_domain_hits(unsigned long long* out, int cap) {
+  if (cap < DOM_NSITES) return DOM_NSITES;
+  if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+  if (cudaMemcpyFromSymbol(out, g_domain_hits, sizeof(unsigned long long) * DOM_NSITES) != cudaSuccess) return -1;
+  static const unsigned long long zero[DOM_NSITES] = {};
+  return cudaMemcpyToSymbol(g_domain_hits, zero, sizeof zero) == cudaSuccess ? DOM_NSITES : -1;
 }
 #endif

@@ -507,6 +507,23 @@ def debug_replaygain(channels, samplerate, kbps, left, right=None, resample=Fals
             "reruns": int(stats[2]), "ms": float(stats[3:4].view(np.float32)[0])}
 
 
+DOMAIN_SITES = ("trunc_mask_idx", "trunc_log16", "trunc_quant", "trunc_noise", "dmax", "dmin", "pack_search", "pack_outer",
+                "region_mx", "bitsum_field", "log16_table", "f32_overflow")     # DomainSite (mp3_device.cuh)
+
+
+def debug_domain_hits():
+    """A library built with -DMP3_DOMAIN_CHECK only: per DomainSite, how many arguments fell outside the domain the site is
+    exact on since the last call (the counters are cleared).  int64 array indexed like DOMAIN_SITES."""
+    fn = getattr(lib(), "mp3b200_debug_domain_hits", None)
+    if fn is None:
+        raise Mp3B200Error("the library was built without MP3_DOMAIN_CHECK")
+    out = np.zeros(len(DOMAIN_SITES), dtype=np.uint64)
+    fn.argtypes = [ctypes.c_void_p, ctypes.c_int]
+    n = _check(fn(out.ctypes.data, len(out)))
+    assert n == len(DOMAIN_SITES), n
+    return out.astype(np.int64)
+
+
 def debug_music_crc(d_buf_ptr, offsets, lengths, timed=False):
     """k_music_crc on byte ranges of a device buffer (raw pointer as int): list of CRC-16 values (+ ms if `timed`)."""
     off = np.ascontiguousarray(offsets, dtype=np.int64)

@@ -63,13 +63,44 @@ def compare_quant_state(g, tr, G, ch, label=""):
             assert d is None, (label, k, "device chain: frame start != predecessor's end at (frame - 1, channel) %s" % d)
 
 
+def differences(g, tr, ref, G, ch):
+    """Every tap of `g` (debug_stages with want=ALL_TAPS) that differs from the oracle trace `tr` / bytes `ref`, as
+    (tap, index of its first differing element) sorted by that index -- (frame, granule, channel, ...) for the per-granule
+    taps, so the first entry names the earliest frame and the tap where the kernel and the oracle part."""
+    sl = (slice(None), slice(0, G), slice(0, ch))
+    pairs = [(k, g[k], tr[k][sl]) for k in ("blocktype", "en_l", "thm_l", "en_s", "thm_s", "xr", "l3_enc", "scalefac",
+                                             "subblock_gain", "max_nonzero_coeff", "xmin", "xrpow_max")]
+    pairs.append(("ath_adjust", g["ath_adjust"], tr["ath_adjust"]))
+    pairs.append(("scfsi", g["scfsi"], tr["scfsi"][:, :ch]))
+    for j, (k, i) in enumerate(GINFO_FIELDS):
+        got = g["ginfo"][..., j]
+        if k == "table_select":
+            got = np.where(got == 14, 16, got)        # see compare()
+        pairs.append(("%s%s" % (k, "" if i is None else "[%d]" % i), got, tr[k][sl] if i is None else tr[k][sl + (i,)]))
+    for k, fields in STATE_FIELDS.items():
+        for j, f in enumerate(fields):
+            pairs.append((f, g[k][:, j], tr[f][:, :ch]))
+    out = []
+    for k, a, b in pairs:
+        d = _first_diff(a, b)
+        if d is not None:
+            out.append((k, d))
+    if g["bytes"].tobytes() != ref:
+        a, b = np.frombuffer(g["bytes"].tobytes(), np.uint8), np.frombuffer(ref, np.uint8)
+        n = min(len(a), len(b))
+        bad = np.nonzero(a[:n] != b[:n])[0]
+        out.append(("bytes", [int(bad[0]) if len(bad) else n]))
+    return sorted(out, key=lambda e: (e[0] == "bytes", e[1][:1], e[1]))
+
+
 def compare(g, tr, ref, G, ch, label=""):
     """Asserts every tap of `g` (debug_stages with want=ALL_TAPS) equals the oracle trace `tr` / bytes `ref`."""
     assert np.array_equal(g["blocktype"], tr["blocktype"][:, :G, :ch]), label
     assert np.array_equal(g["ath_adjust"], tr["ath_adjust"]), label
     for k in ("xr", "en_l", "thm_l", "en_s", "thm_s"):
-        assert bits_equal(g[k], tr[k][:, :G, :ch]), (label, k)          # relative tolerance: 0
-    assert np.array_equal(g["l3_enc"], tr["l3_enc"][:, :G, :ch]), label
+        # relative tolerance: 0
+        assert bits_equal(g[k], tr[k][:, :G, :ch]), (label, k, "first (frame, granule, channel, ...) differing: %s" % _first_diff(g[k], tr[k][:, :G, :ch]))
+    assert np.array_equal(g["l3_enc"], tr["l3_enc"][:, :G, :ch]), (label, "l3_enc", _first_diff(g["l3_enc"], tr["l3_enc"][:, :G, :ch]))
     for j, (k, i) in enumerate(GINFO_FIELDS):
         want = tr[k][:, :G, :ch] if i is None else tr[k][:, :G, :ch, i]
         got = g["ginfo"][..., j]

@@ -2,7 +2,7 @@
 call schedule, host, device and tagged whole streams, and the ReplayGain fixtures through handles and whole streams.  Where
 lamejs encodes, the bytes and per-call sizes are lamejs's; where it throws (a frame's bits do not fit its slot), the
 library refuses the same call with MP3B200_ERR_CONFIG, k_q_pack has not packed the frame, and a refused handle call leaves
-every handle of the call as it was.  Samples beyond 2^35 once scaled (beyond 2^20 x full scale) are refused by the input
+every handle of the call as it was.  Samples beyond 2^40 once scaled (beyond 2^25 x full scale) are refused by the input
 gate.  The loudest encodable rung of each configuration is compared with the oracle stage by stage."""
 import hashlib
 import json
@@ -20,7 +20,7 @@ import stage_taps  # noqa: E402
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLDEN = json.load(open(os.path.join(HERE, "golden", "lamejs_loud_golden.json")))
-GATE = 2.0 ** 35                       # MP3_F32_MAX_SAMPLE (k_resample.cuh)
+GATE = 2.0 ** 40                       # MP3_F32_MAX_SAMPLE (k_resample.cuh)
 FRACTIONAL = (44100, 22050, 11025)     # see tests/test_float_golden_cpu.py
 
 
@@ -68,8 +68,9 @@ def rows(c):
 def test_golden_splits_at_the_gate():
     assert len(ENCODED) > 100 and len(REFUSED_AT_GATE) > 50 and len(REPLAYGAIN) >= 6
     assert any(GOLDEN[n]["thrown"] is not None for n in ENCODED) and any(GOLDEN[n]["thrown"] is None for n in ENCODED)
-    # the loudest rung below the gate holds streams lamejs encodes
-    assert any(GOLDEN[n]["thrown"] is None and GOLDEN[n]["magnitude"] == 2 ** 20 for n in ENCODED)
+    # the loudest rung below the gate (3.3e7 x full scale) holds streams lamejs encodes; 1e9 lies beyond it
+    assert any(GOLDEN[n]["thrown"] is None and GOLDEN[n]["magnitude"] == 3.3e7 for n in ENCODED)
+    assert not any(GOLDEN[n]["magnitude"] == 1e9 for n in ENCODED)
     assert len(loudest_encodable()) == len({cfg_of(GOLDEN[n]) for n in ENCODED})
 
 
@@ -208,32 +209,51 @@ def test_loudest_encodable_rung_matches_the_oracle_stage_by_stage(M, name):
     stage_taps.compare(g, tr, ref, G, ch, name)
 
 
+@pytest.mark.parametrize("entry", ["host", "handle", "device"])
 @pytest.mark.parametrize("name", REFUSED_AT_GATE)
-def test_input_beyond_the_gate_is_refused(M, name):
+def test_input_beyond_the_limit_is_refused(M, name, entry):
+    """every entry point refuses input beyond the limit: the host calls and a handle before anything runs (the handle
+    unchanged), the device call from k_stage_f32's flag"""
+    import torch
+
     c = GOLDEN[name]
     ch, sr, kb = cfg_of(c)
     rs = M.out_samplerate(ch, sr, kb) != sr
     lf, rf, _ = rows(c)
-    with pytest.raises(M.Mp3B200Error, match="2\\^35"):
-        M.encode_streams(ch, sr, kb, [lf], None if rf is None else [rf], resample=rs)
-    e = M.Mp3Encoder(ch, sr, kb, resample=rs)
-    before = e.export_state()
-    with pytest.raises(M.Mp3B200Error, match="2\\^35"):
-        e.encodeBuffer(lf, rf)
-    assert e.export_state() == before
-    e.close()
+    if entry == "host":
+        with pytest.raises(M.Mp3B200Error, match="2\\^40"):
+            M.encode_streams(ch, sr, kb, [lf], None if rf is None else [rf], resample=rs)
+    elif entry == "handle":
+        e = M.Mp3Encoder(ch, sr, kb, resample=rs)
+        before = e.export_state()
+        with pytest.raises(M.Mp3B200Error, match="2\\^40"):
+            e.encodeBuffer(lf, rf)
+        assert e.export_state() == before
+        e.close()
+    else:
+        pcm = np.concatenate([lf, rf]) if ch == 2 else lf
+        d_pcm = torch.from_numpy(pcm).cuda()
+        d_out = torch.zeros(M.stream_bytes(ch, sr, kb, len(lf), resample=rs), dtype=torch.uint8, device="cuda")
+        with pytest.raises(M.Mp3B200Error, match="2\\^40"):
+            M.encode_streams_device(ch, sr, kb, d_pcm.data_ptr(), [0], [len(lf)], d_out.data_ptr(), [0], resample=rs,
+                                    float32=True)
 
 
-def test_seek_refuses_history_beyond_the_gate(M):
-    """seek only sets a handle's state (it encodes nothing): its history is refused at the gate, and the handle stays fresh"""
+def test_seek_refuses_history_beyond_the_limit(M):
+    """seek only sets a handle's state (it encodes nothing): its history is refused beyond the limit, and the handle stays
+    fresh; the same history scaled to peak exactly at the limit is taken"""
     ch, sr, kb = 2, 44100, 128
     frame, fs = 5, 1152
     n = frame * fs + 224 - (frame * fs - 1104)
     l, r = FS.loud("noise", 1e9, n, sr, 3, 1.0)
     e = M.Mp3Encoder(ch, sr, kb)
     before = e.export_state()
-    with pytest.raises(M.Mp3B200Error, match="2\\^35"):
+    with pytest.raises(M.Mp3B200Error, match="2\\^40"):
         e.seek(frame, l.astype(np.float32), r.astype(np.float32))
     assert e.export_state() == before
-    e.seek(frame, (l / 1e9).astype(np.float32), (r / 1e9).astype(np.float32))
+    k = GATE / max(np.abs(l).max(), np.abs(r).max())
+    lk, rk = (l * k).astype(np.float32), (r * k).astype(np.float32)
+    lk[np.argmax(np.abs(lk))] = np.float32(GATE)                # one sample exactly at the limit
+    assert max(np.abs(lk).max(), np.abs(rk).max()) == GATE
+    e.seek(frame, lk, rk)
     e.close()
