@@ -81,6 +81,26 @@ int mp3b200_encode_batch(mp3b200_encoder* const* handles, const int16_t* const* 
                          const int* nsamples, uint8_t* const* out, const int* cap, int nstreams, int* out_bytes);
 int mp3b200_flush_batch(mp3b200_encoder* const* handles, uint8_t* const* out, const int* cap, int nstreams, int* out_bytes);
 
+/* Streaming handles fed from device memory: mp3b200_encode / mp3b200_encode_f32 / mp3b200_encode_batch /
+ * mp3b200_encode_batch_f32 with the sample rows in device memory (a model producing audio on the GPU in chunks feeds them
+ * without a copy to the host).  Everything else means exactly what it means there: bytes, error codes, repeated handles,
+ * failed handles keeping their samples, Float32 mode, tags, ReplayGain, resampling; a handle may take host and device calls
+ * in any mix, and its state blob does not tell them apart.  The output stays in host memory.
+ * Every row (right rows of mono handles aside) must be device or managed memory on the handle's device
+ * (cudaPointerGetAttributes); anything else returns MP3B200_ERR_HANDLE before any handle changes.  Float32 rows are
+ * checked on the device before any handle changes, and refused with MP3B200_ERR_CONFIG like the host calls refuse them.
+ * The call first waits for work already queued on the legacy default stream (where torch / plain CUDA callers produce the
+ * rows), and has finished reading the rows when it returns: the caller may then overwrite or free them.
+ * Without a device these calls return MP3B200_ERR_CUDA. */
+int mp3b200_encode_device(mp3b200_encoder* h, const int16_t* d_left, const int16_t* d_right, int nsamples, uint8_t* out, int cap);
+int mp3b200_encode_device_f32(mp3b200_encoder* h, const float* d_left, const float* d_right, int nsamples, uint8_t* out, int cap);
+int mp3b200_encode_batch_device(mp3b200_encoder* const* handles, const int16_t* const* d_left, const int16_t* const* d_right,
+                                const int* nsamples, uint8_t* const* out, const int* cap, int nstreams, int* out_bytes);
+int mp3b200_encode_batch_device_f32(mp3b200_encoder* const* handles, const float* const* d_left, const float* const* d_right,
+                                    const int* nsamples, uint8_t* const* out, const int* cap, int nstreams, int* out_bytes);
+/* the CUDA device a handle was created on (the device of mp3b200_set_device at mp3b200_create), or MP3B200_ERR_HANDLE */
+int mp3b200_encoder_device(const mp3b200_encoder* h);
+
 /* ---- encoder state: checkpoint / resume, and one stream cut into segments (SURVEY.md 8(e)(2)) ----------------------------
  * lamejs keeps an Mp3Encoder's state in JS objects (gfc.*: ATH adjust, block-type FSM, OldValue / CurrentStep, the previous
  * granule's masking, mfbuf); a JS caller checkpoints by keeping the object alive.  Here the state is a blob:

@@ -8,6 +8,8 @@
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdio.h>
+#include <algorithm>
+#include <array>
 #include <stdlib.h>
 #include <string.h>
 #include <atomic>
@@ -27,6 +29,7 @@
 #include "k_tag.cuh"
 #include "k_resample.cuh"
 #include "k_replaygain.cuh"
+#include "k_stage.cuh"
 #include "mp3_tag.h"
 
 namespace {

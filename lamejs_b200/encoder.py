@@ -98,6 +98,11 @@ def lib():
     L.mp3b200_debug_stages_f32.argtypes = [ctypes.POINTER(DebugTaps), vp, vp]
     L.mp3b200_debug_resample_f32.argtypes = [c_int, c_int, c_int, vp, vp, c_i64, vp, c_i64]
     L.mp3b200_debug_replaygain_f32.argtypes = [c_int, c_int, c_int, c_int, vp, vp, c_i64, vp, vp, c_i64, vp, vp, vp]
+    L.mp3b200_encode_device.argtypes = [vp, vp, vp, c_int, vp, c_int]
+    L.mp3b200_encode_device_f32.argtypes = [vp, vp, vp, c_int, vp, c_int]
+    L.mp3b200_encode_batch_device.argtypes = [vp, vp, vp, vp, vp, vp, c_int, vp]
+    L.mp3b200_encode_batch_device_f32.argtypes = [vp, vp, vp, vp, vp, vp, c_int, vp]
+    L.mp3b200_encoder_device.argtypes = [vp]
     _lib = L
     return L
 
@@ -114,10 +119,36 @@ def _rows(lefts, rights=None):
     return lefts, [l if r is None else np.ascontiguousarray(r, dtype=dt) for l, r in zip(lefts, rights)], f32
 
 
+def _on_cuda(x):
+    """True for a torch tensor in CUDA memory"""
+    return bool(getattr(x, "is_cuda", False))
+
+
+def _device_rows(lefts, rights, device):
+    """_rows for CUDA tensors: contiguous Float32 (floating dtypes, rounded once) or Int16 tensors on `device`, the encoders'
+    CUDA device index.  Raises ValueError for a row in host memory or on another device.  Makes torch's default stream wait
+    for the current one, as the library's calls wait for the default stream: rows produced on a side stream are ordered."""
+    import torch
+    rights = [None] * len(lefts) if rights is None else list(rights)
+    rows = [x for x in (*lefts, *rights) if x is not None]
+    if not all(_on_cuda(x) for x in rows):
+        raise ValueError("one call takes rows either all in host memory or all in CUDA memory")
+    if any(x.device.index != device for x in rows):
+        raise ValueError("CUDA rows must be on the encoders' device (cuda:%d)" % device)
+    f32 = any(x.dtype.is_floating_point or x.dtype.is_complex for x in rows)
+    dt = torch.float32 if f32 else torch.int16
+    lefts = [x.to(dt).contiguous() for x in lefts]
+    rights = [l if r is None else r.to(dt).contiguous() for l, r in zip(lefts, rights)]
+    torch.cuda.default_stream(device).wait_stream(torch.cuda.current_stream(device))
+    return lefts, rights, f32
+
+
 # each Int16 entry point and its Float32 twin, which takes the same arguments with Float32 rows
 _F32_TWIN = {
     "mp3b200_encode": "mp3b200_encode_f32",
     "mp3b200_encode_batch": "mp3b200_encode_batch_f32",
+    "mp3b200_encode_device": "mp3b200_encode_device_f32",
+    "mp3b200_encode_batch_device": "mp3b200_encode_batch_device_f32",
     "mp3b200_seek": "mp3b200_seek_f32",
     "mp3b200_encode_streams_ex": "mp3b200_encode_streams_f32",
     "mp3b200_encode_streams_tagged_ex": "mp3b200_encode_streams_tagged_f32",
@@ -296,6 +327,7 @@ class Mp3Encoder:
         flags = RESAMPLE if resample else 0
         rc = self._L.mp3b200_create_ex(channels, samplerate, kbps, flags, ctypes.byref(self._h))
         _check(rc)
+        self.device = _check(self._L.mp3b200_encoder_device(self._h))     # CUDA tensors fed to it must live there
         self.tag_on = bool(write_vbr_tag) and _check(self._L.mp3b200_set_write_vbr_tag(self._h, 1)) == 1
         self._tag_room = _check(self._L.mp3b200_lametag_size_ex(channels, samplerate, kbps, flags)) if self.tag_on else 0
         self.replay_gain_on = bool(find_replay_gain) and _check(self._L.mp3b200_set_find_replay_gain(self._h, 1)) == 1
@@ -328,12 +360,19 @@ class Mp3Encoder:
 
     def encodeBuffer(self, left, right=None):
         """Int16 samples, or floating-point samples (Float32Array / plain Array in lamejs: rounded to Float32 once and
-        scaled like lamejs scales them; non-finite values are refused)"""
-        (left,), (right,), f32 = _rows([left], [None if self.channels == 1 else right])
+        scaled like lamejs scales them; non-finite values are refused).  CUDA torch tensors are encoded from device memory
+        (mp3b200_encode_device): the same bytes, without a copy of the samples to the host."""
+        right = None if self.channels == 1 else right
+        if _on_cuda(left) or _on_cuda(right):
+            (left,), (right,), f32 = _device_rows([left], [right], self.device)
+            name, ptr = "mp3b200_encode_device", (lambda x: x.data_ptr())
+        else:
+            (left,), (right,), f32 = _rows([left], [right])
+            name, ptr = "mp3b200_encode", (lambda x: x.ctypes.data)
         assert len(left) == len(right)
         cap = int(1.25 * len(left) + 7200) + self._tag_room     # index.js:114,124
         buf = np.empty(cap, dtype=np.uint8)
-        n = _check(_entry("mp3b200_encode", f32)(self._h, left.ctypes.data, right.ctypes.data, len(left), buf.ctypes.data, cap))
+        n = _check(_entry(name, f32)(self._h, ptr(left), ptr(right), len(left), buf.ctypes.data, cap))
         return buf[:n].tobytes()
 
     def flush(self):
@@ -376,18 +415,27 @@ class Mp3Encoder:
 
 def encode_batch(encoders, lefts, rights=None):
     """encodeBuffer on many live Mp3Encoder objects of one configuration in ONE pipeline launch (SURVEY 8(b) batch row):
-    returns [enc.encodeBuffer(l, r) for ...] byte strings."""
+    returns [enc.encodeBuffer(l, r) for ...] byte strings.  CUDA torch tensors are encoded from device memory
+    (mp3b200_encode_batch_device); one call takes rows all in host memory or all on the encoders' CUDA device."""
     S = len(encoders)
-    lefts, rights, f32 = _rows(lefts, rights)
+    if any(_on_cuda(x) for x in (*lefts, *(() if rights is None else rights))):
+        devs = {e.device for e in encoders}
+        if len(devs) != 1:
+            raise ValueError("CUDA rows need encoders of one device")
+        lefts, rights, f32 = _device_rows(lefts, rights, devs.pop())
+        name, ptr = "mp3b200_encode_batch_device", (lambda x: x.data_ptr())
+    else:
+        lefts, rights, f32 = _rows(lefts, rights)
+        name, ptr = "mp3b200_encode_batch", (lambda x: x.ctypes.data)
     ns = np.array([len(x) for x in lefts], dtype=np.int32)
     caps = np.array([int(1.25 * n + 7200) for n in ns], dtype=np.int32)
     outs = [np.empty(int(c), dtype=np.uint8) for c in caps]
     hp = (ctypes.c_void_p * S)(*[e._h for e in encoders])
-    lp = (ctypes.c_void_p * S)(*[x.ctypes.data for x in lefts])
-    rp = (ctypes.c_void_p * S)(*[x.ctypes.data for x in rights])
+    lp = (ctypes.c_void_p * S)(*[ptr(x) for x in lefts])
+    rp = (ctypes.c_void_p * S)(*[ptr(x) for x in rights])
     op = (ctypes.c_void_p * S)(*[x.ctypes.data for x in outs])
     got = np.zeros(S, dtype=np.int32)
-    _check(_entry("mp3b200_encode_batch", f32)(hp, lp, rp, ns.ctypes.data, op, caps.ctypes.data, S, got.ctypes.data))
+    _check(_entry(name, f32)(hp, lp, rp, ns.ctypes.data, op, caps.ctypes.data, S, got.ctypes.data))
     for g in got:
         _check(int(g))
     return [o[: int(g)].tobytes() for o, g in zip(outs, got)]
