@@ -423,6 +423,41 @@ int mp3b200_debug_replaygain_f32(int channels, int samplerate, int kbps, int fla
                                  int64_t nsamples, double* win_sums, int32_t* win_idx, int64_t nwin_cap, int32_t* hist,
                                  double* title_db, int32_t* stats);
 
+/* ---- Encode sessions: whole device-resident streams, queued on the caller's CUDA stream (DESIGN.md 14) ----------------
+ * A session is bound to one CUDA stream of the device that is current when it is created (NULL: the legacy default
+ * stream).  mp3b200_encode_streams_async / _async_f32 encode what mp3b200_encode_streams_device_ex / _device_f32 encode, with
+ * the same layout of d_pcm and d_out and the same bytes, but they only queue the work on the session's stream and return:
+ * it runs after everything queued there before the call, and work queued there afterwards sees the bytes and d_status.
+ * Nothing else orders the call: it does not wait for the legacy default stream.
+ *   flags       MP3B200_RESAMPLE or 0 (MP3B200_REPLAYGAIN is refused: the tag is built on the host).
+ *   d_status    int32[4] of device memory, written by the call's last queued operation: [0] a Float32 sample was refused
+ *               (not finite, or beyond 2^40 once scaled), [1] a frame did not fit its bit budget (where lamejs throws),
+ *               [2] the number of quantizer passes (timings_ms[7] of the synchronous call), [3] an internal fault.  When [0],
+ *               [1] or [3] is non-zero the output must not be used; mp3b200_check_status turns the words, copied to the host
+ *               once the stream has reached them, into the error code and mp3b200_last_error text of the synchronous call.
+ * What the host can see is refused before anything is queued, with the codes and texts of the synchronous call: unknown
+ * flags, a bad configuration, nstreams < 0; a stream that is capturing a graph returns MP3B200_ERR_HANDLE.
+ * The call does not wait for the device, except: on the first use of a configuration on the device (its tables are
+ * uploaded), when the session's workspace or pinned staging grows (which may synchronise the device), and when
+ * MP3B200_SESSION_SLOTS calls of the session are still in flight (it waits for the oldest).  A session that has seen a
+ * launch shape before never waits.  The quantizer's re-validation loop runs on the device (a CUDA graph with a conditional
+ * WHILE node, captured once per launch shape and kept by the session).
+ * One call runs at a time per session; sessions share no buffer, so several may be used from one thread or from many.
+ * The buffers must stay alive until the stream has reached the call's end.  mp3b200_session_destroy waits for the session's
+ * queued work, then frees it. */
+#define MP3B200_SESSION_SLOTS 4
+typedef struct mp3b200_session mp3b200_session;
+int mp3b200_session_create(void* cuda_stream, mp3b200_session** out);
+int mp3b200_session_destroy(mp3b200_session* s);
+int mp3b200_encode_streams_async(mp3b200_session* s, int channels, int samplerate, int kbps, int flags, int nstreams,
+                                 const int16_t* d_pcm, const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
+                                 const int64_t* out_off, int32_t* d_status);
+int mp3b200_encode_streams_async_f32(mp3b200_session* s, int channels, int samplerate, int kbps, int flags, int nstreams,
+                                     const float* d_pcm, const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
+                                     const int64_t* out_off, int32_t* d_status);
+/* status: the 4 words of d_status in host memory.  0, or the error the synchronous call returns (last_error set). */
+int mp3b200_check_status(const int32_t* status);
+
 const char* mp3b200_last_error(void);
 /* total number of kernel launches issued by this library since load (bench.py "gpu_launches") */
 int64_t mp3b200_launch_count(void);

@@ -250,6 +250,12 @@ struct Workspace {
                         counter.fit(Q_NCOUNTERS) || scan.fit((size_t)(F / SCAN_FRAMES + S + 1));
     return failed ? MP3B200_ERR_CUDA : 0;
   }
+  /* the workspace's generation as far as the quantizer's buffers go: capacities only grow, so this sum changes exactly when
+   * one of them has been reallocated (and a graph holding their addresses is stale) */
+  size_t generation() const {
+    return streams.cap + qstate.cap + ginfo.cap + l3enc.cap + xrq.cap + xrpow.cap + neg.cap + prep.cap + dirty.cap + counter.cap +
+           refusals.cap;
+  }
   void release() {
     streams.release(); bt_final.release(); bt_prev.release(); xr.release(); slab.release(); psy.release(); scan_in.release();
     ratio.release(); ath_psy.release(); ath_q.release(); qstate.release(); ginfo.release(); l3enc.release(); xrq.release();
@@ -258,14 +264,22 @@ struct Workspace {
   }
 };
 
+/* Pinned host memory the descriptors of an asynchronous call are uploaded from (a slot of a session's ring): `used` bytes
+ * of `cap` are taken. */
+struct PinnedArena { uint8_t* p = nullptr; size_t cap = 0, used = 0; };
+
 /* Everything a host thread needs to drive the GPU: its own non-blocking stream (threads encoding through distinct handles
  * or batches never serialise on the legacy default stream), events, workspace and staging buffers.  Bound to one device;
- * re-created when the thread is used with a configuration of another device. */
+ * re-created when the thread is used with a configuration of another device.
+ * An encode session (mp3b200_session) holds one too, bound to the caller's stream instead (session = true): its launches
+ * are ordered by that stream alone, with no wait for the legacy default stream, and upload their descriptors from `arena`. */
 enum { MP3_MAX_PCM_CHUNKS = 8 };
 /* The stream index is a grid y / z coordinate of several kernels (CUDA limit 65535): larger batches run in groups */
 enum { MP3_MAX_LAUNCH_STREAMS = 65535 };
 struct ThreadCtx {
   int device = -1;
+  bool session = false;                   /* st is the caller's stream (not owned) */
+  PinnedArena* arena = nullptr;           /* sessions: where the current call's uploads are staged */
   cudaStream_t st = nullptr, up_st = nullptr, aux_st = nullptr;   /* main, PCM upload, quantizer repair chain */
   cudaEvent_t ev[8] = {}, evq[QE_COUNT] = {}, ev_in = nullptr, ev_fork = nullptr, ev_join = nullptr, ready[MP3_MAX_PCM_CHUNKS] = {};
   cudaEvent_t ev_rs[2] = {};              /* around k_resample */
@@ -302,7 +316,8 @@ struct ThreadCtx {
     if (ev_fork) { cudaEventDestroy(ev_fork); ev_fork = nullptr; }
     if (ev_join) { cudaEventDestroy(ev_join); ev_join = nullptr; }
     if (aux_st) { cudaStreamDestroy(aux_st); aux_st = nullptr; }
-    if (st) { cudaStreamDestroy(st); st = nullptr; }
+    if (st && !session) cudaStreamDestroy(st);
+    st = nullptr;
     if (up_st) { cudaStreamDestroy(up_st); up_st = nullptr; }
     device = -1;
   }
@@ -312,6 +327,16 @@ struct ThreadCtx {
     if (device == dev) return 0;
     release();
     CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    return create(dev);
+  }
+  /* a session's context on the current device `dev`, launching on the caller's stream `s` */
+  int bind(int dev, cudaStream_t s) {
+    release();
+    session = true;
+    st = s;
+    return create(dev);
+  }
+  int create(int dev) {
     CK(cudaStreamCreateWithFlags(&up_st, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&rg_st, cudaStreamNonBlocking));
     for (auto& e : ev_rg) CK(cudaEventCreate(&e));
@@ -333,14 +358,25 @@ struct ThreadCtx {
 };
 thread_local ThreadCtx t_ctx;
 
+int config_on(int dev, int ch, int sr, int kbps, int flags, Config** out);
+
 /* The configuration for a launch on the current device (g_device): uploads its tables there on first use and binds the
  * calling thread's context (t_ctx) to that device, so cfg->dev[t_ctx.device] holds them. */
 int get_config(int ch, int sr, int kbps, int flags, Config** out) {
-  if (flags & ~MP3B200_RESAMPLE) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
   int dev = 0;
   {
     std::lock_guard<std::mutex> lk(g_mu);
     dev = g_device;
+  }
+  const int rc = config_on(dev, ch, sr, kbps, flags, out);
+  return rc ? rc : t_ctx.use(dev);
+}
+
+/* get_config on device `dev`, binding no context (an encode session has its own) */
+int config_on(int dev, int ch, int sr, int kbps, int flags, Config** out) {
+  if (flags & ~MP3B200_RESAMPLE) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
+  {
+    std::lock_guard<std::mutex> lk(g_mu);
     int rc = ensure_device(dev);
     if (rc) return rc;
     Config* c = find_config(ch, sr, kbps, flags);
@@ -355,7 +391,7 @@ int get_config(int ch, int sr, int kbps, int flags, Config** out) {
     }
     *out = c;
   }
-  return t_ctx.use(dev);
+  return 0;
 }
 
 /* MP3B200_DEBUG_SYNC=1: synchronise after every launch and name the failing kernel */
@@ -380,16 +416,24 @@ struct PcmArrival { int chunks = 1; cudaEvent_t* ready = nullptr; };
  * find after its launch, and then undoes: handles_call) */
 thread_local bool t_over_budget = false;
 
+/* The error of a launch whose ws.refusals read refused / over_budget (and, for an asynchronous call, fault: its device
+ * fixed-point loop hit the bound), with g_err set; 0 when the output stands. */
+int refusal_error(int refused, int over_budget, int fault) {
+  if (refused) { g_err = "non-finite input sample (or one beyond 2^40 once scaled)"; return MP3B200_ERR_CONFIG; }
+  if (over_budget) { g_err = "frame over its bit budget (input too loud to encode)"; return MP3B200_ERR_CONFIG; }
+  if (fault) { g_err = "quantizer stage failed: the fixed-point loop did not converge"; return MP3B200_ERR_CUDA; }
+  return 0;
+}
+
 /* After a launch has drained, one read-back of ws.refusals: MP3B200_ERR_CONFIG when k_stage_f32 refused a Float32 sample,
  * or when a frame's bits did not fit its slot (k_q_pack left it unpacked), where lamejs throws out of the call
  * (BitStream.js:856-885).  The call's output must not be used. */
-int check_refusals() {
+int check_refusals(ThreadCtx& c) {
   int r[2] = {0, 0};
-  CK(cudaMemcpyAsync(r, t_ctx.ws.refusals.p, sizeof r, cudaMemcpyDeviceToHost, t_ctx.st));
-  CK(cudaStreamSynchronize(t_ctx.st));
-  if (r[0]) { g_err = "non-finite input sample (or one beyond 2^40 once scaled)"; return MP3B200_ERR_CONFIG; }
-  if (r[1]) { g_err = "frame over its bit budget (input too loud to encode)"; t_over_budget = true; return MP3B200_ERR_CONFIG; }
-  return 0;
+  CK(cudaMemcpyAsync(r, c.ws.refusals.p, sizeof r, cudaMemcpyDeviceToHost, c.st));
+  CK(cudaStreamSynchronize(c.st));
+  if (!r[0] && r[1]) t_over_budget = true;
+  return refusal_error(r[0], r[1], 0);
 }
 
 /* Options of launch_streams */
@@ -398,13 +442,48 @@ struct LaunchOpts {
   bool stop_after_mdct = false;          /* debug: no quantizer, no bytes */
   const PcmArrival* arrival = nullptr;   /* PCM still landing on the upload stream */
   float* timings_ms = nullptr;           /* the 16 timing slots of include/mp3b200.h */
-  bool sync = true;                      /* false: return with the work queued on t_ctx.st (no timings) */
+  bool sync = true;                      /* false: return with the work queued on the context's stream (no timings) */
   StreamDesc* committed = nullptr;       /* host: each stream's descriptor as the pipeline left it (the carried state),
-                                            valid once t_ctx.st has drained */
+                                            valid once the context's stream has drained */
   struct RgJob* rg = nullptr;            /* ReplayGain of every stream, beside the encoder (one launch group only) */
   bool f32_in = false;                   /* the descriptors point at the caller's Float32 rows (k_stage_f32 stages them); with
                                             sync, a non-finite sample makes the launch return MP3B200_ERR_CONFIG */
+  struct LoopGraphs* loops = nullptr;    /* run the quantizer's fixed-point loop on the device, as the cached graphs of a session
+                                            (no host round trip; needs !sync) */
 };
+
+/* The quantizer's fixed-point loop graphs of a session (QuantLoop), one per launch shape: (configuration, streams, frames,
+ * longest stream's frames).  They hold the workspace's addresses, so they are all dropped when its generation changes. */
+struct LoopGraphs {
+  cudaStream_t capture = nullptr;
+  size_t generation = 0;
+  std::map<std::tuple<const Config*, int, long long, int>, cudaGraphExec_t> exec;
+  void clear() { for (auto& e : exec) cudaGraphExecDestroy(e.second); exec.clear(); }
+};
+
+/* Queues the copy of n bytes of host descriptors to dst on c.st.  A session's call stages them in its pinned slot first, so
+ * the copy never waits for the device; a thread's context copies from `src` (pageable) as it is. */
+int upload(ThreadCtx& c, void* dst, const void* src, size_t n) {
+  if (c.arena) {
+    PinnedArena& a = *c.arena;
+    const size_t at = (a.used + 255) & ~(size_t)255;
+    if (at + n > a.cap) { g_err = "descriptor staging overflow"; return MP3B200_ERR_CUDA; }
+    memcpy(a.p + at, src, n);
+    a.used = at + n;
+    src = a.p + at;
+  }
+  CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, c.st));
+  return 0;
+}
+
+/* Makes c.st wait for the work the caller queued on the legacy default stream (torch and plain CUDA callers produce their
+ * device buffers there).  A session's stream is the only ordering of its calls: nothing to do. */
+int wait_legacy(ThreadCtx& c) {
+  if (c.session) return 0;
+  CK(cudaEventRecord(c.ev_in, cudaStreamLegacy));
+  CK(cudaStreamWaitEvent(c.st, c.ev_in, 0));
+  return 0;
+}
 
 /* The rows the descriptors of a launch point at: the caller's Int16 samples, {false, host.scale_applied}, or Float32 rows
  * already scaled by k_stage_f32 or k_resample, SCALED_F32.  The kernels that read them are instantiated for `f32`. */
@@ -412,16 +491,16 @@ struct Rows { bool f32; int scale_applied; };
 constexpr Rows SCALED_F32 = {true, 0};
 
 /* One pipeline launch for the streams sds[0 .. S) (at most MP3_MAX_LAUNCH_STREAMS, unit / frame bases set, the workspace
- * large enough).  All launches go to the calling thread's stream (t_ctx.st), which first waits for whatever the caller
- * queued on the legacy default stream (torch and plain CUDA callers produce their device buffers there); with o.sync the
- * call returns after the stream has drained, so the results are visible to any stream afterwards. */
-int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, const LaunchOpts& o, const PcmArrival* arrival,
-                 Rows rows, Timings* tm) {
-  cudaStream_t st = t_ctx.st;
-  cudaEvent_t* ev = t_ctx.ev;
-  Workspace& ws = t_ctx.ws;
+ * large enough).  All launches go to the context's stream (c.st: the calling thread's, t_ctx.st, or a session's), which
+ * first waits for whatever the caller queued on the legacy default stream (wait_legacy); with o.sync the call returns after
+ * the stream has drained, so the results are visible to any stream afterwards. */
+int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, const LaunchOpts& o,
+                 const PcmArrival* arrival, Rows rows, Timings* tm) {
+  cudaStream_t st = c.st;
+  cudaEvent_t* ev = c.ev;
+  Workspace& ws = c.ws;
 
-  const Mp3Tables* const tab = cfg->dev[t_ctx.device];
+  const Mp3Tables* const tab = cfg->dev[c.device];
   const int nch = cfg->host.nch;
   const bool f32_pcm = rows.f32;
   int max_frames = 0;
@@ -436,9 +515,8 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
     s.scan_base = scan_rows;
     scan_rows += (s.nframes + SCAN_FRAMES - 1) / SCAN_FRAMES;
   }
-  CK(cudaEventRecord(t_ctx.ev_in, cudaStreamLegacy));
-  CK(cudaStreamWaitEvent(st, t_ctx.ev_in, 0));
-  CK(cudaMemcpyAsync(ws.streams.p, h_streams, sizeof(StreamDesc) * S, cudaMemcpyHostToDevice, st));
+  int rc = wait_legacy(c);
+  if (rc || (rc = upload(c, ws.streams.p, h_streams, sizeof(StreamDesc) * S))) return rc;
   CK(cudaEventRecord(ev[0], st));
 
   /* K2: psy analysis, one block per (granule incl. 1 halo, channel, stream) */
@@ -489,7 +567,7 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
       void (*const k_fb)(const Mp3Tables*, const StreamDesc*, float*) = f32_pcm ? k_subband_analysis<true> : k_subband_analysis<false>;
       {
         std::lock_guard<std::mutex> lk(g_mu);   /* the attribute is per device */
-        if (!g_fb_attr_done[t_ctx.device][f32_pcm]) { CK(cudaFuncSetAttribute(k_fb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); g_fb_attr_done[t_ctx.device][f32_pcm] = true; }
+        if (!g_fb_attr_done[c.device][f32_pcm]) { CK(cudaFuncSetAttribute(k_fb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); g_fb_attr_done[c.device][f32_pcm] = true; }
       }
       cudaLaunchConfig_t lc = {};
       lc.gridDim = dim3((G * max_frames + 1 + FB_SLABS - 1) / FB_SLABS, nch, S);
@@ -535,7 +613,20 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
     qb.xr = ws.xr.p; qb.ratio = ws.ratio.p; qb.bt = ws.bt_final.p; qb.ath_q = ws.ath_q.p; qb.qs = ws.qstate.p; qb.ginfo = ws.ginfo.p;
     qb.l3enc = ws.l3enc.p; qb.xrq = ws.xrq.p; qb.xrpow = ws.xrpow.p; qb.neg = ws.neg.p; qb.prep = ws.prep.p; qb.list = ws.dirty.p; qb.counter = ws.counter.p;
     qb.over_budget = ws.refusals.p + 1;
-    int rc = quant_run(tab, cfg->host, ws.streams.p, S, streams_with_frames, max_frames, total_frames, qb, d_out, st, t_ctx.aux_st, t_ctx.ev_fork, t_ctx.ev_join, ev[5], t_ctx.evq, t_ctx.evq_pred, &passes, &g_launches);
+    QuantLoop dloop;
+    cudaGraphExec_t* cached = nullptr;
+    if (o.loops) {                         /* the session's graph for this shape, captured by quant_run if there is none */
+      LoopGraphs& lg = *o.loops;
+      if (lg.generation != ws.generation()) { lg.clear(); lg.generation = ws.generation(); }
+      cached = &lg.exec[std::make_tuple((const Config*)cfg, S, total_frames, max_frames)];
+      dloop.capture = lg.capture; dloop.st = ws.refusals.p + 2; dloop.exec = *cached;
+    }
+    rc = quant_run(tab, cfg->host, ws.streams.p, S, streams_with_frames, max_frames, total_frames, qb, d_out, st, c.aux_st, c.ev_fork, c.ev_join, ev[5], c.evq, c.evq_pred, &passes, &g_launches,
+                   o.loops ? &dloop : nullptr);
+    if (cached) {
+      *cached = dloop.exec;
+      if (!dloop.exec) o.loops->exec.erase(std::make_tuple((const Config*)cfg, S, total_frames, max_frames));
+    }
     if (rc) { g_err = "quantizer stage failed: " + std::string(cudaGetErrorString(cudaGetLastError())); return rc; }
   } else {
     CK(cudaEventRecord(ev[5], st));
@@ -554,7 +645,7 @@ int run_pipeline(Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, cons
     cudaEventElapsedTime(&tm->total, ev[0], ev[6]);
     tm->passes = passes;
     if (!o.stop_after_mdct && passes > 0) {
-      auto span = [&](int slot) { float v = 0; const int p = t_ctx.evq_pred[slot]; if (p >= 0) cudaEventElapsedTime(&v, t_ctx.evq[p], t_ctx.evq[slot]); return v; };
+      auto span = [&](int slot) { float v = 0; const int p = c.evq_pred[slot]; if (p >= 0) cudaEventElapsedTime(&v, c.evq[p], c.evq[slot]); return v; };
       tm->q_prepare = span(QE_PREP);
       tm->q_search = span(QE_S0) + span(QE_S1);
       tm->q_outer = span(QE_O0) + span(QE_O1);
@@ -584,9 +675,9 @@ long long hist_base_at(int mode_gr, long long frame) {
 /* Float32 input: the descriptors sds[0 .. S) point at the caller's Float32 rows.  Queues k_stage_f32, which writes them
  * scaled into the workspace (ws.refusals[0] flags a refused sample), and points the descriptors at the staged rows; the
  * sample indices stay as they were. */
-int stage_streams(Config* cfg, StreamDesc* sds, int S) {
+int stage_streams(ThreadCtx& c, Config* cfg, StreamDesc* sds, int S) {
   const int nch = cfg->host.nch;
-  Workspace& ws = t_ctx.ws;
+  Workspace& ws = c.ws;
   std::vector<StageDesc> d((size_t)S);
   long long tot = 0, max_n = 0;
   for (int i = 0; i < S; i++) {
@@ -606,10 +697,8 @@ int stage_streams(Config* cfg, StreamDesc* sds, int S) {
     off += d[i].n * nch;
     for (int c = 0; c < 2; c++) sds[i].pcm[c] = d[i].y[c];
   }
-  cudaStream_t st = t_ctx.st;
-  CK(cudaEventRecord(t_ctx.ev_in, cudaStreamLegacy));      /* the input may come from the legacy default stream */
-  CK(cudaStreamWaitEvent(st, t_ctx.ev_in, 0));
-  CK(cudaMemcpyAsync(ws.st_desc.p, d.data(), sizeof(StageDesc) * S, cudaMemcpyHostToDevice, st));
+  cudaStream_t st = c.st;
+  if ((rc = wait_legacy(c)) || (rc = upload(c, ws.st_desc.p, d.data(), sizeof(StageDesc) * S))) return rc;
   if (max_n > 0) {
     const long long per = (long long)STAGE_THREADS * STAGE_PER_THREAD;
     dim3 grid((unsigned)((max_n + per - 1) / per), nch, S);
@@ -622,13 +711,12 @@ int stage_streams(Config* cfg, StreamDesc* sds, int S) {
 
 /* Queues k_resample for the S descriptors rd (uploaded here), whose input rows `in` describes; ev_rs[0 / 1] bracket the
  * kernel (timing slot 14). */
-int queue_resample(const Config* cfg, const ResampleDesc* rd, int S, long long max_ny, Rows in) {
-  Workspace& ws = t_ctx.ws;
-  cudaStream_t st = t_ctx.st;
+int queue_resample(ThreadCtx& c, const Config* cfg, const ResampleDesc* rd, int S, long long max_ny, Rows in) {
+  Workspace& ws = c.ws;
+  cudaStream_t st = c.st;
   int rc = ws.rs_desc.fit((size_t)S);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(ws.rs_desc.p, rd, sizeof(ResampleDesc) * S, cudaMemcpyHostToDevice, st));
-  CK(cudaEventRecord(t_ctx.ev_rs[0], st));
+  if (rc || (rc = upload(c, ws.rs_desc.p, rd, sizeof(ResampleDesc) * S))) return rc;
+  CK(cudaEventRecord(c.ev_rs[0], st));
   if (max_ny > 0) {
     dim3 grid((unsigned)((max_ny + RS_THREADS - 1) / RS_THREADS), cfg->host.nch, S);
     if (in.f32) k_resample<float><<<grid, RS_THREADS, 0, st>>>(ws.rs_desc.p, cfg->rs.ratio, in.scale_applied, cfg->host.scale);
@@ -636,7 +724,7 @@ int queue_resample(const Config* cfg, const ResampleDesc* rd, int S, long long m
     g_launches++;
     DBG("k_resample");
   }
-  CK(cudaEventRecord(t_ctx.ev_rs[1], st));
+  CK(cudaEventRecord(c.ev_rs[1], st));
   return 0;
 }
 
@@ -645,9 +733,9 @@ int queue_resample(const Config* cfg, const ResampleDesc* rd, int S, long long m
  * Queues k_resample for the outputs the streams' frames read -- from hist_base_at(frame0) up to the last output the input
  * reaches; later outputs are 0 -- into the workspace, and points the descriptors at them: from then on pcm_base / pcm_end
  * count outputs, and the stream reads like PCM at the output rate. */
-int resample_streams(Config* cfg, StreamDesc* sds, int S, Rows in) {
+int resample_streams(ThreadCtx& c, Config* cfg, StreamDesc* sds, int S, Rows in) {
   const int r = cfg->rs.ratio, nch = cfg->host.nch;
-  Workspace& ws = t_ctx.ws;
+  Workspace& ws = c.ws;
   std::vector<ResampleDesc> rd((size_t)S);
   long long tot = 0, max_ny = 0;
   for (int i = 0; i < S; i++) {
@@ -673,9 +761,8 @@ int resample_streams(Config* cfg, StreamDesc* sds, int S, Rows in) {
     for (int c = 0; c < 2; c++) sds[i].pcm[c] = d.y[c];
     sds[i].pcm_base = d.y_base; sds[i].pcm_end = d.y_base + d.ny;
   }
-  CK(cudaEventRecord(t_ctx.ev_in, cudaStreamLegacy));      /* the input may come from the legacy default stream */
-  CK(cudaStreamWaitEvent(t_ctx.st, t_ctx.ev_in, 0));
-  return queue_resample(cfg, rd.data(), S, max_ny, in);
+  if ((rc = wait_legacy(c))) return rc;                     /* the input may come from the legacy default stream */
+  return queue_resample(c, cfg, rd.data(), S, max_ny, in);
 }
 
 /* ---- ReplayGain (lamejs findReplayGain; k_replaygain.cuh) ----
@@ -715,10 +802,9 @@ int rg_req_index(int sr) {
   return -1;
 }
 
-/* queues pass 1 and the first RG_QUEUED_PASSES repair passes on t_ctx.rg_st, after the PCM (the upload slices in `arrival`,
- * or everything queued on t_ctx.st so far: uploads and the resampler) */
-int rg_queue(Config* cfg, const StreamDesc* sds, RgJob& job, const PcmArrival* arrival, Rows rows) {
-  ThreadCtx& c = t_ctx;
+/* queues pass 1 and the first RG_QUEUED_PASSES repair passes on c.rg_st, after the PCM (the upload slices in `arrival`,
+ * or everything queued on c.st so far: uploads and the resampler) */
+int rg_queue(ThreadCtx& c, Config* cfg, const StreamDesc* sds, RgJob& job, const PcmArrival* arrival, Rows rows) {
   const int sr = cfg->host.samplerate, W = (sr + 19) / 20, nch = cfg->host.nch, req = rg_req_index(sr);
   if (req < 0) { g_err = "no ReplayGain filter for this rate"; return MP3B200_ERR_CONFIG; }
   const int T = (int)job.specs.size();
@@ -797,9 +883,8 @@ int rg_queue(Config* cfg, const StreamDesc* sds, RgJob& job, const PcmArrival* a
 }
 
 /* after the encoder has been queued: runs repair passes until one changes nothing, then the histograms, the gains of the
- * titles that end and the carries; reads the results.  Returns with t_ctx.rg_st drained. */
-int rg_finish(Config* cfg, RgJob& job) {
-  ThreadCtx& c = t_ctx;
+ * titles that end and the carries; reads the results.  Returns with c.rg_st drained. */
+int rg_finish(ThreadCtx& c, Config* cfg, RgJob& job) {
   cudaStream_t st = c.rg_st;
   RgParams& p = job.prm;
   const int nch = cfg->host.nch, T = (int)job.specs.size();
@@ -864,27 +949,29 @@ int rg_finish(Config* cfg, RgJob& job) {
 }
 
 /* Encodes the streams `sds` into d_out: the caller sets each descriptor's PCM, pcm_base / pcm_end, frame0, nframes,
- * out_base and carried state; this assigns unit_base / frame_base, grows the thread's workspace and runs the pipeline.
+ * out_base and carried state; this assigns unit_base / frame_base, grows the context's workspace and runs the pipeline.
  * The stream index is a grid y / z coordinate of several kernels (CUDA limit 65535): a larger batch runs as consecutive
- * launches of at most MP3_MAX_LAUNCH_STREAMS streams on the thread's stream, the later ones behind every PCM upload.
+ * launches of at most MP3_MAX_LAUNCH_STREAMS streams on the context's stream, the later ones behind every PCM upload.
  * Timings add up over the launches; the pass count is the largest any of them needed.
  * With resampling (cfg->rs.ratio > 1) the descriptors hold the caller's input as resample_streams describes; each launch
  * first resamples it (timing slot 14). */
-int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, const LaunchOpts& o) {
+int launch_streams(ThreadCtx& c, Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, const LaunchOpts& o) {
   if (o.timings_ms) for (int i = 0; i < 16; i++) o.timings_ms[i] = 0.0f;
   const PcmArrival* arrival = o.arrival;
   const int nstreams = (int)sds.size();
   if (o.rg && nstreams > MP3_MAX_LAUNCH_STREAMS) { g_err = "ReplayGain batches hold at most 65535 streams"; return MP3B200_ERR_HANDLE; }
   {
-    int rc = t_ctx.ws.refusals.fit(2);
+    int rc = c.ws.refusals.fit(2);
     if (rc) return rc;
-    CK(cudaMemsetAsync(t_ctx.ws.refusals.p, 0, 2 * sizeof(int), t_ctx.st));
+    CK(cudaMemsetAsync(c.ws.refusals.p, 0, 2 * sizeof(int), c.st));
   }
   /* Before anything reads the descriptors' rows: the caller's device rows may come from the legacy default stream, and
-   * rg_queue forks the analysis stream from t_ctx.st ahead of run_pipeline's own wait (Int16 rows that are neither staged
+   * rg_queue forks the analysis stream from c.st ahead of run_pipeline's own wait (Int16 rows that are neither staged
    * nor resampled are read by k_rg_pass1 where the caller left them). */
-  CK(cudaEventRecord(t_ctx.ev_in, cudaStreamLegacy));
-  CK(cudaStreamWaitEvent(t_ctx.st, t_ctx.ev_in, 0));
+  {
+    const int rc = wait_legacy(c);
+    if (rc) return rc;
+  }
   for (int g0 = 0; g0 < nstreams; g0 += MP3_MAX_LAUNCH_STREAMS) {
     const int n = nstreams - g0 < MP3_MAX_LAUNCH_STREAMS ? nstreams - g0 : MP3_MAX_LAUNCH_STREAMS;
     StreamDesc* group = sds.data() + g0;
@@ -894,41 +981,41 @@ int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, co
       U += (long long)cfg->host.mode_gr * group[i].nframes; F += group[i].nframes;
     }
     if (F == 0) continue;                     /* empty group: nothing to launch */
-    int rc = t_ctx.ws.fit(n, cfg->host.nch, U, F);
+    int rc = c.ws.fit(n, cfg->host.nch, U, F);
     if (rc) return rc;
     const bool resampled = cfg->rs.ratio > 1;
     if (resampled || o.f32_in) {
       if (arrival)                              /* the resampler / stager reads all of the input: wait for every slice */
-        for (int j = 0; j < arrival->chunks; j++) CK(cudaStreamWaitEvent(t_ctx.st, arrival->ready[j], 0));
+        for (int j = 0; j < arrival->chunks; j++) CK(cudaStreamWaitEvent(c.st, arrival->ready[j], 0));
       arrival = nullptr;
     }
     Rows rows = {false, cfg->host.scale_applied};
     if (o.f32_in) {
-      rc = stage_streams(cfg, group, n);
+      rc = stage_streams(c, cfg, group, n);
       if (rc) return rc;
       rows = SCALED_F32;
     }
     if (resampled) {
-      rc = resample_streams(cfg, group, n, rows);
+      rc = resample_streams(c, cfg, group, n, rows);
       if (rc) return rc;
       rows = SCALED_F32;
     }
     if (o.rg) {
-      rc = rg_queue(cfg, group, *o.rg, arrival, rows);
+      rc = rg_queue(c, cfg, group, *o.rg, arrival, rows);
       if (rc) return rc;
     }
     Timings tm;
-    rc = run_pipeline(cfg, group, n, d_out, o, arrival, rows, &tm);
+    rc = run_pipeline(c, cfg, group, n, d_out, o, arrival, rows, &tm);
     if (rc) return rc;
     if (o.rg) {
-      rc = rg_finish(cfg, *o.rg);
+      rc = rg_finish(c, cfg, *o.rg);
       if (rc) return rc;
     }
     arrival = nullptr;
     float rs_ms = 0.0f;
-    if (resampled && o.timings_ms && o.sync) CK(cudaEventElapsedTime(&rs_ms, t_ctx.ev_rs[0], t_ctx.ev_rs[1]));
+    if (resampled && o.timings_ms && o.sync) CK(cudaEventElapsedTime(&rs_ms, c.ev_rs[0], c.ev_rs[1]));
     if (o.committed)
-      CK(cudaMemcpyAsync(o.committed + g0, t_ctx.ws.streams.p, sizeof(StreamDesc) * n, cudaMemcpyDeviceToHost, t_ctx.st));
+      CK(cudaMemcpyAsync(o.committed + g0, c.ws.streams.p, sizeof(StreamDesc) * n, cudaMemcpyDeviceToHost, c.st));
     if (o.timings_ms) {
       const float t[16] = {tm.psy, tm.scan, tm.mask, tm.fb, tm.q1, tm.qn, tm.total, 0.0f,
                            tm.q_prepare, tm.q_search, tm.q_outer, tm.q_finish, tm.q_pack, tm.q_mid, rs_ms, 0.0f};
@@ -936,7 +1023,7 @@ int launch_streams(Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, co
       if ((float)tm.passes > o.timings_ms[7]) o.timings_ms[7] = (float)tm.passes;
     }
   }
-  return o.sync && (o.f32_in || !o.stop_after_mdct) ? check_refusals() : 0;
+  return o.sync && (o.f32_in || !o.stop_after_mdct) ? check_refusals(c) : 0;
 }
 
 }  // namespace
@@ -1093,7 +1180,7 @@ int encode_host_streams(Config* cfg, int nstreams, const T* const* left, const T
   o.arrival = &arr;
   o.rg = rg;
   o.f32_in = std::is_same_v<T, float>;
-  return launch_streams(cfg, sds, t_ctx.out.p, o);
+  return launch_streams(t_ctx, cfg, sds, t_ctx.out.p, o);
 }
 
 }  // namespace
@@ -1120,7 +1207,7 @@ int encode_device(int channels, int samplerate, int kbps, int flags, int nstream
   LaunchOpts o;
   o.timings_ms = timings_ms;
   o.f32_in = std::is_same_v<T, float>;
-  return launch_streams(cfg, sds, d_out, o);
+  return launch_streams(t_ctx, cfg, sds, d_out, o);
 }
 
 template <class T>
@@ -1227,7 +1314,7 @@ int debug_stages(const mp3b200_debug_taps* tp, const T* left, const T* right) {
   opts.f32_in = std::is_same_v<T, float>;
   opts.force_bt = force_blocktype;
   opts.stop_after_mdct = !(l3_enc || bytes_out || want_gi || want_prep || want_q);
-  rc = launch_streams(cfg, sds, d_out, opts);
+  rc = launch_streams(t_ctx, cfg, sds, d_out, opts);
   /* read-back on the thread's stream (the launch has drained it) */
   auto fetch = [](void* dst, const void* src, size_t bytes) {
     const cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, t_ctx.st);
@@ -1341,14 +1428,14 @@ int debug_resample(int channels, int samplerate, int kbps, const T* left, const 
   if (std::is_same_v<T, float>) {                   /* the launch path's staging: Float32(x * scale) rows */
     rc = t_ctx.ws.refusals.fit(2);
     if (rc) return rc;
-    rc = stage_streams(cfg, &sd, 1);
+    rc = stage_streams(t_ctx, cfg, &sd, 1);
     if (rc) return rc;
     rows = SCALED_F32;
   }
   ResampleDesc d;
   d.x[0] = sd.pcm[0]; d.x[1] = sd.pcm[1]; d.x_base = 0; d.x_end = nsamples;
   d.y[0] = t_ctx.ws.rs_y.p; d.y[1] = d.y[0] + (nch == 2 ? ny : 0); d.y_base = 0; d.ny = ny;
-  rc = queue_resample(cfg, &d, 1, ny, rows);
+  rc = queue_resample(t_ctx, cfg, &d, 1, ny, rows);
   if (rc) return rc;
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(y, t_ctx.ws.rs_y.p, sizeof(float) * (size_t)(ny * nch), cudaMemcpyDeviceToHost, t_ctx.st));
@@ -1630,7 +1717,7 @@ struct DeviceTagged {
     LaunchOpts o;
     o.rg = rg;
     o.f32_in = std::is_same_v<T, float>;
-    int rc = launch_streams(cfg, sds, d_out, o);
+    int rc = launch_streams(t_ctx, cfg, sds, d_out, o);
     if (rc || ntags == 0) return rc;
     rc = t_ctx.pin.fit(staging_bytes());
     if (rc) return rc;
@@ -1765,6 +1852,7 @@ int mp3b200_debug_replaygain_f32(int channels, int samplerate, int kbps, int fla
 }  // extern "C"
 
 #include "mp3_handle.inc"
+#include "mp3_session.inc"
 
 #ifdef Q_TASKSTAT
 extern "C" int mp3b200_debug_taskstat(int* out, int rows) {

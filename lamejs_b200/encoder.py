@@ -103,6 +103,11 @@ def lib():
     L.mp3b200_encode_batch_device.argtypes = [vp, vp, vp, vp, vp, vp, c_int, vp]
     L.mp3b200_encode_batch_device_f32.argtypes = [vp, vp, vp, vp, vp, vp, c_int, vp]
     L.mp3b200_encoder_device.argtypes = [vp]
+    L.mp3b200_session_create.argtypes = [vp, ctypes.POINTER(vp)]
+    L.mp3b200_session_destroy.argtypes = [vp]
+    L.mp3b200_encode_streams_async.argtypes = [vp, c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp]
+    L.mp3b200_encode_streams_async_f32.argtypes = [vp, c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp]
+    L.mp3b200_check_status.argtypes = [vp]
     _lib = L
     return L
 
@@ -617,6 +622,89 @@ def encode_streams_device_tagged(channels, samplerate, kbps, d_pcm_ptr, pcm_off,
                                                                     got.ctypes.data, title.ctypes.data, ctypes.byref(album)))
     return ([int(g) for g in got[:S]], [float(t) for t in title[:S]],
             float(album.value) if S else float(GAIN_NOT_ENOUGH_SAMPLES))
+
+
+class EncodeSession:
+    """Whole device-resident streams encoded on one CUDA stream without blocking the calling thread (mp3b200_session,
+    DESIGN.md 14).  `stream` is a torch.cuda.Stream (None: torch.cuda.current_stream() now).  encode_streams queues the
+    encode behind everything already queued on that stream and returns; later work on the stream sees `out` and the
+    returned status.  A session must not be used from two threads at once; separate sessions share nothing."""
+
+    def __init__(self, stream=None):
+        import torch
+        self.stream = torch.cuda.current_stream() if stream is None else stream
+        self.device = self.stream.device
+        h = ctypes.c_void_p()
+        with torch.cuda.device(self.device):
+            _check(lib().mp3b200_session_create(ctypes.c_void_p(self.stream.cuda_stream or None), ctypes.byref(h)))
+        self._h = h
+
+    def encode_streams(self, channels, samplerate, kbps, pcm, pcm_off, nsamples, out, out_off, resample=False):
+        """encode_streams_device on tensors, queued: `pcm` is a 1-D CUDA tensor of int16 or float32 samples (float32 is
+        encoded as lamejs encodes a Float32Array), laid out as encode_streams_device reads d_pcm; `out` a uint8 CUDA tensor,
+        stream s written at out_off[s].  pcm_off, nsamples and out_off are host sequences.  Returns the int32[4] status
+        tensor the call fills on the session's stream (check_status reads it)."""
+        import torch
+        if self._h is None:
+            raise ValueError("the session is closed")
+        if pcm.dtype not in (torch.int16, torch.float32):
+            raise TypeError("pcm must be int16 or float32, not %s" % pcm.dtype)
+        if out.dtype != torch.uint8:
+            raise TypeError("out must be uint8, not %s" % out.dtype)
+        for name, t in (("pcm", pcm), ("out", out)):
+            if not _on_cuda(t) or t.device != self.device:
+                raise ValueError("%s must be a CUDA tensor on the session's device (%s)" % (name, self.device))
+            if t.dim() != 1 or not t.is_contiguous():
+                raise ValueError("%s must be a contiguous 1-D tensor" % name)
+        pcm_off = np.ascontiguousarray(pcm_off, dtype=np.int64)
+        nsamples = np.ascontiguousarray(nsamples, dtype=np.int64)
+        out_off = np.ascontiguousarray(out_off, dtype=np.int64)
+        S = len(nsamples)
+        if len(pcm_off) != S or len(out_off) != S:
+            raise ValueError("pcm_off, nsamples and out_off must have one entry per stream")
+        if S:
+            nb = {int(n): stream_bytes(channels, samplerate, kbps, int(n), resample) for n in np.unique(nsamples) if n >= 0}
+            if all(b >= 0 for b in nb.values()) and (nsamples >= 0).all():
+                room = np.array([nb[int(n)] for n in nsamples], dtype=np.int64)
+                if ((pcm_off < 0) | (pcm_off + nsamples * channels > pcm.numel()) | (out_off < 0) |
+                        (out_off + room > out.numel())).any():
+                    raise ValueError("a stream lies outside pcm or out")
+        with torch.cuda.stream(self.stream):
+            status = torch.empty(4, dtype=torch.int32, device=self.device)
+        fn = lib().mp3b200_encode_streams_async_f32 if pcm.dtype == torch.float32 else lib().mp3b200_encode_streams_async
+        _check(fn(self._h, channels, samplerate, kbps, RESAMPLE if resample else 0, S, pcm.data_ptr(), pcm_off.ctypes.data,
+                  nsamples.ctypes.data, out.data_ptr(), out_off.ctypes.data, status.data_ptr()))
+        for t in (pcm, out, status):
+            t.record_stream(self.stream)
+        return status
+
+    def close(self):
+        """Waits for the session's queued work and frees it."""
+        if self._h is not None:
+            h, self._h = self._h, None
+            _check(lib().mp3b200_session_destroy(h))
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def check_status(status):
+    """Synchronises the device, then raises Mp3B200Error as encode_streams_device would have for the call that filled
+    `status` (a refused Float32 sample, a frame over its bit budget, an internal fault).  Returns the quantizer pass count."""
+    import torch
+    torch.cuda.synchronize(status.device)
+    words = np.ascontiguousarray(status.cpu().numpy(), dtype=np.int32)
+    _check(lib().mp3b200_check_status(words.ctypes.data))
+    return int(words[2])
 
 
 def debug_resample(channels, samplerate, kbps, left, right=None, ny=None):
