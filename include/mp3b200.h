@@ -429,7 +429,7 @@ int mp3b200_debug_replaygain_f32(int channels, int samplerate, int kbps, int fla
  * the same layout of d_pcm and d_out and the same bytes, but they only queue the work on the session's stream and return:
  * it runs after everything queued there before the call, and work queued there afterwards sees the bytes and d_status.
  * Nothing else orders the call: it does not wait for the legacy default stream.
- *   flags       MP3B200_RESAMPLE or 0 (MP3B200_REPLAYGAIN is refused: the tag is built on the host).
+ *   flags       MP3B200_RESAMPLE or 0 (MP3B200_REPLAYGAIN is refused: mp3b200_encode_streams_tagged_async below takes it).
  *   d_status    int32[4] of device memory, written by the call's last queued operation: [0] a Float32 sample was refused
  *               (not finite, or beyond 2^40 once scaled), [1] a frame did not fit its bit budget (where lamejs throws),
  *               [2] the number of quantizer passes (timings_ms[7] of the synchronous call), [3] an internal fault.  When [0],
@@ -455,8 +455,32 @@ int mp3b200_encode_streams_async(mp3b200_session* s, int channels, int samplerat
 int mp3b200_encode_streams_async_f32(mp3b200_session* s, int channels, int samplerate, int kbps, int flags, int nstreams,
                                      const float* d_pcm, const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
                                      const int64_t* out_off, int32_t* d_status);
-/* status: the 4 words of d_status in host memory.  0, or the error the synchronous call returns (last_error set). */
+/* status: the first 4 words of d_status in host memory.  0, or the error the synchronous call returns (last_error set). */
 int mp3b200_check_status(const int32_t* status);
+
+/* Finished files from a session (DESIGN.md 15): mp3b200_encode_streams_tagged_device / _f32 queued on the session's stream.
+ * The same layout and bytes: stream s becomes one file at d_out + out_off[s], its Info / LAME tag frame and then its audio,
+ * for flags within MP3B200_RESAMPLE | MP3B200_REPLAYGAIN.  The tag frame is finished on the device (music CRC, Radio Replay
+ * Gain field, the tag's own CRC), and the ReplayGain repair loop runs there as a second conditional-WHILE graph, so the
+ * call never waits for a result.
+ *   out_bytes   host, [nstreams]: each file's length (audio + tag frame), known in closed form and filled when the call
+ *               returns.
+ *   d_gain      device, [nstreams + 1], written on the session's stream: GetTitleGain of each stream and, last, the album
+ *               gain in dB; -24601 wherever the synchronous call hands that out (less than one RMS window, no
+ *               MP3B200_REPLAYGAIN, a configuration whose tag does not fit).  May be NULL without MP3B200_REPLAYGAIN.
+ *   d_status    device, int32[8]: [0 .. 3] as above (mp3b200_check_status reads them; a ReplayGain loop that hits its bound
+ *               raises [3] and reads as the synchronous call's "ReplayGain repair did not converge"), [4] the analysis's
+ *               pass count, [5] the chunks it ran again, [6] and [7] zero.
+ * Refused before anything is queued, with the synchronous call's codes and texts: unknown flags, a bad configuration,
+ * nstreams < 0, MP3B200_REPLAYGAIN with more than 65535 streams; and with MP3B200_ERR_HANDLE: MP3B200_REPLAYGAIN with a NULL
+ * d_gain, a NULL d_status or out_bytes, a capturing stream.  The call waits for the device only where
+ * mp3b200_encode_streams_async does: everything it uploads is staged in the call's pinned slot. */
+int mp3b200_encode_streams_tagged_async(mp3b200_session* s, int channels, int samplerate, int kbps, int flags, int nstreams,
+                                        const int16_t* d_pcm, const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
+                                        const int64_t* out_off, int64_t* out_bytes, double* d_gain, int32_t* d_status);
+int mp3b200_encode_streams_tagged_async_f32(mp3b200_session* s, int channels, int samplerate, int kbps, int flags, int nstreams,
+                                            const float* d_pcm, const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
+                                            const int64_t* out_off, int64_t* out_bytes, double* d_gain, int32_t* d_status);
 
 const char* mp3b200_last_error(void);
 /* total number of kernel launches issued by this library since load (bench.py "gpu_launches") */

@@ -259,7 +259,10 @@ __global__ void __launch_bounds__(RG_THREADS) k_rg_pass1(RgParams p) {
   p.end_in[row] = RgEnd{st, sum};
 }
 
-__global__ void __launch_bounds__(RG_THREADS) k_rg_repair(RgParams p, int pass) {
+/* one repair pass, thread = (chunk, channel) as in k_rg_pass1.  The pass index is `pass`, or with At what `at` points to,
+ * read where it is used so that it holds no register through the run. */
+template <bool At>
+__device__ __forceinline__ void rg_repair_pass(const RgParams& p, int pass, const int* at) {
   if (*p.done) return;
   const RgTitle t = p.titles[blockIdx.y];
   const int i = blockIdx.x * RG_THREADS + threadIdx.x;
@@ -278,16 +281,48 @@ __global__ void __launch_bounds__(RG_THREADS) k_rg_repair(RgParams p, int pass) 
   if (merged) { p.end_out[row] = p.end_in[row]; return; }
   p.end_out[row] = RgEnd{st, sum};
   if (!rg_same(st, p.end_in[row].st) || __double_as_longlong(sum) != __double_as_longlong(p.end_in[row].sum))
-    atomicAdd(p.pass_changed + pass, 1);
+    atomicAdd(p.pass_changed + (At ? *at : pass), 1);
 }
 
 /* after pass `pass`: done when it changed no end state; otherwise its end states become the next pass's input */
-__global__ void k_rg_check(RgParams p, int pass, long long rows) {
+__device__ __forceinline__ void rg_check_pass(const RgParams& p, int pass, long long rows) {
   if (*p.done) return;
   const bool stop = p.pass_changed[pass] == 0;
   for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (long long)gridDim.x * blockDim.x)
     p.end_in[r] = p.end_out[r];
   if (stop && blockIdx.x == 0 && threadIdx.x == 0) *p.done = 1;
+}
+
+__global__ void __launch_bounds__(RG_THREADS) k_rg_repair(RgParams p, int pass) { rg_repair_pass<false>(p, pass, nullptr); }
+__global__ void k_rg_check(RgParams p, int pass, long long rows) { rg_check_pass(p, pass, rows); }
+
+/* ---- the repair loop on the device (an encode session's tagged calls: no host round trip per pass) ----
+ * A CUDA graph whose conditional WHILE node has one pass as its body: k_rg_repair_at and k_rg_check_at, which are k_rg_repair
+ * and k_rg_check taking the pass index from device memory, then k_rg_loop_cond.  loop[0] is that index (the host sets it to
+ * RG_QUEUED_PASSES, the passes queued ahead of the graph); k_rg_report leaves the counts of the call in loop[1 .. 2]. */
+__global__ void __launch_bounds__(RG_THREADS) k_rg_repair_at(RgParams p, const int* loop) { rg_repair_pass<true>(p, 0, loop); }
+__global__ void k_rg_check_at(RgParams p, const int* __restrict__ loop, long long rows) { rg_check_pass(p, loop[0], rows); }
+
+/* one thread, after each pass of the body: counts it and lets the body run again unless a pass has changed nothing.  With
+ * max_passes run and still no such pass (the bound of the host loop, rg_finish, which cannot be reached) it ends the loop
+ * with *fault = RG_FAULT. */
+#define RG_FAULT 2
+__global__ void k_rg_loop_cond(cudaGraphConditionalHandle handle, int* __restrict__ loop, int* __restrict__ done, int max_passes,
+                               int* __restrict__ fault) {
+  const int passes = loop[0] + 1;
+  loop[0] = passes;
+  bool more = *done == 0;
+  if (more && passes >= max_passes) { *done = 1; *fault = RG_FAULT; more = false; }
+  cudaGraphSetConditional(handle, more ? 1u : 0u);
+}
+
+/* one thread, after the loop: loop[1] = the passes the analysis needed, counted like rg_finish counts them -- up to and
+ * including the first of the loop[0] passes run that changed nothing (later ones returned at once); loop[2] = chunks run again */
+__global__ void k_rg_report(int* __restrict__ loop, const int* __restrict__ pass_changed, const int* __restrict__ reruns) {
+  int used = 0;
+  while (used < loop[0] && pass_changed[used] != 0) used++;
+  loop[1] = used + 1;
+  loop[2] = *reruns;
 }
 
 /* grid (ceil(max windows / 256), titles): histogram index of every completed window (GainAnalysis.js:466-475) */

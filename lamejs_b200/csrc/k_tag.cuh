@@ -1,5 +1,5 @@
-/* k_tag.cuh -- the music CRC of the Xing / LAME tag on the GPU (SURVEY.md 8(f3)), and the placement of the tag frames of
- * device-resident streams (k_tag_scatter).
+/* k_tag.cuh -- the music CRC of the Xing / LAME tag on the GPU (SURVEY.md 8(f3)), the placement of the tag frames of
+ * device-resident streams (k_tag_scatter), and the frames an encode session finishes on the device (k_tag_finish).
  *
  * lamejs keeps gfc.nMusicCRC by pushing every byte copy_buffer hands out through a table-driven CRC-16 (polynomial
  * x^16 + x^15 + x^2 + 1, reflected, start 0; reference src/js/VBRTag.js:547-556, BitStream.js:924-928): one dependent table
@@ -21,10 +21,12 @@
  */
 #ifndef MP3B200_K_TAG_CUH
 #define MP3B200_K_TAG_CUH
+#include <math.h>
 #include <stdint.h>
+#include "mp3_config.h"
 
 #ifndef __CUDACC__
-#define MP3_HD
+#define MP3_HD inline
 #else
 #define MP3_HD __host__ __device__ __forceinline__
 #endif
@@ -99,6 +101,45 @@ inline void crc_host_tables(CrcTables* t) {
     }
 }
 
+/* ---- the bytes of a tag frame that depend on the encoded data (mp3_tag_frame, mp3_tag.cpp; k_tag_finish below) ----
+ * Everything else in the frame follows from the configuration and the stream's length.  One definition for the host and
+ * the device; tests/tag_patch_emul.cpp compiles it with g++. */
+
+/* gfc.RadioGain = Math.floor(title gain * 10 + 0.5) | 0 (BitStream.js:785) */
+MP3_HD int mp3_radio_gain(double title_db) { return (int)floor(title_db * 10.0 + 0.5); }
+
+/* the tag's Radio Replay Gain field (VBRTag.js:640-661): name code 1, originator 3 (determined automatically), sign bit,
+ * |RadioGain| clamped to 0x1FE */
+MP3_HD int mp3_radio_gain_field(int radio_gain) {
+  if (radio_gain > 0x1FE) radio_gain = 0x1FE;
+  if (radio_gain < -0x1FE) radio_gain = -0x1FE;
+  return radio_gain >= 0 ? (0x2000 | 0xC00 | radio_gain) : (0x2000 | 0xC00 | 0x200 | -radio_gain);
+}
+
+/* CRC-16 of the tag's own bytes (the music CRC's polynomial; under two hundred bytes, bit by bit) */
+MP3_HD unsigned mp3_tag_crc16(const uint8_t* p, int n) {
+  unsigned c = 0;
+  for (int i = 0; i < n; i++) {
+    c ^= p[i];
+    for (int k = 0; k < 8; k++) c = (c & 1u) ? (c >> 1) ^ 0xA001u : c >> 1;
+  }
+  return c;
+}
+
+/* offset of the LAME extension in a tag frame, and the bytes of the frame up to and including its CRC */
+MP3_HD int mp3_tag_lame_at(const Mp3TagParams& p) { return p.sideinfo_len + 116; }
+MP3_HD int mp3_tag_head_bytes(const Mp3TagParams& p) { return mp3_tag_lame_at(p) + 40; }
+
+/* Completes a frame whose other bytes are in place: the Radio Replay Gain field (0: nobody analysed), the music CRC, and
+ * then the frame's own CRC over everything in front of it. */
+MP3_HD void mp3_tag_patch(uint8_t* frame, const Mp3TagParams& p, unsigned music_crc, int radio_gain_field) {
+  uint8_t* q = frame + mp3_tag_lame_at(p);
+  q[19] = (uint8_t)(radio_gain_field >> 8); q[20] = (uint8_t)radio_gain_field;
+  q[36] = (uint8_t)(music_crc >> 8); q[37] = (uint8_t)music_crc;
+  const unsigned own = mp3_tag_crc16(frame, mp3_tag_lame_at(p) + 38);
+  q[38] = (uint8_t)(own >> 8); q[39] = (uint8_t)own;
+}
+
 #ifdef __CUDACC__
 /* grid (pieces of the longest range / CRC_WARPS, ranges); crc_out[r] must be zero before the launch.
  * off[r] / len[r]: byte range r inside `buf`. */
@@ -135,6 +176,29 @@ k_tag_scatter(const long long* __restrict__ dst, const uint8_t* __restrict__ fra
   const uint8_t* src = frames + (size_t)blockIdx.x * frame_bytes;
   uint8_t* d = out + dst[blockIdx.x];
   for (int i = threadIdx.x; i < frame_bytes; i += TAG_SCATTER_THREADS) d[i] = src[i];
+}
+
+/* The tag frames an encode session finishes without the host: grid (frames), one block per frame.  templates + i *
+ * p.frame_bytes is mp3_tag_frame with music CRC 0 and gain field 0, built on the host before anything ran; it goes to
+ * dst[i].at, completed by mp3_tag_patch with the music CRC k_music_crc left in crc[dst[i].stream] and, when the call analysed
+ * (gain != NULL), the field of gain[dst[i].stream].  The patched head is staged in shared memory, so the frame's own CRC reads
+ * no global memory. */
+struct TagDest { uint8_t* at; long long stream; };
+enum { TAG_FINISH_THREADS = 128, TAG_HEAD_MAX = 4 + 32 + 116 + 40 };      /* the longest side info: MPEG-1 stereo */
+__global__ void __launch_bounds__(TAG_FINISH_THREADS)
+k_tag_finish(const TagDest* __restrict__ dst, const uint8_t* __restrict__ templates, Mp3TagParams p, const unsigned* __restrict__ crc,
+             const double* __restrict__ gain) {
+  __shared__ uint8_t head[TAG_HEAD_MAX];
+  const TagDest d = dst[blockIdx.x];
+  const uint8_t* src = templates + (size_t)blockIdx.x * p.frame_bytes;
+  const int nhead = mp3_tag_head_bytes(p);
+  for (int i = threadIdx.x; i < nhead; i += TAG_FINISH_THREADS) head[i] = src[i];
+  for (int i = nhead + threadIdx.x; i < p.frame_bytes; i += TAG_FINISH_THREADS) d.at[i] = src[i];
+  __syncthreads();
+  if (threadIdx.x == 0)
+    mp3_tag_patch(head, p, crc[d.stream] & 0xffffu, gain ? mp3_radio_gain_field(mp3_radio_gain(gain[d.stream])) : 0);
+  __syncthreads();
+  for (int i = threadIdx.x; i < nhead; i += TAG_FINISH_THREADS) d.at[i] = head[i];
 }
 #endif
 

@@ -300,6 +300,10 @@ struct ThreadCtx {
   Buf<RgEnd> rg_end_a, rg_end_b;
   Buf<RgCarry> rg_carry;
   Buf<int> rg_idx, rg_hist, rg_count;
+  /* Workspace::generation for the buffers RgParams names (a graph of the repair loop holds their addresses) */
+  size_t rg_generation() const {
+    return rg_titles.cap + rg_sum.cap + rg_wstate.cap + rg_cstart.cap + rg_end_a.cap + rg_end_b.cap + rg_count.cap + ws.refusals.cap;
+  }
   void release() {
     if (device < 0) return;
     cudaSetDevice(device);
@@ -421,6 +425,7 @@ thread_local bool t_over_budget = false;
 int refusal_error(int refused, int over_budget, int fault) {
   if (refused) { g_err = "non-finite input sample (or one beyond 2^40 once scaled)"; return MP3B200_ERR_CONFIG; }
   if (over_budget) { g_err = "frame over its bit budget (input too loud to encode)"; return MP3B200_ERR_CONFIG; }
+  if (fault == RG_FAULT) { g_err = "ReplayGain repair did not converge"; return MP3B200_ERR_CUDA; }
   if (fault) { g_err = "quantizer stage failed: the fixed-point loop did not converge"; return MP3B200_ERR_CUDA; }
   return 0;
 }
@@ -453,17 +458,22 @@ struct LaunchOpts {
 };
 
 /* The quantizer's fixed-point loop graphs of a session (QuantLoop), one per launch shape: (configuration, streams, frames,
- * longest stream's frames).  They hold the workspace's addresses, so they are all dropped when its generation changes. */
+ * longest stream's frames).  They hold the workspace's addresses, so they are all dropped when its generation changes.
+ * The graphs of the ReplayGain repair loop (rg_finish_queued) are kept the same way: one per (configuration, Float32 rows,
+ * titles, longest title's chunks, chunk rows) -- what RgParams and the launch grids are made of -- dropped when the
+ * context's rg_generation changes. */
 struct LoopGraphs {
   cudaStream_t capture = nullptr;
-  size_t generation = 0;
+  size_t generation = 0, rg_generation = 0;
   std::map<std::tuple<const Config*, int, long long, int>, cudaGraphExec_t> exec;
+  std::map<std::tuple<const Config*, bool, int, int, long long>, cudaGraphExec_t> rg_exec;
+  void clear_rg() { for (auto& e : rg_exec) cudaGraphExecDestroy(e.second); rg_exec.clear(); }
   void clear() { for (auto& e : exec) cudaGraphExecDestroy(e.second); exec.clear(); }
 };
 
-/* Queues the copy of n bytes of host descriptors to dst on c.st.  A session's call stages them in its pinned slot first, so
- * the copy never waits for the device; a thread's context copies from `src` (pageable) as it is. */
-int upload(ThreadCtx& c, void* dst, const void* src, size_t n) {
+/* Queues the copy of n bytes of host descriptors to dst on `on` (NULL: c.st).  A session's call stages them in its pinned
+ * slot first, so the copy never waits for the device; a thread's context copies from `src` (pageable) as it is. */
+int upload(ThreadCtx& c, void* dst, const void* src, size_t n, cudaStream_t on = nullptr) {
   if (c.arena) {
     PinnedArena& a = *c.arena;
     const size_t at = (a.used + 255) & ~(size_t)255;
@@ -472,7 +482,7 @@ int upload(ThreadCtx& c, void* dst, const void* src, size_t n) {
     a.used = at + n;
     src = a.p + at;
   }
-  CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, c.st));
+  CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, on ? on : c.st));
   return 0;
 }
 
@@ -855,8 +865,9 @@ int rg_queue(ThreadCtx& c, Config* cfg, const StreamDesc* sds, RgJob& job, const
   CK(cudaEventRecord(c.ev_rg[0], c.st));
   CK(cudaStreamWaitEvent(st, c.ev_rg[0], 0));
   CK(cudaEventRecord(c.ev_rg[1], st));
-  CK(cudaMemcpyAsync(c.rg_piece.p, starts.data(), sizeof(long long) * (size_t)(npiece + 1), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(c.rg_titles.p, t.data(), sizeof(RgTitle) * (size_t)T, cudaMemcpyHostToDevice, st));
+  if ((rc = upload(c, c.rg_piece.p, starts.data(), sizeof(long long) * (size_t)(npiece + 1), st)) ||
+      (rc = upload(c, c.rg_titles.p, t.data(), sizeof(RgTitle) * (size_t)T, st)))
+    return rc;
   CK(cudaMemsetAsync(c.rg_count.p, 0, sizeof(int) * (size_t)(max_passes + 2), st));
   CK(cudaMemsetAsync(c.rg_hist.p, 0, sizeof(int) * (size_t)(T + 1) * RG_HIST, st));
   CK(cudaMemsetAsync(c.rg_carry.p, 0, sizeof(RgCarry) * (size_t)(T + 1), st));
@@ -882,12 +893,88 @@ int rg_queue(ThreadCtx& c, Config* cfg, const StreamDesc* sds, RgJob& job, const
   return 0;
 }
 
+/* once the repair passes have ended: queues the titles' histograms, the album's, and the gains (c.rg_gain: [t] of the
+ * titles that end, [T] the album's) on c.rg_st */
+int rg_queue_results(ThreadCtx& c, RgJob& job) {
+  cudaStream_t st = c.rg_st;
+  const RgParams& p = job.prm;
+  const int T = (int)job.specs.size();
+  if (job.max_win > 0) {
+    k_rg_hist<<<dim3((unsigned)((job.max_win + 255) / 256), (unsigned)T), 256, 0, st>>>(p.titles, p.W, p.win_sum, c.rg_idx.p);
+    g_launches++;
+  }
+  int* album = c.rg_hist.p + (size_t)T * RG_HIST;
+  k_rg_album<<<(RG_HIST + 255) / 256, 256, 0, st>>>(p.titles, T, album);
+  CK(cudaMemsetAsync(c.rg_gain.p, 0, sizeof(double) * (size_t)(T + 1), st));
+  k_rg_result<<<T + 1, 256, 0, st>>>(p.titles, T, album, c.rg_gain.p);
+  g_launches += 2;
+  return 0;
+}
+
+/* rg_finish for a session, which must not wait for the device: the repair loop runs as a graph on c.rg_st (k_rg_loop_cond),
+ * kept in `lg` per shape and captured here when there is none; then the same results and carries.  `loop` is three words
+ * of device memory: the pass index, and what k_rg_report leaves there (RgJob::passes and reruns of rg_finish); *fault is
+ * set to RG_FAULT if the loop hits rg_finish's bound.  Nothing is read back. */
+int rg_finish_queued(ThreadCtx& c, Config* cfg, RgJob& job, LoopGraphs& lg, int* loop, int* fault) {
+  cudaStream_t st = c.rg_st;
+  RgParams& p = job.prm;
+  const int nch = cfg->host.nch, T = (int)job.specs.size();
+  if (job.max_chunks > 0) {
+    if (lg.rg_generation != c.rg_generation()) { lg.clear_rg(); lg.rg_generation = c.rg_generation(); }
+    const auto key = std::make_tuple((const Config*)cfg, p.f32 != 0, T, job.max_chunks, job.chunk_rows);
+    cudaGraphExec_t& exec = lg.rg_exec[key];
+    if (!exec) {
+      cudaGraph_t g = nullptr;
+      cudaGraphConditionalHandle cond;
+      cudaGraphNode_t node;
+      cudaGraphNodeParams cp = {};
+      cp.type = cudaGraphNodeTypeConditional;
+      bool ok = cudaGraphCreate(&g, 0) == cudaSuccess;
+      ok = ok && cudaGraphConditionalHandleCreate(&cond, g, 1, cudaGraphCondAssignDefault) == cudaSuccess;
+      cp.conditional.handle = cond; cp.conditional.type = cudaGraphCondTypeWhile; cp.conditional.size = 1;
+      ok = ok && cudaGraphAddNode(&node, g, nullptr, 0, &cp) == cudaSuccess;
+      cudaGraph_t body = ok ? cp.conditional.phGraph_out[0] : nullptr;
+      if (ok && cudaStreamBeginCaptureToGraph(lg.capture, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
+        dim3 grid((unsigned)((job.max_chunks * nch + RG_THREADS - 1) / RG_THREADS), (unsigned)T);
+        k_rg_repair_at<<<grid, RG_THREADS, 0, lg.capture>>>(p, loop);
+        k_rg_check_at<<<(unsigned)((job.chunk_rows + 255) / 256), 256, 0, lg.capture>>>(p, loop, job.chunk_rows);
+        k_rg_loop_cond<<<1, 1, 0, lg.capture>>>(cond, loop, p.done, job.max_chunks + RG_QUEUED_PASSES + 1, fault);
+        cudaGraph_t captured = nullptr;
+        ok = cudaStreamEndCapture(lg.capture, &captured) == cudaSuccess && captured == body &&
+             cudaGraphInstantiate(&exec, g, 0) == cudaSuccess;
+      } else {
+        ok = false;
+      }
+      if (g) cudaGraphDestroy(g);
+      if (!ok) {
+        exec = nullptr;
+        lg.rg_exec.erase(key);
+        g_err = "ReplayGain loop graph failed: " + std::string(cudaGetErrorString(cudaGetLastError()));
+        return MP3B200_ERR_CUDA;
+      }
+    }
+    const int first = RG_QUEUED_PASSES;              /* the pass index the graph starts at */
+    int rc = upload(c, loop, &first, sizeof first, st);
+    if (rc) return rc;
+    CK(cudaGraphLaunch(exec, st));
+    k_rg_report<<<1, 1, 0, st>>>(loop, p.pass_changed, p.reruns);
+    g_launches += 2;
+  }
+  const int rc = rg_queue_results(c, job);
+  if (rc) return rc;
+  k_rg_finish<<<T, 256, 0, st>>>(p.titles, p.end_in, nch);
+  g_launches++;
+  CK(cudaGetLastError());
+  return 0;
+}
+
 /* after the encoder has been queued: runs repair passes until one changes nothing, then the histograms, the gains of the
  * titles that end and the carries; reads the results.  Returns with c.rg_st drained. */
 int rg_finish(ThreadCtx& c, Config* cfg, RgJob& job) {
   cudaStream_t st = c.rg_st;
   RgParams& p = job.prm;
   const int nch = cfg->host.nch, T = (int)job.specs.size();
+  int rc = 0;
   if (job.max_chunks > 0) {
     dim3 grid((unsigned)((job.max_chunks * nch + RG_THREADS - 1) / RG_THREADS), (unsigned)T);
     for (;;) {
@@ -910,14 +997,8 @@ int rg_finish(ThreadCtx& c, Config* cfg, RgJob& job) {
     while (used < job.passes && pc[used] != 0) used++;
     job.passes = used + 1;
   }
-  if (job.max_win > 0) {
-    k_rg_hist<<<dim3((unsigned)((job.max_win + 255) / 256), (unsigned)T), 256, 0, st>>>(p.titles, p.W, p.win_sum, c.rg_idx.p);
-    g_launches++;
-  }
-  int* album = c.rg_hist.p + (size_t)T * RG_HIST;
-  k_rg_album<<<(RG_HIST + 255) / 256, 256, 0, st>>>(p.titles, T, album);
-  CK(cudaMemsetAsync(c.rg_gain.p, 0, sizeof(double) * (size_t)(T + 1), st));
-  k_rg_result<<<T + 1, 256, 0, st>>>(p.titles, T, album, c.rg_gain.p);
+  rc = rg_queue_results(c, job);
+  if (rc) return rc;
   std::vector<int> hist0;
   if (job.want_windows && T > 0) {
     job.hist0.assign(RG_HIST, 0);
@@ -927,7 +1008,7 @@ int rg_finish(ThreadCtx& c, Config* cfg, RgJob& job) {
     CK(cudaMemcpyAsync(job.hist0.data(), t0.hist, sizeof(int) * RG_HIST, cudaMemcpyDeviceToHost, st));
   }
   k_rg_finish<<<T, 256, 0, st>>>(p.titles, p.end_in, nch);
-  g_launches += 3;
+  g_launches++;
   CK(cudaEventRecord(c.ev_rg[2], st));
   std::vector<double> g((size_t)T + 1);
   CK(cudaMemcpyAsync(g.data(), c.rg_gain.p, sizeof(double) * (size_t)(T + 1), cudaMemcpyDeviceToHost, st));
@@ -1007,8 +1088,8 @@ int launch_streams(ThreadCtx& c, Config* cfg, std::vector<StreamDesc>& sds, uint
     Timings tm;
     rc = run_pipeline(c, cfg, group, n, d_out, o, arrival, rows, &tm);
     if (rc) return rc;
-    if (o.rg) {
-      rc = rg_finish(c, cfg, *o.rg);
+    if (o.rg) {                                /* a session: ws.refusals[3] is its fault word, [5 .. 8) the loop's words */
+      rc = o.loops ? rg_finish_queued(c, cfg, *o.rg, *o.loops, c.ws.refusals.p + 5, c.ws.refusals.p + 3) : rg_finish(c, cfg, *o.rg);
       if (rc) return rc;
     }
     arrival = nullptr;
@@ -1472,22 +1553,27 @@ const CrcTables& crc_host() {
   return g_crc_host;
 }
 
+/* uploads the CRC tables to `device` on first use there (g_crc_dev) */
+int crc_tables_on(int device) {
+  const CrcTables& ht = crc_host();
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (!g_crc_dev[device]) {
+    CK(cudaMalloc(&g_crc_dev[device], sizeof(CrcTables)));
+    CK(cudaMemcpy(g_crc_dev[device], &ht, sizeof(CrcTables), cudaMemcpyHostToDevice));
+  }
+  return 0;
+}
+
 /* CRC-16 (start 0) of the byte ranges [off[i], off[i] + len[i]) of d_buf, one k_music_crc launch per 65535 ranges, on the
  * calling thread's stream behind whatever wrote the bytes.  crc[i] is valid when the call returns. */
 int music_crc_ranges(int device, const uint8_t* d_buf, const std::vector<long long>& off, const std::vector<long long>& len, std::vector<unsigned>& crc) {
   const int R = (int)off.size();
   crc.assign((size_t)R, 0u);
   if (R == 0) return 0;
-  const CrcTables& ht = crc_host();
-  {
-    std::lock_guard<std::mutex> lk(g_mu);
-    if (!g_crc_dev[device]) {
-      CK(cudaMalloc(&g_crc_dev[device], sizeof(CrcTables)));
-      CK(cudaMemcpy(g_crc_dev[device], &ht, sizeof(CrcTables), cudaMemcpyHostToDevice));
-    }
-  }
+  int rc = crc_tables_on(device);
+  if (rc) return rc;
   ThreadCtx& sc = t_ctx;
-  int rc = sc.crc_ranges.fit((size_t)2 * R);
+  rc = sc.crc_ranges.fit((size_t)2 * R);
   if (rc) return rc;
   rc = sc.crc.fit((size_t)R);
   if (rc) return rc;
@@ -1613,6 +1699,33 @@ namespace {
  *   io.frame(s)                              host memory for stream s's tag frame, once the launch has succeeded
  *   io.finish(tag, audio, at)                puts the frames and the audio where they belong, and drains t_ctx.st
  * out_bytes[s] receives the file's length; `rg` (flags & MP3B200_REPLAYGAIN) receives the analysis. */
+/* What is known about tagged whole streams before anything runs, in closed form from the lamejs FIFO: each stream's frames,
+ * its end padding and the size of its tag frame (tfs, or 0: no frame), and, with `rg`, the pieces the analysis sees
+ * (rg->specs).  `rg` is reset to NULL where lamejs does not analyse: it does so only when the tag is written
+ * (Lame.js:911-916). */
+struct TaggedPlan {
+  int tfs = 0;
+  std::vector<long long> frames;
+  std::vector<int> padding, tag;
+};
+TaggedPlan tagged_plan(const Config* cfg, int nstreams, const int64_t* nsamples, RgJob*& rg) {
+  TaggedPlan pl;
+  pl.tfs = cfg->tag.fits ? cfg->tag.frame_bytes : 0;
+  if (rg && pl.tfs == 0) rg = nullptr;
+  if (rg) rg->specs.assign((size_t)nstreams, RgSpec());
+  pl.frames.resize((size_t)nstreams); pl.padding.resize((size_t)nstreams); pl.tag.resize((size_t)nstreams);
+  for (int s = 0; s < nstreams; s++) {
+    LameFifo fifo(cfg->host.mode_gr, cfg->rs.ratio);
+    if (rg) { rg->specs[s].stream = s; fifo.pieces = &rg->specs[s].pieces; }
+    const long long fed = fifo.feed(nsamples[s]);
+    const FifoFlush fl = fifo.flush();
+    pl.frames[s] = fed + fl.frames;
+    pl.padding[s] = fl.end_padding;
+    pl.tag[s] = pl.tfs > 0 && pl.frames[s] > 0 ? pl.tfs : 0;
+  }
+  return pl;
+}
+
 template <class Io>
 int encode_tagged(int channels, int samplerate, int kbps, int flags, int nstreams, const int64_t* nsamples, int64_t* out_bytes,
                   RgJob* rg, Io& io) {
@@ -1622,21 +1735,10 @@ int encode_tagged(int channels, int samplerate, int kbps, int flags, int nstream
   int rc = get_config(channels, samplerate, kbps, flags & MP3B200_RESAMPLE, &cfg);
   if (rc || (rc = io.check_input(cfg))) return rc;
   const Mp3TagParams& p = cfg->tag;
-  const int tfs = p.fits ? p.frame_bytes : 0;
-  if (rg && tfs == 0) rg = nullptr;               /* lamejs analyses only when the tag is written (Lame.js:911-916) */
-  if (rg) rg->specs.assign((size_t)nstreams, RgSpec());
-  /* each stream's frames and end padding, and the pieces the analysis sees: closed form, before anything runs */
-  std::vector<long long> frames((size_t)nstreams);
-  std::vector<int> padding((size_t)nstreams), tag((size_t)nstreams);
-  for (int s = 0; s < nstreams; s++) {
-    LameFifo fifo(cfg->host.mode_gr, cfg->rs.ratio);
-    if (rg) { rg->specs[s].stream = s; fifo.pieces = &rg->specs[s].pieces; }
-    const long long fed = fifo.feed(nsamples[s]);
-    const FifoFlush fl = fifo.flush();
-    frames[s] = fed + fl.frames;
-    padding[s] = fl.end_padding;
-    tag[s] = tfs > 0 && frames[s] > 0 ? tfs : 0;
-  }
+  const TaggedPlan plan = tagged_plan(cfg, nstreams, nsamples, rg);
+  const int tfs = plan.tfs;
+  const std::vector<long long>& frames = plan.frames;
+  const std::vector<int>&padding = plan.padding, &tag = plan.tag;
   std::vector<long long> audio, at;
   rc = io.launch(cfg, tfs, tag, rg, audio, at);
   if (rc || nstreams == 0) return rc;

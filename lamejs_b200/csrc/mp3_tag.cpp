@@ -20,16 +20,6 @@ inline void put_be(uint8_t* p, int nbytes, long long v) {
   for (int i = 0; i < nbytes; i++) p[i] = (uint8_t)(v >> (8 * (nbytes - 1 - i)));
 }
 
-/* CRC-16 of the tag's own bytes (same polynomial as the music CRC; a hundred-odd bytes, done in place) */
-unsigned crc16_bytes(const uint8_t* p, int n) {
-  unsigned c = 0;
-  for (int i = 0; i < n; i++) {
-    c ^= p[i];
-    for (int k = 0; k < 8; k++) c = (c & 1u) ? (c >> 1) ^ 0xA001u : c >> 1;
-  }
-  return c;
-}
-
 }  // namespace
 
 void Mp3SeekBag::reset() { sum = 0; seen = 0; want = 1; pos = 0; frames = 0; }
@@ -62,14 +52,6 @@ int mp3_tag_placeholder(const Mp3TagParams& p, uint8_t* out) {
   return p.frame_bytes;
 }
 
-int mp3_radio_gain(double title_db) { return (int)floor(title_db * 10.0 + 0.5); }
-
-int mp3_radio_gain_field(int radio_gain) {
-  if (radio_gain > 0x1FE) radio_gain = 0x1FE;
-  if (radio_gain < -0x1FE) radio_gain = -0x1FE;
-  return radio_gain >= 0 ? (0x2000 | 0xC00 | radio_gain) : (0x2000 | 0xC00 | 0x200 | -radio_gain);
-}
-
 int mp3_tag_frame(const Mp3TagParams& p, const Mp3SeekBag& bag, long long music_bytes, unsigned music_crc, int encoder_padding, uint8_t* out,
                   int radio_gain_field) {
   if (!p.fits || bag.pos <= 0) return 0;
@@ -89,14 +71,13 @@ int mp3_tag_frame(const Mp3TagParams& p, const Mp3SeekBag& bag, long long music_
     int seek = (int)(256. * (double)bag.bag[at] / (double)bag.sum);
     toc[i] = (uint8_t)(seek > 255 ? 255 : seek);
   }
-  uint8_t* q = w + 116;                                      /* the LAME extension */
+  uint8_t* q = out + mp3_tag_lame_at(p);                     /* the LAME extension */
   put_be(q, 4, p.quality_byte);
   memcpy(q + 4, "LAME3.98r", 9);                             /* Version.js:56-59 */
   q[13] = 1;                                                 /* tag revision 0, method 1 = CBR */
   q[14] = (uint8_t)p.lowpass_byte;
-  /* q[15..18] peak amplitude: zero (it needs the decoder); q[19..20] Radio Replay Gain when analysed (0 otherwise),
+  /* q[15..18] peak amplitude: zero (it needs the decoder); q[19..20] Radio Replay Gain: mp3_tag_patch;
    * q[21..22] Audiophile Replay Gain: zero (lamejs never sets it) */
-  put_be(q + 19, 2, radio_gain_field);
   q[23] = (uint8_t)p.flags_byte;
   q[24] = (uint8_t)(p.kbps >= 255 ? 255 : p.kbps);
   const int delay = 576;                                     /* Encoder.ENCDELAY */
@@ -107,8 +88,7 @@ int mp3_tag_frame(const Mp3TagParams& p, const Mp3SeekBag& bag, long long music_
   q[29] = 0;
   put_be(q + 30, 2, p.kbps);                                 /* gfp.preset = the bitrate (Presets.js:415) */
   put_be(q + 32, 4, stream_bytes);
-  put_be(q + 36, 2, music_crc & 0xffffu);
-  put_be(q + 38, 2, crc16_bytes(out, (int)(q + 38 - out)));
+  mp3_tag_patch(out, p, music_crc & 0xffffu, radio_gain_field);      /* q[19..20], q[36..39] */
   return p.frame_bytes;
 }
 

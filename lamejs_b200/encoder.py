@@ -108,6 +108,8 @@ def lib():
     L.mp3b200_encode_streams_async.argtypes = [vp, c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp]
     L.mp3b200_encode_streams_async_f32.argtypes = [vp, c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp]
     L.mp3b200_check_status.argtypes = [vp]
+    L.mp3b200_encode_streams_tagged_async.argtypes = [vp, c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.mp3b200_encode_streams_tagged_async_f32.argtypes = [vp, c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp, vp, vp]
     _lib = L
     return L
 
@@ -159,6 +161,7 @@ _F32_TWIN = {
     "mp3b200_encode_streams_tagged_ex": "mp3b200_encode_streams_tagged_f32",
     "mp3b200_encode_streams_device_ex": "mp3b200_encode_streams_device_f32",
     "mp3b200_encode_streams_tagged_device": "mp3b200_encode_streams_tagged_device_f32",
+    "mp3b200_encode_streams_tagged_async": "mp3b200_encode_streams_tagged_async_f32",
     "mp3b200_debug_resample": "mp3b200_debug_resample_f32",
     "mp3b200_debug_replaygain": "mp3b200_debug_replaygain_f32",
 }
@@ -639,11 +642,8 @@ class EncodeSession:
             _check(lib().mp3b200_session_create(ctypes.c_void_p(self.stream.cuda_stream or None), ctypes.byref(h)))
         self._h = h
 
-    def encode_streams(self, channels, samplerate, kbps, pcm, pcm_off, nsamples, out, out_off, resample=False):
-        """encode_streams_device on tensors, queued: `pcm` is a 1-D CUDA tensor of int16 or float32 samples (float32 is
-        encoded as lamejs encodes a Float32Array), laid out as encode_streams_device reads d_pcm; `out` a uint8 CUDA tensor,
-        stream s written at out_off[s].  pcm_off, nsamples and out_off are host sequences.  Returns the int32[4] status
-        tensor the call fills on the session's stream (check_status reads it)."""
+    def _checked(self, channels, samplerate, kbps, pcm, pcm_off, nsamples, out, out_off, resample, tag_bytes):
+        """the tensor and layout checks of a call; tag_bytes: room of a stream's tag frame.  Returns the three int64 arrays."""
         import torch
         if self._h is None:
             raise ValueError("the session is closed")
@@ -665,18 +665,53 @@ class EncodeSession:
         if S:
             nb = {int(n): stream_bytes(channels, samplerate, kbps, int(n), resample) for n in np.unique(nsamples) if n >= 0}
             if all(b >= 0 for b in nb.values()) and (nsamples >= 0).all():
-                room = np.array([nb[int(n)] for n in nsamples], dtype=np.int64)
+                room = np.array([nb[int(n)] + tag_bytes for n in nsamples], dtype=np.int64)
                 if ((pcm_off < 0) | (pcm_off + nsamples * channels > pcm.numel()) | (out_off < 0) |
                         (out_off + room > out.numel())).any():
                     raise ValueError("a stream lies outside pcm or out")
+        return pcm_off, nsamples, out_off
+
+    def encode_streams(self, channels, samplerate, kbps, pcm, pcm_off, nsamples, out, out_off, resample=False):
+        """encode_streams_device on tensors, queued: `pcm` is a 1-D CUDA tensor of int16 or float32 samples (float32 is
+        encoded as lamejs encodes a Float32Array), laid out as encode_streams_device reads d_pcm; `out` a uint8 CUDA tensor,
+        stream s written at out_off[s].  pcm_off, nsamples and out_off are host sequences.  Returns the int32[4] status
+        tensor the call fills on the session's stream (check_status reads it)."""
+        import torch
+        pcm_off, nsamples, out_off = self._checked(channels, samplerate, kbps, pcm, pcm_off, nsamples, out, out_off, resample, 0)
         with torch.cuda.stream(self.stream):
             status = torch.empty(4, dtype=torch.int32, device=self.device)
         fn = lib().mp3b200_encode_streams_async_f32 if pcm.dtype == torch.float32 else lib().mp3b200_encode_streams_async
-        _check(fn(self._h, channels, samplerate, kbps, RESAMPLE if resample else 0, S, pcm.data_ptr(), pcm_off.ctypes.data,
+        _check(fn(self._h, channels, samplerate, kbps, RESAMPLE if resample else 0, len(nsamples), pcm.data_ptr(), pcm_off.ctypes.data,
                   nsamples.ctypes.data, out.data_ptr(), out_off.ctypes.data, status.data_ptr()))
         for t in (pcm, out, status):
             t.record_stream(self.stream)
         return status
+
+    def encode_streams_tagged(self, channels, samplerate, kbps, pcm, pcm_off, nsamples, out, out_off, resample=False,
+                              find_replay_gain=False):
+        """encode_streams_device_tagged on tensors, queued (DESIGN.md 15): stream s becomes one finished file at
+        out[out_off[s]:], its Info / LAME tag frame and then its audio, and needs stream_bytes(...) + lametag_size(...) bytes
+        of room.  Returns (out_bytes, gains, status): the files' lengths, a host list known at once; with find_replay_gain a
+        float64 CUDA tensor of the title gains and, last, the album gain in dB (-24601: nothing to analyse), else None; and
+        the int32[8] status tensor (check_status reads it; [4] and [5] are the analysis's passes and reruns).  Tensors and
+        status are filled on the session's stream."""
+        import torch
+        tfs = lametag_size(channels, samplerate, kbps, resample)
+        pcm_off, nsamples, out_off = self._checked(channels, samplerate, kbps, pcm, pcm_off, nsamples, out, out_off, resample,
+                                                   max(tfs, 0))
+        S = len(nsamples)
+        got = np.zeros(max(S, 1), dtype=np.int64)
+        with torch.cuda.stream(self.stream):
+            status = torch.empty(8, dtype=torch.int32, device=self.device)
+            gains = torch.empty(S + 1, dtype=torch.float64, device=self.device) if find_replay_gain else None
+        flags = (REPLAYGAIN if find_replay_gain else 0) | (RESAMPLE if resample else 0)
+        fn = _entry("mp3b200_encode_streams_tagged_async", pcm.dtype == torch.float32)
+        _check(fn(self._h, channels, samplerate, kbps, flags, S, pcm.data_ptr(), pcm_off.ctypes.data, nsamples.ctypes.data,
+                  out.data_ptr(), out_off.ctypes.data, got.ctypes.data, gains.data_ptr() if find_replay_gain else None,
+                  status.data_ptr()))
+        for t in (pcm, out, status) + ((gains,) if find_replay_gain else ()):
+            t.record_stream(self.stream)
+        return [int(g) for g in got[:S]], gains, status
 
     def close(self):
         """Waits for the session's queued work and frees it."""
