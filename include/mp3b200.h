@@ -482,6 +482,37 @@ int mp3b200_encode_streams_tagged_async_f32(mp3b200_session* s, int channels, in
                                             const float* d_pcm, const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
                                             const int64_t* out_off, int64_t* out_bytes, double* d_gain, int32_t* d_status);
 
+/* Streaming handles in a session (DESIGN.md 16): encodeBuffer / flush() on n live handles of one configuration, queued on the
+ * session's stream.  Entry i's bytes go to d_out + out_off[i]; out_bytes[i] (host) is filled when the call returns and equals
+ * what mp3b200_encode_batch_device / _f32 / mp3b200_flush_batch return for the same handles and calls.  d_status is the
+ * int32[4] of mp3b200_encode_streams_async (mp3b200_check_status reads it).  Rows are device (or managed) memory on the
+ * session's device and may be freed once the stream has passed the call.
+ * A handle's first session call binds it to the session (this may block): its tail and carried state then live on the
+ * device, and every host-side call on it (encode, flush, the batch calls, export / import, seek, the tag and ReplayGain
+ * setters and getters) and any other session's call returns MP3B200_ERR_HANDLE until mp3b200_session_release moves them
+ * back to the host.  mp3b200_destroy and mp3b200_session_destroy release first.
+ * A call refused on the device (a non-finite Float32 sample or one beyond 2^40 once scaled, a frame over its bit budget)
+ * commits nothing: each handle it names is marked refused, every later call that names one reports the same refusal in its
+ * status, and at release each such handle is exactly where it stood before the refused call.
+ * Refused before anything is queued: NULL or repeated handles, a handle with the tag or ReplayGain on, a handle bound to
+ * another session, rows that are not device memory on the session's device, a capturing stream, more than 65535 handles
+ * (MP3B200_ERR_HANDLE); handles of different configurations or of another device (MP3B200_ERR_CONFIG).  The call waits for
+ * the device only where mp3b200_encode_streams_async does, and when it binds a handle. */
+int mp3b200_session_encode_batch(mp3b200_session* s, mp3b200_encoder* const* handles, const int16_t* const* d_left,
+                                 const int16_t* const* d_right, const int* nsamples, int n, uint8_t* d_out, const int64_t* out_off,
+                                 int* out_bytes, int32_t* d_status);
+int mp3b200_session_encode_batch_f32(mp3b200_session* s, mp3b200_encoder* const* handles, const float* const* d_left,
+                                     const float* const* d_right, const int* nsamples, int n, uint8_t* d_out, const int64_t* out_off,
+                                     int* out_bytes, int32_t* d_status);
+int mp3b200_session_flush_batch(mp3b200_session* s, mp3b200_encoder* const* handles, int n, uint8_t* d_out, const int64_t* out_off,
+                                int* out_bytes, int32_t* d_status);
+/* the exact bytes the handle's next call of nsamples samples (-1: flush) hands out; host arithmetic only, bound or not */
+int mp3b200_encode_bytes(const mp3b200_encoder* h, int nsamples);
+/* waits for the session's work, settles refusals and gives the handles back to the host calls (unbound handles: no-op) */
+int mp3b200_session_release(mp3b200_session* s, mp3b200_encoder* const* handles, int n);
+/* the samples per channel a bound handle's tail buffer holds: the most any handle of the configuration retains after a call */
+int64_t mp3b200_session_tail_capacity(int channels, int samplerate, int kbps, int flags);
+
 const char* mp3b200_last_error(void);
 /* total number of kernel launches issued by this library since load (bench.py "gpu_launches") */
 int64_t mp3b200_launch_count(void);

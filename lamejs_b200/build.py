@@ -9,7 +9,8 @@ LIB = os.path.join(HERE, "libmp3b200.so")
 STAMP = LIB + ".flags"          # the flags LIB was built with: a library built with other flags is rebuilt
 SOURCES = ["mp3_encoder.cu", "mp3_config.cpp", "mp3_tag.cpp", "mp3_id3.cpp"]
 DEPS = SOURCES + ["mp3_config.h", "mp3_device.cuh", "mp3_math.cuh", "mp3_tables.h", "k_filterbank.cuh", "k_psy.cuh",
-                  "k_quant.cuh", "k_tag.cuh", "k_resample.cuh", "k_replaygain.cuh", "k_stage.cuh", "mp3_tag.h", "mp3_handle.inc", "mp3_session.inc", "../../include/mp3b200.h"]
+                  "k_quant.cuh", "k_tag.cuh", "k_resample.cuh", "k_replaygain.cuh", "k_stage.cuh", "k_handle.cuh", "mp3_tag.h", "mp3_handle.inc",
+                  "mp3_session.inc", "mp3_session_handles.inc", "../../include/mp3b200.h"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     # bit-exactness contract: no FMA contraction, IEEE div/sqrt, no flush-to-zero (DESIGN.md "numerics")

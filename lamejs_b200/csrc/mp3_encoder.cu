@@ -30,6 +30,7 @@
 #include "k_resample.cuh"
 #include "k_replaygain.cuh"
 #include "k_stage.cuh"
+#include "k_handle.cuh"
 #include "mp3_tag.h"
 
 namespace {
@@ -455,7 +456,12 @@ struct LaunchOpts {
                                             sync, a non-finite sample makes the launch return MP3B200_ERR_CONFIG */
   struct LoopGraphs* loops = nullptr;    /* run the quantizer's fixed-point loop on the device, as the cached graphs of a session
                                             (no host round trip; needs !sync) */
+  const struct HandleCarry* carry = nullptr;   /* streaming handles bound to a session: their carried state is on the device
+                                                  (k_handle_carry_in; one launch group only) */
 };
+
+/* LaunchOpts::carry: recs[z] is the record of stream z (device array); halo_scratch takes the masking of refused handles */
+struct HandleCarry { HandleRecord* const* recs; float* halo_scratch; };
 
 /* The quantizer's fixed-point loop graphs of a session (QuantLoop), one per launch shape: (configuration, streams, frames,
  * longest stream's frames).  They hold the workspace's addresses, so they are all dropped when its generation changes.
@@ -527,6 +533,11 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, uint8_
   }
   int rc = wait_legacy(c);
   if (rc || (rc = upload(c, ws.streams.p, h_streams, sizeof(StreamDesc) * S))) return rc;
+  if (o.carry) {
+    k_handle_carry_in<<<(S + 127) / 128, 128, 0, st>>>(ws.streams.p, S, o.carry->recs, o.carry->halo_scratch);
+    g_launches++;
+    DBG("k_handle_carry_in");
+  }
   CK(cudaEventRecord(ev[0], st));
 
   /* K2: psy analysis, one block per (granule incl. 1 halo, channel, stream) */
@@ -1955,6 +1966,7 @@ int mp3b200_debug_replaygain_f32(int channels, int samplerate, int kbps, int fla
 
 #include "mp3_handle.inc"
 #include "mp3_session.inc"
+#include "mp3_session_handles.inc"
 
 #ifdef Q_TASKSTAT
 extern "C" int mp3b200_debug_taskstat(int* out, int rows) {

@@ -110,6 +110,13 @@ def lib():
     L.mp3b200_check_status.argtypes = [vp]
     L.mp3b200_encode_streams_tagged_async.argtypes = [vp, c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp, vp, vp]
     L.mp3b200_encode_streams_tagged_async_f32.argtypes = [vp, c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.mp3b200_session_encode_batch.argtypes = [vp, vp, vp, vp, vp, c_int, vp, vp, vp, vp]
+    L.mp3b200_session_encode_batch_f32.argtypes = [vp, vp, vp, vp, vp, c_int, vp, vp, vp, vp]
+    L.mp3b200_session_flush_batch.argtypes = [vp, vp, c_int, vp, vp, vp, vp]
+    L.mp3b200_encode_bytes.argtypes = [vp, c_int]
+    L.mp3b200_session_release.argtypes = [vp, vp, c_int]
+    L.mp3b200_session_tail_capacity.argtypes = [c_int, c_int, c_int, c_int]
+    L.mp3b200_session_tail_capacity.restype = c_i64
     _lib = L
     return L
 
@@ -712,6 +719,80 @@ class EncodeSession:
         for t in (pcm, out, status) + ((gains,) if find_replay_gain else ()):
             t.record_stream(self.stream)
         return [int(g) for g in got[:S]], gains, status
+
+    def _handles(self, encoders):
+        if self._h is None:
+            raise ValueError("the session is closed")
+        if any(not isinstance(e, Mp3Encoder) or not e._h for e in encoders):
+            raise ValueError("encoders must be open Mp3Encoder objects")
+        if len({id(e) for e in encoders}) != len(encoders):
+            raise ValueError("a session call names each encoder once (make two calls instead)")
+        return (ctypes.c_void_p * max(len(encoders), 1))(*[e._h for e in encoders])
+
+    def _queue(self, encoders, lengths, call, *tensors):
+        """allocates `out` for the calls' exact lengths on the session's stream and runs call(hp, out, offsets, got, status)"""
+        import torch
+        S = len(encoders)
+        hp = self._handles(encoders)
+        lengths = [_check(int(lib().mp3b200_encode_bytes(e._h, n))) for e, n in zip(encoders, lengths)]
+        offsets = np.zeros(max(S, 1), dtype=np.int64)
+        if S > 1:
+            offsets[1:S] = np.cumsum(lengths[:-1])
+        with torch.cuda.stream(self.stream):
+            out = torch.empty(max(sum(lengths), 1), dtype=torch.uint8, device=self.device)
+            status = torch.empty(4, dtype=torch.int32, device=self.device)
+        got = np.zeros(max(S, 1), dtype=np.int32)
+        _check(call(hp, out.data_ptr(), offsets.ctypes.data, got.ctypes.data, status.data_ptr()))
+        for t in (out, status) + tensors:
+            t.record_stream(self.stream)
+        assert [int(g) for g in got[:S]] == lengths
+        return out, [int(o) for o in offsets[:S]], lengths, status
+
+    def encode_batch(self, encoders, lefts, rights=None):
+        """encodeBuffer on live Mp3Encoder objects of one configuration, queued on the session's stream (DESIGN.md 16):
+        `lefts` / `rights` are CUDA tensors on the session's device (floating dtypes are encoded as Float32, like
+        Mp3Encoder.encodeBuffer).  Each encoder's first session call binds it to the session: until release() its host
+        calls raise Mp3B200Error.  Returns (out, offsets, lengths, status): a uint8 CUDA tensor filled on the stream, encoder
+        i's bytes at out[offsets[i]:offsets[i] + lengths[i]] (host lists, known at once), and the int32[4] status tensor
+        check_status reads.  Nothing here orders the rows: produce them on the session's stream, or make it wait."""
+        import torch
+        if self._h is None:
+            raise ValueError("the session is closed")
+        S = len(encoders)
+        if len(lefts) != S or (rights is not None and len(rights) != S):
+            raise ValueError("one row (pair) per encoder")
+        rights = [None] * S if rights is None else list(rights)
+        rows = [x for x in (*lefts, *rights) if x is not None]
+        if not all(_on_cuda(x) and x.device == self.device for x in rows):
+            raise ValueError("rows must be CUDA tensors on the session's device (%s)" % self.device)
+        if any(x.dim() != 1 for x in rows):
+            raise ValueError("rows must be 1-D")
+        f32 = any(x.dtype.is_floating_point for x in rows)
+        dt = torch.float32 if f32 else torch.int16
+        with torch.cuda.stream(self.stream):
+            lefts = [x.to(dt).contiguous() for x in lefts]
+            rights = [l if (r is None or e.channels == 1) else r.to(dt).contiguous() for e, l, r in zip(encoders, lefts, rights)]
+        if any(len(l) != len(r) for l, r in zip(lefts, rights)):
+            raise ValueError("left and right rows differ in length")
+        ns = np.array([len(x) for x in lefts] or [0], dtype=np.int32)
+        lp = (ctypes.c_void_p * max(S, 1))(*[x.data_ptr() for x in lefts])
+        rp = (ctypes.c_void_p * max(S, 1))(*[x.data_ptr() for x in rights])
+        fn = lib().mp3b200_session_encode_batch_f32 if f32 else lib().mp3b200_session_encode_batch
+        return self._queue(encoders, [int(n) for n in ns[:S]],
+                           lambda hp, o, off, got, st: fn(self._h, hp, lp, rp, ns.ctypes.data, S, o, off, got, st),
+                           *lefts, *rights)
+
+    def flush_batch(self, encoders):
+        """flush() on live Mp3Encoder objects, queued on the session's stream; returns what encode_batch returns"""
+        S = len(encoders)
+        return self._queue(encoders, [-1] * S,
+                           lambda hp, o, off, got, st: lib().mp3b200_session_flush_batch(self._h, hp, S, o, off, got, st))
+
+    def release(self, encoders):
+        """Waits for the session's work on `encoders` and gives them back to their host calls: each continues its stream
+        exactly where it stands (a handle of a refused call: where it stood before that call)."""
+        hp = self._handles(encoders)
+        _check(lib().mp3b200_session_release(self._h, hp, len(encoders)))
 
     def close(self):
         """Waits for the session's queued work and frees it."""
