@@ -508,10 +508,46 @@ int mp3b200_session_flush_batch(mp3b200_session* s, mp3b200_encoder* const* hand
                                 int* out_bytes, int32_t* d_status);
 /* the exact bytes the handle's next call of nsamples samples (-1: flush) hands out; host arithmetic only, bound or not */
 int mp3b200_encode_bytes(const mp3b200_encoder* h, int nsamples);
-/* waits for the session's work, settles refusals and gives the handles back to the host calls (unbound handles: no-op) */
+/* the same for every call of a schedule on a fresh handle of the configuration (flags: MP3B200_RESAMPLE), with the tag
+ * switched on when write_vbr_tag is non-zero and the tag fits: out_bytes[i] for the call of nsamples[i] samples (-1: flush),
+ * the placeholder included.  Host arithmetic only: needs no device. */
+int mp3b200_encode_bytes_schedule(int channels, int samplerate, int kbps, int flags, int write_vbr_tag, const int* nsamples, int n,
+                                  int* out_bytes);
+/* waits for the session's work, settles refusals and gives the handles back to the host calls (unbound handles: no-op),
+ * a tagged handle with its music CRC and a ReplayGain handle with its title gain, RadioGain and title count */
 int mp3b200_session_release(mp3b200_session* s, mp3b200_encoder* const* handles, int n);
 /* the samples per channel a bound handle's tail buffer holds: the most any handle of the configuration retains after a call */
 int64_t mp3b200_session_tail_capacity(int channels, int samplerate, int kbps, int flags);
+
+/* Tagged and ReplayGain handles in a session (DESIGN.md 17).  mp3b200_session_encode_batch_tagged / _f32 and
+ * mp3b200_session_flush_batch_tagged take the arguments of the three calls above and live handles of one configuration in
+ * any mix: plain, with the tag (mp3b200_set_write_vbr_tag), and with the tag and ReplayGain (mp3b200_set_find_replay_gain).
+ * out_bytes[i] is what mp3b200_encode_bytes says, and the bytes are those of mp3b200_encode_batch_device / _f32 /
+ * mp3b200_flush_batch, the all-zero placeholder a tagged handle's first feeding call (or flush) hands out included.  The
+ * music CRC, the analysis and the title gains stay on the device and commit only when the call stands.
+ *   d_status    int32[8]: [0 .. 3] as for mp3b200_encode_streams_async (mp3b200_check_status reads them; a ReplayGain repair
+ *               loop that hits its bound raises [3]: "ReplayGain repair did not converge"), [4] the analysis's pass count,
+ *               [5] the chunks it ran again, [6] and [7] zero.
+ * Refused before anything is queued: what the calls above refuse, less the rule on the tag and ReplayGain. */
+int mp3b200_session_encode_batch_tagged(mp3b200_session* s, mp3b200_encoder* const* handles, const int16_t* const* d_left,
+                                        const int16_t* const* d_right, const int* nsamples, int n, uint8_t* d_out, const int64_t* out_off,
+                                        int* out_bytes, int32_t* d_status);
+int mp3b200_session_encode_batch_tagged_f32(mp3b200_session* s, mp3b200_encoder* const* handles, const float* const* d_left,
+                                            const float* const* d_right, const int* nsamples, int n, uint8_t* d_out,
+                                            const int64_t* out_off, int* out_bytes, int32_t* d_status);
+int mp3b200_session_flush_batch_tagged(mp3b200_session* s, mp3b200_encoder* const* handles, int n, uint8_t* d_out,
+                                       const int64_t* out_off, int* out_bytes, int32_t* d_status);
+/* Queues, for each handle (one configuration), the frame mp3b200_get_lametag_frame would return at this point of the
+ * stream to d_out + out_off[i]; out_bytes[i] (host, known at return) is its size, 0 with the tag off or before the first
+ * frame.  The music CRC and the Radio Replay Gain field come from the device.  d_status: int32[4] as for
+ * mp3b200_encode_streams_async, non-zero where a handle named was refused by an earlier call.  Binds unbound handles. */
+int mp3b200_session_lametag_frames(mp3b200_session* s, mp3b200_encoder* const* handles, int n, uint8_t* d_out, const int64_t* out_off,
+                                   int* out_bytes, int32_t* d_status);
+/* mp3b200_album_gain queued on the session's stream: GetAlbumGain over the B histograms of the handles that analyse, one double
+ * written to device memory d_album (-24601: nothing analysed).  d_status as for mp3b200_session_lametag_frames. */
+int mp3b200_session_album_gain(mp3b200_session* s, mp3b200_encoder* const* handles, int n, double* d_album, int32_t* d_status);
+/* the loop graphs (quantizer and ReplayGain repair) the session has instantiated so far: flat once its shapes are warm */
+int64_t mp3b200_session_graph_instantiations(mp3b200_session* s);
 
 const char* mp3b200_last_error(void);
 /* total number of kernel launches issued by this library since load (bench.py "gpu_launches") */

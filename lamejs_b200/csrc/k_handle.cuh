@@ -20,6 +20,10 @@ struct HandleRecord {
   int refused;                      /* a call that named the handle was refused: nothing has been committed since */
   int words[3];                     /* that call's status words [0], [1] and [3] */
   unsigned long long call;          /* that call's index in its session */
+  /* tagged handles (DESIGN.md 17): gfc.nMusicCRC, and the titles ended so far with the last one's gain (GetTitleGain) */
+  unsigned music_crc;
+  int titles;
+  double title_db;
 };
 
 /* one handle's tail of a call: dst[c][i] = src[c][i] for i < n_src, else 0 (flush zeros), i < n; nothing when rec is refused */
@@ -107,6 +111,84 @@ k_handle_commit(const StreamDesc* __restrict__ streams, const CommitDesc* __rest
         r.old_value[c] = sd.old_value[c]; r.current_step[c] = sd.current_step[c];
       }
     }
+  }
+}
+
+/* ---- tagged and ReplayGain handles (mp3b200_session_encode_batch_tagged and its twins, DESIGN.md 17) ----
+ * These need k_tag.cuh (crc_append) and k_replaygain.cuh (RgCarry, RG_HIST), which mp3_encoder.cu includes first.
+ * A call's refusal is known only after the packer, so nothing that analyses or checksums a call writes a handle's own state:
+ * the analysis works on a copy of each handle's carry and histogram A (k_rg_stage_in), and the commit kernels below, which
+ * run behind k_handle_commit, take the results into the handle only when words[7] says the call stood. */
+
+/* one analysing handle of a call: its RgCarry + A (d_rg) and their copy in session workspace; q is its title in the job */
+struct RgStageDesc {
+  uint8_t* handle;
+  uint8_t* stage;
+  HandleRecord* rec;
+  int q, title_end;
+};
+enum { RG_STAGE_BYTES = (int)sizeof(RgCarry) + 4 * RG_HIST, RG_STAGE_THREADS = 256 };
+static_assert(RG_STAGE_BYTES % 16 == 0, "RgCarry + A copied as 16-byte words");
+
+/* grid (handles): stage = the handle's carry and A */
+__global__ void __launch_bounds__(RG_STAGE_THREADS) k_rg_stage_in(const RgStageDesc* __restrict__ d) {
+  const RgStageDesc e = d[blockIdx.x];
+  const uint4* src = reinterpret_cast<const uint4*>(e.handle);
+  uint4* dst = reinterpret_cast<uint4*>(e.stage);
+  for (int i = threadIdx.x; i < RG_STAGE_BYTES / 16; i += RG_STAGE_THREADS) dst[i] = src[i];
+}
+
+/* grid (handles), behind k_handle_commit: when the call stood, the staged carry and A become the handle's; at a title end
+ * (GetTitleGain) A is added to B instead and cleared, and the record takes the title's gain (gain[q]) and counts it */
+__global__ void __launch_bounds__(RG_STAGE_THREADS)
+k_rg_commit(const RgStageDesc* __restrict__ d, const int* __restrict__ words, const double* __restrict__ gain) {
+  if (words[7]) return;
+  const RgStageDesc e = d[blockIdx.x];
+  if (!e.title_end) {
+    const uint4* src = reinterpret_cast<const uint4*>(e.stage);
+    uint4* dst = reinterpret_cast<uint4*>(e.handle);
+    for (int i = threadIdx.x; i < RG_STAGE_BYTES / 16; i += RG_STAGE_THREADS) dst[i] = src[i];
+    return;
+  }
+  const int* a = reinterpret_cast<const int*>(e.stage + sizeof(RgCarry));
+  int* ha = reinterpret_cast<int*>(e.handle + sizeof(RgCarry));
+  int* hb = ha + RG_HIST;
+  for (int b = threadIdx.x; b < RG_HIST; b += RG_STAGE_THREADS) { hb[b] += a[b]; ha[b] = 0; }
+  const unsigned* cs = reinterpret_cast<const unsigned*>(e.stage);     /* the carry k_rg_finish zeroed */
+  unsigned* ch = reinterpret_cast<unsigned*>(e.handle);
+  for (int i = threadIdx.x; i < (int)(sizeof(RgCarry) / 4); i += RG_STAGE_THREADS) ch[i] = cs[i];
+  if (threadIdx.x == 0) { e.rec->title_db = gain[e.q]; e.rec->titles++; }
+}
+
+/* one tagged handle whose frames a call encodes: k_music_crc's word crc[k] of its `bytes` audio bytes */
+struct CrcCommitDesc {
+  HandleRecord* rec;
+  long long bytes;
+};
+
+/* behind k_handle_commit: when the call stood, each record's music CRC continues over the call's audio (copy_buffer's
+ * running CRC, BitStream.js:924-928) */
+__global__ void k_crc_commit(const CrcCommitDesc* __restrict__ d, int n, const unsigned* __restrict__ crc,
+                             const CrcTables* __restrict__ tables, const int* __restrict__ words) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n || words[7]) return;
+  HandleRecord& r = *d[k].rec;
+  r.music_crc = crc_append(r.music_crc, crc[k] & 0xffffu, (unsigned long long)d[k].bytes, tables->pow);
+}
+
+/* the records' tag fields for k_tag_finish (crc, title_db: NULL to skip) and the refusals of the handles named, ORed into
+ * status[0], [1], [3] (zeroed before) as k_handle_commit merges them */
+__global__ void k_tag_gather(HandleRecord* const* __restrict__ recs, int n, unsigned* __restrict__ crc, double* __restrict__ title_db,
+                             int* __restrict__ status) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const HandleRecord& r = *recs[i];
+  if (crc) crc[i] = r.music_crc;
+  if (title_db) title_db[i] = r.title_db;
+  if (r.refused) {
+    if (r.words[0]) atomicOr(&status[0], r.words[0]);
+    if (r.words[1]) atomicOr(&status[1], r.words[1]);
+    if (r.words[2]) atomicOr(&status[3], r.words[2]);
   }
 }
 

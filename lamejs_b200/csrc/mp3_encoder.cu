@@ -458,6 +458,7 @@ struct LaunchOpts {
                                             (no host round trip; needs !sync) */
   const struct HandleCarry* carry = nullptr;   /* streaming handles bound to a session: their carried state is on the device
                                                   (k_handle_carry_in; one launch group only) */
+  int* rg_loop = nullptr;                /* a session's three words of the ReplayGain loop (rg_finish_queued); NULL: ws.refusals + 5 */
 };
 
 /* LaunchOpts::carry: recs[z] is the record of stream z (device array); halo_scratch takes the masking of refused handles */
@@ -466,14 +467,19 @@ struct HandleCarry { HandleRecord* const* recs; float* halo_scratch; };
 /* The quantizer's fixed-point loop graphs of a session (QuantLoop), one per launch shape: (configuration, streams, frames,
  * longest stream's frames).  They hold the workspace's addresses, so they are all dropped when its generation changes.
  * The graphs of the ReplayGain repair loop (rg_finish_queued) are kept the same way: one per (configuration, Float32 rows,
- * titles, longest title's chunks, chunk rows) -- what RgParams and the launch grids are made of -- dropped when the
- * context's rg_generation changes. */
+ * titles, longest title's chunks, chunk rows, loop words) -- what RgParams and the launch grids are made of -- dropped when
+ * the context's rg_generation changes.  Streaming handles vary those shapes far more than whole streams do, so at most
+ * MP3_RG_GRAPHS of them are kept, the least recently used going first. */
+enum { MP3_RG_GRAPHS = 32 };
 struct LoopGraphs {
   cudaStream_t capture = nullptr;
   size_t generation = 0, rg_generation = 0;
+  long long instantiated = 0;            /* graphs instantiated over the session's life (mp3b200_session_graph_instantiations) */
+  unsigned long long rg_tick = 0;
   std::map<std::tuple<const Config*, int, long long, int>, cudaGraphExec_t> exec;
-  std::map<std::tuple<const Config*, bool, int, int, long long>, cudaGraphExec_t> rg_exec;
-  void clear_rg() { for (auto& e : rg_exec) cudaGraphExecDestroy(e.second); rg_exec.clear(); }
+  struct RgGraph { cudaGraphExec_t exec = nullptr; unsigned long long used = 0; };
+  std::map<std::tuple<const Config*, bool, int, int, long long, const int*>, RgGraph> rg_exec;
+  void clear_rg() { for (auto& e : rg_exec) cudaGraphExecDestroy(e.second.exec); rg_exec.clear(); }
   void clear() { for (auto& e : exec) cudaGraphExecDestroy(e.second); exec.clear(); }
 };
 
@@ -645,6 +651,7 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, uint8_
     rc = quant_run(tab, cfg->host, ws.streams.p, S, streams_with_frames, max_frames, total_frames, qb, d_out, st, c.aux_st, c.ev_fork, c.ev_join, ev[5], c.evq, c.evq_pred, &passes, &g_launches,
                    o.loops ? &dloop : nullptr);
     if (cached) {
+      if (!*cached && dloop.exec) o.loops->instantiated++;
       *cached = dloop.exec;
       if (!dloop.exec) o.loops->exec.erase(std::make_tuple((const Config*)cfg, S, total_frames, max_frames));
     }
@@ -932,8 +939,16 @@ int rg_finish_queued(ThreadCtx& c, Config* cfg, RgJob& job, LoopGraphs& lg, int*
   const int nch = cfg->host.nch, T = (int)job.specs.size();
   if (job.max_chunks > 0) {
     if (lg.rg_generation != c.rg_generation()) { lg.clear_rg(); lg.rg_generation = c.rg_generation(); }
-    const auto key = std::make_tuple((const Config*)cfg, p.f32 != 0, T, job.max_chunks, job.chunk_rows);
-    cudaGraphExec_t& exec = lg.rg_exec[key];
+    const auto key = std::make_tuple((const Config*)cfg, p.f32 != 0, T, job.max_chunks, job.chunk_rows, (const int*)loop);
+    if (!lg.rg_exec.count(key) && lg.rg_exec.size() >= MP3_RG_GRAPHS) {
+      auto lru = lg.rg_exec.begin();
+      for (auto e = lg.rg_exec.begin(); e != lg.rg_exec.end(); ++e) if (e->second.used < lru->second.used) lru = e;
+      cudaGraphExecDestroy(lru->second.exec);
+      lg.rg_exec.erase(lru);
+    }
+    LoopGraphs::RgGraph& slot = lg.rg_exec[key];
+    slot.used = ++lg.rg_tick;
+    cudaGraphExec_t& exec = slot.exec;
     if (!exec) {
       cudaGraph_t g = nullptr;
       cudaGraphConditionalHandle cond;
@@ -963,6 +978,7 @@ int rg_finish_queued(ThreadCtx& c, Config* cfg, RgJob& job, LoopGraphs& lg, int*
         g_err = "ReplayGain loop graph failed: " + std::string(cudaGetErrorString(cudaGetLastError()));
         return MP3B200_ERR_CUDA;
       }
+      lg.instantiated++;
     }
     const int first = RG_QUEUED_PASSES;              /* the pass index the graph starts at */
     int rc = upload(c, loop, &first, sizeof first, st);
@@ -1100,7 +1116,8 @@ int launch_streams(ThreadCtx& c, Config* cfg, std::vector<StreamDesc>& sds, uint
     rc = run_pipeline(c, cfg, group, n, d_out, o, arrival, rows, &tm);
     if (rc) return rc;
     if (o.rg) {                                /* a session: ws.refusals[3] is its fault word, [5 .. 8) the loop's words */
-      rc = o.loops ? rg_finish_queued(c, cfg, *o.rg, *o.loops, c.ws.refusals.p + 5, c.ws.refusals.p + 3) : rg_finish(c, cfg, *o.rg);
+      rc = o.loops ? rg_finish_queued(c, cfg, *o.rg, *o.loops, o.rg_loop ? o.rg_loop : c.ws.refusals.p + 5, c.ws.refusals.p + 3)
+                   : rg_finish(c, cfg, *o.rg);
       if (rc) return rc;
     }
     arrival = nullptr;

@@ -116,6 +116,14 @@ def lib():
     L.mp3b200_encode_bytes.argtypes = [vp, c_int]
     L.mp3b200_session_release.argtypes = [vp, vp, c_int]
     L.mp3b200_session_tail_capacity.argtypes = [c_int, c_int, c_int, c_int]
+    L.mp3b200_session_encode_batch_tagged.argtypes = [vp, vp, vp, vp, vp, c_int, vp, vp, vp, vp]
+    L.mp3b200_session_encode_batch_tagged_f32.argtypes = [vp, vp, vp, vp, vp, c_int, vp, vp, vp, vp]
+    L.mp3b200_session_flush_batch_tagged.argtypes = [vp, vp, c_int, vp, vp, vp, vp]
+    L.mp3b200_session_lametag_frames.argtypes = [vp, vp, c_int, vp, vp, vp, vp]
+    L.mp3b200_session_album_gain.argtypes = [vp, vp, c_int, vp, vp]
+    L.mp3b200_session_graph_instantiations.argtypes = [vp]
+    L.mp3b200_encode_bytes_schedule.argtypes = [c_int, c_int, c_int, c_int, c_int, vp, c_int, vp]
+    L.mp3b200_session_graph_instantiations.restype = c_i64
     L.mp3b200_session_tail_capacity.restype = c_i64
     _lib = L
     return L
@@ -169,6 +177,8 @@ _F32_TWIN = {
     "mp3b200_encode_streams_device_ex": "mp3b200_encode_streams_device_f32",
     "mp3b200_encode_streams_tagged_device": "mp3b200_encode_streams_tagged_device_f32",
     "mp3b200_encode_streams_tagged_async": "mp3b200_encode_streams_tagged_async_f32",
+    "mp3b200_session_encode_batch": "mp3b200_session_encode_batch_f32",
+    "mp3b200_session_encode_batch_tagged": "mp3b200_session_encode_batch_tagged_f32",
     "mp3b200_debug_resample": "mp3b200_debug_resample_f32",
     "mp3b200_debug_replaygain": "mp3b200_debug_replaygain_f32",
 }
@@ -729,7 +739,7 @@ class EncodeSession:
             raise ValueError("a session call names each encoder once (make two calls instead)")
         return (ctypes.c_void_p * max(len(encoders), 1))(*[e._h for e in encoders])
 
-    def _queue(self, encoders, lengths, call, *tensors):
+    def _queue(self, encoders, lengths, call, *tensors, status_words=4):
         """allocates `out` for the calls' exact lengths on the session's stream and runs call(hp, out, offsets, got, status)"""
         import torch
         S = len(encoders)
@@ -740,7 +750,7 @@ class EncodeSession:
             offsets[1:S] = np.cumsum(lengths[:-1])
         with torch.cuda.stream(self.stream):
             out = torch.empty(max(sum(lengths), 1), dtype=torch.uint8, device=self.device)
-            status = torch.empty(4, dtype=torch.int32, device=self.device)
+            status = torch.empty(status_words, dtype=torch.int32, device=self.device)
         got = np.zeros(max(S, 1), dtype=np.int32)
         _check(call(hp, out.data_ptr(), offsets.ctypes.data, got.ctypes.data, status.data_ptr()))
         for t in (out, status) + tensors:
@@ -755,6 +765,17 @@ class EncodeSession:
         calls raise Mp3B200Error.  Returns (out, offsets, lengths, status): a uint8 CUDA tensor filled on the stream, encoder
         i's bytes at out[offsets[i]:offsets[i] + lengths[i]] (host lists, known at once), and the int32[4] status tensor
         check_status reads.  Nothing here orders the rows: produce them on the session's stream, or make it wait."""
+        return self._encode(encoders, lefts, rights, False)
+
+    def encode_batch_tagged(self, encoders, lefts, rights=None):
+        """encode_batch for encoders in any mix of plain, write_vbr_tag and find_replay_gain (DESIGN.md 17), queued on the
+        session's stream: the same rows, the same (out, offsets, lengths, status), where a tagged encoder's first feeding
+        call hands out the all-zero placeholder frame first, and status is int32[8] ([4] and [5]: the analysis's passes and
+        reruns).  The music CRC and ReplayGain stay on the device until release(); lametag_frames and album_gain read them
+        there, ordered behind this call by the session's stream."""
+        return self._encode(encoders, lefts, rights, True)
+
+    def _encode(self, encoders, lefts, rights, tagged):
         import torch
         if self._h is None:
             raise ValueError("the session is closed")
@@ -777,16 +798,66 @@ class EncodeSession:
         ns = np.array([len(x) for x in lefts] or [0], dtype=np.int32)
         lp = (ctypes.c_void_p * max(S, 1))(*[x.data_ptr() for x in lefts])
         rp = (ctypes.c_void_p * max(S, 1))(*[x.data_ptr() for x in rights])
-        fn = lib().mp3b200_session_encode_batch_f32 if f32 else lib().mp3b200_session_encode_batch
+        fn = _entry("mp3b200_session_encode_batch_tagged" if tagged else "mp3b200_session_encode_batch", f32)
         return self._queue(encoders, [int(n) for n in ns[:S]],
                            lambda hp, o, off, got, st: fn(self._h, hp, lp, rp, ns.ctypes.data, S, o, off, got, st),
-                           *lefts, *rights)
+                           *lefts, *rights, status_words=8 if tagged else 4)
 
     def flush_batch(self, encoders):
         """flush() on live Mp3Encoder objects, queued on the session's stream; returns what encode_batch returns"""
         S = len(encoders)
         return self._queue(encoders, [-1] * S,
                            lambda hp, o, off, got, st: lib().mp3b200_session_flush_batch(self._h, hp, S, o, off, got, st))
+
+    def flush_batch_tagged(self, encoders):
+        """flush() on encoders in any mix of plain, tagged and ReplayGain, queued on the session's stream; returns what
+        encode_batch_tagged returns.  Each flush ends a ReplayGain title on the device, ordered by the session's stream."""
+        S = len(encoders)
+        return self._queue(encoders, [-1] * S,
+                           lambda hp, o, off, got, st: lib().mp3b200_session_flush_batch_tagged(self._h, hp, S, o, off, got, st),
+                           status_words=8)
+
+    def lametag_frames(self, encoders):
+        """The frame lametag_frame() would return for each encoder (one configuration) at this point of its stream, written
+        on the session's stream behind every call queued before: (out, offsets, lengths, status) as encode_batch returns
+        them, a length 0 where the tag is off or no frame has been encoded; status int32[4] (check_status raises where an
+        encoder was refused by an earlier call).  Binds the encoders that are not bound yet."""
+        import torch
+        S = len(encoders)
+        hp = self._handles(encoders)
+        room = [e._tag_room if e.tag_on else 0 for e in encoders]     # the call says which frames exist
+        offsets = np.zeros(max(S, 1), dtype=np.int64)
+        if S > 1:
+            offsets[1:S] = np.cumsum(room[:-1])
+        with torch.cuda.stream(self.stream):
+            out = torch.empty(max(sum(room), 1), dtype=torch.uint8, device=self.device)
+            status = torch.empty(4, dtype=torch.int32, device=self.device)
+        got = np.zeros(max(S, 1), dtype=np.int32)
+        _check(lib().mp3b200_session_lametag_frames(self._h, hp, S, out.data_ptr(), offsets.ctypes.data, got.ctypes.data,
+                                                    status.data_ptr()))
+        for t in (out, status):
+            t.record_stream(self.stream)
+        return out, [int(o) for o in offsets[:S]], [int(g) for g in got[:S]], status
+
+    def album_gain(self, encoders):
+        """album_gain(encoders) on the session's stream, behind every call queued before: a float64 CUDA tensor of one
+        element (-24601: nothing analysed) and an int32[4] status (check_status raises where an encoder was refused).
+        Binds the encoders that are not bound yet."""
+        import torch
+        hp = self._handles(encoders)
+        with torch.cuda.stream(self.stream):
+            album = torch.empty(1, dtype=torch.float64, device=self.device)
+            status = torch.empty(4, dtype=torch.int32, device=self.device)
+        _check(lib().mp3b200_session_album_gain(self._h, hp, len(encoders), album.data_ptr(), status.data_ptr()))
+        for t in (album, status):
+            t.record_stream(self.stream)
+        return album, status
+
+    def graph_instantiations(self):
+        """loop graphs the session has instantiated so far (constant once a steady workload's shapes are warm)"""
+        if self._h is None:
+            raise ValueError("the session is closed")
+        return int(lib().mp3b200_session_graph_instantiations(self._h))
 
     def release(self, encoders):
         """Waits for the session's work on `encoders` and gives them back to their host calls: each continues its stream
