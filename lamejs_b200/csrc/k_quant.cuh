@@ -256,7 +256,7 @@ __device__ Q_HELPER int region_pick(int mx, const RegionClass& rc, int a, int b,
 }
 
 /* Huffman table and bits of the pairs [begin, end) (even bounds) */
-__device__ __noinline__ int region_table_w(const short* ix, int begin, int end, int* bits) {
+__device__ __forceinline__ int region_table_w(const short* ix, int begin, int end, int* bits) {
   const int lane = LANE;
   const unsigned* w32 = reinterpret_cast<const unsigned*>(ix);
   const int p0 = (begin >> 1) + lane, p1 = end >> 1;
@@ -294,7 +294,7 @@ Q_UNROLL(Q_RT_UNROLL)
 /* noquant_count_bits (Takehiro.js:521-628).  gi scalars are updated by lane 0. */
 /* `top`: per lane, end (2p + 2) of its last non-zero pair below i0 = min(576, (max_nonzero_coeff + 2) & ~1), found by
  * the quantising loop of the caller while it had the pair in a register */
-__device__ __noinline__ int noquant_count_bits_w(const Mp3Tables* T, const short* ix, GranuleInfoDev* gi, GcWork* wk, bool use_prev, int top) {
+__device__ __forceinline__ int noquant_count_bits_w(const Mp3Tables* T, const short* ix, GranuleInfoDev* gi, GcWork* wk, bool use_prev, int top) {
   const int lane = LANE;
   const unsigned* w32 = reinterpret_cast<const unsigned*>(ix);
   /* count1 = end of the last non-zero pair below i0 */
@@ -349,7 +349,7 @@ __device__ __noinline__ int noquant_count_bits_w(const Mp3Tables* T, const short
     b1 = min(b1, bigv);
     b2 = min(b2, bigv);
     /* same order as the reference: region 2 (long blocks only), then 0, then 1; empty regions keep their table.
-     * One small routine called three times: the kernel is instruction-fetch bound, code reuse beats a fused sweep. */
+     * One small routine inlined at three call sites: calls and their stack frame cost more than the code size (DESIGN.md §6). */
     if (bt == BT_NORM && b2 < bigv) { QSTAT(15); ts2 = region_table_w(ix, b2, bigv, &bits); }
     if (0 < b1) { QSTAT(15); ts0 = region_table_w(ix, 0, b1, &bits); }
     if (b1 < b2) { QSTAT(15); ts1 = region_table_w(ix, b1, b2, &bits); }
@@ -383,7 +383,7 @@ __device__ __forceinline__ int sfb_step(const GranuleInfoDev* gi, const GcWork* 
 
 /* count_bits (Takehiro.js:630-660) = range check + quantize_xrpow (:171-314) + noquant_count_bits */
 template <bool use_prev>
-__device__ __noinline__ int count_bits_w(const Mp3Tables* T, GcWork* wk, GranuleInfoDev* gi, short* ix) {
+__device__ __forceinline__ int count_bits_w(const Mp3Tables* T, GcWork* wk, GranuleInfoDev* gi, short* ix) {
   const int lane = LANE;
   const double istep = (double)T->ipow20[gi->global_gain];
   if (gi->xrpow_max > T->ixmax_over_istep[gi->global_gain]) return Q_LARGE_BITS;
@@ -484,7 +484,7 @@ Q_UNROLL(Q_CB_UNROLL)
 
 /* calc_noise (QuantizePVT.js:725-878) for quant_comp 9: over_count, over_SSD, max_noise (+ distort[]) */
 struct NoiseRes { int over_count; double over_SSD, max_noise; int bits; };
-__device__ __noinline__ void calc_noise_w(const Mp3Tables* T, GcWork* wk, const GranuleInfoDev* gi, const short* ix, NoiseRes* res) {
+__device__ __forceinline__ void calc_noise_w(const Mp3Tables* T, GcWork* wk, const GranuleInfoDev* gi, const short* ix, NoiseRes* res) {
   const int lane = LANE;
   const int psymax = gi->psymax, mnz = gi->max_nonzero_coeff;
   /* Line cursor: a band starts where the previous one stopped.  Cached bands and bands that end at or below
@@ -570,7 +570,7 @@ Q_UNROLL(Q_CN_UNROLL)
 }
 
 /* scale_bitcount (Takehiro.js:980-1030), MPEG-1, all lanes; returns true when no legal scalefac_compress exists */
-__device__ __noinline__ bool scale_bitcount_w(GranuleInfoDev* gi) {
+__device__ __forceinline__ bool scale_bitcount_w(GranuleInfoDev* gi) {
   const int lane = LANE;
   int* scalefac = gi->scalefac;
   const bool is_short = gi->block_type == BT_SHORT;
@@ -608,7 +608,7 @@ __device__ __noinline__ bool scale_bitcount_w(GranuleInfoDev* gi) {
  * exceeds its range (the side info fields are then left as they were, like the reference).  preflag is never set on the LSF
  * path (scale_bitcount and the pre-emphasis step of best_scalefac_store are MPEG-1 only; inc_scalefac_scale clears it), so
  * only partition table 0 occurs: long {6,5,5,5}, short {9,9,9,9} bands, ranges {15,15,7,7}. */
-__device__ __noinline__ bool scale_bitcount_lsf_w(GranuleInfoDev* gi) {
+__device__ __forceinline__ bool scale_bitcount_lsf_w(GranuleInfoDev* gi) {
   const int lane = LANE;
   const bool is_short = gi->block_type == BT_SHORT;
   __syncwarp();
@@ -650,7 +650,7 @@ __device__ __forceinline__ bool loop_break_w(const GranuleInfoDev* gi, const GcW
 
 /* multiply xrpow of the bands flagged in wk->mode[] by `factor[band]` (amp_scalefac_bands / inc_scalefac_scale
  * line loops, Quantize.js:650-655,690-695) and fold the new values into xrpow_max */
-__device__ __noinline__ void scale_xrpow_w(GcWork* wk, GranuleInfoDev* gi, double f34) {
+__device__ __forceinline__ void scale_xrpow_w(GcWork* wk, GranuleInfoDev* gi, double f34) {
   const int lane = LANE;
   const int sfbmax = gi->sfbmax;
   float mx = 0.0f;
@@ -763,7 +763,7 @@ __device__ __noinline__ bool balance_escalate_w(const Mp3Tables* T, GcWork* wk) 
 
 
 /* balance_noise (Quantize.js:783-846) on cod_info_w.  Returns true when a new scalefactor combination exists. */
-__device__ __noinline__ bool balance_noise_w(const Mp3Tables* T, GcWork* wk) {
+__device__ __forceinline__ bool balance_noise_w(const Mp3Tables* T, GcWork* wk) {
   const int lane = LANE;
   GranuleInfoDev* gi = &wk->w;
   /* ---- amp_scalefac_bands, noise_shaping_amp == 1 (Quantize.js:597-660) ---- */
@@ -794,7 +794,7 @@ __device__ __noinline__ bool balance_noise_w(const Mp3Tables* T, GcWork* wk) {
   return balance_escalate_w(T, wk);
 }
 
-__device__ __noinline__ void copy_gi_w(GranuleInfoDev* dst, const GranuleInfoDev* src) {
+__device__ __forceinline__ void copy_gi_w(GranuleInfoDev* dst, const GranuleInfoDev* src) {
   const int n = sizeof(GranuleInfoDev) / 4;
   const int* s = reinterpret_cast<const int*>(src);
   int* d = reinterpret_cast<int*>(dst);
@@ -807,7 +807,7 @@ __device__ __noinline__ void copy_gi_w(GranuleInfoDev* dst, const GranuleInfoDev
   for (int k = 0; k < 3; k++) { const int i = LANE + 32 * k; if (i < n) d[i] = v[k]; }
   __syncwarp();
 }
-__device__ __noinline__ void copy_ix_w(short* dst, const short* src) {
+__device__ __forceinline__ void copy_ix_w(short* dst, const short* src) {
   const int* s = reinterpret_cast<const int*>(src);
   int* d = reinterpret_cast<int*>(dst);
   __syncwarp();
@@ -817,7 +817,7 @@ __device__ __noinline__ void copy_ix_w(short* dst, const short* src) {
 }
 
 /* bin_search_StepSize (Quantize.js:322-381) on cod_info (wk->b / ixb) */
-__device__ __noinline__ int bin_search_w(const Mp3Tables* T, GcWork* wk, int desired_rate, int* old_value, int* current_step, int stat_base = 0) {
+__device__ __forceinline__ int bin_search_w(const Mp3Tables* T, GcWork* wk, int desired_rate, int* old_value, int* current_step, int stat_base = 0) {
   GranuleInfoDev* gi = &wk->b;
   int nBits;
   int CurrentStep = *current_step;
@@ -865,7 +865,7 @@ __device__ __noinline__ int bin_search_w(const Mp3Tables* T, GcWork* wk, int des
 
 /* fingerprint of a GranuleInfoDev (every lane returns the same value): each lane mixes its words with their position,
  * the warp combines them with a sum and an xor (order-free, so no serial chain) */
-__device__ __noinline__ unsigned long long gi_hash(const GranuleInfoDev* gi) {
+__device__ __forceinline__ unsigned long long gi_hash(const GranuleInfoDev* gi) {
   const unsigned* w = reinterpret_cast<const unsigned*>(gi);
   unsigned sum = 0, x = 0;
 #pragma unroll 1
@@ -882,7 +882,7 @@ __device__ __noinline__ unsigned long long gi_hash(const GranuleInfoDev* gi) {
 /* outer_loop (Quantize.js:871-1052) for noise_shaping_amp 1, full_outer_loop 0, substep_shaping 0 */
 /* The bin search that opens outer_loop (Quantize.js:884) runs in its own kernel (k_q_search); this is everything after it.
  * gfc.OldValue / CurrentStep are final right after the search (outer_loop never touches them again). */
-__device__ __noinline__ void outer_loop_w(const Mp3Tables* T, GcWork* wk, int targ_bits) {
+__device__ __forceinline__ void outer_loop_w(const Mp3Tables* T, GcWork* wk, int targ_bits) {
   const int lane = LANE;
   NoiseRes best, cur;
   int best_part2_3_length = 9999999;
@@ -1700,15 +1700,16 @@ __device__ __forceinline__ int granule_budget(int nch, int mean_bits, int gr, in
  *     k_q_search  (gr1), k_q_outer (gr1)
  *     k_q_pack               format_bitstream                                                task = frame
  * A task is one warp; warps pull tasks from an atomic counter (persistent blocks), so uneven loop counts balance at warp
- * granularity and no warp ever waits for another.  Every kernel's code fits the SM's 32 KB instruction cache level (the
- * single fused kernel of round 1 had a 135 KB body and was instruction-fetch bound) and all resident warps run the same few
- * loops.  The hand-over (prepared xr / xrpow rows, the quantised lines, side info) goes through HBM/L2: ~20 KB per
+ * granularity and no warp ever waits for another.  Code run once per task stays out of the rate loop's kernel (the single
+ * fused kernel of round 1 had a 135 KB body and was instruction-fetch bound; code bytes per kernel: DESIGN.md §4) and all
+ * warps run the same few loops.  The hand-over (prepared xr / xrpow rows, the quantised lines, side info) goes through HBM/L2: ~20 KB per
  * granule-channel per pass against ~35 k warp instructions of work. */
 #ifndef Q_WARPS
 #define Q_WARPS 4
 #endif
 #ifndef Q_BLOCKS_PER_SM
-#define Q_BLOCKS_PER_SM 6     /* C2 step on an H100 SXM (400 W): 6 / 7 blocks -> 5.02 / 5.13 ms (k_q_outer: 80 / 72 registers, 8 / 48 bytes spilled) */
+#define Q_BLOCKS_PER_SM 7     /* k_q_outer with its rate loop inlined: 72 registers, no stack.  C2 on an H100 80GB HBM3 (700 W), k_q_outer
+                                 * 6 / 7 blocks -> 2.012 / 1.939 ms per step (the call-based loop: 80 registers and an 80-byte frame at 6) */
 #endif
 #define Q_THREADS (32 * Q_WARPS)
 
