@@ -140,6 +140,18 @@ def hf_tone(n, sr, seed=8):
     return l.astype(np.int16), r.astype(np.int16)
 
 
+def tone_comb(n, sr, level):
+    """40 tones spaced evenly in log frequency from 60 Hz to 0.45 fs, each at (f / 1 kHz) x level / 10 (rising 6 dB per
+    octave), the right channel 1 radian later: quantizes to values of at most 15 with table 14 best in region 2, the
+    region whose table 14 -> 16 remap the side-info writer has."""
+    t = np.arange(n, dtype=np.float64)
+    out = []
+    for ph in (0.0, 1.0):
+        x = sum((f / 1000.0) * np.sin(2 * np.pi * f * t / sr + f + ph) for f in np.geomspace(60.0, sr * 0.45, 40))
+        out.append(np.clip(np.rint(x * level / 10.0), -FULL - 1, FULL).astype(np.int16))
+    return out[0], out[1]
+
+
 def make(kind, n, sr, framesize, ratio=1):
     """`n` samples of `kind` at `sr`; `framesize` and `ratio` are in input samples (a resampled configuration's output frame
     and granule are `ratio` times longer at the input)."""
@@ -171,6 +183,8 @@ def make(kind, n, sr, framesize, ratio=1):
         return loud_silent(n, framesize)
     if kind == "hf_tone":
         return hf_tone(n, sr)
+    if kind.startswith("tone_comb"):
+        return tone_comb(n, sr, int(kind[9:]))
     raise ValueError(kind)
 
 
@@ -191,6 +205,7 @@ CASES = [
     ("l_minus_r", 2, 48000, 256, 30), ("l_minus_r", 2, 16000, 48, 60),
     ("loud_silent", 2, 44100, 128, 60), ("loud_silent", 1, 24000, 56, 80),
     ("hf_tone", 2, 44100, 320, 30), ("hf_tone", 1, 48000, 128, 30),
+    ("tone_comb5000", 2, 44100, 128, 12),
 ]
 
 

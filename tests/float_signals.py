@@ -43,6 +43,8 @@ LOUD_KINDS = ("burst", "noise", "nyquist", "impulse", "dcstep")
 LOUD_MAGNITUDES = (16, 256, 4096, 65536, 2 ** 18, 2 ** 20, 2 ** 22, 2 ** 24, 3.3e7, 1e9, 1e15, 1e20, 1e30, "max")
 # across the magnitude at which lamejs's frames stop fitting their slots (between 2e5 and 1e6 x full scale)
 LOUD_FINE = (3e5, 4e5, 5e5, 6e5, 7e5, 8e5)
+# the library's input limit (MP3_F32_MAX_SAMPLE, k_resample.cuh): it refuses samples beyond it once scaled
+LOUD_GATE = 2.0 ** 40
 
 
 def _unit(kind, n, sr, seed):

@@ -46,6 +46,12 @@ def lib():
         tmp = os.path.join(d, "liboracle_f32.%d.so" % os.getpid())
         subprocess.check_call(["g++"] + CXXFLAGS + ["-shared", "-o", tmp] + srcs + ["-lm"])
         os.replace(tmp, so)
+    _lib = bind(so)
+    return _lib
+
+
+def bind(so):
+    """the ctypes library of a build of oracle_f32.cpp with the oracle's sources (lib()'s, or another build of them)"""
     L = ctypes.CDLL(so)
     vp, ci = ctypes.c_void_p, ctypes.c_int
     L.lj_create.restype = vp
@@ -63,7 +69,6 @@ def lib():
     L.lj_gain_clamps.argtypes = [vp]
     L.lj_get_scale.restype = ctypes.c_double
     assert L.lj_trace_size() == oracle_lib.TRACE_DTYPE.itemsize
-    _lib = L
     return L
 
 

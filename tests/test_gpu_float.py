@@ -9,6 +9,7 @@ import pytest
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import edge_signals  # noqa: E402
 import oracle_f32  # noqa: E402
+import oracle_inputs  # noqa: E402
 import resample_tap  # noqa: E402
 import stage_taps  # noqa: E402
 from synth import make_signal  # noqa: E402
@@ -25,38 +26,9 @@ def M():
     return lamejs_b200
 
 
-# MPEG-1, MPEG-2, MPEG-2.5 and resampled (48 -> 24, 44.1 -> 22.05, 48 -> 8 kHz) configurations
-CFGS = [(2, 44100, 128), (1, 48000, 160), (2, 32000, 96), (2, 22050, 64), (1, 24000, 48), (2, 16000, 40), (1, 11025, 24),
-        (2, 12000, 32), (1, 8000, 16), (2, 48000, 64), (2, 44100, 48), (1, 48000, 8)]
-
-
-def float_signal(kind, n, sr, seed):
-    """the float inputs lamejs callers pass: Web Audio x * 32767 with fractions, unscaled [-1, 1], 1.5 and 4 x full scale,
-    +-0.5 dither, Float32 denormals and -0.0"""
-    l, r = make_signal("noise" if kind in ("dither", "denormal") else "burst", n, sr, seed=seed)
-    u = np.stack([l, r]).astype(np.float64) / 32768.0
-    rng = np.random.default_rng(seed)
-    if kind == "webaudio":
-        x = u * 32767.0
-    elif kind == "unit":
-        x = u
-    elif kind == "x1.5":
-        x = u * 32768.0 * 1.5
-    elif kind == "x4":
-        x = u * 32768.0 * 4.0
-    elif kind == "dither":
-        x = rng.uniform(-0.5, 0.5, size=u.shape)
-    elif kind == "denormal":
-        x = rng.integers(-3, 4, size=u.shape) * np.float64(np.float32(1e-45))
-        x[:, ::7] = -0.0
-        x[:, 5::11] = np.float32(1.1754942e-38)
-    else:
-        raise ValueError(kind)
-    x = x.astype(np.float32)
-    return x[0].copy(), x[1].copy()
-
-
-KINDS = ["webaudio", "unit", "x1.5", "x4", "dither", "denormal"]
+CFGS = oracle_inputs.FLOAT_CFGS
+KINDS = oracle_inputs.FLOAT_KINDS
+float_signal = oracle_inputs.float_signal
 
 
 def accepted(M, cfg):
@@ -120,7 +92,8 @@ def test_entry_points_match_the_oracle(M, cfg):
     rs = resampled(M, cfg)
     fs = 576 * M.granules_per_frame(ch, sr, kb, resample=rs) * (sr // M.out_samplerate(ch, sr, kb))
     n = 6 * fs + 123
-    sigs = [float_signal(k, n, sr, 30 + i) for i, k in enumerate(KINDS)]
+    sigs = oracle_inputs.float_entry_signals(cfg)
+    assert len(sigs[0][0]) == n
     wants = [oracle_f32.encode_stream(ch, sr, kb, l, r if ch == 2 else None)[0] for l, r in sigs]
     got = M.encode_streams(ch, sr, kb, [l for l, _ in sigs], [r for _, r in sigs] if ch == 2 else None, resample=rs)
     for k, g, w in zip(KINDS, got, wants):
@@ -177,7 +150,8 @@ def test_stage_taps_match_the_oracle(M, cfg):
     rs = resampled(M, cfg)
     G = M.granules_per_frame(ch, sr, kb, resample=rs)
     n = (sr // M.out_samplerate(ch, sr, kb)) * (12 * 576 * G + 211) + 5
-    for kind in ("webaudio", "unit"):
+    assert n == oracle_inputs.float_tap_samples(cfg)
+    for kind in oracle_inputs.FLOAT_TAP_KINDS:
         l, r = float_signal(kind, n, sr, 7)
         rr = r if ch == 2 else None
         F = M.stream_frames(n, ch, sr, kb, resample=rs)
@@ -230,7 +204,7 @@ def test_replaygain_of_float_input(M):
         assert tag + stream[len(tag):] == whole[0]
 
 
-@pytest.mark.parametrize("case", edge_signals.CASES[::2] + edge_signals.RESAMPLED_CASES[::3], ids=edge_signals.case_id)
+@pytest.mark.parametrize("case", oracle_inputs.EDGE_AS_FLOAT_CASES, ids=edge_signals.case_id)
 def test_edge_corpus_as_floats(M, case):
     """edge corpus cases as integer-valued floats give the Int16 bytes; the same signals / 32768 (Web Audio's range) equal
     the oracle's Float32 store"""
@@ -240,8 +214,7 @@ def test_edge_corpus_as_floats(M, case):
     want = M.encode_streams(ch, sr, kb, [l], None if rr is None else [rr], resample=rs)
     got = M.encode_streams(ch, sr, kb, [l.astype(np.float32)], None if rr is None else [rr.astype(np.float32)], resample=rs)
     assert got == want, case
-    lf = (l.astype(np.float64) / 32768.0).astype(np.float32)
-    rf = None if rr is None else (rr.astype(np.float64) / 32768.0).astype(np.float32)
+    lf, rf = oracle_inputs.edge_as_float(case)
     got = M.encode_streams(ch, sr, kb, [lf], None if rf is None else [rf], resample=rs)[0]
     assert got == oracle_f32.encode_stream(ch, sr, kb, lf, rf)[0], case
 

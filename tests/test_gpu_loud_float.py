@@ -5,7 +5,6 @@ library refuses the same call with MP3B200_ERR_CONFIG, k_q_pack has not packed t
 every handle of the call as it was.  Samples beyond 2^40 once scaled (beyond 2^25 x full scale) are refused by the input
 gate.  The loudest encodable rung of each configuration is compared with the oracle stage by stage."""
 import hashlib
-import json
 import os
 import sys
 
@@ -15,12 +14,12 @@ import pytest
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import float_signals as FS  # noqa: E402
 import oracle_f32  # noqa: E402
+import oracle_inputs  # noqa: E402
 import stage_taps  # noqa: E402
 
 pytestmark = pytest.mark.gpu
-HERE = os.path.dirname(os.path.abspath(__file__))
-GOLDEN = json.load(open(os.path.join(HERE, "golden", "lamejs_loud_golden.json")))
-GATE = 2.0 ** 40                       # MP3_F32_MAX_SAMPLE (k_resample.cuh)
+GOLDEN = oracle_inputs.loud_golden()
+GATE = FS.LOUD_GATE
 FRACTIONAL = (44100, 22050, 11025)     # see tests/test_float_golden_cpu.py
 
 

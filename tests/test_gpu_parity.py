@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import mp3_parse
+import oracle_inputs
 import stage_taps
 from stage_taps import bits_equal
 from synth import make_signal, white, octave_hold, bursts
@@ -21,13 +22,9 @@ def M():
     return lamejs_b200
 
 
-@pytest.mark.parametrize("kind,ch,sr,kbps,frames", [
-    ("noise", 2, 44100, 128, 60), ("burst", 2, 44100, 128, 80), ("white", 2, 48000, 320, 50), ("sine", 1, 44100, 128, 40),
-    ("octave", 1, 44100, 128, 60), ("sweep", 2, 44100, 128, 120), ("noise", 2, 32000, 160, 40), ("white", 1, 48000, 320, 30),
-    ("silence", 2, 44100, 128, 12), ("burst", 1, 44100, 192, 60)])
+@pytest.mark.parametrize("kind,ch,sr,kbps,frames", oracle_inputs.STAGE_PARITY_CASES)
 def test_stage_parity(M, oracle, kind, ch, sr, kbps, frames):
-    l, r = make_signal(kind, frames * 1152 + 211, sr, 21)
-    r = r if ch == 2 else None
+    l, r = oracle_inputs.stage_parity_signal((kind, ch, sr, kbps, frames))
     F = M.stream_frames(len(l))
     ref, _, tr = oracle.encode_stream(ch, sr, kbps, l, r, trace_frames=F + 2)
     g = M.debug_stages(ch, sr, kbps, l, r, want=stage_taps.ALL_TAPS)
@@ -158,15 +155,14 @@ def test_batched_live_encoders_one_launch_per_call(M, oracle):
         e.close(); r.close()
 
 
-@pytest.mark.parametrize("sr", [8000, 11025, 12000, 16000, 22050, 24000, 32000, 44100, 48000])
+@pytest.mark.parametrize("sr", oracle_inputs.CONFIG_MATRIX_RATES)
 def test_config_matrix(M, oracle, sr):
     """Every bitrate of the rate's MPEG version (and an off-ladder one that lamejs snaps, worker-realtime.js passes 123) x
     mono/stereo at each sample rate: short noisy + transient streams, byte-exact against the oracle.  The C ABI must reject
     exactly the configurations in which lamejs resamples (oracle.out_samplerate != sr)."""
-    l, r = make_signal("burst", 9 * 1152 + 100, sr, 77)
-    l2, r2 = make_signal("noise", 7 * 1152, sr, 78)
+    (l, r), (l2, r2) = oracle_inputs.config_matrix_signals(sr)
     tried = 0
-    for kbps in (8, 16, 24, 32, 40, 48, 56, 64, 80, 96, 112, 123, 128, 144, 160, 192, 224, 256, 320):
+    for kbps in oracle_inputs.CONFIG_MATRIX_KBPS:
         for ch in (1, 2):
             native = oracle.out_samplerate(ch, sr, kbps) == sr
             try:
@@ -246,15 +242,11 @@ def test_empty_batch_and_error_paths_keep_the_stream_intact(oracle):
     assert bytes(got) == ref
 
 
-@pytest.mark.parametrize("kind,ch,sr,kbps,frames", [
-    ("noise", 2, 22050, 64, 80), ("burst", 2, 24000, 96, 100), ("octave", 1, 16000, 32, 80), ("white", 2, 16000, 160, 60),
-    ("burst", 1, 22050, 32, 90), ("noise", 1, 8000, 8, 60), ("burst", 2, 12000, 32, 70), ("sine", 2, 11025, 40, 50), ("sine", 1, 11025, 24, 50),
-    ("silence", 2, 24000, 64, 14)])
+@pytest.mark.parametrize("kind,ch,sr,kbps,frames", oracle_inputs.LSF_STAGE_PARITY_CASES)
 def test_stage_parity_lsf(M, oracle, kind, ch, sr, kbps, frames):
     """MPEG-2 / MPEG-2.5 (one granule per frame, 576-sample frames, scale_bitcount_lsf, 9/17-byte side info): every stage
     tap bit-equal to the oracle, which is byte-identical to real lamejs on these configurations (test_lamejs_pin)."""
-    l, r = make_signal(kind, frames * 576 + 211, sr, 23)
-    r = r if ch == 2 else None
+    l, r = oracle_inputs.lsf_stage_parity_signal((kind, ch, sr, kbps, frames))
     assert M.granules_per_frame(ch, sr, kbps) == 1
     F = M.stream_frames(len(l), ch, sr, kbps)
     ref, _, tr = oracle.encode_stream(ch, sr, kbps, l, r, trace_frames=F + 2)
