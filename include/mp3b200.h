@@ -249,7 +249,8 @@ int mp3b200_encode_streams_tagged_ex(int channels, int samplerate, int kbps, int
  * batches run as consecutive launches, as mp3b200_encode_streams_device does.  The call runs on a stream of its own that
  * first waits for work already queued on the legacy default stream (where torch / plain CUDA callers produced d_pcm and
  * d_out) and returns after that stream has drained.  The packer writes each stream's audio straight behind the room of its
- * tag frame; the frames are built on the host, uploaded in one copy and put in place by one kernel (k_tag_scatter).
+ * tag frame; the frames are finished on the device (music CRC, Radio Replay Gain field, the tag's own CRC) by one kernel
+ * (k_tag_finish), as the session's tagged calls finish them.
  * _device_f32 takes Float32 samples, laid out the same way, as mp3b200_encode_streams_device_f32 does; a sample that is not
  * finite, or beyond 2^40 once scaled, returns MP3B200_ERR_CONFIG, and no tag frame is placed (the audio bytes in d_out are
  * then unspecified). */

@@ -1,5 +1,6 @@
-/* k_tag.cuh -- the music CRC of the Xing / LAME tag on the GPU (SURVEY.md 8(f3)), the placement of the tag frames of
- * device-resident streams (k_tag_scatter), and the frames an encode session finishes on the device (k_tag_finish).
+/* k_tag.cuh -- the music CRC of the Xing / LAME tag on the GPU (SURVEY.md 8(f3)), the placement of a session's tag
+ * placeholder frames (k_tag_scatter), and the tag frames of whole streams and session handles finished on the device
+ * (k_tag_finish).
  *
  * lamejs keeps gfc.nMusicCRC by pushing every byte copy_buffer hands out through a table-driven CRC-16 (polynomial
  * x^16 + x^15 + x^2 + 1, reflected, start 0; reference src/js/VBRTag.js:547-556, BitStream.js:924-928): one dependent table
@@ -167,9 +168,9 @@ k_music_crc(const uint8_t* __restrict__ buf, const long long* __restrict__ off, 
   if (lane == 0) atomicXor(&crc_out[r], crc_shift(c, (unsigned long long)p.after_piece, s_t.pow));
 }
 
-/* The tag frames of a batch of device-resident streams, built on the host (mp3_tag_frame) and uploaded in one copy, put in
- * front of their streams: grid (frames), frame i is frame_bytes bytes at frames + i * frame_bytes and goes to out + dst[i].
- * One block per frame, so a batch of any size is one launch. */
+/* Frames built on the host and uploaded in one copy (a session's tag placeholders), put in front of their streams: grid
+ * (frames), frame i is frame_bytes bytes at frames + i * frame_bytes and goes to out + dst[i].  One block per frame, so a
+ * batch of any size is one launch. */
 enum { TAG_SCATTER_THREADS = 128 };
 __global__ void __launch_bounds__(TAG_SCATTER_THREADS)
 k_tag_scatter(const long long* __restrict__ dst, const uint8_t* __restrict__ frames, int frame_bytes, uint8_t* __restrict__ out) {
@@ -178,7 +179,7 @@ k_tag_scatter(const long long* __restrict__ dst, const uint8_t* __restrict__ fra
   for (int i = threadIdx.x; i < frame_bytes; i += TAG_SCATTER_THREADS) d[i] = src[i];
 }
 
-/* The tag frames an encode session finishes without the host: grid (frames), one block per frame.  templates + i *
+/* The tag frames finished without the host: grid (frames), one block per frame.  templates + i *
  * p.frame_bytes is mp3_tag_frame with music CRC 0 and gain field 0, built on the host before anything ran; it goes to
  * dst[i].at, completed by mp3_tag_patch with the music CRC k_music_crc left in crc[dst[i].stream] and, when the call analysed
  * (gain != NULL), the field of gain[dst[i].stream].  The patched head is staged in shared memory, so the frame's own CRC reads

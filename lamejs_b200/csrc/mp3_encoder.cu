@@ -291,7 +291,7 @@ struct ThreadCtx {
   Buf<uint8_t, true> pin;                 /* pinned host staging */
   Buf<long long> crc_ranges;              /* music CRC: [2][R] offsets / lengths */
   Buf<unsigned> crc;                      /* music CRC: [R] results */
-  Buf<uint8_t> tags;                      /* tagged device streams: the uploaded tag frames and their offsets (k_tag_scatter) */
+  Buf<uint8_t> tags;                      /* tagged whole streams: the template frames and their destinations (k_tag_finish) */
   cudaStream_t rg_st = nullptr;           /* ReplayGain analysis, beside the encoder */
   cudaEvent_t ev_rg[3] = {};              /* fork, start, end */
   Buf<RgTitle> rg_titles;
@@ -1242,26 +1242,27 @@ int check_input(const Config* cfg, int nstreams, const float* const* left, const
   return MP3B200_OK;
 }
 
-/* Whole streams from host buffers: checks that out[s] has room for the stream's audio[s] bytes plus `extra`
- * (out_bytes[s] = their sum), stages the PCM (Int16 or Float32) in the thread's buffers and encodes the batch into t_ctx.out,
- * stream s at out_off[s].  Stereo input with right == NULL or right[s] == NULL encodes left[s] on both channels. */
+/* Whole streams from host buffers, laid out as files in t_ctx.out: file s at out_off[s] is room[s] bytes (room NULL: none)
+ * and then the stream's audio.  Checks that out[s] has room for the file (out_bytes[s] = its length), stages the PCM (Int16
+ * or Float32) in the thread's buffers and fills the descriptors `sds` (out_base: the file's offset, where the audio goes when
+ * there is no room) and the upload's arrival `arr`.  Stereo input with right == NULL or right[s] == NULL encodes left[s] on
+ * both channels. */
 template <class T>
-int encode_host_streams(Config* cfg, int nstreams, const T* const* left, const T* const* right,
-                        const int64_t* nsamples, const int64_t* cap, int extra, int64_t* out_bytes,
-                        std::vector<int64_t>& out_off, std::vector<long long>& audio, RgJob* rg = nullptr) {
+int stage_host_streams(Config* cfg, int nstreams, const T* const* left, const T* const* right, const int64_t* nsamples,
+                       const int64_t* cap, const int* room, int64_t* out_bytes, std::vector<int64_t>& out_off,
+                       std::vector<StreamDesc>& sds, PcmArrival& arr) {
   const int nch = cfg->host.nch;
   std::vector<int64_t> pcm_off(nstreams);
   out_off.assign(nstreams, 0);
-  audio.assign(nstreams, 0);
   long long tot_samples = 0, tot_bytes = 0;
   for (int s = 0; s < nstreams; s++) {
     pcm_off[s] = tot_samples;
     tot_samples += nsamples[s] * nch;
     out_off[s] = tot_bytes;
-    audio[s] = bytes_of_frames(cfg->host, 0, frames_for(nsamples[s], cfg->host.mode_gr, cfg->rs.ratio));
-    if (cap[s] < audio[s] + extra) { g_err = "output buffer too small"; return MP3B200_ERR_BUFFER; }
-    out_bytes[s] = audio[s] + extra;
-    tot_bytes += audio[s];
+    const long long n = bytes_of_frames(cfg->host, 0, frames_for(nsamples[s], cfg->host.mode_gr, cfg->rs.ratio)) + (room ? room[s] : 0);
+    if (cap[s] < n) { g_err = "output buffer too small"; return MP3B200_ERR_BUFFER; }
+    out_bytes[s] = n;
+    tot_bytes += n;
   }
   if (nstreams == 0) return MP3B200_OK;
   T* d_pcm = staging_pcm<T>((size_t)tot_samples + 8);
@@ -1270,7 +1271,6 @@ int encode_host_streams(Config* cfg, int nstreams, const T* const* left, const T
   if (rc) return rc;
   /* Upload in time slices on a copy stream; the psy analysis of a slice starts when it has landed, so only the first
    * slice's transfer is exposed.  Many small streams are uploaded whole (one slice): per-copy overhead would win. */
-  PcmArrival arr;
   arr.chunks = (nstreams <= 8 && tot_samples >= (1 << 20)) ? MP3_MAX_PCM_CHUNKS : 1;
   arr.ready = t_ctx.ready;
   for (int j = 0; j < arr.chunks; j++) {
@@ -1284,12 +1284,8 @@ int encode_host_streams(Config* cfg, int nstreams, const T* const* left, const T
     }
     CK(cudaEventRecord(t_ctx.ready[j], t_ctx.up_st));
   }
-  std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off.data(), nsamples, out_off.data());
-  LaunchOpts o;
-  o.arrival = &arr;
-  o.rg = rg;
-  o.f32_in = std::is_same_v<T, float>;
-  return launch_streams(t_ctx, cfg, sds, t_ctx.out.p, o);
+  sds = whole_streams(cfg, nstreams, d_pcm, pcm_off.data(), nsamples, out_off.data());
+  return MP3B200_OK;
 }
 
 }  // namespace
@@ -1327,11 +1323,16 @@ int encode_host(int channels, int samplerate, int kbps, int flags, int nstreams,
   int rc = get_config(channels, samplerate, kbps, flags, &cfg);
   if (rc || (rc = check_input(cfg, nstreams, left, right, nsamples))) return rc;
   std::vector<int64_t> out_off;
-  std::vector<long long> audio;
-  rc = encode_host_streams(cfg, nstreams, left, right, nsamples, cap, 0, out_bytes, out_off, audio);
+  std::vector<StreamDesc> sds;
+  PcmArrival arr;
+  rc = stage_host_streams(cfg, nstreams, left, right, nsamples, cap, nullptr, out_bytes, out_off, sds, arr);
   if (rc || nstreams == 0) return rc;
+  LaunchOpts o;
+  o.arrival = &arr;
+  o.f32_in = std::is_same_v<T, float>;
+  if ((rc = launch_streams(t_ctx, cfg, sds, t_ctx.out.p, o))) return rc;
   for (int s = 0; s < nstreams; s++)
-    if (cudaMemcpyAsync(out[s], t_ctx.out.p + out_off[s], (size_t)audio[s], cudaMemcpyDeviceToHost, t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
+    if (cudaMemcpyAsync(out[s], t_ctx.out.p + out_off[s], (size_t)out_bytes[s], cudaMemcpyDeviceToHost, t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
   if (cudaStreamSynchronize(t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
   return rc;
 }
@@ -1592,36 +1593,27 @@ int crc_tables_on(int device) {
   return 0;
 }
 
-/* CRC-16 (start 0) of the byte ranges [off[i], off[i] + len[i]) of d_buf, one k_music_crc launch per 65535 ranges, on the
- * calling thread's stream behind whatever wrote the bytes.  crc[i] is valid when the call returns. */
-int music_crc_ranges(int device, const uint8_t* d_buf, const std::vector<long long>& off, const std::vector<long long>& len, std::vector<unsigned>& crc) {
-  const int R = (int)off.size();
-  crc.assign((size_t)R, 0u);
+/* Queues on c.st, behind whatever wrote the bytes, the music CRC (CRC-16, start 0) of the byte ranges [at[r], at[r] + len[r])
+ * (absolute device addresses, like the packer's output offsets) into c.crc[r]: one k_music_crc launch per 65535 ranges.
+ * The ranges go up through upload(); the CRC tables must already be on the device (crc_tables_on). */
+int queue_music_crc(ThreadCtx& c, const std::vector<long long>& at, const std::vector<long long>& len) {
+  const int R = (int)at.size();
   if (R == 0) return 0;
-  int rc = crc_tables_on(device);
-  if (rc) return rc;
-  ThreadCtx& sc = t_ctx;
-  rc = sc.crc_ranges.fit((size_t)2 * R);
-  if (rc) return rc;
-  rc = sc.crc.fit((size_t)R);
-  if (rc) return rc;
   std::vector<long long> ranges((size_t)2 * R);
   long long longest = 0;
-  for (int i = 0; i < R; i++) { ranges[i] = off[i]; ranges[(size_t)R + i] = len[i]; longest = len[i] > longest ? len[i] : longest; }
-  CK(cudaMemcpyAsync(sc.crc_ranges.p, ranges.data(), sizeof(long long) * ranges.size(), cudaMemcpyHostToDevice, sc.st));
-  CK(cudaMemsetAsync(sc.crc.p, 0, sizeof(unsigned) * (size_t)R, sc.st));
-  if (longest > 0) {
-    const long long pieces = (longest + CRC_PIECE_BYTES - 1) / CRC_PIECE_BYTES;
-    for (int r0 = 0; r0 < R; r0 += 65535) {
-      const int nr = R - r0 < 65535 ? R - r0 : 65535;
-      dim3 grid((unsigned)((pieces + CRC_WARPS - 1) / CRC_WARPS), (unsigned)nr);
-      k_music_crc<<<grid, CRC_WARPS * 32, 0, sc.st>>>(d_buf, sc.crc_ranges.p + r0, sc.crc_ranges.p + R + r0, g_crc_dev[device], sc.crc.p + r0);
-      g_launches++;
-    }
+  for (int i = 0; i < R; i++) { ranges[i] = at[i]; ranges[(size_t)R + i] = len[i]; longest = len[i] > longest ? len[i] : longest; }
+  int rc = 0;
+  if ((rc = c.crc_ranges.fit((size_t)2 * R)) || (rc = c.crc.fit((size_t)R)) ||
+      (rc = upload(c, c.crc_ranges.p, ranges.data(), sizeof(long long) * ranges.size())))
+    return rc;
+  CK(cudaMemsetAsync(c.crc.p, 0, sizeof(unsigned) * (size_t)R, c.st));
+  const long long pieces = (longest + CRC_PIECE_BYTES - 1) / CRC_PIECE_BYTES;
+  for (int r0 = 0; r0 < R && longest > 0; r0 += 65535) {
+    const int nr = R - r0 < 65535 ? R - r0 : 65535;
+    dim3 grid((unsigned)((pieces + CRC_WARPS - 1) / CRC_WARPS), (unsigned)nr);
+    k_music_crc<<<grid, CRC_WARPS * 32, 0, c.st>>>(nullptr, c.crc_ranges.p + r0, c.crc_ranges.p + R + r0, g_crc_dev[c.device], c.crc.p + r0);
+    g_launches++;
   }
-  CK(cudaMemcpyAsync(crc.data(), sc.crc.p, sizeof(unsigned) * (size_t)R, cudaMemcpyDeviceToHost, sc.st));
-  CK(cudaStreamSynchronize(sc.st));
-  CK(cudaGetLastError());
   return 0;
 }
 
@@ -1659,22 +1651,18 @@ int mp3b200_debug_music_crc(const uint8_t* d_buf, const int64_t* off, const int6
   int dev = 0;
   { std::lock_guard<std::mutex> lk(g_mu); dev = g_device; int rc = ensure_device(dev); if (rc) return rc; }
   int rc = t_ctx.use(dev);
-  if (rc) return rc;
-  std::vector<long long> o(off, off + nranges), l(len, len + nranges);
-  std::vector<unsigned> c;
-  CK(cudaEventRecord(t_ctx.ev_in, cudaStreamLegacy));
-  CK(cudaStreamWaitEvent(t_ctx.st, t_ctx.ev_in, 0));
-  rc = music_crc_ranges(dev, d_buf, o, l, c);              /* first call: uploads the tables */
-  if (rc) return rc;
-  if (ms) {
-    CK(cudaEventRecord(t_ctx.ev[0], t_ctx.st));
-    rc = music_crc_ranges(dev, d_buf, o, l, c);
-    if (rc) return rc;
-    CK(cudaEventRecord(t_ctx.ev[1], t_ctx.st));
-    CK(cudaEventSynchronize(t_ctx.ev[1]));
-    CK(cudaEventElapsedTime(ms, t_ctx.ev[0], t_ctx.ev[1]));
+  if (rc || (rc = crc_tables_on(dev)) || (rc = wait_legacy(t_ctx))) return rc;
+  std::vector<long long> at(off, off + nranges), l(len, len + nranges);
+  for (long long& a : at) a += (long long)(uintptr_t)d_buf;
+  for (int run = 0; run < (ms ? 2 : 1); run++) {          /* with ms, a second run is timed */
+    if (run) CK(cudaEventRecord(t_ctx.ev[0], t_ctx.st));
+    if ((rc = queue_music_crc(t_ctx, at, l))) return rc;
+    if (nranges > 0) CK(cudaMemcpyAsync(crc, t_ctx.crc.p, sizeof(uint32_t) * (size_t)nranges, cudaMemcpyDeviceToHost, t_ctx.st));
+    if (run) CK(cudaEventRecord(t_ctx.ev[1], t_ctx.st));
+    CK(cudaStreamSynchronize(t_ctx.st));
+    CK(cudaGetLastError());
   }
-  for (int i = 0; i < nranges; i++) crc[i] = c[i];
+  if (ms) CK(cudaEventElapsedTime(ms, t_ctx.ev[0], t_ctx.ev[1]));
   return 0;
 }
 
@@ -1718,15 +1706,6 @@ int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int ns
 }  // extern "C"
 
 namespace {
-/* The tagged whole streams (encodeBuffer(everything) + flush() on fresh encoders with the tag on) of both kinds of buffers.
- * `io` says where the PCM comes from and where the files go (HostTagged, DeviceTagged):
- *   io.check_input(cfg)                      the input gate of the host entry points (device rows: k_stage_f32)
- *   io.launch(cfg, tfs, tag, rg, audio, at)  encodes the batch, with the analysis `rg` when set; stream s's audio[s] bytes
- *                                            then lie at io.buf() + at[s].  tag[s] is the size of stream s's tag frame
- *                                            (tfs, or 0: no frame)
- *   io.frame(s)                              host memory for stream s's tag frame, once the launch has succeeded
- *   io.finish(tag, audio, at)                puts the frames and the audio where they belong, and drains t_ctx.st
- * out_bytes[s] receives the file's length; `rg` (flags & MP3B200_REPLAYGAIN) receives the analysis. */
 /* What is known about tagged whole streams before anything runs, in closed form from the lamejs FIFO: each stream's frames,
  * its end padding and the size of its tag frame (tfs, or 0: no frame), and, with `rg`, the pieces the analysis sees
  * (rg->specs).  `rg` is reset to NULL where lamejs does not analyse: it does so only when the tag is written
@@ -1754,152 +1733,121 @@ TaggedPlan tagged_plan(const Config* cfg, int nstreams, const int64_t* nsamples,
   return pl;
 }
 
-template <class Io>
-int encode_tagged(int channels, int samplerate, int kbps, int flags, int nstreams, const int64_t* nsamples, int64_t* out_bytes,
-                  RgJob* rg, Io& io) {
-  if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
-  if (flags & ~(MP3B200_RESAMPLE | MP3B200_REPLAYGAIN)) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
-  Config* cfg;
-  int rc = get_config(channels, samplerate, kbps, flags & MP3B200_RESAMPLE, &cfg);
-  if (rc || (rc = io.check_input(cfg))) return rc;
+/* Queues, behind the packer on c.st, what turns the audio of tagged whole streams into files: the music CRC of each stream
+ * where its audio lies (sds[i].out_base, an absolute address), and k_tag_finish, which completes each template frame with
+ * it and with the field of gain[i] (device; NULL: nothing was analysed, the field is 0) and writes it to d_out + out_off[i].
+ * The templates are mp3_tag_frame with music CRC 0 and gain field 0.  Every upload goes through upload(). */
+int finish_tagged(ThreadCtx& c, Config* cfg, const TaggedPlan& plan, const std::vector<StreamDesc>& sds, const std::vector<long long>& audio,
+                  uint8_t* d_out, const int64_t* out_off, const double* gain) {
+  const int S = (int)sds.size();
   const Mp3TagParams& p = cfg->tag;
-  const TaggedPlan plan = tagged_plan(cfg, nstreams, nsamples, rg);
-  const int tfs = plan.tfs;
-  const std::vector<long long>& frames = plan.frames;
-  const std::vector<int>&padding = plan.padding, &tag = plan.tag;
-  std::vector<long long> audio, at;
-  rc = io.launch(cfg, tfs, tag, rg, audio, at);
-  if (rc || nstreams == 0) return rc;
-  /* the music CRC of every stream, where the bytes are */
-  std::vector<unsigned> crc;
-  rc = music_crc_ranges(t_ctx.device, io.buf(), at, audio, crc);
+  int ntags = 0;
+  for (int i = 0; i < S; i++) ntags += plan.tag[i] ? 1 : 0;
+  if (ntags == 0) return 0;
+  std::vector<long long> at((size_t)S);
+  for (int i = 0; i < S; i++) at[i] = sds[i].out_base;
+  int rc = queue_music_crc(c, at, audio);
   if (rc) return rc;
+  /* the template frames: everything but the music CRC, the gain field and the frame's own CRC */
+  const size_t tfs = (size_t)plan.tfs;
+  std::vector<TagDest> dst((size_t)ntags);
+  std::vector<uint8_t> frames(tfs * (size_t)ntags);
   Mp3SeekBag* bag = new Mp3SeekBag();
-  for (int s = 0; s < nstreams; s++) {
-    if (tag[s]) {
-      bag->reset();
-      bag->add_frames(frames[s], p.kbps);
-      const int field = rg ? mp3_radio_gain_field(mp3_radio_gain(rg->title_db[s])) : 0;
-      mp3_tag_frame(p, *bag, audio[s], crc[s], padding[s], io.frame(s), field);
-    }
-    out_bytes[s] = audio[s] + tag[s];
+  for (int i = 0, k = 0; i < S; i++) {
+    if (!plan.tag[i]) continue;
+    bag->reset();
+    bag->add_frames(plan.frames[i], p.kbps);
+    mp3_tag_frame(p, *bag, audio[i], 0, plan.padding[i], frames.data() + tfs * (size_t)k, 0);
+    dst[k].at = d_out + out_off[i]; dst[k].stream = i;
+    k++;
   }
   delete bag;
-  return io.finish(tag, audio, at);
-}
-
-/* Host rows in, host files out: the PCM is uploaded like mp3b200_encode_streams uploads it, out[s] (cap[s] bytes) receives
- * the tag frame and then the audio, read back from t_ctx.out. */
-template <class T>
-struct HostTagged {
-  int nstreams;
-  const T* const* left;
-  const T* const* right;
-  const int64_t* nsamples;
-  uint8_t* const* out;
-  const int64_t* cap;
-  int64_t* out_bytes;
-  int check_input(const Config* cfg) const { return ::check_input(cfg, nstreams, left, right, nsamples); }
-  int launch(Config* cfg, int tfs, const std::vector<int>&, RgJob* rg, std::vector<long long>& audio, std::vector<long long>& at) {
-    std::vector<int64_t> out_off;
-    const int rc = encode_host_streams(cfg, nstreams, left, right, nsamples, cap, tfs, out_bytes, out_off, audio, rg);
-    at.assign(out_off.begin(), out_off.end());
+  const size_t dst_bytes = (sizeof(TagDest) * (size_t)ntags + 255) & ~(size_t)255;
+  if ((rc = c.tags.fit(dst_bytes + frames.size())) || (rc = upload(c, c.tags.p, dst.data(), sizeof(TagDest) * dst.size())) ||
+      (rc = upload(c, c.tags.p + dst_bytes, frames.data(), frames.size())))
     return rc;
-  }
-  const uint8_t* buf() const { return t_ctx.out.p; }
-  uint8_t* frame(int s) { return out[s]; }
-  int finish(const std::vector<int>& tag, const std::vector<long long>& audio, const std::vector<long long>& at) {
-    int rc = 0;
-    for (int s = 0; s < nstreams; s++)
-      if (audio[s] > 0 && cudaMemcpyAsync(out[s] + tag[s], t_ctx.out.p + at[s], (size_t)audio[s], cudaMemcpyDeviceToHost, t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
-    if (cudaStreamSynchronize(t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
-    return rc;
-  }
-};
-
-/* Device rows in (laid out as mp3b200_encode_streams_device reads them), device files out: stream s's file starts at
- * d_out + out_off[s].  The packer writes the audio straight behind the room of its tag frame; the frames are built on the
- * host into one pinned buffer (t_ctx.pin: [k] destination offsets, then the k frames), uploaded with one copy and put in
- * place by k_tag_scatter. */
-template <class T>
-struct DeviceTagged {
-  int nstreams;
-  const T* d_pcm;
-  const int64_t* pcm_off;
-  const int64_t* nsamples;
-  uint8_t* d_out;
-  const int64_t* out_off;
-  std::vector<int> slot;                  /* stream s's frame is frame slot[s] of the staging buffer */
-  int ntags = 0, tfs = 0;            /* tag frames of the batch, and their size */
-  int check_input(const Config*) const { return MP3B200_OK; }
-  int launch(Config* cfg, int tfs_, const std::vector<int>& tag, RgJob* rg, std::vector<long long>& audio, std::vector<long long>& at) {
-    tfs = tfs_;
-    std::vector<int64_t> audio_off((size_t)nstreams);
-    for (int s = 0; s < nstreams; s++) audio_off[s] = out_off[s] + tag[s];
-    std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off, nsamples, audio_off.data());
-    audio.assign((size_t)nstreams, 0);
-    at.assign(audio_off.begin(), audio_off.end());
-    slot.assign((size_t)nstreams, -1);
-    for (int s = 0; s < nstreams; s++) {
-      audio[s] = bytes_of_frames(cfg->host, 0, sds[s].nframes);
-      if (tag[s]) slot[s] = ntags++;
-    }
-    LaunchOpts o;
-    o.rg = rg;
-    o.f32_in = std::is_same_v<T, float>;
-    int rc = launch_streams(t_ctx, cfg, sds, d_out, o);
-    if (rc || ntags == 0) return rc;
-    rc = t_ctx.pin.fit(staging_bytes());
-    if (rc) return rc;
-    long long* dst = reinterpret_cast<long long*>(t_ctx.pin.p);
-    for (int s = 0; s < nstreams; s++) if (slot[s] >= 0) dst[slot[s]] = out_off[s];
-    return 0;
-  }
-  size_t staging_bytes() const { return (sizeof(long long) + (size_t)tfs) * (size_t)ntags; }
-  const uint8_t* buf() const { return d_out; }
-  uint8_t* frame(int s) { return t_ctx.pin.p + sizeof(long long) * (size_t)ntags + (size_t)tfs * (size_t)slot[s]; }
-  int finish(const std::vector<int>&, const std::vector<long long>&, const std::vector<long long>&) {
-    if (ntags == 0) return 0;
-    int rc = t_ctx.tags.fit(staging_bytes());
-    if (rc) return rc;
-    CK(cudaMemcpyAsync(t_ctx.tags.p, t_ctx.pin.p, staging_bytes(), cudaMemcpyHostToDevice, t_ctx.st));
-    k_tag_scatter<<<ntags, TAG_SCATTER_THREADS, 0, t_ctx.st>>>(reinterpret_cast<const long long*>(t_ctx.tags.p),
-                                                               t_ctx.tags.p + sizeof(long long) * (size_t)ntags, tfs, d_out);
-    g_launches++;
-    CK(cudaStreamSynchronize(t_ctx.st));
-    CK(cudaGetLastError());
-    return 0;
-  }
-};
-
-/* encode_tagged with the gains handed out: title_db[s] / album_db (optional), RG_NOT_ENOUGH_SAMPLES where nothing ran */
-template <class Io>
-int encode_tagged_rg(int channels, int samplerate, int kbps, int flags, int nstreams, const int64_t* nsamples, int64_t* out_bytes,
-                     double* title_db, double* album_db, Io& io) {
-  RgJob job;
-  const bool want = (flags & MP3B200_REPLAYGAIN) != 0;
-  const int rc = encode_tagged(channels, samplerate, kbps, flags, nstreams, nsamples, out_bytes, want ? &job : nullptr, io);
-  if (rc) return rc;
-  const bool ran = want && (int)job.title_db.size() == nstreams && nstreams > 0;
-  for (int s = 0; title_db && s < nstreams; s++) title_db[s] = ran ? job.title_db[s] : RG_NOT_ENOUGH_SAMPLES;
-  if (album_db) *album_db = ran ? job.album_db : RG_NOT_ENOUGH_SAMPLES;
+  k_tag_finish<<<ntags, TAG_FINISH_THREADS, 0, c.st>>>(reinterpret_cast<const TagDest*>(c.tags.p), c.tags.p + dst_bytes, p, c.crc.p, gain);
+  g_launches++;
+  CK(cudaGetLastError());
   return 0;
 }
 
+/* The synchronous tagged whole streams (encodeBuffer(everything) + flush() on fresh encoders with the tag on), once their PCM
+ * is on the device: `sds` are the batch's whole_streams descriptors, and o.arrival / o.f32_in say how their rows arrive.
+ * File s -- its tag frame (plan.tag[s] bytes), then its audio -- is written at d_out + out_off[s]; with `out` (host callers,
+ * d_out in t_ctx.out) it is then copied into out[s].  out_bytes[s] receives the file's length, `rg` (as tagged_plan left
+ * it) the analysis, and title_db[s] / album_db (optional) its gains, RG_NOT_ENOUGH_SAMPLES where nothing ran. */
+int encode_tagged(Config* cfg, const TaggedPlan& plan, RgJob* rg, std::vector<StreamDesc>& sds, LaunchOpts o, uint8_t* d_out,
+                  const int64_t* out_off, uint8_t* const* out, int64_t* out_bytes, double* title_db, double* album_db) {
+  const int S = (int)sds.size();
+  if (S > 0) {
+    /* The packer gets a null base and each stream's absolute output address, its audio behind the room of its tag frame */
+    std::vector<long long> audio((size_t)S);
+    for (int s = 0; s < S; s++) {
+      sds[s].out_base = (long long)(uintptr_t)(d_out + out_off[s] + plan.tag[s]);
+      audio[s] = bytes_of_frames(cfg->host, 0, sds[s].nframes);
+    }
+    o.rg = rg;
+    int rc = launch_streams(t_ctx, cfg, sds, nullptr, o);     /* returns with the refusals checked: no tag for a refused call */
+    if (rc || (rc = crc_tables_on(t_ctx.device)) ||
+        (rc = finish_tagged(t_ctx, cfg, plan, sds, audio, d_out, out_off, rg ? t_ctx.rg_gain.p : nullptr)))
+      return rc;
+    for (int s = 0; s < S; s++) {
+      out_bytes[s] = audio[s] + plan.tag[s];
+      if (out) CK(cudaMemcpyAsync(out[s], d_out + out_off[s], (size_t)out_bytes[s], cudaMemcpyDeviceToHost, t_ctx.st));
+    }
+    CK(cudaStreamSynchronize(t_ctx.st));
+    CK(cudaGetLastError());
+  }
+  const bool ran = rg && (int)rg->title_db.size() == S && S > 0;
+  for (int s = 0; title_db && s < S; s++) title_db[s] = ran ? rg->title_db[s] : RG_NOT_ENOUGH_SAMPLES;
+  if (album_db) *album_db = ran ? rg->album_db : RG_NOT_ENOUGH_SAMPLES;
+  return 0;
+}
+
+/* The checks a synchronous tagged call starts with, and its configuration */
+int tagged_config(int channels, int samplerate, int kbps, int flags, int nstreams, Config** cfg) {
+  if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
+  if (flags & ~(MP3B200_RESAMPLE | MP3B200_REPLAYGAIN)) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
+  return get_config(channels, samplerate, kbps, flags & MP3B200_RESAMPLE, cfg);
+}
+
+/* Host rows in, host files out: the PCM is checked and uploaded as mp3b200_encode_streams does it, and out[s] (cap[s] bytes)
+ * receives file s.  With MP3B200_REPLAYGAIN, `job` receives the analysis. */
 template <class T>
 int encode_tagged_host(int channels, int samplerate, int kbps, int flags, int nstreams, const T* const* left, const T* const* right,
                        const int64_t* nsamples, uint8_t* const* out, const int64_t* cap, int64_t* out_bytes, double* title_db,
-                       double* album_db) {
-  HostTagged<T> io{nstreams, left, right, nsamples, out, cap, out_bytes};
-  return encode_tagged_rg(channels, samplerate, kbps, flags, nstreams, nsamples, out_bytes, title_db, album_db, io);
+                       double* album_db, RgJob& job) {
+  Config* cfg;
+  int rc = tagged_config(channels, samplerate, kbps, flags, nstreams, &cfg);
+  if (rc || (rc = check_input(cfg, nstreams, left, right, nsamples))) return rc;
+  RgJob* rg = flags & MP3B200_REPLAYGAIN ? &job : nullptr;
+  const TaggedPlan plan = tagged_plan(cfg, nstreams, nsamples, rg);
+  std::vector<int64_t> file_off;
+  std::vector<StreamDesc> sds;
+  PcmArrival arr;
+  if ((rc = stage_host_streams(cfg, nstreams, left, right, nsamples, cap, plan.tag.data(), out_bytes, file_off, sds, arr))) return rc;
+  LaunchOpts o;
+  o.arrival = &arr;
+  o.f32_in = std::is_same_v<T, float>;
+  return encode_tagged(cfg, plan, rg, sds, o, t_ctx.out.p, file_off.data(), out, out_bytes, title_db, album_db);
 }
 
+/* Device rows in (laid out as mp3b200_encode_streams_device reads them), device files out: file s at d_out + out_off[s] */
 template <class T>
 int encode_tagged_device(int channels, int samplerate, int kbps, int flags, int nstreams, const T* d_pcm, const int64_t* pcm_off,
                          const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off, int64_t* out_bytes, double* title_db,
                          double* album_db) {
-  DeviceTagged<T> io{nstreams, d_pcm, pcm_off, nsamples, d_out, out_off};
-  return encode_tagged_rg(channels, samplerate, kbps, flags, nstreams, nsamples, out_bytes, title_db, album_db, io);
+  Config* cfg;
+  const int rc = tagged_config(channels, samplerate, kbps, flags, nstreams, &cfg);
+  if (rc) return rc;
+  RgJob job;
+  RgJob* rg = flags & MP3B200_REPLAYGAIN ? &job : nullptr;
+  const TaggedPlan plan = tagged_plan(cfg, nstreams, nsamples, rg);
+  std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off, nsamples, out_off);
+  LaunchOpts o;
+  o.f32_in = std::is_same_v<T, float>;
+  return encode_tagged(cfg, plan, rg, sds, o, d_out, out_off, nullptr, out_bytes, title_db, album_db);
 }
 }  // namespace
 
@@ -1908,12 +1856,14 @@ extern "C" {
 int mp3b200_encode_streams_tagged_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
                                      const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
                                      const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db) {
-  return encode_tagged_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, title_db, album_db);
+  RgJob job;
+  return encode_tagged_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, title_db, album_db, job);
 }
 int mp3b200_encode_streams_tagged_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* const* left,
                                       const float* const* right, const int64_t* nsamples, uint8_t* const* out,
                                       const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db) {
-  return encode_tagged_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, title_db, album_db);
+  RgJob job;
+  return encode_tagged_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, title_db, album_db, job);
 }
 
 int mp3b200_encode_streams_tagged_device(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
@@ -1951,8 +1901,8 @@ int debug_replaygain(int channels, int samplerate, int kbps, int flags, const T*
   std::vector<uint8_t> out((size_t)cap);
   uint8_t* outp = out.data();
   int64_t ob = 0;
-  HostTagged<T> io{1, &left, &right, &nsamples, &outp, &cap, &ob};
-  const int rc = encode_tagged(channels, samplerate, kbps, (flags & MP3B200_RESAMPLE) | MP3B200_REPLAYGAIN, 1, &nsamples, &ob, &job, io);
+  const int rc = encode_tagged_host(channels, samplerate, kbps, (flags & MP3B200_RESAMPLE) | MP3B200_REPLAYGAIN, 1, &left, &right,
+                                    &nsamples, &outp, &cap, &ob, nullptr, nullptr, job);
   if (rc) return rc;
   const long long n = (long long)job.win_idx.size();
   for (long long w = 0; w < n && w < nwin_cap; w++) {
