@@ -262,12 +262,56 @@ int mp3b200_encode_streams_tagged_device_f32(int channels, int samplerate, int k
                                              int64_t* out_bytes, double* title_db, double* album_db);
 /* mp3b200_lametag_build with flags (MP3B200_RESAMPLE) and the Radio Replay Gain field of an analysed stream: radio_gain is
  * gfc.RadioGain = floor(title_db * 10 + 0.5), clamped to +-51.0 dB like lamejs; for segment callers that analyse the whole
- * stream themselves (ReplayGain is not combined across segments). */
+ * stream themselves (ReplayGain is not combined across segments).  mp3b200_replaygain_streams below is that analysis, and
+ * mp3b200_finish_tags_device the whole tag step on the joined audio in device memory. */
 int mp3b200_set_find_replay_gain(mp3b200_encoder* h, int on);
 int mp3b200_get_replay_gain(mp3b200_encoder* h, double* title_db, int* radio_gain);
 int mp3b200_album_gain(mp3b200_encoder* const* handles, int n, double* album_db);
 int mp3b200_lametag_build_ex(int channels, int samplerate, int kbps, int flags, int64_t nframes, int64_t music_bytes, int music_crc,
                              int encoder_padding, int radio_gain, uint8_t* buf, int cap);
+/* ReplayGain of whole streams without the encoder: the analysis lamejs runs for a fresh Mp3Encoder with findReplayGain fed
+ * encodeBuffer(whole stream) and then flush() -- the same pieces, the flush zeros, and under MP3B200_RESAMPLE the
+ * resampler's output -- and nothing else: no encoder kernel runs.  For segment callers, which encode one stream in pieces
+ * (lamejs_b200/sharding.py) and analyse it once beside them.
+ *   left, right, nsamples      as for mp3b200_encode_streams_ex / _f32 (Int16 rows, or Float32 rows rounded and scaled as
+ *                              lamejs's Float32Array store does; a sample that is not finite, or beyond 2^40 once scaled,
+ *                              returns MP3B200_ERR_CONFIG).  Stereo with right == NULL or right[s] == NULL takes left[s].
+ *   _device / _device_f32      rows laid out as mp3b200_encode_streams_device_ex reads them: stream s at d_pcm + pcm_off[s],
+ *                              the right channel behind the left.  The call waits for work queued on the legacy default
+ *                              stream and returns after its own stream has drained, as mp3b200_encode_streams_tagged_device.
+ *   flags                      0 or MP3B200_RESAMPLE; any other bit returns MP3B200_ERR_CONFIG.
+ *   title_db, album_db         (optional) GetTitleGain of each stream in dB and GetAlbumGain of the batch, -24601 for less
+ *                              than one RMS window.  Bit-identical to what mp3b200_encode_streams_tagged_ex with
+ *                              MP3B200_REPLAYGAIN returns for the same rows wherever the tag fits the configuration.  Where it
+ *                              does not (mp3b200_lametag_size_ex == 0) that call analyses nothing and returns -24601; these
+ *                              calls still analyse.
+ * nstreams < 0, a NULL array (left / d_pcm, pcm_off, nsamples, or a NULL left[s]) or a negative nsamples[s] returns
+ * MP3B200_ERR_HANDLE before the device is touched; at most 65535 streams per call (MP3B200_ERR_HANDLE). */
+int mp3b200_replaygain_streams(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
+                               const int16_t* const* right, const int64_t* nsamples, double* title_db, double* album_db);
+int mp3b200_replaygain_streams_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* const* left,
+                                   const float* const* right, const int64_t* nsamples, double* title_db, double* album_db);
+int mp3b200_replaygain_streams_device(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
+                                      const int64_t* pcm_off, const int64_t* nsamples, double* title_db, double* album_db);
+int mp3b200_replaygain_streams_device_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* d_pcm,
+                                          const int64_t* pcm_off, const int64_t* nsamples, double* title_db, double* album_db);
+/* The tag step of mp3b200_encode_streams_tagged_device on audio already in device memory: turns the untagged audio of whole
+ * streams (one stream encoded in segments and joined, say) into finished files.
+ *   d_files, file_off, nsamples   file s lies at d_files + file_off[s]: mp3b200_lametag_size_ex bytes of room, then the
+ *                              mp3b200_stream_bytes_ex(..., nsamples[s]) audio bytes of encodeBuffer(nsamples[s] samples) +
+ *                              flush() on a fresh encoder.  The tag frame is written into the room: music CRC of the audio
+ *                              (k_music_crc), frame / byte counts, seek table and encoder padding from nsamples[s].
+ *   title_db                   host array (may be NULL): the Radio Replay Gain field of file s from title_db[s], rounded and
+ *                              clamped to +-51.0 dB as lamejs does; NULL writes the field as 0 (nothing analysed).
+ *   file_bytes                 host array: file_bytes[s] receives the file's length.
+ *   flags                      0 or MP3B200_RESAMPLE.
+ * Where the tag does not fit the configuration there is no room and nothing is written; nothing outside
+ * [file_off[s], file_off[s] + file_bytes[s]) is ever written.  The files are byte-identical to what
+ * mp3b200_encode_streams_tagged_device writes for the same samples: with MP3B200_REPLAYGAIN when title_db comes from
+ * mp3b200_replaygain_streams, without it when title_db is NULL.  Ordering as mp3b200_replaygain_streams_device; argument
+ * errors as there (d_files, file_off, nsamples and file_bytes must not be NULL). */
+int mp3b200_finish_tags_device(int channels, int samplerate, int kbps, int flags, int nstreams, uint8_t* d_files,
+                               const int64_t* file_off, const int64_t* nsamples, const double* title_db, int64_t* file_bytes);
 /* Test tap: one whole stream through mp3b200_encode_streams_tagged_ex with MP3B200_REPLAYGAIN (flags: MP3B200_RESAMPLE).
  * win_sums [w][2] = lsum, rsum of RMS window w (bit-exact), win_idx[w] its histogram index, for w < nwin_cap; hist (12000
  * bins), title_db; stats[0] windows, [1] repair passes, [2] chunks run again, [3] the analysis time in ms (a float's bits).

@@ -12,3 +12,4 @@ from .encoder import Mp3Encoder, WavHeader, id3v1_tag, id3v2_tag, ID3_ADD_V2, ID
 from .encoder import REPLAYGAIN, GAIN_NOT_ENOUGH_SAMPLES, radio_gain, lametag_build_ex, debug_replaygain, encode_streams_replaygain, album_gain  # noqa: F401
 from .encoder import DOMAIN_SITES, debug_domain_hits  # noqa: F401
 from .encoder import EncodeSession, check_status  # noqa: F401
+from .encoder import replay_gain_streams, replay_gain_streams_device, finish_tags_device  # noqa: F401

@@ -459,6 +459,8 @@ struct LaunchOpts {
   const struct HandleCarry* carry = nullptr;   /* streaming handles bound to a session: their carried state is on the device
                                                   (k_handle_carry_in; one launch group only) */
   int* rg_loop = nullptr;                /* a session's three words of the ReplayGain loop (rg_finish_queued); NULL: ws.refusals + 5 */
+  bool analyse_only = false;             /* stop after staging, resampling and the ReplayGain analysis of o.rg: no encoder
+                                            kernels, no bytes, no workspace beyond the staged rows */
 };
 
 /* LaunchOpts::carry: recs[z] is the record of stream z (device array); halo_scratch takes the masking of refused handles */
@@ -1089,7 +1091,7 @@ int launch_streams(ThreadCtx& c, Config* cfg, std::vector<StreamDesc>& sds, uint
       U += (long long)cfg->host.mode_gr * group[i].nframes; F += group[i].nframes;
     }
     if (F == 0) continue;                     /* empty group: nothing to launch */
-    int rc = c.ws.fit(n, cfg->host.nch, U, F);
+    int rc = o.analyse_only ? 0 : c.ws.fit(n, cfg->host.nch, U, F);
     if (rc) return rc;
     const bool resampled = cfg->rs.ratio > 1;
     if (resampled || o.f32_in) {
@@ -1113,7 +1115,7 @@ int launch_streams(ThreadCtx& c, Config* cfg, std::vector<StreamDesc>& sds, uint
       if (rc) return rc;
     }
     Timings tm;
-    rc = run_pipeline(c, cfg, group, n, d_out, o, arrival, rows, &tm);
+    rc = o.analyse_only ? 0 : run_pipeline(c, cfg, group, n, d_out, o, arrival, rows, &tm);
     if (rc) return rc;
     if (o.rg) {                                /* a session: ws.refusals[3] is its fault word, [5 .. 8) the loop's words */
       rc = o.loops ? rg_finish_queued(c, cfg, *o.rg, *o.loops, o.rg_loop ? o.rg_loop : c.ws.refusals.p + 5, c.ws.refusals.p + 3)
@@ -1242,33 +1244,21 @@ int check_input(const Config* cfg, int nstreams, const float* const* left, const
   return MP3B200_OK;
 }
 
-/* Whole streams from host buffers, laid out as files in t_ctx.out: file s at out_off[s] is room[s] bytes (room NULL: none)
- * and then the stream's audio.  Checks that out[s] has room for the file (out_bytes[s] = its length), stages the PCM (Int16
- * or Float32) in the thread's buffers and fills the descriptors `sds` (out_base: the file's offset, where the audio goes when
- * there is no room) and the upload's arrival `arr`.  Stereo input with right == NULL or right[s] == NULL encodes left[s] on
- * both channels. */
+/* Stages the rows of host streams (Int16 or Float32) in the thread's buffer, stream s at d_pcm + pcm_off[s] laid out as
+ * whole_streams reads it, and fills the upload's arrival `arr`.  Stereo input with right == NULL or right[s] == NULL takes
+ * left[s] for both channels. */
 template <class T>
-int stage_host_streams(Config* cfg, int nstreams, const T* const* left, const T* const* right, const int64_t* nsamples,
-                       const int64_t* cap, const int* room, int64_t* out_bytes, std::vector<int64_t>& out_off,
-                       std::vector<StreamDesc>& sds, PcmArrival& arr) {
+int upload_host_rows(const Config* cfg, int nstreams, const T* const* left, const T* const* right, const int64_t* nsamples,
+                     std::vector<int64_t>& pcm_off, T*& d_pcm, PcmArrival& arr) {
   const int nch = cfg->host.nch;
-  std::vector<int64_t> pcm_off(nstreams);
-  out_off.assign(nstreams, 0);
-  long long tot_samples = 0, tot_bytes = 0;
+  pcm_off.assign(nstreams, 0);
+  long long tot_samples = 0;
   for (int s = 0; s < nstreams; s++) {
     pcm_off[s] = tot_samples;
     tot_samples += nsamples[s] * nch;
-    out_off[s] = tot_bytes;
-    const long long n = bytes_of_frames(cfg->host, 0, frames_for(nsamples[s], cfg->host.mode_gr, cfg->rs.ratio)) + (room ? room[s] : 0);
-    if (cap[s] < n) { g_err = "output buffer too small"; return MP3B200_ERR_BUFFER; }
-    out_bytes[s] = n;
-    tot_bytes += n;
   }
-  if (nstreams == 0) return MP3B200_OK;
-  T* d_pcm = staging_pcm<T>((size_t)tot_samples + 8);
+  d_pcm = staging_pcm<T>((size_t)tot_samples + 8);
   if (!d_pcm) return MP3B200_ERR_CUDA;
-  int rc = t_ctx.out.fit((size_t)tot_bytes + 8);
-  if (rc) return rc;
   /* Upload in time slices on a copy stream; the psy analysis of a slice starts when it has landed, so only the first
    * slice's transfer is exposed.  Many small streams are uploaded whole (one slice): per-copy overhead would win. */
   arr.chunks = (nstreams <= 8 && tot_samples >= (1 << 20)) ? MP3_MAX_PCM_CHUNKS : 1;
@@ -1284,6 +1274,31 @@ int stage_host_streams(Config* cfg, int nstreams, const T* const* left, const T*
     }
     CK(cudaEventRecord(t_ctx.ready[j], t_ctx.up_st));
   }
+  return MP3B200_OK;
+}
+
+/* Whole streams from host buffers, laid out as files in t_ctx.out: file s at out_off[s] is room[s] bytes (room NULL: none)
+ * and then the stream's audio.  Checks that out[s] has room for the file (out_bytes[s] = its length), stages the PCM
+ * (upload_host_rows) and fills the descriptors `sds` (out_base: the file's offset, where the audio goes when there is no
+ * room) and the upload's arrival `arr`. */
+template <class T>
+int stage_host_streams(Config* cfg, int nstreams, const T* const* left, const T* const* right, const int64_t* nsamples,
+                       const int64_t* cap, const int* room, int64_t* out_bytes, std::vector<int64_t>& out_off,
+                       std::vector<StreamDesc>& sds, PcmArrival& arr) {
+  out_off.assign(nstreams, 0);
+  long long tot_bytes = 0;
+  for (int s = 0; s < nstreams; s++) {
+    out_off[s] = tot_bytes;
+    const long long n = bytes_of_frames(cfg->host, 0, frames_for(nsamples[s], cfg->host.mode_gr, cfg->rs.ratio)) + (room ? room[s] : 0);
+    if (cap[s] < n) { g_err = "output buffer too small"; return MP3B200_ERR_BUFFER; }
+    out_bytes[s] = n;
+    tot_bytes += n;
+  }
+  if (nstreams == 0) return MP3B200_OK;
+  std::vector<int64_t> pcm_off;
+  T* d_pcm = nullptr;
+  int rc = upload_host_rows(cfg, nstreams, left, right, nsamples, pcm_off, d_pcm, arr);
+  if (rc || (rc = t_ctx.out.fit((size_t)tot_bytes + 8))) return rc;
   sds = whole_streams(cfg, nstreams, d_pcm, pcm_off.data(), nsamples, out_off.data());
   return MP3B200_OK;
 }
@@ -1708,17 +1723,15 @@ int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int ns
 namespace {
 /* What is known about tagged whole streams before anything runs, in closed form from the lamejs FIFO: each stream's frames,
  * its end padding and the size of its tag frame (tfs, or 0: no frame), and, with `rg`, the pieces the analysis sees
- * (rg->specs).  `rg` is reset to NULL where lamejs does not analyse: it does so only when the tag is written
- * (Lame.js:911-916). */
+ * (rg->specs), whether or not the tag fits. */
 struct TaggedPlan {
   int tfs = 0;
   std::vector<long long> frames;
   std::vector<int> padding, tag;
 };
-TaggedPlan tagged_plan(const Config* cfg, int nstreams, const int64_t* nsamples, RgJob*& rg) {
+TaggedPlan stream_plan(const Config* cfg, int nstreams, const int64_t* nsamples, RgJob* rg) {
   TaggedPlan pl;
   pl.tfs = cfg->tag.fits ? cfg->tag.frame_bytes : 0;
-  if (rg && pl.tfs == 0) rg = nullptr;
   if (rg) rg->specs.assign((size_t)nstreams, RgSpec());
   pl.frames.resize((size_t)nstreams); pl.padding.resize((size_t)nstreams); pl.tag.resize((size_t)nstreams);
   for (int s = 0; s < nstreams; s++) {
@@ -1731,6 +1744,13 @@ TaggedPlan tagged_plan(const Config* cfg, int nstreams, const int64_t* nsamples,
     pl.tag[s] = pl.tfs > 0 && pl.frames[s] > 0 ? pl.tfs : 0;
   }
   return pl;
+}
+
+/* stream_plan for the tagged encodes: `rg` is reset to NULL where lamejs does not analyse, which it does only when the tag
+ * is written (Lame.js:911-916) */
+TaggedPlan tagged_plan(const Config* cfg, int nstreams, const int64_t* nsamples, RgJob*& rg) {
+  if (rg && !cfg->tag.fits) rg = nullptr;
+  return stream_plan(cfg, nstreams, nsamples, rg);
 }
 
 /* Queues, behind the packer on c.st, what turns the audio of tagged whole streams into files: the music CRC of each stream
@@ -1772,6 +1792,22 @@ int finish_tagged(ThreadCtx& c, Config* cfg, const TaggedPlan& plan, const std::
   return 0;
 }
 
+/* The tag step of the synchronous tagged whole streams, once their audio lies at sds[s].out_base (audio[s] bytes, queued
+ * on t_ctx.st or already there): finish_tagged with gain[s] (device; NULL: field 0), out_bytes[s] = the file's length, and
+ * with `out` each file copied from d_out + out_off[s] into out[s].  Returns with t_ctx.st drained. */
+int finish_files(Config* cfg, const TaggedPlan& plan, const std::vector<StreamDesc>& sds, const std::vector<long long>& audio,
+                 uint8_t* d_out, const int64_t* out_off, const double* gain, uint8_t* const* out, int64_t* out_bytes) {
+  int rc = crc_tables_on(t_ctx.device);
+  if (rc || (rc = finish_tagged(t_ctx, cfg, plan, sds, audio, d_out, out_off, gain))) return rc;
+  for (size_t s = 0; s < sds.size(); s++) {
+    out_bytes[s] = audio[s] + plan.tag[s];
+    if (out) CK(cudaMemcpyAsync(out[s], d_out + out_off[s], (size_t)out_bytes[s], cudaMemcpyDeviceToHost, t_ctx.st));
+  }
+  CK(cudaStreamSynchronize(t_ctx.st));
+  CK(cudaGetLastError());
+  return 0;
+}
+
 /* The synchronous tagged whole streams (encodeBuffer(everything) + flush() on fresh encoders with the tag on), once their PCM
  * is on the device: `sds` are the batch's whole_streams descriptors, and o.arrival / o.f32_in say how their rows arrive.
  * File s -- its tag frame (plan.tag[s] bytes), then its audio -- is written at d_out + out_off[s]; with `out` (host callers,
@@ -1789,15 +1825,7 @@ int encode_tagged(Config* cfg, const TaggedPlan& plan, RgJob* rg, std::vector<St
     }
     o.rg = rg;
     int rc = launch_streams(t_ctx, cfg, sds, nullptr, o);     /* returns with the refusals checked: no tag for a refused call */
-    if (rc || (rc = crc_tables_on(t_ctx.device)) ||
-        (rc = finish_tagged(t_ctx, cfg, plan, sds, audio, d_out, out_off, rg ? t_ctx.rg_gain.p : nullptr)))
-      return rc;
-    for (int s = 0; s < S; s++) {
-      out_bytes[s] = audio[s] + plan.tag[s];
-      if (out) CK(cudaMemcpyAsync(out[s], d_out + out_off[s], (size_t)out_bytes[s], cudaMemcpyDeviceToHost, t_ctx.st));
-    }
-    CK(cudaStreamSynchronize(t_ctx.st));
-    CK(cudaGetLastError());
+    if (rc || (rc = finish_files(cfg, plan, sds, audio, d_out, out_off, rg ? t_ctx.rg_gain.p : nullptr, out, out_bytes))) return rc;
   }
   const bool ran = rg && (int)rg->title_db.size() == S && S > 0;
   for (int s = 0; title_db && s < S; s++) title_db[s] = ran ? rg->title_db[s] : RG_NOT_ENOUGH_SAMPLES;
@@ -1849,6 +1877,68 @@ int encode_tagged_device(int channels, int samplerate, int kbps, int flags, int 
   o.f32_in = std::is_same_v<T, float>;
   return encode_tagged(cfg, plan, rg, sds, o, d_out, out_off, nullptr, out_bytes, title_db, album_db);
 }
+
+/* The argument checks of the standalone analysis and tag step, made before anything touches the device: `rows` is the
+ * call's row array (left, or d_pcm / d_files) and `offs` its offsets, which host rows (host_rows) do not have */
+int whole_stream_args(int nstreams, int flags, const void* rows, const int64_t* offs, bool host_rows, const int64_t* nsamples) {
+  if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
+  if (flags & ~MP3B200_RESAMPLE) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
+  if (nstreams == 0) return MP3B200_OK;
+  if (!rows || !nsamples || (!host_rows && !offs)) { g_err = "null array"; return MP3B200_ERR_HANDLE; }
+  for (int s = 0; s < nstreams; s++)
+    if (nsamples[s] < 0) { g_err = "negative sample count"; return MP3B200_ERR_HANDLE; }
+  return MP3B200_OK;
+}
+
+/* The ReplayGain analysis of whole streams (descriptors `sds` from whole_streams) without the encoder: the RgSpecs of the
+ * tagged whole-stream path (stream_plan), analysed by launch_streams on the staged or resampled rows (o.analyse_only) */
+int analyse_streams(Config* cfg, int nstreams, const int64_t* nsamples, std::vector<StreamDesc>& sds, LaunchOpts o,
+                    double* title_db, double* album_db) {
+  RgJob job;
+  stream_plan(cfg, nstreams, nsamples, &job);
+  o.rg = &job;
+  o.analyse_only = true;
+  const int rc = launch_streams(t_ctx, cfg, sds, nullptr, o);
+  if (rc) return rc;
+  const bool ran = (int)job.title_db.size() == nstreams && nstreams > 0;
+  for (int s = 0; title_db && s < nstreams; s++) title_db[s] = ran ? job.title_db[s] : RG_NOT_ENOUGH_SAMPLES;
+  if (album_db) *album_db = ran ? job.album_db : RG_NOT_ENOUGH_SAMPLES;
+  return 0;
+}
+
+template <class T>
+int replaygain_host(int channels, int samplerate, int kbps, int flags, int nstreams, const T* const* left, const T* const* right,
+                    const int64_t* nsamples, double* title_db, double* album_db) {
+  int rc = whole_stream_args(nstreams, flags, left, nullptr, true, nsamples);
+  if (rc) return rc;
+  for (int s = 0; s < nstreams; s++)
+    if (!left[s]) { g_err = "null row"; return MP3B200_ERR_HANDLE; }
+  Config* cfg;
+  if ((rc = get_config(channels, samplerate, kbps, flags, &cfg)) || (rc = check_input(cfg, nstreams, left, right, nsamples))) return rc;
+  std::vector<int64_t> pcm_off, out_off((size_t)nstreams, 0);
+  T* d_pcm = nullptr;
+  PcmArrival arr;
+  if (nstreams > 0 && (rc = upload_host_rows(cfg, nstreams, left, right, nsamples, pcm_off, d_pcm, arr))) return rc;
+  std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off.data(), nsamples, out_off.data());
+  LaunchOpts o;
+  o.arrival = nstreams > 0 ? &arr : nullptr;
+  o.f32_in = std::is_same_v<T, float>;
+  return analyse_streams(cfg, nstreams, nsamples, sds, o, title_db, album_db);
+}
+
+template <class T>
+int replaygain_device(int channels, int samplerate, int kbps, int flags, int nstreams, const T* d_pcm, const int64_t* pcm_off,
+                      const int64_t* nsamples, double* title_db, double* album_db) {
+  int rc = whole_stream_args(nstreams, flags, d_pcm, pcm_off, false, nsamples);
+  if (rc) return rc;
+  Config* cfg;
+  if ((rc = get_config(channels, samplerate, kbps, flags, &cfg))) return rc;
+  std::vector<int64_t> out_off((size_t)nstreams, 0);
+  std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off, nsamples, out_off.data());
+  LaunchOpts o;
+  o.f32_in = std::is_same_v<T, float>;
+  return analyse_streams(cfg, nstreams, nsamples, sds, o, title_db, album_db);
+}
 }  // namespace
 
 extern "C" {
@@ -1883,6 +1973,47 @@ int mp3b200_lametag_build_ex(int channels, int samplerate, int kbps, int flags, 
                              int encoder_padding, int radio_gain, uint8_t* buf, int cap) {
   return build_lametag(channels, samplerate, kbps, flags, nframes, music_bytes, music_crc, encoder_padding,
                        mp3_radio_gain_field(radio_gain), buf, cap);
+}
+
+int mp3b200_replaygain_streams(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
+                               const int16_t* const* right, const int64_t* nsamples, double* title_db, double* album_db) {
+  return replaygain_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, title_db, album_db);
+}
+int mp3b200_replaygain_streams_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* const* left,
+                                   const float* const* right, const int64_t* nsamples, double* title_db, double* album_db) {
+  return replaygain_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, title_db, album_db);
+}
+int mp3b200_replaygain_streams_device(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
+                                      const int64_t* pcm_off, const int64_t* nsamples, double* title_db, double* album_db) {
+  return replaygain_device(channels, samplerate, kbps, flags, nstreams, d_pcm, pcm_off, nsamples, title_db, album_db);
+}
+int mp3b200_replaygain_streams_device_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* d_pcm,
+                                          const int64_t* pcm_off, const int64_t* nsamples, double* title_db, double* album_db) {
+  return replaygain_device(channels, samplerate, kbps, flags, nstreams, d_pcm, pcm_off, nsamples, title_db, album_db);
+}
+
+int mp3b200_finish_tags_device(int channels, int samplerate, int kbps, int flags, int nstreams, uint8_t* d_files,
+                               const int64_t* file_off, const int64_t* nsamples, const double* title_db, int64_t* file_bytes) {
+  int rc = whole_stream_args(nstreams, flags, d_files, file_off, false, nsamples);
+  if (rc) return rc;
+  if (nstreams > 0 && !file_bytes) { g_err = "file_bytes is NULL"; return MP3B200_ERR_HANDLE; }
+  Config* cfg;
+  if ((rc = get_config(channels, samplerate, kbps, flags, &cfg)) || (rc = wait_legacy(t_ctx))) return rc;
+  const TaggedPlan plan = stream_plan(cfg, nstreams, nsamples, nullptr);
+  std::vector<StreamDesc> sds((size_t)nstreams);
+  std::vector<long long> audio((size_t)nstreams);
+  for (int s = 0; s < nstreams; s++) {
+    memset(&sds[s], 0, sizeof(StreamDesc));
+    sds[s].out_base = (long long)(uintptr_t)(d_files + file_off[s] + plan.tag[s]);
+    audio[s] = bytes_of_frames(cfg->host, 0, plan.frames[s]);
+  }
+  const double* gain = nullptr;
+  if (title_db && nstreams > 0) {
+    if ((rc = t_ctx.rg_gain.fit((size_t)nstreams)) || (rc = upload(t_ctx, t_ctx.rg_gain.p, title_db, sizeof(double) * (size_t)nstreams)))
+      return rc;
+    gain = t_ctx.rg_gain.p;
+  }
+  return finish_files(cfg, plan, sds, audio, d_files, file_off, gain, nullptr, file_bytes);
 }
 
 }  // extern "C"

@@ -124,6 +124,10 @@ def lib():
     L.mp3b200_session_graph_instantiations.argtypes = [vp]
     L.mp3b200_encode_bytes_schedule.argtypes = [c_int, c_int, c_int, c_int, c_int, vp, c_int, vp]
     L.mp3b200_session_graph_instantiations.restype = c_i64
+    for name in ("mp3b200_replaygain_streams", "mp3b200_replaygain_streams_f32", "mp3b200_replaygain_streams_device",
+                 "mp3b200_replaygain_streams_device_f32"):
+        getattr(L, name).argtypes = [c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp]
+    L.mp3b200_finish_tags_device.argtypes = [c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp]
     L.mp3b200_session_tail_capacity.restype = c_i64
     _lib = L
     return L
@@ -181,6 +185,8 @@ _F32_TWIN = {
     "mp3b200_session_encode_batch_tagged": "mp3b200_session_encode_batch_tagged_f32",
     "mp3b200_debug_resample": "mp3b200_debug_resample_f32",
     "mp3b200_debug_replaygain": "mp3b200_debug_replaygain_f32",
+    "mp3b200_replaygain_streams": "mp3b200_replaygain_streams_f32",
+    "mp3b200_replaygain_streams_device": "mp3b200_replaygain_streams_device_f32",
 }
 
 
@@ -422,7 +428,8 @@ class Mp3Encoder:
 
     def seek(self, frame, left_hist, right_hist=None):
         """fresh encoder -> frame `frame` of a stream with start-of-stream sequential state; *_hist = samples
-        [max(0, frame*framesize-1104), frame*framesize+224)"""
+        [max(0, frame*framesize-1104), frame*framesize+224) (CUDA tensors are copied to the host: at most 1328 samples)"""
+        left_hist, right_hist = [x.cpu() if _on_cuda(x) else x for x in (left_hist, right_hist)]
         (left_hist,), (right_hist,), f32 = _rows([left_hist], [None if self.channels == 1 else right_hist])
         _check(_entry("mp3b200_seek", f32)(self._h, int(frame), left_hist.ctypes.data, right_hist.ctypes.data, len(left_hist)))
 
@@ -533,6 +540,54 @@ def encode_streams_replaygain(channels, samplerate, kbps, lefts, rights=None, re
     out = _encode_host_streams("mp3b200_encode_streams_tagged_ex", flags, channels, samplerate, kbps, lefts, rights, max(room, 0),
                                resample, title.ctypes.data, ctypes.byref(album))
     return out, [float(t) for t in title[:len(lefts)]], float(album.value) if lefts else float(GAIN_NOT_ENOUGH_SAMPLES)
+
+
+def replay_gain_streams(channels, samplerate, kbps, lefts, rights=None, resample=False):
+    """The ReplayGain analysis of encode_streams_replaygain without the encoder (mp3b200_replaygain_streams): returns
+    (title_db list, album_db), bit-identical to its gains wherever the tag fits; where it does not, the encode analyses
+    nothing (-24601) and this still analyses.  Host rows with the dtype rules of encode_streams."""
+    S = len(lefts)
+    lefts, rights, f32 = _rows(lefts, None if channels == 1 else rights)
+    ns = np.array([len(x) for x in lefts] or [0], dtype=np.int64)
+    lp = (ctypes.c_void_p * max(S, 1))(*[x.ctypes.data for x in lefts])
+    rp = (ctypes.c_void_p * max(S, 1))(*[x.ctypes.data for x in rights])
+    title = np.zeros(max(S, 1), dtype=np.float64)
+    album = ctypes.c_double(0.0)
+    _check(_entry("mp3b200_replaygain_streams", f32)(channels, samplerate, kbps, RESAMPLE if resample else 0, S, lp, rp,
+                                                     ns.ctypes.data, title.ctypes.data, ctypes.byref(album)))
+    return [float(t) for t in title[:S]], float(album.value)
+
+
+def replay_gain_streams_device(channels, samplerate, kbps, d_pcm_ptr, pcm_off, nsamples, resample=False, float32=False):
+    """replay_gain_streams on device rows (raw device pointer as int), laid out as encode_streams_device reads them:
+    returns (title_db list, album_db).  float32=True: d_pcm holds Float32 samples; a non-finite one raises Mp3B200Error."""
+    pcm_off = np.ascontiguousarray(pcm_off, dtype=np.int64)
+    nsamples = np.ascontiguousarray(nsamples, dtype=np.int64)
+    S = len(nsamples)
+    title = np.zeros(max(S, 1), dtype=np.float64)
+    album = ctypes.c_double(0.0)
+    _check(_entry("mp3b200_replaygain_streams_device", float32)(channels, samplerate, kbps, RESAMPLE if resample else 0, S, d_pcm_ptr,
+                                                                pcm_off.ctypes.data, nsamples.ctypes.data, title.ctypes.data,
+                                                                ctypes.byref(album)))
+    return [float(t) for t in title[:S]], float(album.value)
+
+
+def finish_tags_device(channels, samplerate, kbps, d_files_ptr, file_off, nsamples, title_db=None, resample=False):
+    """The tag step of encode_streams_device_tagged on audio already in device memory (mp3b200_finish_tags_device): file s
+    at d_files + file_off[s] is lametag_size(...) bytes of room followed by the stream_bytes(..., nsamples[s]) audio bytes
+    of a whole encodeBuffer + flush; the finished tag frame is written into the room, its Radio Replay Gain field from
+    title_db[s] (None: 0).  Returns each file's length."""
+    file_off = np.ascontiguousarray(file_off, dtype=np.int64)
+    nsamples = np.ascontiguousarray(nsamples, dtype=np.int64)
+    S = len(nsamples)
+    got = np.zeros(max(S, 1), dtype=np.int64)
+    gains = None if title_db is None else np.ascontiguousarray(title_db, dtype=np.float64)
+    if gains is not None and len(gains) != S:
+        raise ValueError("title_db needs one gain per stream")
+    _check(lib().mp3b200_finish_tags_device(channels, samplerate, kbps, RESAMPLE if resample else 0, S, d_files_ptr,
+                                            file_off.ctypes.data, nsamples.ctypes.data,
+                                            None if gains is None else gains.ctypes.data, got.ctypes.data))
+    return [int(g) for g in got[:S]]
 
 
 def album_gain(encoders):

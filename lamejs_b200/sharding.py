@@ -5,6 +5,8 @@ rank j % world (round-robin, like config C4), every rank encodes its shard with 
 encoded bytes are gathered to rank 0 at the end.  CBR without reservoir makes every stream's byte count a closed form of
 its sample count (mp3b200_stream_bytes), so each rank knows all sizes up front and the gather needs no size exchange.
 Backend-agnostic: NCCL on GPUs (bench.py), gloo in the CPU tests."""
+from concurrent.futures import ThreadPoolExecutor
+
 import numpy as np
 import torch
 import torch.distributed as dist
@@ -147,3 +149,104 @@ def encode_stream_segments(make_encoder, left, right, framesize, warmup=8, group
     if rank != 0:
         return None, int(cnt.item())
     return b"".join(bufs[r][: int(sizes[r].item())].cpu().numpy().tobytes() for r in range(world)), int(cnt.item())
+
+
+# ---- finished files from segments ----------------------------------------------------------------------------------------
+# The segments are encoded untagged, exactly as above; the file is finished afterwards on rank 0.  Every field of the tag
+# frame is a closed form of the sample count (frames, bytes, seek table, encoder padding) or a function of the joined audio
+# (music CRC), and lamejs's ReplayGain depends only on the PCM and on the pieces one encodeBuffer(whole) + flush() feeds it,
+# not on the encoded bytes.  So rank 0 analyses the whole stream once on a second host thread (its own CUDA stream) while
+# its range encodes, joins the ranges' audio behind the tag frame's room in one buffer and finishes the frame there
+# (mp3b200_finish_tags_device).  The result is the file encode_streams_replaygain makes of the whole stream.
+
+def _finished(encode_audio, room, analyse, finish, file_device):
+    """encode_audio() -> (joined audio bytes, or None off rank 0; ranges re-encoded).  analyse() (None: no analysis) runs on
+    a second thread beside it and returns the title gain.  finish(buf, title_db) writes the tag frame into buf[:room] of the
+    buffer holding the audio behind it and returns the file's length.  Returns (file bytes, ranges re-encoded, title_db),
+    with title_db None when nothing was analysed, or (None, redone, None) where encode_audio gave no audio."""
+    with ThreadPoolExecutor(max_workers=1) as pool:
+        gain = pool.submit(analyse) if analyse is not None else None
+        try:
+            audio, redone = encode_audio()
+        finally:
+            title_db = gain.result() if gain is not None else None     # joins the thread; re-raises its error
+    if audio is None:
+        return None, redone, None
+    buf = torch.zeros(room + len(audio), dtype=torch.uint8, device=file_device)
+    if audio:
+        buf[room:] = torch.frombuffer(bytearray(audio), dtype=torch.uint8).to(file_device)
+    n = finish(buf, title_db)
+    return buf[:n].cpu().numpy().tobytes(), redone, title_db
+
+
+def encode_segments_tagged_local(make_encoder, left, right, framesize, nseg, warmup, room, analyse, finish, file_device="cpu"):
+    """encode_stream_segments_local made into a finished file by _finished (its arguments: room, analyse, finish)"""
+    return _finished(lambda: encode_stream_segments_local(make_encoder, left, right, framesize, nseg, warmup), room, analyse,
+                     finish, file_device)
+
+
+def encode_segments_tagged(make_encoder, left, right, framesize, room, analyse, finish, warmup=8, group=None, device="cpu",
+                           file_device="cpu"):
+    """encode_stream_segments made into a finished file on rank 0 by _finished; only rank 0 runs `analyse`"""
+    rank = dist.get_rank(group)
+    return _finished(lambda: encode_stream_segments(make_encoder, left, right, framesize, warmup, group, device), room,
+                     analyse if rank == 0 else None, finish, file_device)
+
+
+def _library_parts(channels, samplerate, kbps, left, right, find_replay_gain):
+    """the libmp3b200 pieces of a segmented finished file: (make_encoder, framesize, room, analyse, finish, file_device)"""
+    from . import encoder as E
+    if E.out_samplerate(channels, samplerate, kbps) != samplerate:
+        raise ValueError("(%d, %d, %d) is resampled by lamejs: a resampled stream cannot be cut into segments (seek does not "
+                         "take resampling encoders)" % (channels, samplerate, kbps))
+    gr = E.granules_per_frame(channels, samplerate, kbps)
+    if gr < 0:
+        raise E.Mp3B200Error("unsupported configuration: channels=%d samplerate=%d kbps=%d" % (channels, samplerate, kbps))
+    right = None if channels == 1 else right
+    probe = E.Mp3Encoder(channels, samplerate, kbps)
+    device = probe.device                                   # the library's device: where the encoders and the file live
+    probe.close()
+    room = E.lametag_size(channels, samplerate, kbps)
+    n = len(left)
+
+    def analyse():
+        if E._on_cuda(left) or E._on_cuda(right):
+            (l,), (r,), f32 = E._device_rows([left], [right], device)
+            pcm = l if channels == 1 else torch.cat([l, r])
+            return E.replay_gain_streams_device(channels, samplerate, kbps, pcm.data_ptr(), [0], [n], float32=f32)[0][0]
+        return E.replay_gain_streams(channels, samplerate, kbps, [left], None if right is None else [right])[0][0]
+
+    def finish(buf, title_db):
+        return E.finish_tags_device(channels, samplerate, kbps, buf.data_ptr(), [0], [n],
+                                    None if title_db is None else [title_db])[0]
+
+    # lamejs analyses only when the tag is written (Lame.js:911-916)
+    return (lambda: E.Mp3Encoder(channels, samplerate, kbps), 576 * gr, room, analyse if find_replay_gain and room > 0 else None,
+            finish, "cuda:%d" % device)
+
+
+def _title(title_db):
+    from .encoder import GAIN_NOT_ENOUGH_SAMPLES
+    return float(GAIN_NOT_ENOUGH_SAMPLES) if title_db is None else title_db
+
+
+def encode_stream_segments_tagged_local(channels, samplerate, kbps, left, right, nseg, warmup=8, find_replay_gain=False):
+    """One stream cut into `nseg` frame ranges, encoded one after another in this process, as one finished file: returns (file
+    bytes, ranges re-encoded, title_db), the file byte-identical to encode_streams_replaygain([left], [right],
+    find_replay_gain=...)[0][0] and title_db to its title gain (-24601 when nothing was analysed).  Int16 or floating-point
+    rows, in host memory or CUDA tensors on the library's device; configurations lamejs resamples raise ValueError."""
+    make, fs, room, analyse, finish, file_device = _library_parts(channels, samplerate, kbps, left, right, find_replay_gain)
+    out, redone, title_db = encode_segments_tagged_local(make, left, None if channels == 1 else right, fs, nseg, warmup, room,
+                                                         analyse, finish, file_device)
+    return out, redone, _title(title_db)
+
+
+def encode_stream_segments_tagged(channels, samplerate, kbps, left, right, warmup=8, find_replay_gain=False, group=None,
+                                  device="cpu"):
+    """encode_stream_segments_tagged_local over the ranks of `group` (one range each; `device` is the collectives' device, as
+    for encode_stream_segments): returns the same on rank 0, (None, ranges re-encoded, None) elsewhere.  Rank 0 analyses
+    the whole stream beside its own range and finishes the file on the library's device."""
+    make, fs, room, analyse, finish, file_device = _library_parts(channels, samplerate, kbps, left, right, find_replay_gain)
+    out, redone, title_db = encode_segments_tagged(make, left, None if channels == 1 else right, fs, room, analyse, finish,
+                                                   warmup, group, device, file_device)
+    return (None, redone, None) if out is None else (out, redone, _title(title_db))
