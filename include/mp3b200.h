@@ -405,7 +405,11 @@ int mp3b200_debug_stages(int channels, int samplerate, int kbps, const int16_t* 
  * `flags` selects the configuration like the _ex entry points (mp3b200_debug_stages: 0).  With MP3B200_RESAMPLE a
  * configuration lamejs resamples is tapped after k_resample: left / right / nsamples are input samples, and every shape above
  * is that of the output rate ([F] = mp3b200_stream_frames_ex(..., flags, nsamples), [G] = mp3b200_granules_per_frame_ex).
- * Any output pointer may be NULL. */
+ * Any output pointer may be NULL.
+ * The encoder computes the short-block half of the psy model (en_s / thm_s) only for the units whose masking a short
+ * granule reads, and for each stream's last unit (DESIGN.md 2); the taps compute it for every unit, unless `flags` holds
+ * MP3B200_DEBUG_SKIP_SHORT: then en_s / thm_s are defined for those units only, as in an encode. */
+#define MP3B200_DEBUG_SKIP_SHORT 0x10000
 typedef struct mp3b200_debug_taps {
   int32_t size, channels, samplerate, kbps;
   const int16_t *left, *right;
@@ -418,6 +422,9 @@ typedef struct mp3b200_debug_taps {
   int32_t flags;
 } mp3b200_debug_taps;
 int mp3b200_debug_stages_ex(const mp3b200_debug_taps* t);
+/* (unit, channel) pairs the calling thread's last launch ran the short-block psy half for (halo units included); -1 before
+ * its first launch */
+int64_t mp3b200_debug_short_units(void);
 
 /* Test tap of k_resample: y[c * ny + m], m < ny, = output m of channel c (nch rows) of the resampler of a configuration that
  * MP3B200_RESAMPLE accepts with resampling, for the input left / right (nsamples each; right NULL: left) extended with zeros

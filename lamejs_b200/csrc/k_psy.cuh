@@ -7,13 +7,16 @@
  *
  * lamejs runs one psy call per granule ("unit" c, analysing stream samples [576c-224, 576c+800)) and carries
  * state from call to call.  Here the work is split by what it depends on:
- *   k_psy_analysis   pure function of PCM: fs/4 HPF + 9 sub-block peaks, 1024-pt and 3x256-pt FHT, line
- *                    energies, partition energies / tonality index, short-block spreading sums
+ *   k_psy_analysis   pure function of PCM, every unit: fs/4 HPF + 9 sub-block peaks, 1024-pt FHT, line energies,
+ *                    long partition energies / tonality index
  *                    (and the ordered 512-term loudness sum, psycho_loudness_approx: terms in parallel, additions on one thread)
  *   k_attack_prepass pure function of two consecutive units: attack candidates (before the lastAttacks FSM)
  *   k_stream_scan    the only sequential part: per stream, the attack / block-type FSM and the ATH-adjust IIR
+ *   k_psy_short_list after the scan: the units whose short-block half is read (psy_short_read, DESIGN.md 2)
+ *   k_psy_short      pure function of PCM, listed units only: 3x256-pt FHT, short partition energies, short spreading sums
  *   k_psy_masking    long-block spreading with mask_add (needs ATH.adjust), short thresholds (need the previous
- *                    block type), partition -> scalefactor-band conversion, inter-channel masking
+ *                    block type; units whose short half is read only), partition -> scalefactor-band conversion,
+ *                    inter-channel masking
  * With the reservoir disabled pcfact == 0 (PsyModel.js:1036-1038), so every NS_INTERP pre-echo branch returns
  * its second argument and nb_1/nb_2 are never read; PE (pecalc_*) feeds only dead values (SURVEY.md 7.6).
  */
@@ -28,9 +31,8 @@
 #endif
 #define MASK_THREADS 128
 
+/* long half of a psy unit, written for every unit */
 struct PsyUnit {
-  double ecb_s[3][MP3_CBANDS];      /* short-block spreading sums (double; float32 of it is lamejs nb_s1) */
-  float eb_s[3][MP3_CBANDS];
   float eb_l[MP3_CBANDS];
   float peaks[9];                   /* en_subshort[3..11] */
   float loudness;                   /* psycho_loudness_approx */
@@ -38,6 +40,12 @@ struct PsyUnit {
   unsigned char attack[4];          /* pre-FSM ns_attacks[0..3] */
   unsigned char pad_;
 };
+/* short half, a separate array: written by k_psy_short for the units on the short list only; the other rows are stale */
+struct PsyShort {
+  double ecb_s[3][MP3_CBANDS];      /* short-block spreading sums (double; float32 of it is lamejs nb_s1) */
+  float eb_s[3][MP3_CBANDS];
+};
+/* en_s / thm_s are written only for the units whose short half is read (psy_short_read); elsewhere they are stale */
 struct PsyRatioDev { float en_l[22], thm_l[22], en_s[13][3], thm_s[13][3]; };
 
 __constant__ unsigned char c_fft_rv[128];
@@ -160,6 +168,31 @@ __device__ __forceinline__ void fht_task(f32w* fz, int stage, int task, const do
 /* psy row of (stream z, relative unit u >= -1): unit_base + z + u + 1 */
 __device__ __forceinline__ size_t psy_row(const StreamDesc& sd, int z, int u) { return (size_t)sd.unit_base + z + u + 1; }
 
+/* the unit's PCM span [x0, x0 + 1024) widened to double (zero outside the stream), all of a thread's loads in flight at once
+ * (they were one dependent HBM round trip per iteration) */
+template <bool F32_PCM, int NT>
+__device__ __forceinline__ void psy_load_span(const Mp3Tables* __restrict__ T, const StreamDesc& sd, int ch, long long x0, double* xs) {
+  using Sample = pcm_sample_t<F32_PCM>;
+  const int tid = threadIdx.x;
+  const int scale_applied = T->scale_applied;
+  const double scale = T->scale;
+  const Sample* __restrict__ pbuf = static_cast<const Sample*>(sd.pcm[ch]);
+  const long long pbase = sd.pcm_base, pend = sd.pcm_end;
+  constexpr int NB = (1024 + NT - 1) / NT;
+  Sample v[NB];
+#pragma unroll
+  for (int k = 0; k < NB; k++) {
+    const int j = tid + k * NT;
+    const long long i = x0 + j;
+    v[k] = (j < 1024 && i >= 0 && i < pend) ? __ldg(&pbuf[i - pbase]) : (Sample)0;
+  }
+#pragma unroll
+  for (int k = 0; k < NB; k++) {
+    const int j = tid + k * NT;
+    if (j < 1024) xs[j] = pcm_value(v[k], scale_applied, scale);
+  }
+}
+
 /* grid (max_units + 1, nch, nstreams).  F32_PCM: sd.pcm[ch] points at Float32 samples already at the encoding rate and
  * scaled (the resampler's output, k_resample) instead of Int16 input. */
 #ifndef PSY_MIN_BLOCKS
@@ -190,7 +223,6 @@ k_psy_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ s
   const int tid = threadIdx.x;
 
   if (c < 0) {   /* before the first call: psymodel_init values (PsyModel.js:2573-2595) */
-    for (int i = tid; i < 3 * MP3_CBANDS; i += PSY_THREADS) { (&o->ecb_s[0][0])[i] = 1.0; (&o->eb_s[0][0])[i] = 0.0f; }
     if (tid < MP3_CBANDS) { o->eb_l[tid] = 0.0f; o->mask_idx[tid] = 0; }
     if (tid < 9) o->peaks[tid] = 10.0f;
     if (tid == 0) o->loudness = 0.0f;
@@ -203,49 +235,24 @@ k_psy_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ s
   __shared__ __align__(16) unsigned char s_u[sizeof(double) * 1024];
   double* const xs = reinterpret_cast<double*>(s_u);
   f32s* const fe = reinterpret_cast<f32s*>(s_u);                                  /* [513] */
-  f32s (*const fes)[129] = reinterpret_cast<f32s (*)[129]>(s_u + 2064);           /* [3][129] */
-  f32s* const s_max = reinterpret_cast<f32s*>(s_u + 2064 + 1552);                 /* [64] */
+  f32s* const s_max = reinterpret_cast<f32s*>(s_u + 2064);                        /* [64] */
   f32s* const s_avg = s_max + MP3_CBANDS;                                         /* [64] */
-  f32s (*const s_ebs)[MP3_CBANDS] = reinterpret_cast<f32s (*)[MP3_CBANDS]>(s_avg + MP3_CBANDS);   /* [3][64] */
-  static_assert(2064 + 1552 + 2 * 4 * MP3_CBANDS + 3 * 4 * MP3_CBANDS <= (int)sizeof(s_u), "energies must fit the PCM span");
   /* psycho_loudness_approx (PsyModel.js:241-249) is ONE ordered 512-term double sum per unit.  Its terms energy[i] * eql_w[i]
    * are computed by the threads that produce the energies (double products, 2 x 256 of them parked in shared memory that is
    * dead by then: the high-pass output and the tail of the PCM span); the thread that owns no partition then only walks the
    * additions -- an 8-cycle step instead of the 60-cycle load / convert / multiply / add step that stalled the block when
    * the whole sum sat on one thread (measured slower) -- half in each of the two partition phases. */
-  constexpr int PROD_HI_OFF = 2064 + 1552 + 2 * 4 * MP3_CBANDS + 3 * 4 * MP3_CBANDS;
+  constexpr int PROD_HI_OFF = 2064 + 2 * 4 * MP3_CBANDS;
   static_assert(PROD_HI_OFF % 8 == 0 && PROD_HI_OFF + 256 * 8 <= (int)sizeof(s_u), "second half of the loudness terms");
   double* const prod_hi = reinterpret_cast<double*>(s_u + PROD_HI_OFF);                /* terms 256..511 */
   __shared__ f32w wl[1024 + 64];
-  __shared__ f32w wsh[3][256 + 16];
   __shared__ __align__(8) f32s hp[576];
   double* const prod_lo = reinterpret_cast<double*>(hp);                               /* terms 0..255 (hp is dead by then) */
   static_assert(sizeof(f32s) * 576 >= 256 * 8, "first half of the loudness terms");
   __shared__ int s_peak[9];
   if (tid < 9) s_peak[tid] = __float_as_int(1.0f);
 
-  const int scale_applied = T->scale_applied;
-  const double scale = T->scale;
-  const long long x0 = 576 * c - 224;                /* stream sample of bufPos */
-  {
-    /* all of a thread's loads in flight at once (they were one dependent HBM round trip per iteration) */
-    using Sample = pcm_sample_t<F32_PCM>;
-    const Sample* __restrict__ pbuf = static_cast<const Sample*>(sd.pcm[ch]);
-    const long long pbase = sd.pcm_base, pend = sd.pcm_end;
-    constexpr int NB = (1024 + PSY_THREADS - 1) / PSY_THREADS;
-    Sample v[NB];
-#pragma unroll
-    for (int k = 0; k < NB; k++) {
-      const int j = tid + k * PSY_THREADS;
-      const long long i = x0 + j;
-      v[k] = (j < 1024 && i >= 0 && i < pend) ? __ldg(&pbuf[i - pbase]) : (Sample)0;
-    }
-#pragma unroll
-    for (int k = 0; k < NB; k++) {
-      const int j = tid + k * PSY_THREADS;
-      if (j < 1024) xs[j] = pcm_value(v[k], scale_applied, scale);
-    }
-  }
+  psy_load_span<F32_PCM, PSY_THREADS>(T, sd, ch, 576 * c - 224, xs);
   __syncthreads();
 
   /* fs/4 high-pass (PsyModel.js:1051-1069): firbuf index = bufPos + 397 + i + j */
@@ -260,9 +267,8 @@ k_psy_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ s
     hp[i] = sum1 + sum2;
   }
   /* windowing + first radix-4 pass of fft_long (FFT.js:185-224): iteration jj writes y[4jj..4jj+3], y[512+4jj..] */
-  for (int vt = tid; vt < 128 + 96; vt += PSY_THREADS) {
-  if (vt < 128) {
-    const int jj = vt, i = c_fft_rv[jj], x = 4 * jj;
+  for (int jj = tid; jj < 128; jj += PSY_THREADS) {
+    const int i = c_fft_rv[jj], x = 4 * jj;
     const float* w = T->fft_window;
     double f0, f1, f2, f3, wv;
     f0 = (double)w[i] * (double)xs[i];
@@ -279,43 +285,17 @@ k_psy_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ s
     wv = (double)w[i + 0x301] * (double)xs[i + 0x301];
     f3 = f2 - wv; f2 = f2 + wv;
     wl[FHT_PAD(x + 512 + 0)] = f0 + f2; wl[FHT_PAD(x + 512 + 2)] = f0 - f2; wl[FHT_PAD(x + 512 + 1)] = f1 + f3; wl[FHT_PAD(x + 512 + 3)] = f1 - f3;
-  } else {
-    /* fft_short (FFT.js:140-183): block b, iteration j writes x_real[b][4j..], [128+4j..] */
-    const int q = vt - 128, b = q >> 5, j = q & 31;
-    const int i = c_fft_rv[j << 2], x = 4 * j, k = 192 * (b + 1);
-    const float* w = T->fft_window_s;
-    const double* bx = xs + i + k;
-    double f0, f1, f2, f3, wv;
-    f0 = (double)w[i] * (double)bx[0];
-    wv = (double)w[0x7f - i] * (double)bx[0x80];
-    f1 = f0 - wv; f0 = f0 + wv;
-    f2 = (double)w[i + 0x40] * (double)bx[0x40];
-    wv = (double)w[0x3f - i] * (double)bx[0xc0];
-    f3 = f2 - wv; f2 = f2 + wv;
-    wsh[b][FHT_PAD(x + 0)] = f0 + f2; wsh[b][FHT_PAD(x + 2)] = f0 - f2; wsh[b][FHT_PAD(x + 1)] = f1 + f3; wsh[b][FHT_PAD(x + 3)] = f1 - f3;
-    f0 = (double)w[i + 0x01] * (double)bx[0x01];
-    wv = (double)w[0x7e - i] * (double)bx[0x81];
-    f1 = f0 - wv; f0 = f0 + wv;
-    f2 = (double)w[i + 0x41] * (double)bx[0x41];
-    wv = (double)w[0x3e - i] * (double)bx[0xc1];
-    f3 = f2 - wv; f2 = f2 + wv;
-    wsh[b][FHT_PAD(x + 128 + 0)] = f0 + f2; wsh[b][FHT_PAD(x + 128 + 2)] = f0 - f2; wsh[b][FHT_PAD(x + 128 + 1)] = f1 + f3; wsh[b][FHT_PAD(x + 128 + 3)] = f1 - f3;
-  }
   }
   __syncthreads();
 
   /* 9 sub-block peaks of the high-passed signal (PsyModel.js:1125-1132): max(1, |hp|) over 64 samples each; the
    * values are non-negative float32, whose order is the order of their bit patterns */
   for (int i = tid; i < 576; i += PSY_THREADS) atomicMax(&s_peak[i >> 6], __float_as_int(fabsf(hp[i].v)));
-  /* FHT stages: 128 tasks per stage for the long transform (4 stages), 32 for each short one (3 stages); task numbers map to
-   * butterflies by shifts (the earlier enumeration needed integer divisions: 16 % of this kernel's instructions) */
+  /* FHT stages: 128 tasks per stage (task numbers map to butterflies by shifts: the earlier enumeration needed integer
+   * divisions, 16 % of this kernel's instructions) */
 #pragma unroll
   for (int stage = 0; stage < 4; stage++) {
-    const int nt = 128 + (stage < 3 ? 96 : 0);
-    for (int t = tid; t < nt; t += PSY_THREADS) {
-      if (t < 128) fht_task(wl, stage, t, T->tw, T->tw_off);
-      else fht_task(wsh[(t - 128) >> 5], stage, (t - 128) & 31, T->tw, T->tw_off);
-    }
+    for (int t = tid; t < 128; t += PSY_THREADS) fht_task(wl, stage, t, T->tw, T->tw_off);
     __syncthreads();
   }
 
@@ -328,33 +308,16 @@ k_psy_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ s
     if (k < 512) { const double p = (double)e * (double)T->eql_w[k]; if (k < 256) prod_lo[k] = p; else prod_hi[k - 256] = p; }
   }
   if (tid == 0) { f32s t0; t0 = (double)wl[0]; t0 *= (double)t0; fe[0] = (double)t0; prod_lo[0] = (double)t0 * (double)T->eql_w[0]; }
-  for (int t = tid; t < 3 * 128; t += PSY_THREADS) {
-    const int b = t >> 7, j = t & 127;
-    const double re = wsh[b][FHT_PAD(128 - j)], im = wsh[b][FHT_PAD(128 + j)];
-    fes[b][128 - j] = (re * re + im * im) * 0.5;
-  }
-  if (tid < 3) { f32s t0; t0 = (double)wsh[tid][0]; t0 *= (double)t0; fes[tid][0] = (double)t0; }
   __syncthreads();
 
-  const int npl = T->npart_l, nps = T->npart_s;
-  for (int vt = tid; vt < 256; vt += PSY_THREADS) {
-  if (vt < npl) {                                    /* calc_energy (PsyModel.js:906-928) */
+  const int npl = T->npart_l;
+  for (int b = tid; b < npl; b += PSY_THREADS) {     /* calc_energy (PsyModel.js:906-928) */
     double ebb = 0, m = 0;
-    const int l0 = T->line0_l[vt], l1 = T->line0_l[vt + 1];
+    const int l0 = T->line0_l[b], l1 = T->line0_l[b + 1];
     for (int j = l0; j < l1; j++) { const double el = fe[j]; ebb += el; if (m < el) m = el; }
-    o->eb_l[vt] = (float)ebb;
-    s_max[vt] = m;
-    s_avg[vt] = ebb * (double)T->rnumlines_l[vt];
-  } else if (vt >= 64 && vt < 64 + 3 * 64) {         /* short partition energies (compute_masking_s :740-750) */
-    const int q = vt - 64, sb = q >> 6, b = q & 63;
-    if (b < nps) {
-      double ebb = 0;
-      const int l0 = T->line0_s[b], l1 = T->line0_s[b + 1];
-      for (int j = l0; j < l1; j++) ebb += (double)fes[sb][j];
-      s_ebs[sb][b] = ebb;
-      o->eb_s[sb][b] = (float)ebb;
-    }
-  }
+    o->eb_l[b] = (float)ebb;
+    s_max[b] = m;
+    s_avg[b] = ebb * (double)T->rnumlines_l[b];
   }
   double loud = 0.0;
   if (tid == PSY_THREADS - 1) {
@@ -364,9 +327,7 @@ k_psy_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ s
   if (tid < 9) o->peaks[tid] = __int_as_float(s_peak[tid]);
   __syncthreads();
 
-  for (int vt = tid; vt < 256; vt += PSY_THREADS) {
-  if (vt < npl) {                                    /* calc_mask_index_l (PsyModel.js:930-992) */
-    const int b = vt;
+  for (int b = tid; b < npl; b += PSY_THREADS) {     /* calc_mask_index_l (PsyModel.js:930-992) */
     const int lo = b > 0 ? b - 1 : b, hi = b < npl - 1 ? b + 1 : b;
     double a = 0; double m = 0; int lines = 0;
     for (int q = lo; q <= hi; q++) {
@@ -382,23 +343,142 @@ k_psy_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ s
       if (k > 8) k = 8;
     }
     o->mask_idx[b] = (unsigned char)k;
-  } else if (vt >= 64 && vt < 64 + 3 * 64) {         /* short spreading sums (compute_masking_s :753-761) */
-    const int q = vt - 64, sb = q >> 6, b = q & 63;
-    if (b < nps) {
-      int kk = T->s3lo_s[b];
-      int j = T->s3off_s[b];
-      double ecb = (double)T->s3_ss[j++] * (double)s_ebs[sb][kk];
-      ++kk;
-      while (kk <= T->s3hi_s[b]) { ecb += (double)T->s3_ss[j] * (double)s_ebs[sb][kk]; ++j; ++kk; }
-      o->ecb_s[sb][b] = ecb;
-    }
-  }
   }
   if (tid == PSY_THREADS - 1) {
 #pragma unroll 8
     for (int i = 0; i < 256; ++i) loud += prod_hi[i];
     loud *= (1. / (14752. * 14752.) / 512);
     o->loudness = (float)loud;
+  }
+}
+
+/* ---- the short-block half (PsyModel.js:1000-1383 for shortblock, compute_masking_s :740-761) --------------------------
+ * Read only for granules encoded as short blocks and their neighbours (psy_short_read): computed after the block-type scan
+ * for a compacted list of (unit, channel) pairs. */
+
+/* R(u): the ratio row of unit u (relative, of stream sd) needs en_s / thm_s.  The quantizer of granule u + 1 reads it
+ * (calc_xmin's short branch) when either channel of that granule is a short block (per unit: inter-channel masking mixes
+ * both channels' thm_s); a stream's last unit is always complete, as its row is carried to the next call (halo_out) and
+ * into state blobs.  The halo row (u = -1) is never computed by the masking.  all: every unit (the stage taps). */
+__device__ __forceinline__ bool psy_short_read(const Mp3Tables* __restrict__ T, const StreamDesc& sd,
+                                               const signed char* __restrict__ bt_final, int u, int all) {
+  const int n = T->mode_gr * sd.nframes;
+  if (u < 0 || u >= n) return false;
+  if (all || u == n - 1) return true;
+  const size_t row = (size_t)(sd.unit_base + u + 1) * 2;
+  return bt_final[row] == BT_SHORT || (T->nch == 2 && bt_final[row + 1] == BT_SHORT);
+}
+
+/* grid ((max_units + 1 + 127) / 128, nstreams) x 128.  Appends (stream, unit, channel) for every unit u >= -1 with
+ * S(u) = R(u) || R(u + 1) (the thresholds of unit u + 1 read ecb_s of unit u: nb_s1 / nb_s2) to list; count[0] is its
+ * length and count[1] k_psy_short's task counter, both zero on entry. */
+__global__ void __launch_bounds__(128)
+k_psy_short_list(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ streams, const signed char* __restrict__ bt_final,
+                 int all, int2* __restrict__ list, int* __restrict__ count) {
+  const int z = blockIdx.y;
+  const StreamDesc& sd = streams[z];
+  const int u = (int)(blockIdx.x * blockDim.x + threadIdx.x) - 1;
+  if (u >= T->mode_gr * sd.nframes) return;
+  if (!psy_short_read(T, sd, bt_final, u, all) && !psy_short_read(T, sd, bt_final, u + 1, all)) return;
+  const int nch = T->nch;
+  const int at = atomicAdd(count, nch);
+  for (int ch = 0; ch < nch; ch++) list[at + ch] = make_int2(z, ((u + 1) << 1) | ch);
+}
+
+/* persistent blocks of PSY_THREADS pulling (stream, unit, channel) tasks from the list k_psy_short_list built */
+#ifndef PSY_SHORT_BLOCKS
+#define PSY_SHORT_BLOCKS 8    /* resident blocks per SM */
+#endif
+template <bool F32_PCM>
+__global__ void __launch_bounds__(PSY_THREADS)
+k_psy_short(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ streams, PsyShort* __restrict__ out,
+            const int2* __restrict__ list, int* __restrict__ count) {
+  const int ntasks = count[0];
+  if (ntasks == 0) return;
+  const int tid = threadIdx.x;
+  const int nch = T->nch, nps = T->npart_s;
+  __shared__ double xs[1024];
+  __shared__ f32w wsh[3][256 + 16];
+  __shared__ f32s fes[3][129];
+  __shared__ f32s s_ebs[3][MP3_CBANDS];
+  __shared__ int s_task;
+  for (;;) {
+    if (tid == 0) s_task = atomicAdd(count + 1, 1);
+    __syncthreads();
+    const int t = s_task;
+    if (t >= ntasks) return;
+    const int2 e = list[t];
+    const int z = e.x, u = (e.y >> 1) - 1, ch = e.y & 1;
+    const StreamDesc& sd = streams[z];
+    const long long c = (long long)T->mode_gr * sd.frame0 + u;
+    PsyShort* o = out + psy_row(sd, z, u) * nch + ch;
+    if (c < 0) {   /* before the first call: psymodel_init values (PsyModel.js:2573-2595) */
+      for (int i = tid; i < 3 * MP3_CBANDS; i += PSY_THREADS) { (&o->ecb_s[0][0])[i] = 1.0; (&o->eb_s[0][0])[i] = 0.0f; }
+      __syncthreads();
+      continue;
+    }
+    psy_load_span<F32_PCM, PSY_THREADS>(T, sd, ch, 576 * c - 224, xs);
+    __syncthreads();
+    /* fft_short (FFT.js:140-183): block b, iteration j writes x_real[b][4j..], [128+4j..] */
+    for (int q = tid; q < 96; q += PSY_THREADS) {
+      const int b = q >> 5, j = q & 31;
+      const int i = c_fft_rv[j << 2], x = 4 * j, k = 192 * (b + 1);
+      const float* w = T->fft_window_s;
+      const double* bx = xs + i + k;
+      double f0, f1, f2, f3, wv;
+      f0 = (double)w[i] * (double)bx[0];
+      wv = (double)w[0x7f - i] * (double)bx[0x80];
+      f1 = f0 - wv; f0 = f0 + wv;
+      f2 = (double)w[i + 0x40] * (double)bx[0x40];
+      wv = (double)w[0x3f - i] * (double)bx[0xc0];
+      f3 = f2 - wv; f2 = f2 + wv;
+      wsh[b][FHT_PAD(x + 0)] = f0 + f2; wsh[b][FHT_PAD(x + 2)] = f0 - f2; wsh[b][FHT_PAD(x + 1)] = f1 + f3; wsh[b][FHT_PAD(x + 3)] = f1 - f3;
+      f0 = (double)w[i + 0x01] * (double)bx[0x01];
+      wv = (double)w[0x7e - i] * (double)bx[0x81];
+      f1 = f0 - wv; f0 = f0 + wv;
+      f2 = (double)w[i + 0x41] * (double)bx[0x41];
+      wv = (double)w[0x3e - i] * (double)bx[0xc1];
+      f3 = f2 - wv; f2 = f2 + wv;
+      wsh[b][FHT_PAD(x + 128 + 0)] = f0 + f2; wsh[b][FHT_PAD(x + 128 + 2)] = f0 - f2; wsh[b][FHT_PAD(x + 128 + 1)] = f1 + f3; wsh[b][FHT_PAD(x + 128 + 3)] = f1 - f3;
+    }
+    __syncthreads();
+    /* FHT stages 0..2: 32 tasks per stage for each of the three transforms */
+#pragma unroll
+    for (int stage = 0; stage < 3; stage++) {
+      for (int q = tid; q < 96; q += PSY_THREADS) fht_task(wsh[q >> 5], stage, q & 31, T->tw, T->tw_off);
+      __syncthreads();
+    }
+    /* line energies (PsyModel.js:300-316) */
+    for (int q = tid; q < 3 * 128; q += PSY_THREADS) {
+      const int b = q >> 7, j = q & 127;
+      const double re = wsh[b][FHT_PAD(128 - j)], im = wsh[b][FHT_PAD(128 + j)];
+      fes[b][128 - j] = (re * re + im * im) * 0.5;
+    }
+    if (tid < 3) { f32s t0; t0 = (double)wsh[tid][0]; t0 *= (double)t0; fes[tid][0] = (double)t0; }
+    __syncthreads();
+    for (int q = tid; q < 3 * MP3_CBANDS; q += PSY_THREADS) {   /* short partition energies (compute_masking_s :740-750) */
+      const int sb = q >> 6, b = q & 63;
+      if (b < nps) {
+        double ebb = 0;
+        const int l0 = T->line0_s[b], l1 = T->line0_s[b + 1];
+        for (int j = l0; j < l1; j++) ebb += (double)fes[sb][j];
+        s_ebs[sb][b] = ebb;
+        o->eb_s[sb][b] = (float)ebb;
+      }
+    }
+    __syncthreads();
+    for (int q = tid; q < 3 * MP3_CBANDS; q += PSY_THREADS) {   /* short spreading sums (compute_masking_s :753-761) */
+      const int sb = q >> 6, b = q & 63;
+      if (b < nps) {
+        int kk = T->s3lo_s[b];
+        int j = T->s3off_s[b];
+        double ecb = (double)T->s3_ss[j++] * (double)s_ebs[sb][kk];
+        ++kk;
+        while (kk <= T->s3hi_s[b]) { ecb += (double)T->s3_ss[j] * (double)s_ebs[sb][kk]; ++j; ++kk; }
+        o->ecb_s[sb][b] = ecb;
+      }
+    }
+    __syncthreads();   /* s_task, xs and the work arrays are reused by the next task */
   }
 }
 
@@ -648,10 +728,12 @@ __device__ __forceinline__ double mask_add_dev(double m1, double m2, int kk, int
   return m1 * c_table1[i];
 }
 
-/* grid (max_units + 1, 1, nstreams); threads: 64 per channel */
+/* grid (max_units + 1, 1, nstreams); threads: 64 per channel.  The short half (thresholds, conversion, pre-echo factor,
+ * inter-channel masking) only where psy_short_read holds. */
 __global__ void __launch_bounds__(MASK_THREADS)
 k_psy_masking(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ streams, const PsyUnit* __restrict__ psy,
-              const signed char* __restrict__ bt_prev, const double* __restrict__ ath_psy, PsyRatioDev* __restrict__ ratio) {
+              const PsyShort* __restrict__ psy_s, const signed char* __restrict__ bt_prev, const signed char* __restrict__ bt_final,
+              int all_short, const double* __restrict__ ath_psy, PsyRatioDev* __restrict__ ratio) {
   const int z = blockIdx.z;
   const StreamDesc& sd = streams[z];
   const int u = (int)blockIdx.x - 1;
@@ -676,7 +758,9 @@ k_psy_masking(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ st
   const int npl = T->npart_l, nps = T->npart_s;
   /* (staging these rows in shared memory was measured slower: the extra barrier costs more than the L1 hits) */
   const PsyUnit* pu = (ch < nch) ? psy + psy_row(sd, z, u) * nch + ch : nullptr;
-  const PsyUnit* pp = (ch < nch) ? psy + psy_row(sd, z, u - 1) * nch + ch : nullptr;
+  const PsyShort* ps = (ch < nch) ? psy_s + psy_row(sd, z, u) * nch + ch : nullptr;
+  const PsyShort* pp = (ch < nch) ? psy_s + psy_row(sd, z, u - 1) * nch + ch : nullptr;
+  const bool short_read = psy_short_read(T, sd, bt_final, u, all_short);
   const double ath_adjust = ath_psy[sd.frame_base + u / T->mode_gr];
 
   if (ch < nch) {
@@ -696,11 +780,11 @@ k_psy_masking(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ st
     } else { s_thr[ch][b] = 0.0; s_eb[ch][b] = 0.0; }
     /* short-block thresholds (compute_masking_s :753-777); nb_s1/nb_s2 = float32 ecb of the two previous sub-blocks */
     const int prev_short = bt_prev[(size_t)(sd.unit_base + u) * 2 + ch] == BT_SHORT;
-    for (int sb = 0; sb < 3; sb++) {
+    for (int sb = 0; short_read && sb < 3; sb++) {
       if (b < nps) {
-        const double ecb = pu->ecb_s[sb][b];
-        const float nb1 = sb >= 1 ? (float)pu->ecb_s[sb - 1][b] : (float)pp->ecb_s[2][b];
-        const float nb2 = sb == 2 ? (float)pu->ecb_s[0][b] : (sb == 1 ? (float)pp->ecb_s[2][b] : (float)pp->ecb_s[1][b]);
+        const double ecb = ps->ecb_s[sb][b];
+        const float nb1 = sb >= 1 ? (float)ps->ecb_s[sb - 1][b] : (float)pp->ecb_s[2][b];
+        const float nb2 = sb == 2 ? (float)ps->ecb_s[0][b] : (sb == 1 ? (float)pp->ecb_s[2][b] : (float)pp->ecb_s[1][b]);
         f32s t;
         t = js_dmin(ecb, 2 * (double)nb1);
         if (prev_short) { const double x = 16 * (double)nb2, y = (double)t; t = js_dmin(x, y); }
@@ -735,7 +819,7 @@ k_psy_masking(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ st
         thm[sbi] += w_curr * (double)s_thr[ch][bd];
       }
     }
-  } else if (ch < nch && b >= 22 && b < 22 + 39) {
+  } else if (short_read && ch < nch && b >= 22 && b < 22 + 39) {
     const int q = b - 22, sbi = q / 3, sblock = q - 3 * sbi;
     f32s(*en)[3] = reinterpret_cast<f32s(*)[3]>(s_out[ch].en_s);
     f32s(*thm)[3] = reinterpret_cast<f32s(*)[3]>(s_out[ch].thm_s);
@@ -745,16 +829,16 @@ k_psy_masking(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ st
       double enn = 0.0, thmm = 0.0;
       if (init >= 0) {
         const double w_next = 1.0 - (double)T->bo_s_weight[sbi - 1];
-        enn = w_next * (double)pu->eb_s[sblock][init];
+        enn = w_next * (double)ps->eb_s[sblock][init];
         thmm = w_next * (double)s_thr_s[ch][sblock][init];
       }
       const int p1 = T->conv_s.end[sbi];
-      for (int p = T->conv_s.start[sbi]; p < p1; p++) { enn += (double)pu->eb_s[sblock][p]; thmm += (double)s_thr_s[ch][sblock][p]; }
+      for (int p = T->conv_s.start[sbi]; p < p1; p++) { enn += (double)ps->eb_s[sblock][p]; thmm += (double)s_thr_s[ch][sblock][p]; }
       en[sbi][sblock] = enn; thm[sbi][sblock] = thmm;
       const int bd = T->conv_s.bound[sbi];
       if (bd >= 0) {
         const double w_curr = (double)T->bo_s_weight[sbi];
-        en[sbi][sblock] += w_curr * (double)pu->eb_s[sblock][bd];
+        en[sbi][sblock] += w_curr * (double)ps->eb_s[sblock][bd];
         thm[sbi][sblock] += w_curr * (double)s_thr_s[ch][sblock][bd];
       }
     }
@@ -768,7 +852,7 @@ k_psy_masking(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ st
   }
   __syncthreads();
   /* inter-channel masking (PsyModel.js:525-543), stereo with interChRatio > 0 */
-  if (nch == 2 && T->interch_ratio > 0.0 && tid < 22 + 39) {
+  if (nch == 2 && T->interch_ratio > 0.0 && tid < (short_read ? 22 + 39 : 22)) {
     const double r = T->interch_ratio;
     f32s* t0 = reinterpret_cast<f32s*>(tid < 22 ? &s_out[0].thm_l[tid] : &s_out[0].thm_s[0][0] + (tid - 22));
     f32s* t1 = reinterpret_cast<f32s*>(tid < 22 ? &s_out[1].thm_l[tid] : &s_out[1].thm_s[0][0] + (tid - 22));
@@ -777,7 +861,8 @@ k_psy_masking(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ st
     *t1 += l * r;
   }
   __syncthreads();
-  for (int i = tid; i < nch * 122; i += MASK_THREADS) (&out[0].en_l[0])[i] = (&s_out[0].en_l[0])[i];
+  for (int i = tid; i < nch * 122; i += MASK_THREADS)
+    if (short_read || i % 122 < 44) (&out[0].en_l[0])[i] = (&s_out[0].en_l[0])[i];
   if (sd.halo_out && u == T->mode_gr * sd.nframes - 1)
     for (int i = tid; i < nch * 122; i += MASK_THREADS) sd.halo_out[i] = (&s_out[0].en_l[0])[i];
 }

@@ -222,6 +222,9 @@ struct Workspace {
   Buf<float> xr;                          /* [U][nch][576] */
   Buf<float> slab;                        /* [U + S][nch][18][32] subband samples (gfc.sb_sample), psy row numbering */
   Buf<PsyUnit> psy;                       /* [U + S][nch]  (one halo unit per stream in front) */
+  Buf<PsyShort> psy_s;                    /* [U + S][nch]  short half of the units on the short list, psy row numbering */
+  Buf<int2> short_list;                   /* [U + S][nch]  (stream, unit, channel) tasks of k_psy_short */
+  Buf<int> short_count;                   /* [2]: the short list's length, k_psy_short's task counter */
   Buf<ScanIn> scan_in;                    /* [U + S][nch] attack candidates + loudness for the scans */
   Buf<PsyRatioDev> ratio;                 /* [U + S][nch]  masking of unit c (used by granule c+1) */
   Buf<double> ath_psy;                    /* [F] ATH.adjust seen by the psy calls of the frame */
@@ -245,7 +248,8 @@ struct Workspace {
   int fit(int S, int nch, long long U, long long F) {
     const size_t gc = (size_t)U * nch, rows = (size_t)(U + S) * nch, f = (size_t)F + 1;
     const bool failed = streams.fit(S) || bt_final.fit((size_t)U * 2 + 16) || bt_prev.fit((size_t)U * 2 + 16) ||
-                        xr.fit(gc * 576) || slab.fit(rows * 576) || psy.fit(rows) || scan_in.fit(rows) || ratio.fit(rows) ||
+                        xr.fit(gc * 576) || slab.fit(rows * 576) || psy.fit(rows) || psy_s.fit(rows) || short_list.fit(rows) ||
+                        short_count.fit(2) || scan_in.fit(rows) || ratio.fit(rows) ||
                         ath_psy.fit(f) || ath_q.fit(f) || qstate.fit(f) || ginfo.fit(gc) || l3enc.fit(gc * 576) ||
                         xrq.fit(gc * 576) || xrpow.fit(gc * 576) || neg.fit(gc * 18) || prep.fit(gc) || dirty.fit(3 * f) ||
                         counter.fit(Q_NCOUNTERS) || scan.fit((size_t)(F / SCAN_FRAMES + S + 1));
@@ -258,7 +262,8 @@ struct Workspace {
            refusals.cap;
   }
   void release() {
-    streams.release(); bt_final.release(); bt_prev.release(); xr.release(); slab.release(); psy.release(); scan_in.release();
+    streams.release(); bt_final.release(); bt_prev.release(); xr.release(); slab.release(); psy.release(); psy_s.release(); short_list.release();
+    short_count.release(); scan_in.release();
     ratio.release(); ath_psy.release(); ath_q.release(); qstate.release(); ginfo.release(); l3enc.release(); xrq.release();
     xrpow.release(); neg.release(); prep.release(); dirty.release(); counter.release(); scan.release();
     rs_desc.release(); rs_y.release(); st_desc.release(); st_y.release(); refusals.release();
@@ -446,6 +451,7 @@ int check_refusals(ThreadCtx& c) {
 struct LaunchOpts {
   const int32_t* force_bt = nullptr;     /* debug: host [units][nch] block types overriding the psy model's decision */
   bool stop_after_mdct = false;          /* debug: no quantizer, no bytes */
+  bool all_short = false;                /* debug: the short-block psy half of every unit, as if each were read (stage taps) */
   const PcmArrival* arrival = nullptr;   /* PCM still landing on the upload stream */
   float* timings_ms = nullptr;           /* the 16 timing slots of include/mp3b200.h */
   bool sync = true;                      /* false: return with the work queued on the context's stream (no timings) */
@@ -619,10 +625,27 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, uint8_
     CK(cudaMemcpyAsync(ws.bt_final.p, bt.data(), bt.size(), cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));
   }
+  /* K2b: the short-block psy half of the units whose short thresholds are read, listed from the final block types (after
+   * force_bt); persistent blocks that leave at once when the list is empty */
+  {
+    CK(cudaMemsetAsync(ws.short_count.p, 0, 2 * sizeof(int), st));
+    dim3 grid((cfg->host.mode_gr * max_frames + 1 + 127) / 128, S);
+    k_psy_short_list<<<grid, 128, 0, st>>>(tab, ws.streams.p, ws.bt_final.p, o.all_short ? 1 : 0, ws.short_list.p, ws.short_count.p);
+    DBG("k_psy_short_list");
+    int sms = 132;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c.device));
+    const long long tasks = ((long long)cfg->host.mode_gr * total_frames + S) * nch;
+    const int blocks = (int)std::min<long long>(std::max<long long>(tasks, 1), (long long)sms * PSY_SHORT_BLOCKS);
+    if (f32_pcm) k_psy_short<true><<<blocks, PSY_THREADS, 0, st>>>(tab, ws.streams.p, ws.psy_s.p, ws.short_list.p, ws.short_count.p);
+    else k_psy_short<false><<<blocks, PSY_THREADS, 0, st>>>(tab, ws.streams.p, ws.psy_s.p, ws.short_list.p, ws.short_count.p);
+    g_launches += 2;
+    DBG("k_psy_short");
+  }
   /* K3b: masking thresholds */
   {
     dim3 grid(cfg->host.mode_gr * max_frames + 1, 1, S);
-    k_psy_masking<<<grid, MASK_THREADS, 0, st>>>(tab, ws.streams.p, ws.psy.p, ws.bt_prev.p, ws.ath_psy.p, ws.ratio.p);
+    k_psy_masking<<<grid, MASK_THREADS, 0, st>>>(tab, ws.streams.p, ws.psy.p, ws.psy_s.p, ws.bt_prev.p, ws.bt_final.p,
+                                                 o.all_short ? 1 : 0, ws.ath_psy.p, ws.ratio.p);
     g_launches++;
     DBG("k_psy_masking");
   }
@@ -1150,6 +1173,13 @@ int mp3b200_debug_qstats(unsigned long long* out16, int reset) {
 }
 #endif
 int64_t mp3b200_launch_count(void) { return g_launches; }
+int64_t mp3b200_debug_short_units(void) {
+  if (!t_ctx.ws.short_count.p) return -1;
+  int n = 0;
+  CK(cudaMemcpyAsync(&n, t_ctx.ws.short_count.p, sizeof n, cudaMemcpyDeviceToHost, t_ctx.st));
+  CK(cudaStreamSynchronize(t_ctx.st));
+  return n;
+}
 
 int mp3b200_set_device(int device) {
   int n = 0;
@@ -1414,7 +1444,7 @@ int debug_stages(const mp3b200_debug_taps* tp, const T* left, const T* right) {
   uint8_t* bytes_out = tp->bytes_out;
   const int64_t bytes_cap = tp->bytes_cap;
   Config* cfg;
-  int rc = get_config(channels, tp->samplerate, tp->kbps, tp->flags, &cfg);
+  int rc = get_config(channels, tp->samplerate, tp->kbps, tp->flags & ~MP3B200_DEBUG_SKIP_SHORT, &cfg);
   if (rc || (rc = check_input(cfg, 1, &left, &right, &nsamples))) return rc;
   if (!right) right = left;
   const int nch = cfg->host.nch;
@@ -1438,6 +1468,7 @@ int debug_stages(const mp3b200_debug_taps* tp, const T* left, const T* right) {
   LaunchOpts opts;
   opts.f32_in = std::is_same_v<T, float>;
   opts.force_bt = force_blocktype;
+  opts.all_short = !(tp->flags & MP3B200_DEBUG_SKIP_SHORT);
   opts.stop_after_mdct = !(l3_enc || bytes_out || want_gi || want_prep || want_q);
   rc = launch_streams(t_ctx, cfg, sds, d_out, opts);
   /* read-back on the thread's stream (the launch has drained it) */
