@@ -539,17 +539,17 @@ int mp3b200_encode_streams_tagged_async_f32(mp3b200_session* s, int channels, in
  * what mp3b200_encode_batch_device / _f32 / mp3b200_flush_batch return for the same handles and calls.  d_status is the
  * int32[4] of mp3b200_encode_streams_async (mp3b200_check_status reads it).  Rows are device (or managed) memory on the
  * session's device and may be freed once the stream has passed the call.
- * A handle's first session call binds it to the session (this may block): its tail and carried state then live on the
- * device, and every host-side call on it (encode, flush, the batch calls, export / import, seek, the tag and ReplayGain
- * setters and getters) and any other session's call returns MP3B200_ERR_HANDLE until mp3b200_session_release moves them
- * back to the host.  mp3b200_destroy and mp3b200_session_destroy release first.
+ * A handle's first session call binds it to the session (nothing is uploaded, nothing blocks; a handle's tail and carried
+ * state live on its device from mp3b200_create on): until mp3b200_session_release gives it back, every host-side call on it
+ * (encode, flush, the batch calls, export / import, seek, the tag and ReplayGain setters and getters) and any other
+ * session's call returns MP3B200_ERR_HANDLE.  mp3b200_destroy and mp3b200_session_destroy release first.
  * A call refused on the device (a non-finite Float32 sample or one beyond 2^40 once scaled, a frame over its bit budget)
  * commits nothing: each handle it names is marked refused, every later call that names one reports the same refusal in its
  * status, and at release each such handle is exactly where it stood before the refused call.
  * Refused before anything is queued: NULL or repeated handles, a handle with the tag or ReplayGain on, a handle bound to
  * another session, rows that are not device memory on the session's device, a capturing stream, more than 65535 handles
  * (MP3B200_ERR_HANDLE); handles of different configurations or of another device (MP3B200_ERR_CONFIG).  The call waits for
- * the device only where mp3b200_encode_streams_async does, and when it binds a handle. */
+ * the device only where mp3b200_encode_streams_async does. */
 int mp3b200_session_encode_batch(mp3b200_session* s, mp3b200_encoder* const* handles, const int16_t* const* d_left,
                                  const int16_t* const* d_right, const int* nsamples, int n, uint8_t* d_out, const int64_t* out_off,
                                  int* out_bytes, int32_t* d_status);
@@ -568,7 +568,8 @@ int mp3b200_encode_bytes_schedule(int channels, int samplerate, int kbps, int fl
 /* waits for the session's work, settles refusals and gives the handles back to the host calls (unbound handles: no-op),
  * a tagged handle with its music CRC and a ReplayGain handle with its title gain, RadioGain and title count */
 int mp3b200_session_release(mp3b200_session* s, mp3b200_encoder* const* handles, int n);
-/* the samples per channel a bound handle's tail buffer holds: the most any handle of the configuration retains after a call */
+/* the samples per channel a handle's tail buffer holds: the most any handle of the configuration retains after a call that
+ * encodes its pending frames (host calls grow a handle's tails when refused calls leave it more) */
 int64_t mp3b200_session_tail_capacity(int channels, int samplerate, int kbps, int flags);
 
 /* Tagged and ReplayGain handles in a session (DESIGN.md 17).  mp3b200_session_encode_batch_tagged / _f32 and

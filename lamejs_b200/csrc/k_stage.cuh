@@ -1,9 +1,9 @@
 /* k_stage.cuh -- streaming handles fed from device memory (mp3b200_encode_device and its batch / Float32 twins).
  *
- * A handle keeps its retained samples on the host (HandleSamples); a device call's rows stay where the caller left them.
- * Per round, k_gather_rows puts, for every handle that encodes, [retained | caller's rows] into the contiguous rows the launch
- * reads, in the launch's input format, and packs the part of the caller's rows each handle keeps after the call for the
- * download.  k_check_rows_f32 refuses a Float32 call before anything changes, with k_stage_f32's rule.
+ * A handle keeps its retained samples in its device tail (k_handle.cuh); a device call's rows stay where the caller left
+ * them.  Per launch, k_gather_rows puts, for every handle that encodes, [retained | caller's rows] into the contiguous rows
+ * the launch reads, in the launch's input format (GatherDesc::pack is unused by the handle calls: NULL).
+ * k_check_rows_f32 refuses a Float32 call before anything changes, with k_stage_f32's rule.
  *
  * Included after k_resample.cuh (MP3_F32_MAX_SAMPLE); defines no __constant__ data.
  */

@@ -297,6 +297,11 @@ struct ThreadCtx {
   Buf<long long> crc_ranges;              /* music CRC: [2][R] offsets / lengths */
   Buf<unsigned> crc;                      /* music CRC: [R] results */
   Buf<uint8_t> tags;                      /* tagged whole streams: the template frames and their destinations (k_tag_finish) */
+  /* streaming handle calls (queue_handle_call): their device descriptors, the masking row of refused handles, the staged
+   * ReplayGain carry and A of analysing handles; for host calls the pinned descriptor arena and the caller's rows */
+  Buf<uint8_t> hdesc, rg_stage, hrows;
+  Buf<float> halo_scratch;
+  Buf<uint8_t, true> hpin;
   cudaStream_t rg_st = nullptr;           /* ReplayGain analysis, beside the encoder */
   cudaEvent_t ev_rg[3] = {};              /* fork, start, end */
   Buf<RgTitle> rg_titles;
@@ -314,6 +319,7 @@ struct ThreadCtx {
     if (device < 0) return;
     cudaSetDevice(device);
     ws.release(); pcm.release(); out.release(); pin.release(); crc_ranges.release(); crc.release(); tags.release();
+    hdesc.release(); rg_stage.release(); hrows.release(); halo_scratch.release(); hpin.release();
     rg_titles.release(); rg_piece.release(); rg_sum.release(); rg_gain.release(); rg_wstate.release(); rg_cstart.release();
     rg_end_a.release(); rg_end_b.release(); rg_carry.release(); rg_idx.release(); rg_hist.release(); rg_count.release();
     for (auto& e : ev_rg) if (e) { cudaEventDestroy(e); e = nullptr; }
@@ -422,10 +428,6 @@ struct Timings { float psy = 0, scan = 0, mask = 0, fb = 0, q1 = 0, qn = 0, tota
  * slice j; the psy analysis of slice j starts as soon as it has landed. */
 struct PcmArrival { int chunks = 1; cudaEvent_t* ready = nullptr; };
 
-/* set by check_refusals when it refuses a launch for a frame over its bit budget (the one refusal a handle call can only
- * find after its launch, and then undoes: handles_call) */
-thread_local bool t_over_budget = false;
-
 /* The error of a launch whose ws.refusals read refused / over_budget (and, for an asynchronous call, fault: its device
  * fixed-point loop hit the bound), with g_err set; 0 when the output stands. */
 int refusal_error(int refused, int over_budget, int fault) {
@@ -443,7 +445,6 @@ int check_refusals(ThreadCtx& c) {
   int r[2] = {0, 0};
   CK(cudaMemcpyAsync(r, c.ws.refusals.p, sizeof r, cudaMemcpyDeviceToHost, c.st));
   CK(cudaStreamSynchronize(c.st));
-  if (!r[0] && r[1]) t_over_budget = true;
   return refusal_error(r[0], r[1], 0);
 }
 
@@ -455,15 +456,13 @@ struct LaunchOpts {
   const PcmArrival* arrival = nullptr;   /* PCM still landing on the upload stream */
   float* timings_ms = nullptr;           /* the 16 timing slots of include/mp3b200.h */
   bool sync = true;                      /* false: return with the work queued on the context's stream (no timings) */
-  StreamDesc* committed = nullptr;       /* host: each stream's descriptor as the pipeline left it (the carried state),
-                                            valid once the context's stream has drained */
   struct RgJob* rg = nullptr;            /* ReplayGain of every stream, beside the encoder (one launch group only) */
   bool f32_in = false;                   /* the descriptors point at the caller's Float32 rows (k_stage_f32 stages them); with
                                             sync, a non-finite sample makes the launch return MP3B200_ERR_CONFIG */
   struct LoopGraphs* loops = nullptr;    /* run the quantizer's fixed-point loop on the device, as the cached graphs of a session
                                             (no host round trip; needs !sync) */
-  const struct HandleCarry* carry = nullptr;   /* streaming handles bound to a session: their carried state is on the device
-                                                  (k_handle_carry_in; one launch group only) */
+  const struct HandleCarry* carry = nullptr;   /* streaming handles: their carried state is on the device (k_handle_carry_in;
+                                                  one launch group only) */
   int* rg_loop = nullptr;                /* a session's three words of the ReplayGain loop (rg_finish_queued); NULL: ws.refusals + 5 */
   bool analyse_only = false;             /* stop after staging, resampling and the ReplayGain analysis of o.rg: no encoder
                                             kernels, no bytes, no workspace beyond the staged rows */
@@ -1148,8 +1147,6 @@ int launch_streams(ThreadCtx& c, Config* cfg, std::vector<StreamDesc>& sds, uint
     arrival = nullptr;
     float rs_ms = 0.0f;
     if (resampled && o.timings_ms && o.sync) CK(cudaEventElapsedTime(&rs_ms, c.ev_rs[0], c.ev_rs[1]));
-    if (o.committed)
-      CK(cudaMemcpyAsync(o.committed + g0, c.ws.streams.p, sizeof(StreamDesc) * n, cudaMemcpyDeviceToHost, c.st));
     if (o.timings_ms) {
       const float t[16] = {tm.psy, tm.scan, tm.mask, tm.fb, tm.q1, tm.qn, tm.total, 0.0f,
                            tm.q_prepare, tm.q_search, tm.q_outer, tm.q_finish, tm.q_pack, tm.q_mid, rs_ms, 0.0f};
@@ -2093,8 +2090,8 @@ int mp3b200_debug_replaygain_f32(int channels, int samplerate, int kbps, int fla
 
 }  // extern "C"
 
-#include "mp3_handle.inc"
 #include "mp3_session.inc"
+#include "mp3_handle.inc"
 #include "mp3_session_handles.inc"
 
 #ifdef Q_TASKSTAT

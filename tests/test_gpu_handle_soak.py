@@ -129,6 +129,52 @@ def test_failed_handle_inside_a_batch(M, oracle):
         e.close()
 
 
+def test_failed_handle_retains_more_than_the_tail_capacity(M, oracle):
+    """Calls refused for a too small buffer keep their samples and frames, so the handle comes to retain more samples than
+    mp3b200_session_tail_capacity: its tails grow.  The call that succeeds hands out everything held back, the stream equals
+    the oracle's, and a blob exported while the frames were pending continues identically in a fresh handle."""
+    l, r = make_signal("noise", 30000, 44100, 21)
+    cap = int(M.lib().mp3b200_session_tail_capacity(2, 44100, 128, 0))
+    a, c = M.Mp3Encoder(2, 44100, 128), M.Mp3Encoder(2, 44100, 128)
+    ref = oracle.OracleEncoder(2, 44100, 128)
+    held, at = b"", 0
+    while at <= cap + 1500:                                 # nothing encoded: the handle retains every sample fed
+        held += ref.encode_buffer(l[at:at + 1500], r[at:at + 1500])
+        got, rc = _raw_batch(M, [a._h], [l[at:at + 1500]], [r[at:at + 1500]], [1])
+        assert rc == 0 and got == [HS.ERR_BUFFER]
+        at += 1500
+    assert len(held) > 1
+    c.import_state(a.export_state())
+    for lo, hi in [(at, at + 4000), (at + 4000, 30000)]:
+        want = held + ref.encode_buffer(l[lo:hi], r[lo:hi])
+        held = b""
+        assert a.encodeBuffer(l[lo:hi], r[lo:hi]) == want
+        assert c.encodeBuffer(l[lo:hi], r[lo:hi]) == want
+    assert a.flush() == c.flush() == ref.flush()
+    for e in (a, c, ref):
+        e.close()
+
+
+def test_tag_switched_on_again_after_an_imported_fresh_state(M):
+    """A tagged handle that has finished a stream, given a fresh handle's state and its tag switched on again, starts the
+    next stream's music CRC from 0: its tag frame and CRC equal a fresh tagged handle's for that stream."""
+    l, r = make_signal("noise", 20000, 44100, 31)
+    a, b = M.Mp3Encoder(2, 44100, 128, write_vbr_tag=True), M.Mp3Encoder(2, 44100, 128, write_vbr_tag=True)
+    fresh = M.Mp3Encoder(2, 44100, 128)
+    a.encodeBuffer(l[:9000], r[:9000])
+    a.flush()
+    assert a.music_crc() != 0
+    a.import_state(fresh.export_state())
+    assert M.lib().mp3b200_set_write_vbr_tag(a._h, 1) == 1
+    for e in (a, b):
+        e.encodeBuffer(l[9000:], r[9000:])
+        e.flush()
+    assert a.music_crc() == b.music_crc() and a.bytes_written() == b.bytes_written()
+    assert a.lametag_frame() == b.lametag_frame()
+    for e in (a, b, fresh):
+        e.close()
+
+
 def test_handle_of_another_configuration_in_a_batch(M, oracle):
     """A handle of another configuration than the batch's first one gets -1; it keeps its samples and frames, and a later
     call of its own hands them out."""

@@ -151,11 +151,14 @@ def test_replaygain_fixture(M, name):
     assert sha(streams[0][len(tag):]) == sha(b"".join(out)[len(tag):]), name
 
 
-@pytest.mark.parametrize("rg", [False, True], ids=["plain", "replaygain"])
-def test_refused_batch_call_leaves_every_handle_as_it_was(M, rg):
+@pytest.mark.parametrize("rg,twice", [(False, False), (True, False), (False, True), (True, True)],
+                         ids=["plain", "replaygain", "plain-twice", "replaygain-twice"])
+def test_refused_batch_call_leaves_every_handle_as_it_was(M, rg, twice):
     """A loud handle batched with a quiet one: the call that reaches an over-budget frame is refused as a whole, both
     handles export the state they had before it, and quiet input then continues as if the loud call had never been made --
-    the bytes (and with ReplayGain the title gain and tag) of the oracle / a handle that never saw it."""
+    the bytes (and with ReplayGain the title gain and tag) of the oracle / a handle that never saw it.  `twice`: the loud
+    handle is listed twice, quiet input first, so the over-budget frame falls in the second round, after the first round
+    has committed."""
     ch, sr, kb = 2, 32000, 128
     q = lambda n, seed: FS.loud("burst", 1, n, sr, seed, 1.0)                   # noqa: E731  full scale
     # the input of fixture rg_burst_262144_2_32000_128_whole, on which lamejs throws in its first call
@@ -169,8 +172,14 @@ def test_refused_batch_call_leaves_every_handle_as_it_was(M, rg):
         o.append(x)
     state = lambda: None if rg else (A.export_state(), B.export_state())        # noqa: E731  (blobs carry no ReplayGain)
     before = state()
+    c = q(2300, 5)
+    if twice:   # round 1 (c for A, b2 for B) is encodable on its own, so it commits before round 2 is refused
+        oracle_f32.encode_calls(ch, sr, kb, [(f32(a1[0]), f32(a1[1])), (f32(c[0]), f32(c[1]))])
     with pytest.raises(M.Mp3B200Error, match="bit budget"):
-        M.encode_batch([A, B], [f32(loud_l), f32(b2[0])], [f32(loud_r), f32(b2[1])])
+        if twice:
+            M.encode_batch([A, B, A], [f32(c[0]), f32(b2[0]), f32(loud_l)], [f32(c[1]), f32(b2[1]), f32(loud_r)])
+        else:
+            M.encode_batch([A, B], [f32(loud_l), f32(b2[0])], [f32(loud_r), f32(b2[1])])
     assert state() == before
     for o, x in zip((outA, outB), M.encode_batch([A, B], [f32(a2[0]), f32(b2[0])], [f32(a2[1]), f32(b2[1])])):
         o.append(x)
