@@ -140,9 +140,26 @@ int mp3b200_granules_per_frame(int channels, int samplerate, int kbps);
 int64_t mp3b200_stream_frames_ex(int channels, int samplerate, int kbps, int flags, int64_t nsamples);
 int mp3b200_granules_per_frame_ex(int channels, int samplerate, int kbps, int flags);
 
-/* Host buffers.  left[s]/right[s]: nsamples[s] Int16 each; right ignored for mono; with stereo input, right == NULL or
+/* Whole-stream calls.  Every call below that encodes, analyses or tags whole streams (encodeBuffer(everything) + flush()
+ * on fresh encoders: mp3b200_encode_streams*, mp3b200_replaygain_streams*, mp3b200_finish_tags_device and the session calls
+ * mp3b200_encode_streams*_async*) checks its arguments by one set of rules before it looks up the configuration and before
+ * it touches the device, so the answer is the same on a machine without a GPU:
+ *   - nstreams < 0 returns MP3B200_ERR_HANDLE ("negative stream count");
+ *   - a flag the call does not take returns MP3B200_ERR_CONFIG ("unknown flags"): every call takes MP3B200_RESAMPLE, and
+ *     only the tagged encodes take MP3B200_REPLAYGAIN (the ReplayGain-only calls imply it);
+ *   - with the ReplayGain analysis, more than 65535 streams return MP3B200_ERR_HANDLE;
+ *   - with nstreams > 0, each of these returns MP3B200_ERR_HANDLE: a NULL nsamples, a NULL row array (left, or d_pcm / d_files
+ *     and their offsets pcm_off / file_off), a NULL left[s], a negative nsamples[s], or a NULL output array the call
+ *     writes: out, cap and out_bytes of the host encodes, out_off of the device encodes, out_bytes of the device tagged
+ *     encodes, file_bytes of mp3b200_finish_tags_device;
+ *   - a session call also returns MP3B200_ERR_HANDLE for a NULL d_status, for a NULL out_bytes of a tagged call, and for a
+ *     NULL d_gain with MP3B200_REPLAYGAIN, whatever nstreams.
+ * A call with several bad arguments is refused for one of them; which one is not specified.  right, d_out, title_db,
+ * album_db and timings_ms may be NULL.
+ * Host buffers.  left[s]/right[s]: nsamples[s] Int16 each; right ignored for mono; with stereo input, right == NULL or
  * right[s] == NULL encodes left[s] on both channels.  out[s] receives
- * out_bytes[s] = mp3b200_stream_bytes(...) bytes (cap[s] must be >= that).  Returns 0 or a negative error. */
+ * out_bytes[s] = mp3b200_stream_bytes(...) bytes (cap[s] must be >= that).  Returns 0 or a negative error; arguments as
+ * for every whole-stream call (above). */
 int mp3b200_encode_streams(int channels, int samplerate, int kbps, int nstreams, const int16_t* const* left,
                            const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
                            const int64_t* cap, int64_t* out_bytes);
@@ -162,7 +179,8 @@ int mp3b200_encode_streams_ex(int channels, int samplerate, int kbps, int flags,
  * More than 65535 streams run as consecutive launches of at most 65535 streams: the times are summed over them, [7] is the
  * largest pass count of any of them.
  * The call runs on a stream of its own that first waits for work already queued on the legacy default stream (where torch /
- * plain CUDA callers produced d_pcm) and returns after that stream has drained. */
+ * plain CUDA callers produced d_pcm) and returns after that stream has drained.  Arguments as for every whole-stream call
+ * (above). */
 int mp3b200_encode_streams_device(int channels, int samplerate, int kbps, int nstreams, const int16_t* d_pcm,
                                   const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
                                   const int64_t* out_off, float* timings_ms);
@@ -213,7 +231,7 @@ int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int ns
  * (the tag then carries -51.0 dB, the clamp) or when the tag does not fit the frame (lamejs analyses only with the tag on;
  * the streams are then written without either).  The peak amplitude field stays 0: lamejs finds it only by decoding.
  * Flags MP3B200_RESAMPLE and MP3B200_REPLAYGAIN may be combined; flags = 0 is mp3b200_encode_streams_tagged.  A batch with
- * MP3B200_REPLAYGAIN holds at most 65535 streams.
+ * MP3B200_REPLAYGAIN holds at most 65535 streams.  Arguments as for every whole-stream call (above).
  * Streaming handles:
  *   set_find_replay_gain  gfp.findReplayGain, before the first sample and after mp3b200_set_write_vbr_tag (which switches it
  *                         off again).  Returns 1 (on), 0 (off: asked to, or the tag is off: lamejs analyses only with the tag
@@ -285,8 +303,7 @@ int mp3b200_lametag_build_ex(int channels, int samplerate, int kbps, int flags, 
  *                              MP3B200_REPLAYGAIN returns for the same rows wherever the tag fits the configuration.  Where it
  *                              does not (mp3b200_lametag_size_ex == 0) that call analyses nothing and returns -24601; these
  *                              calls still analyse.
- * nstreams < 0, a NULL array (left / d_pcm, pcm_off, nsamples, or a NULL left[s]) or a negative nsamples[s] returns
- * MP3B200_ERR_HANDLE before the device is touched; at most 65535 streams per call (MP3B200_ERR_HANDLE). */
+ * Arguments as for every whole-stream call (above): at most 65535 streams per call. */
 int mp3b200_replaygain_streams(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
                                const int16_t* const* right, const int64_t* nsamples, double* title_db, double* album_db);
 int mp3b200_replaygain_streams_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* const* left,
@@ -308,8 +325,8 @@ int mp3b200_replaygain_streams_device_f32(int channels, int samplerate, int kbps
  * Where the tag does not fit the configuration there is no room and nothing is written; nothing outside
  * [file_off[s], file_off[s] + file_bytes[s]) is ever written.  The files are byte-identical to what
  * mp3b200_encode_streams_tagged_device writes for the same samples: with MP3B200_REPLAYGAIN when title_db comes from
- * mp3b200_replaygain_streams, without it when title_db is NULL.  Ordering as mp3b200_replaygain_streams_device; argument
- * errors as there (d_files, file_off, nsamples and file_bytes must not be NULL). */
+ * mp3b200_replaygain_streams, without it when title_db is NULL.  Ordering as mp3b200_replaygain_streams_device; arguments
+ * as for every whole-stream call (above). */
 int mp3b200_finish_tags_device(int channels, int samplerate, int kbps, int flags, int nstreams, uint8_t* d_files,
                                const int64_t* file_off, const int64_t* nsamples, const double* title_db, int64_t* file_bytes);
 /* Test tap: one whole stream through mp3b200_encode_streams_tagged_ex with MP3B200_REPLAYGAIN (flags: MP3B200_RESAMPLE).
@@ -487,8 +504,9 @@ int mp3b200_debug_replaygain_f32(int channels, int samplerate, int kbps, int fla
  *               [2] the number of quantizer passes (timings_ms[7] of the synchronous call), [3] an internal fault.  When [0],
  *               [1] or [3] is non-zero the output must not be used; mp3b200_check_status turns the words, copied to the host
  *               once the stream has reached them, into the error code and mp3b200_last_error text of the synchronous call.
- * What the host can see is refused before anything is queued, with the codes and texts of the synchronous call: unknown
- * flags, a bad configuration, nstreams < 0; a stream that is capturing a graph returns MP3B200_ERR_HANDLE.
+ * What the host can see is refused before anything is queued, with the codes and texts of the synchronous call: the
+ * arguments by the rules of every whole-stream call (above), a bad configuration; a stream that is capturing a graph returns
+ * MP3B200_ERR_HANDLE.
  * The call does not wait for the device, except: on the first use of a configuration on the device (its tables are
  * uploaded), when the session's workspace or pinned staging grows (which may synchronise the device), and when
  * MP3B200_SESSION_SLOTS calls of the session are still in flight (it waits for the oldest).  A session that has seen a
@@ -523,9 +541,8 @@ int mp3b200_check_status(const int32_t* status);
  *   d_status    device, int32[8]: [0 .. 3] as above (mp3b200_check_status reads them; a ReplayGain loop that hits its bound
  *               raises [3] and reads as the synchronous call's "ReplayGain repair did not converge"), [4] the analysis's
  *               pass count, [5] the chunks it ran again, [6] and [7] zero.
- * Refused before anything is queued, with the synchronous call's codes and texts: unknown flags, a bad configuration,
- * nstreams < 0, MP3B200_REPLAYGAIN with more than 65535 streams; and with MP3B200_ERR_HANDLE: MP3B200_REPLAYGAIN with a NULL
- * d_gain, a NULL d_status or out_bytes, a capturing stream.  The call waits for the device only where
+ * Refused before anything is queued, with the synchronous call's codes and texts: the arguments by the rules of every
+ * whole-stream call (above), a bad configuration; a capturing stream returns MP3B200_ERR_HANDLE.  The call waits for the device only where
  * mp3b200_encode_streams_async does: everything it uploads is staged in the call's pinned slot. */
 int mp3b200_encode_streams_tagged_async(mp3b200_session* s, int channels, int samplerate, int kbps, int flags, int nstreams,
                                         const int16_t* d_pcm, const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,

@@ -2158,7 +2158,7 @@ struct QuantLoop {
 };
 
 static int quant_run(const Mp3Tables* dT, const Mp3Tables& hT, StreamDesc* d_streams, int S, int nstreams_with_frames, int max_frames, long long F,
-                     const QuantBuffers& B, uint8_t* d_out, cudaStream_t st_main, cudaStream_t st_repair, cudaEvent_t ev_fork, cudaEvent_t ev_join,
+                     const QuantBuffers& B, cudaStream_t st_main, cudaStream_t st_repair, cudaEvent_t ev_fork, cudaEvent_t ev_join,
                      cudaEvent_t ev_pass1, cudaEvent_t* evq, int* evq_pred, int* passes_out, std::atomic<long long>* launches,
                      QuantLoop* dloop = nullptr) {
   cudaStream_t st = st_main;       /* the launch helpers below use `st`; the repair chain temporarily points it at st_repair */
@@ -2237,7 +2237,7 @@ static int quant_run(const Mp3Tables* dT, const Mp3Tables& hT, StreamDesc* d_str
     finish(gr, nullptr, nullptr, count, reval); mark(slot_f);
   };
   auto pack = [&](const int* list, const int* cptr, long long count, int reval) {
-    k_q_pack<<<grid_for(count, 9), Q_THREADS, smem_pack, st>>>(dT, d_streams, B.qs, B.ginfo, B.l3enc, B.neg, list, cptr, (int)count, reval, fresh_counter(), d_out, B.over_budget);
+    k_q_pack<<<grid_for(count, 9), Q_THREADS, smem_pack, st>>>(dT, d_streams, B.qs, B.ginfo, B.l3enc, B.neg, list, cptr, (int)count, reval, fresh_counter(), nullptr, B.over_budget);
     (*launches)++;
   };
   auto verify = [&](int predict_step = 0) {

@@ -82,7 +82,7 @@ struct StreamDesc {
   int nframes;             /* frames encoded by this launch */
   int unit_base;           /* row of frame0's granule 0 in the per-granule arrays */
   int frame_base;          /* row of frame0 in the per-frame arrays */
-  long long out_base;      /* byte offset of frame0 in the output buffer */
+  long long out_base;      /* device address of frame0's first byte (the packer's output base is always null) */
   int scan_base;           /* first row of this stream in the scan-chunk scratch */
   int pad_;
   /* streaming handles: masking (en/thm, nch x 122 floats) of the psy unit before frame0, carried on the device between

@@ -523,7 +523,7 @@ constexpr Rows SCALED_F32 = {true, 0};
  * large enough).  All launches go to the context's stream (c.st: the calling thread's, t_ctx.st, or a session's), which
  * first waits for whatever the caller queued on the legacy default stream (wait_legacy); with o.sync the call returns after
  * the stream has drained, so the results are visible to any stream afterwards. */
-int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, uint8_t* d_out, const LaunchOpts& o,
+int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, const LaunchOpts& o,
                  const PcmArrival* arrival, Rows rows, Timings* tm) {
   cudaStream_t st = c.st;
   cudaEvent_t* ev = c.ev;
@@ -672,7 +672,7 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, uint8_
       cached = &lg.exec[std::make_tuple((const Config*)cfg, S, total_frames, max_frames)];
       dloop.capture = lg.capture; dloop.st = ws.refusals.p + 2; dloop.exec = *cached;
     }
-    rc = quant_run(tab, cfg->host, ws.streams.p, S, streams_with_frames, max_frames, total_frames, qb, d_out, st, c.aux_st, c.ev_fork, c.ev_join, ev[5], c.evq, c.evq_pred, &passes, &g_launches,
+    rc = quant_run(tab, cfg->host, ws.streams.p, S, streams_with_frames, max_frames, total_frames, qb, st, c.aux_st, c.ev_fork, c.ev_join, ev[5], c.evq, c.evq_pred, &passes, &g_launches,
                    o.loops ? &dloop : nullptr);
     if (cached) {
       if (!*cached && dloop.exec) o.loops->instantiated++;
@@ -1080,14 +1080,14 @@ int rg_finish(ThreadCtx& c, Config* cfg, RgJob& job) {
   return 0;
 }
 
-/* Encodes the streams `sds` into d_out: the caller sets each descriptor's PCM, pcm_base / pcm_end, frame0, nframes,
- * out_base and carried state; this assigns unit_base / frame_base, grows the context's workspace and runs the pipeline.
+/* Encodes the streams `sds`: the caller sets each descriptor's PCM, pcm_base / pcm_end, frame0, nframes, out_base (the
+ * device address of its bytes) and carried state; this assigns unit_base / frame_base, grows the context's workspace and runs the pipeline.
  * The stream index is a grid y / z coordinate of several kernels (CUDA limit 65535): a larger batch runs as consecutive
  * launches of at most MP3_MAX_LAUNCH_STREAMS streams on the context's stream, the later ones behind every PCM upload.
  * Timings add up over the launches; the pass count is the largest any of them needed.
  * With resampling (cfg->rs.ratio > 1) the descriptors hold the caller's input as resample_streams describes; each launch
  * first resamples it (timing slot 14). */
-int launch_streams(ThreadCtx& c, Config* cfg, std::vector<StreamDesc>& sds, uint8_t* d_out, const LaunchOpts& o) {
+int launch_streams(ThreadCtx& c, Config* cfg, std::vector<StreamDesc>& sds, const LaunchOpts& o) {
   if (o.timings_ms) for (int i = 0; i < 16; i++) o.timings_ms[i] = 0.0f;
   const PcmArrival* arrival = o.arrival;
   const int nstreams = (int)sds.size();
@@ -1137,7 +1137,7 @@ int launch_streams(ThreadCtx& c, Config* cfg, std::vector<StreamDesc>& sds, uint
       if (rc) return rc;
     }
     Timings tm;
-    rc = o.analyse_only ? 0 : run_pipeline(c, cfg, group, n, d_out, o, arrival, rows, &tm);
+    rc = o.analyse_only ? 0 : run_pipeline(c, cfg, group, n, o, arrival, rows, &tm);
     if (rc) return rc;
     if (o.rg) {                                /* a session: ws.refusals[3] is its fault word, [5 .. 8) the loop's words */
       rc = o.loops ? rg_finish_queued(c, cfg, *o.rg, *o.loops, o.rg_loop ? o.rg_loop : c.ws.refusals.p + 5, c.ws.refusals.p + 3)
@@ -1221,12 +1221,167 @@ int mp3b200_out_samplerate(int channels, int samplerate, int kbps) { return mp3_
 
 }  // extern "C"
 
+/* ---- container / metadata step (SURVEY.md 8(f3)): music CRC on the device, tag frames on the host ---- */
 namespace {
-/* Whole streams (encodeBuffer(everything) + flush() on fresh encoders): stream s reads nsamples[s] samples per channel at
- * d_pcm + pcm_off[s] (stereo: the right channel follows the left) and writes its bytes at out_off[s]. */
+CrcTables g_crc_host;                              /* byte table + zero-byte powers (k_tag.cuh), built once */
+bool g_crc_host_ready = false;
+CrcTables* g_crc_dev[MP3_MAX_DEVICES] = {};        /* per device copy */
+
+const CrcTables& crc_host() {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (!g_crc_host_ready) { crc_host_tables(&g_crc_host); g_crc_host_ready = true; }
+  return g_crc_host;
+}
+
+/* uploads the CRC tables to `device` on first use there (g_crc_dev) */
+int crc_tables_on(int device) {
+  const CrcTables& ht = crc_host();
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (!g_crc_dev[device]) {
+    CK(cudaMalloc(&g_crc_dev[device], sizeof(CrcTables)));
+    CK(cudaMemcpy(g_crc_dev[device], &ht, sizeof(CrcTables), cudaMemcpyHostToDevice));
+  }
+  return 0;
+}
+
+/* Queues on c.st, behind whatever wrote the bytes, the music CRC (CRC-16, start 0) of the byte ranges [at[r], at[r] + len[r])
+ * (absolute device addresses, like the packer's output offsets) into c.crc[r]: one k_music_crc launch per 65535 ranges.
+ * The ranges go up through upload(); the CRC tables must already be on the device (crc_tables_on). */
+int queue_music_crc(ThreadCtx& c, const std::vector<long long>& at, const std::vector<long long>& len) {
+  const int R = (int)at.size();
+  if (R == 0) return 0;
+  std::vector<long long> ranges((size_t)2 * R);
+  long long longest = 0;
+  for (int i = 0; i < R; i++) { ranges[i] = at[i]; ranges[(size_t)R + i] = len[i]; longest = len[i] > longest ? len[i] : longest; }
+  int rc = 0;
+  if ((rc = c.crc_ranges.fit((size_t)2 * R)) || (rc = c.crc.fit((size_t)R)) ||
+      (rc = upload(c, c.crc_ranges.p, ranges.data(), sizeof(long long) * ranges.size())))
+    return rc;
+  CK(cudaMemsetAsync(c.crc.p, 0, sizeof(unsigned) * (size_t)R, c.st));
+  const long long pieces = (longest + CRC_PIECE_BYTES - 1) / CRC_PIECE_BYTES;
+  for (int r0 = 0; r0 < R && longest > 0; r0 += 65535) {
+    const int nr = R - r0 < 65535 ? R - r0 : 65535;
+    dim3 grid((unsigned)((pieces + CRC_WARPS - 1) / CRC_WARPS), (unsigned)nr);
+    k_music_crc<<<grid, CRC_WARPS * 32, 0, c.st>>>(nullptr, c.crc_ranges.p + r0, c.crc_ranges.p + R + r0, g_crc_dev[c.device], c.crc.p + r0);
+    g_launches++;
+  }
+  return 0;
+}
+
+/* mp3b200_lametag_build(_ex): `field` is the tag's Radio Replay Gain field, 0 for a stream nobody analysed */
+int build_lametag(int channels, int samplerate, int kbps, int flags, int64_t nframes, int64_t music_bytes, int music_crc,
+                  int encoder_padding, int field, uint8_t* buf, int cap) {
+  const Config* c = host_config(channels, samplerate, kbps, flags);
+  if (!c) return MP3B200_ERR_CONFIG;
+  const Mp3TagParams& p = c->tag;
+  if (!p.fits || nframes <= 0) return 0;
+  if (!buf || cap < p.frame_bytes) return p.frame_bytes;              /* like getLameTagFrame: the size it needs */
+  Mp3SeekBag* bag = new Mp3SeekBag();
+  bag->reset();
+  bag->add_frames(nframes, p.kbps);
+  const int n = mp3_tag_frame(p, *bag, music_bytes, (unsigned)music_crc, encoder_padding, buf, field);
+  delete bag;
+  return n;
+}
+}  // namespace
+
+namespace {
+/* ---- whole streams: encodeBuffer(everything) + flush() on fresh encoders of one configuration ----
+ * Every whole-stream entry point fills in one WholeCall and hands it to one of two drivers: whole_sync (the calling
+ * thread's context, returns with the results on the host) or whole_async (an encode session, mp3_session.inc).  Both check
+ * the arguments (whole_args), get the configuration, plan the streams (stream_plan) and run the one body, whole_run. */
+template <class T>     /* the rows' samples: int16_t or float (uint8_t: the encoded files the tag step alone reads) */
+struct WholeCall {
+  int channels, samplerate, kbps, flags, nstreams;
+  /* the rows, nsamples[s] samples per channel: host rows left[s] / right[s] (right or right[s] NULL: left[s] on both
+   * channels), or device rows at d_pcm + pcm_off[s] (stereo: the right channel follows the left) */
+  const T* const* left = nullptr;
+  const T* const* right = nullptr;
+  const T* d_pcm = nullptr;
+  const int64_t* pcm_off = nullptr;
+  const int64_t* nsamples = nullptr;
+  /* what the call does */
+  bool encode = true;                    /* false: no encoder, the analysis alone or the tag step alone */
+  bool tagged = false;                   /* files: the Info/LAME tag frame, then the audio */
+  bool analyse = false;                  /* the ReplayGain analysis (a tagged call's only where its tag is written) */
+  /* where the results go: device files at d_out + out_off[s], or host files out[s] of cap[s] bytes; out_bytes[s] each
+   * file's length; title_db / album_db (optional) the analysis's gains; timings_ms (optional) the 16 timing slots */
+  uint8_t* d_out = nullptr;
+  const int64_t* out_off = nullptr;
+  uint8_t* const* out = nullptr;
+  const int64_t* cap = nullptr;
+  int64_t* out_bytes = nullptr;
+  double* title_db = nullptr;
+  double* album_db = nullptr;
+  float* timings_ms = nullptr;
+  const double* title_in = nullptr;      /* the tag step alone: the title gains the tags carry (host; NULL: none) */
+  RgJob* job = nullptr;                  /* debug: the caller's job, to read the analysis's windows */
+  /* sessions: the gains ([nstreams] titles, then the album's) and the status words, on the device */
+  bool session = false;
+  double* d_gain = nullptr;
+  int32_t* d_status = nullptr;
+};
+
+/* The argument rules of every whole-stream call (include/mp3b200.h, "Whole-stream calls"), checked before the
+ * configuration and before any CUDA call.  MP3B200_REPLAYGAIN is a flag of the tagged encodes; the analysis alone implies it. */
+template <class T>
+int whole_args(const WholeCall<T>& k) {
+  auto refuse = [](const char* why) { g_err = why; return MP3B200_ERR_HANDLE; };
+  if (k.nstreams < 0) return refuse("negative stream count");
+  if (k.flags & ~(MP3B200_RESAMPLE | (k.encode && k.tagged ? MP3B200_REPLAYGAIN : 0))) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
+  if (k.analyse && k.nstreams > MP3_MAX_LAUNCH_STREAMS) return refuse("ReplayGain batches hold at most 65535 streams");
+  if (k.session) {                       /* written by every call: the album's gain and the status words */
+    if (k.analyse && !k.d_gain) return refuse("d_gain is NULL");
+    if (!k.d_status) return refuse("d_status is NULL");
+    if (k.tagged && !k.out_bytes) return refuse("out_bytes is NULL");
+  }
+  if (k.nstreams == 0) return MP3B200_OK;
+  const bool files = k.encode || k.tagged;
+  if (!k.nsamples || !(k.left || (k.d_pcm && k.pcm_off)) || (files && (k.left ? !k.out || !k.cap : !k.out_off)))
+    return refuse("null array");
+  if (!k.out_bytes && (k.left ? k.encode : k.tagged)) return refuse(k.encode ? "out_bytes is NULL" : "file_bytes is NULL");
+  for (int s = 0; s < k.nstreams; s++) {
+    if (k.left && !k.left[s]) return refuse("null row");
+    if (k.nsamples[s] < 0) return refuse("negative sample count");
+  }
+  return MP3B200_OK;
+}
+
+/* What is known about whole streams before anything runs, in closed form from the lamejs FIFO: each stream's frames, audio
+ * bytes and end padding, the room of its tag frame (tag[s]: tfs, or 0 where no tag is written: untagged calls, a tag that
+ * does not fit, a stream without frames), and with the analysis (rg) the pieces it sees (rg->specs).  A tagged stream is
+ * analysed only when its tag is written (Lame.js:911-916): rg is then NULL where the tag does not fit. */
+struct StreamPlan {
+  int tfs = 0;
+  RgJob* rg = nullptr;
+  std::vector<long long> frames, audio;
+  std::vector<int> padding, tag;
+};
+StreamPlan stream_plan(const Config* cfg, int nstreams, const int64_t* nsamples, bool tagged, RgJob* rg) {
+  StreamPlan pl;
+  pl.tfs = tagged && cfg->tag.fits ? cfg->tag.frame_bytes : 0;
+  pl.rg = tagged && !cfg->tag.fits ? nullptr : rg;
+  if (pl.rg) pl.rg->specs.assign((size_t)nstreams, RgSpec());
+  pl.frames.resize((size_t)nstreams); pl.audio.resize((size_t)nstreams); pl.padding.resize((size_t)nstreams); pl.tag.resize((size_t)nstreams);
+  for (int s = 0; s < nstreams; s++) {
+    LameFifo fifo(cfg->host.mode_gr, cfg->rs.ratio);
+    if (pl.rg) { pl.rg->specs[s].stream = s; fifo.pieces = &pl.rg->specs[s].pieces; }
+    const long long fed = fifo.feed(nsamples[s]);
+    const FifoFlush fl = fifo.flush();
+    pl.frames[s] = fed + fl.frames;
+    pl.audio[s] = bytes_of_frames(cfg->host, 0, pl.frames[s]);
+    pl.padding[s] = fl.end_padding;
+    pl.tag[s] = pl.tfs > 0 && pl.frames[s] > 0 ? pl.tfs : 0;
+  }
+  return pl;
+}
+
+/* The descriptors of whole streams: stream s reads nsamples[s] samples per channel at d_pcm + pcm_off[s] (stereo: the right
+ * channel follows the left) and writes its audio at d_out + out_off[s] + plan.tag[s], behind the room of its tag frame
+ * (out_off NULL: the analysis alone, which writes no bytes). */
 template <class T>     /* int16_t, or float (the launch stages the rows: LaunchOpts::f32_in) */
-std::vector<StreamDesc> whole_streams(Config* cfg, int nstreams, const T* d_pcm, const int64_t* pcm_off,
-                                      const int64_t* nsamples, const int64_t* out_off) {
+std::vector<StreamDesc> whole_streams(const Config* cfg, const StreamPlan& pl, int nstreams, const T* d_pcm, const int64_t* pcm_off,
+                                      const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off) {
   std::vector<StreamDesc> sds(nstreams);
   for (int s = 0; s < nstreams; s++) {
     StreamDesc& sd = sds[s];
@@ -1235,11 +1390,50 @@ std::vector<StreamDesc> whole_streams(Config* cfg, int nstreams, const T* d_pcm,
     sd.pcm[0] = x;
     sd.pcm[1] = cfg->host.nch == 2 ? x + nsamples[s] : x;
     sd.pcm_base = 0; sd.pcm_end = nsamples[s];
-    sd.frame0 = 0; sd.nframes = (int)frames_for(nsamples[s], cfg->host.mode_gr, cfg->rs.ratio);
-    sd.out_base = out_off[s];
+    sd.frame0 = 0; sd.nframes = (int)pl.frames[s];
+    sd.out_base = out_off ? (long long)(uintptr_t)(d_out + out_off[s] + pl.tag[s]) : 0;
     init_stream_state(sd);
   }
   return sds;
+}
+
+/* Queues, behind the packer on c.st, what turns the audio of tagged whole streams into files: the music CRC of each stream
+ * where its audio lies (sds[i].out_base), and k_tag_finish, which completes each template frame with it and with the field
+ * of gain[i] (device; NULL: the field is 0) and writes it to d_out + out_off[i].  The templates are mp3_tag_frame with music
+ * CRC 0 and gain field 0.  Every upload goes through upload(). */
+int finish_tagged(ThreadCtx& c, Config* cfg, const StreamPlan& plan, const std::vector<StreamDesc>& sds, uint8_t* d_out,
+                  const int64_t* out_off, const double* gain) {
+  const int S = (int)sds.size();
+  const Mp3TagParams& p = cfg->tag;
+  int ntags = 0;
+  for (int i = 0; i < S; i++) ntags += plan.tag[i] ? 1 : 0;
+  if (ntags == 0) return 0;
+  std::vector<long long> at((size_t)S);
+  for (int i = 0; i < S; i++) at[i] = sds[i].out_base;
+  int rc = queue_music_crc(c, at, plan.audio);
+  if (rc) return rc;
+  /* the template frames: everything but the music CRC, the gain field and the frame's own CRC */
+  const size_t tfs = (size_t)plan.tfs;
+  std::vector<TagDest> dst((size_t)ntags);
+  std::vector<uint8_t> frames(tfs * (size_t)ntags);
+  Mp3SeekBag* bag = new Mp3SeekBag();
+  for (int i = 0, k = 0; i < S; i++) {
+    if (!plan.tag[i]) continue;
+    bag->reset();
+    bag->add_frames(plan.frames[i], p.kbps);
+    mp3_tag_frame(p, *bag, plan.audio[i], 0, plan.padding[i], frames.data() + tfs * (size_t)k, 0);
+    dst[k].at = d_out + out_off[i]; dst[k].stream = i;
+    k++;
+  }
+  delete bag;
+  const size_t dst_bytes = (sizeof(TagDest) * (size_t)ntags + 255) & ~(size_t)255;
+  if ((rc = c.tags.fit(dst_bytes + frames.size())) || (rc = upload(c, c.tags.p, dst.data(), sizeof(TagDest) * dst.size())) ||
+      (rc = upload(c, c.tags.p + dst_bytes, frames.data(), frames.size())))
+    return rc;
+  k_tag_finish<<<ntags, TAG_FINISH_THREADS, 0, c.st>>>(reinterpret_cast<const TagDest*>(c.tags.p), c.tags.p + dst_bytes, p, c.crc.p, gain);
+  g_launches++;
+  CK(cudaGetLastError());
+  return 0;
 }
 
 /* the thread's device buffer for n samples of host PCM of type T; NULL (g_err set) when it cannot grow */
@@ -1261,7 +1455,7 @@ bool finite_after_scale(const Mp3Tables& T, const float* x, long long n) {
 
 /* The input gate of the host entry points: the caller's rows are checked before anything runs, and refused with
  * MP3B200_ERR_CONFIG.  Int16 rows always pass; Float32 rows must stay finite through lamejs's store and scale. */
-int check_input(const Config*, int, const int16_t* const*, const int16_t* const*, const int64_t*) { return MP3B200_OK; }
+template <class T> int check_input(const Config*, int, const T* const*, const T* const*, const int64_t*) { return MP3B200_OK; }
 int check_input(const Config* cfg, int nstreams, const float* const* left, const float* const* right, const int64_t* nsamples) {
   for (int s = 0; s < nstreams; s++)
     if (!finite_after_scale(cfg->host, left[s], nsamples[s]) ||
@@ -1304,95 +1498,86 @@ int upload_host_rows(const Config* cfg, int nstreams, const T* const* left, cons
   return MP3B200_OK;
 }
 
-/* Whole streams from host buffers, laid out as files in t_ctx.out: file s at out_off[s] is room[s] bytes (room NULL: none)
- * and then the stream's audio.  Checks that out[s] has room for the file (out_bytes[s] = its length), stages the PCM
- * (upload_host_rows) and fills the descriptors `sds` (out_base: the file's offset, where the audio goes when there is no
- * room) and the upload's arrival `arr`. */
+/* The body of every whole-stream call, on context c once it is planned (pl): stages host rows (upload_host_rows), describes
+ * the streams (whole_streams), encodes and / or analyses them (launch_streams; o.arrival, o.rg and o.analyse_only are set
+ * here) and writes the tag frames (finish_tagged).  The files lie at k.d_out + k.out_off[s] on the device; k.out_bytes[s]
+ * (optional) receives each file's length. */
 template <class T>
-int stage_host_streams(Config* cfg, int nstreams, const T* const* left, const T* const* right, const int64_t* nsamples,
-                       const int64_t* cap, const int* room, int64_t* out_bytes, std::vector<int64_t>& out_off,
-                       std::vector<StreamDesc>& sds, PcmArrival& arr) {
-  out_off.assign(nstreams, 0);
-  long long tot_bytes = 0;
-  for (int s = 0; s < nstreams; s++) {
-    out_off[s] = tot_bytes;
-    const long long n = bytes_of_frames(cfg->host, 0, frames_for(nsamples[s], cfg->host.mode_gr, cfg->rs.ratio)) + (room ? room[s] : 0);
-    if (cap[s] < n) { g_err = "output buffer too small"; return MP3B200_ERR_BUFFER; }
-    out_bytes[s] = n;
-    tot_bytes += n;
+int whole_run(ThreadCtx& c, Config* cfg, const WholeCall<T>& k, const StreamPlan& pl, LaunchOpts o) {
+  const int S = k.nstreams;
+  std::vector<int64_t> staged_off;
+  T* staged = nullptr;
+  PcmArrival arr;
+  if (k.left) {
+    const int rc = upload_host_rows(cfg, S, k.left, k.right, k.nsamples, staged_off, staged, arr);
+    if (rc) return rc;
+    o.arrival = &arr;
   }
-  if (nstreams == 0) return MP3B200_OK;
-  std::vector<int64_t> pcm_off;
-  T* d_pcm = nullptr;
-  int rc = upload_host_rows(cfg, nstreams, left, right, nsamples, pcm_off, d_pcm, arr);
-  if (rc || (rc = t_ctx.out.fit((size_t)tot_bytes + 8))) return rc;
-  sds = whole_streams(cfg, nstreams, d_pcm, pcm_off.data(), nsamples, out_off.data());
+  std::vector<StreamDesc> sds = whole_streams(cfg, pl, S, k.left ? staged : k.d_pcm, k.left ? staged_off.data() : k.pcm_off,
+                                              k.nsamples, k.d_out, k.out_off);
+  for (int s = 0; k.out_bytes && s < S; s++) k.out_bytes[s] = pl.audio[s] + pl.tag[s];
+  o.rg = pl.rg;
+  o.analyse_only = !k.encode;
+  /* launch_streams returns with the refusals checked when it synchronises: no tag for a refused call.  The tag step alone
+   * waits for the caller's files as a launch waits for its rows. */
+  int rc = k.encode || pl.rg ? launch_streams(c, cfg, sds, o) : wait_legacy(c);
+  if (!rc && pl.rg && !o.sync) {         /* the analysis, still queued on c.rg_st, joins the call before its gains are read */
+    if (cudaEventRecord(c.ev_rg[2], c.rg_st) != cudaSuccess || cudaStreamWaitEvent(c.st, c.ev_rg[2], 0) != cudaSuccess) {
+      g_err = "ReplayGain join failed"; rc = MP3B200_ERR_CUDA;
+    }
+  }
+  if (rc || !k.tagged) return rc;
+  const double* gain = pl.rg ? c.rg_gain.p : nullptr;
+  if (k.title_in && S > 0) {
+    if ((rc = c.rg_gain.fit((size_t)S)) || (rc = upload(c, c.rg_gain.p, k.title_in, sizeof(double) * (size_t)S))) return rc;
+    gain = c.rg_gain.p;
+  }
+  return finish_tagged(c, cfg, pl, sds, k.d_out, k.out_off, gain);
+}
+
+/* The synchronous driver, on the calling thread's context: host files are laid out in t_ctx.out and copied into out[s];
+ * returns with every result on the host. */
+template <class T>
+int whole_sync(WholeCall<T> k) {
+  Config* cfg = nullptr;
+  int rc = whole_args(k);
+  if (rc || (rc = get_config(k.channels, k.samplerate, k.kbps, k.flags & MP3B200_RESAMPLE, &cfg)) ||
+      (k.left && (rc = check_input(cfg, k.nstreams, k.left, k.right, k.nsamples))) || (k.tagged && (rc = crc_tables_on(t_ctx.device))))
+    return rc;
+  const int S = k.nstreams;
+  RgJob job;
+  const StreamPlan pl = stream_plan(cfg, S, k.nsamples, k.tagged, k.analyse ? (k.job ? k.job : &job) : nullptr);
+  std::vector<int64_t> file_off;
+  if (k.out) {
+    long long tot = 0;
+    file_off.resize((size_t)S);
+    for (int s = 0; s < S; s++) {
+      if (k.cap[s] < pl.audio[s] + pl.tag[s]) { g_err = "output buffer too small"; return MP3B200_ERR_BUFFER; }
+      file_off[s] = tot;
+      tot += pl.audio[s] + pl.tag[s];
+    }
+    if ((rc = t_ctx.out.fit((size_t)tot + 8))) return rc;
+    k.d_out = t_ctx.out.p;
+    k.out_off = file_off.data();
+  }
+  LaunchOpts o;
+  o.f32_in = std::is_same_v<T, float>;
+  o.timings_ms = k.timings_ms;
+  if ((rc = whole_run(t_ctx, cfg, k, pl, o))) return rc;
+  if (k.out || k.tagged) {               /* the copies and the tag step are still queued */
+    for (int s = 0; k.out && s < S; s++)
+      CK(cudaMemcpyAsync(k.out[s], k.d_out + k.out_off[s], (size_t)k.out_bytes[s], cudaMemcpyDeviceToHost, t_ctx.st));
+    CK(cudaStreamSynchronize(t_ctx.st));
+    CK(cudaGetLastError());
+  }
+  const bool ran = pl.rg && (int)pl.rg->title_db.size() == S && S > 0;
+  for (int s = 0; k.title_db && s < S; s++) k.title_db[s] = ran ? pl.rg->title_db[s] : RG_NOT_ENOUGH_SAMPLES;
+  if (k.album_db) *k.album_db = ran ? pl.rg->album_db : RG_NOT_ENOUGH_SAMPLES;
   return MP3B200_OK;
 }
-
 }  // namespace
 
 extern "C" {
-
-int mp3b200_encode_streams_device(int channels, int samplerate, int kbps, int nstreams, const int16_t* d_pcm,
-                                  const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
-                                  const int64_t* out_off, float* timings_ms) {
-  return mp3b200_encode_streams_device_ex(channels, samplerate, kbps, 0, nstreams, d_pcm, pcm_off, nsamples, d_out, out_off, timings_ms);
-}
-
-}  // extern "C"
-
-namespace {
-template <class T>
-int encode_device(int channels, int samplerate, int kbps, int flags, int nstreams, const T* d_pcm, const int64_t* pcm_off,
-                  const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off, float* timings_ms) {
-  if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
-  Config* cfg;
-  const int rc = get_config(channels, samplerate, kbps, flags, &cfg);
-  if (rc) return rc;
-  std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off, nsamples, out_off);
-  LaunchOpts o;
-  o.timings_ms = timings_ms;
-  o.f32_in = std::is_same_v<T, float>;
-  return launch_streams(t_ctx, cfg, sds, d_out, o);
-}
-
-template <class T>
-int encode_host(int channels, int samplerate, int kbps, int flags, int nstreams, const T* const* left, const T* const* right,
-                const int64_t* nsamples, uint8_t* const* out, const int64_t* cap, int64_t* out_bytes) {
-  if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
-  Config* cfg;
-  int rc = get_config(channels, samplerate, kbps, flags, &cfg);
-  if (rc || (rc = check_input(cfg, nstreams, left, right, nsamples))) return rc;
-  std::vector<int64_t> out_off;
-  std::vector<StreamDesc> sds;
-  PcmArrival arr;
-  rc = stage_host_streams(cfg, nstreams, left, right, nsamples, cap, nullptr, out_bytes, out_off, sds, arr);
-  if (rc || nstreams == 0) return rc;
-  LaunchOpts o;
-  o.arrival = &arr;
-  o.f32_in = std::is_same_v<T, float>;
-  if ((rc = launch_streams(t_ctx, cfg, sds, t_ctx.out.p, o))) return rc;
-  for (int s = 0; s < nstreams; s++)
-    if (cudaMemcpyAsync(out[s], t_ctx.out.p + out_off[s], (size_t)out_bytes[s], cudaMemcpyDeviceToHost, t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
-  if (cudaStreamSynchronize(t_ctx.st) != cudaSuccess) rc = MP3B200_ERR_CUDA;
-  return rc;
-}
-}  // namespace
-
-extern "C" {
-
-int mp3b200_encode_streams_device_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
-                                     const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
-                                     const int64_t* out_off, float* timings_ms) {
-  return encode_device(channels, samplerate, kbps, flags, nstreams, d_pcm, pcm_off, nsamples, d_out, out_off, timings_ms);
-}
-
-int mp3b200_encode_streams_device_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* d_pcm,
-                                      const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
-                                      const int64_t* out_off, float* timings_ms) {
-  return encode_device(channels, samplerate, kbps, flags, nstreams, d_pcm, pcm_off, nsamples, d_out, out_off, timings_ms);
-}
 
 int mp3b200_encode_streams(int channels, int samplerate, int kbps, int nstreams, const int16_t* const* left,
                            const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
@@ -1403,14 +1588,118 @@ int mp3b200_encode_streams(int channels, int samplerate, int kbps, int nstreams,
 int mp3b200_encode_streams_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
                               const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
                               const int64_t* cap, int64_t* out_bytes) {
-  return encode_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes);
+  return whole_sync<int16_t>({.channels = channels, .samplerate = samplerate, .kbps = kbps, .flags = flags, .nstreams = nstreams,
+                              .left = left, .right = right, .nsamples = nsamples, .out = out, .cap = cap, .out_bytes = out_bytes});
 }
 
 int mp3b200_encode_streams_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* const* left,
                                const float* const* right, const int64_t* nsamples, uint8_t* const* out,
                                const int64_t* cap, int64_t* out_bytes) {
-  return encode_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes);
+  return whole_sync<float>({.channels = channels, .samplerate = samplerate, .kbps = kbps, .flags = flags, .nstreams = nstreams,
+                            .left = left, .right = right, .nsamples = nsamples, .out = out, .cap = cap, .out_bytes = out_bytes});
 }
+
+int mp3b200_encode_streams_device(int channels, int samplerate, int kbps, int nstreams, const int16_t* d_pcm,
+                                  const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
+                                  const int64_t* out_off, float* timings_ms) {
+  return mp3b200_encode_streams_device_ex(channels, samplerate, kbps, 0, nstreams, d_pcm, pcm_off, nsamples, d_out, out_off, timings_ms);
+}
+
+int mp3b200_encode_streams_device_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
+                                     const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
+                                     const int64_t* out_off, float* timings_ms) {
+  return whole_sync<int16_t>({.channels = channels, .samplerate = samplerate, .kbps = kbps, .flags = flags, .nstreams = nstreams,
+                              .d_pcm = d_pcm, .pcm_off = pcm_off, .nsamples = nsamples, .d_out = d_out, .out_off = out_off,
+                              .timings_ms = timings_ms});
+}
+
+int mp3b200_encode_streams_device_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* d_pcm,
+                                      const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out,
+                                      const int64_t* out_off, float* timings_ms) {
+  return whole_sync<float>({.channels = channels, .samplerate = samplerate, .kbps = kbps, .flags = flags, .nstreams = nstreams,
+                            .d_pcm = d_pcm, .pcm_off = pcm_off, .nsamples = nsamples, .d_out = d_out, .out_off = out_off,
+                            .timings_ms = timings_ms});
+}
+
+int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int nstreams, const int16_t* const* left,
+                                  const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
+                                  const int64_t* cap, int64_t* out_bytes) {
+  return mp3b200_encode_streams_tagged_ex(channels, samplerate, kbps, 0, nstreams, left, right, nsamples, out, cap, out_bytes,
+                                          nullptr, nullptr);
+}
+
+int mp3b200_encode_streams_tagged_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
+                                     const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
+                                     const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db) {
+  return whole_sync<int16_t>({.channels = channels, .samplerate = samplerate, .kbps = kbps, .flags = flags, .nstreams = nstreams,
+                              .left = left, .right = right, .nsamples = nsamples, .tagged = true,
+                              .analyse = (flags & MP3B200_REPLAYGAIN) != 0, .out = out, .cap = cap, .out_bytes = out_bytes,
+                              .title_db = title_db, .album_db = album_db});
+}
+
+int mp3b200_encode_streams_tagged_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* const* left,
+                                      const float* const* right, const int64_t* nsamples, uint8_t* const* out,
+                                      const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db) {
+  return whole_sync<float>({.channels = channels, .samplerate = samplerate, .kbps = kbps, .flags = flags, .nstreams = nstreams,
+                            .left = left, .right = right, .nsamples = nsamples, .tagged = true,
+                            .analyse = (flags & MP3B200_REPLAYGAIN) != 0, .out = out, .cap = cap, .out_bytes = out_bytes,
+                            .title_db = title_db, .album_db = album_db});
+}
+
+int mp3b200_encode_streams_tagged_device(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
+                                         const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off,
+                                         int64_t* out_bytes, double* title_db, double* album_db) {
+  return whole_sync<int16_t>({.channels = channels, .samplerate = samplerate, .kbps = kbps, .flags = flags, .nstreams = nstreams,
+                              .d_pcm = d_pcm, .pcm_off = pcm_off, .nsamples = nsamples, .tagged = true,
+                              .analyse = (flags & MP3B200_REPLAYGAIN) != 0, .d_out = d_out, .out_off = out_off,
+                              .out_bytes = out_bytes, .title_db = title_db, .album_db = album_db});
+}
+
+int mp3b200_encode_streams_tagged_device_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* d_pcm,
+                                             const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off,
+                                             int64_t* out_bytes, double* title_db, double* album_db) {
+  return whole_sync<float>({.channels = channels, .samplerate = samplerate, .kbps = kbps, .flags = flags, .nstreams = nstreams,
+                            .d_pcm = d_pcm, .pcm_off = pcm_off, .nsamples = nsamples, .tagged = true,
+                            .analyse = (flags & MP3B200_REPLAYGAIN) != 0, .d_out = d_out, .out_off = out_off,
+                            .out_bytes = out_bytes, .title_db = title_db, .album_db = album_db});
+}
+
+int mp3b200_replaygain_streams(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
+                               const int16_t* const* right, const int64_t* nsamples, double* title_db, double* album_db) {
+  return whole_sync<int16_t>({.channels = channels, .samplerate = samplerate, .kbps = kbps, .flags = flags, .nstreams = nstreams,
+                              .left = left, .right = right, .nsamples = nsamples, .encode = false, .analyse = true,
+                              .title_db = title_db, .album_db = album_db});
+}
+int mp3b200_replaygain_streams_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* const* left,
+                                   const float* const* right, const int64_t* nsamples, double* title_db, double* album_db) {
+  return whole_sync<float>({.channels = channels, .samplerate = samplerate, .kbps = kbps, .flags = flags, .nstreams = nstreams,
+                            .left = left, .right = right, .nsamples = nsamples, .encode = false, .analyse = true,
+                            .title_db = title_db, .album_db = album_db});
+}
+int mp3b200_replaygain_streams_device(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
+                                      const int64_t* pcm_off, const int64_t* nsamples, double* title_db, double* album_db) {
+  return whole_sync<int16_t>({.channels = channels, .samplerate = samplerate, .kbps = kbps, .flags = flags, .nstreams = nstreams,
+                              .d_pcm = d_pcm, .pcm_off = pcm_off, .nsamples = nsamples, .encode = false, .analyse = true,
+                              .title_db = title_db, .album_db = album_db});
+}
+int mp3b200_replaygain_streams_device_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* d_pcm,
+                                          const int64_t* pcm_off, const int64_t* nsamples, double* title_db, double* album_db) {
+  return whole_sync<float>({.channels = channels, .samplerate = samplerate, .kbps = kbps, .flags = flags, .nstreams = nstreams,
+                            .d_pcm = d_pcm, .pcm_off = pcm_off, .nsamples = nsamples, .encode = false, .analyse = true,
+                            .title_db = title_db, .album_db = album_db});
+}
+
+/* the tag step alone: the encoded files are the call's rows, and its output */
+int mp3b200_finish_tags_device(int channels, int samplerate, int kbps, int flags, int nstreams, uint8_t* d_files,
+                               const int64_t* file_off, const int64_t* nsamples, const double* title_db, int64_t* file_bytes) {
+  return whole_sync<uint8_t>({.channels = channels, .samplerate = samplerate, .kbps = kbps, .flags = flags, .nstreams = nstreams,
+                              .d_pcm = d_files, .pcm_off = file_off, .nsamples = nsamples, .encode = false, .tagged = true,
+                              .d_out = d_files, .out_off = file_off, .out_bytes = file_bytes, .title_in = title_db});
+}
+
+}  // extern "C"
+
+extern "C" {
 
 int mp3b200_debug_stages(int channels, int samplerate, int kbps, const int16_t* left, const int16_t* right,
                          int64_t nsamples, const int32_t* force_blocktype, float* xr, int32_t* blocktype,
@@ -1443,22 +1732,19 @@ int debug_stages(const mp3b200_debug_taps* tp, const T* left, const T* right) {
   Config* cfg;
   int rc = get_config(channels, tp->samplerate, tp->kbps, tp->flags & ~MP3B200_DEBUG_SKIP_SHORT, &cfg);
   if (rc || (rc = check_input(cfg, 1, &left, &right, &nsamples))) return rc;
-  if (!right) right = left;
   const int nch = cfg->host.nch;
   const int G = cfg->host.mode_gr;
-  /* nsamples are the caller's (input) samples; frames and granules are those of the rate the configuration encodes at */
-  const long long F = frames_for(nsamples, G, cfg->rs.ratio), U = G * F;
-  /* one whole stream, staged and encoded like a batch of host streams of one */
-  const long long nbytes = bytes_of_frames(cfg->host, 0, F);
-  T* d_pcm = staging_pcm<T>((size_t)(nsamples * nch + 8));
-  if (!d_pcm) return MP3B200_ERR_CUDA;
-  rc = t_ctx.out.fit((size_t)nbytes + 8);
-  if (rc) return rc;
+  /* one whole stream, staged and encoded like a batch of host streams of one.  nsamples are the caller's (input) samples;
+   * frames and granules are those of the rate the configuration encodes at. */
+  const StreamPlan pl = stream_plan(cfg, 1, &nsamples, false, nullptr);
+  const long long F = pl.frames[0], U = G * F, nbytes = pl.audio[0];
+  std::vector<int64_t> pcm_off;
+  T* d_pcm = nullptr;
+  PcmArrival arr;
+  if ((rc = upload_host_rows(cfg, 1, &left, &right, &nsamples, pcm_off, d_pcm, arr)) || (rc = t_ctx.out.fit((size_t)nbytes + 8))) return rc;
   uint8_t* d_out = t_ctx.out.p;
-  CK(cudaMemcpyAsync(d_pcm, left, sizeof(T) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
-  if (nch == 2) CK(cudaMemcpyAsync(d_pcm + nsamples, right, sizeof(T) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
   const int64_t zero = 0;
-  std::vector<StreamDesc> sds = whole_streams(cfg, 1, d_pcm, &zero, &nsamples, &zero);
+  std::vector<StreamDesc> sds = whole_streams(cfg, pl, 1, d_pcm, pcm_off.data(), &nsamples, d_out, &zero);
   const bool want_gi = ginfo || tp->scalefac || tp->subblock_gain;
   const bool want_prep = tp->xmin || tp->max_nonzero_coeff || tp->xrpow_max;
   const bool want_q = tp->scfsi || tp->old_value || tp->cur_step;
@@ -1467,7 +1753,8 @@ int debug_stages(const mp3b200_debug_taps* tp, const T* left, const T* right) {
   opts.force_bt = force_blocktype;
   opts.all_short = !(tp->flags & MP3B200_DEBUG_SKIP_SHORT);
   opts.stop_after_mdct = !(l3_enc || bytes_out || want_gi || want_prep || want_q);
-  rc = launch_streams(t_ctx, cfg, sds, d_out, opts);
+  opts.arrival = &arr;
+  rc = launch_streams(t_ctx, cfg, sds, opts);
   /* read-back on the thread's stream (the launch has drained it) */
   auto fetch = [](void* dst, const void* src, size_t bytes) {
     const cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, t_ctx.st);
@@ -1561,17 +1848,14 @@ int debug_resample(int channels, int samplerate, int kbps, const T* left, const 
   if (rc) return rc;
   if (cfg->rs.ratio == 1) { g_err = "this configuration does not resample"; return MP3B200_ERR_CONFIG; }
   if ((rc = check_input(cfg, 1, &left, &right, &nsamples))) return rc;
-  if (!right) right = left;
   if (ny == 0) return 0;
   const int nch = cfg->host.nch;
-  T* d_pcm = staging_pcm<T>((size_t)(nsamples * nch + 8));
-  if (!d_pcm) return MP3B200_ERR_CUDA;
-  rc = t_ctx.ws.rs_y.fit((size_t)(ny * nch));
-  if (rc) return rc;
-  if (nsamples > 0) {
-    CK(cudaMemcpyAsync(d_pcm, left, sizeof(T) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
-    if (nch == 2) CK(cudaMemcpyAsync(d_pcm + nsamples, right, sizeof(T) * nsamples, cudaMemcpyHostToDevice, t_ctx.st));
-  }
+  std::vector<int64_t> pcm_off;
+  T* d_pcm = nullptr;
+  PcmArrival arr;
+  if ((rc = upload_host_rows(cfg, 1, &left, &right, &nsamples, pcm_off, d_pcm, arr)) || (rc = t_ctx.ws.rs_y.fit((size_t)(ny * nch))))
+    return rc;
+  for (int j = 0; j < arr.chunks; j++) CK(cudaStreamWaitEvent(t_ctx.st, arr.ready[j], 0));   /* the resampler reads all of it */
   StreamDesc sd;
   memset(&sd, 0, sizeof sd);
   sd.pcm[0] = d_pcm;
@@ -1595,6 +1879,35 @@ int debug_resample(int channels, int samplerate, int kbps, const T* left, const 
   CK(cudaStreamSynchronize(t_ctx.st));
   return 0;
 }
+
+/* one tagged whole stream with the analysis, and the analysis's windows */
+template <class T>
+int debug_replaygain(int channels, int samplerate, int kbps, int flags, const T* left, const T* right, int64_t nsamples,
+                     double* win_sums, int32_t* win_idx, int64_t nwin_cap, int32_t* hist, double* title_db, int32_t* stats) {
+  RgJob job;
+  job.want_windows = true;
+  const Config* c = encodable_config(channels, samplerate, kbps, flags & MP3B200_RESAMPLE);
+  if (!c) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
+  if (!c->tag.fits) { g_err = "the tag does not fit: no ReplayGain"; return MP3B200_ERR_CONFIG; }
+  const int64_t cap = bytes_of_frames(c->host, 0, frames_for(nsamples, c->host.mode_gr, c->rs.ratio)) + c->tag.frame_bytes;
+  std::vector<uint8_t> out((size_t)cap);
+  uint8_t* outp = out.data();
+  int64_t ob = 0;
+  const int rc = whole_sync<T>({.channels = channels, .samplerate = samplerate, .kbps = kbps,
+                                .flags = (flags & MP3B200_RESAMPLE) | MP3B200_REPLAYGAIN, .nstreams = 1, .left = &left, .right = &right,
+                                .nsamples = &nsamples, .tagged = true, .analyse = true, .out = &outp, .cap = &cap, .out_bytes = &ob,
+                                .job = &job});
+  if (rc) return rc;
+  const long long n = (long long)job.win_idx.size();
+  for (long long w = 0; w < n && w < nwin_cap; w++) {
+    if (win_sums) { win_sums[2 * w] = job.win_sum[2 * w]; win_sums[2 * w + 1] = job.win_sum[2 * w + 1]; }
+    if (win_idx) win_idx[w] = job.win_idx[w];
+  }
+  if (hist && !job.hist0.empty()) memcpy(hist, job.hist0.data(), sizeof(int32_t) * RG_HIST);
+  if (title_db) *title_db = job.title_db[0];
+  if (stats) { stats[0] = (int32_t)n; stats[1] = job.passes; stats[2] = job.reruns; memcpy(stats + 3, &job.ms, sizeof(float)); }
+  return 0;
+}
 }  // namespace
 
 extern "C" {
@@ -1611,71 +1924,17 @@ int mp3b200_debug_resample_f32(int channels, int samplerate, int kbps, const flo
   return debug_resample(channels, samplerate, kbps, left, right, nsamples, y, ny);
 }
 
+int mp3b200_debug_replaygain(int channels, int samplerate, int kbps, int flags, const int16_t* left, const int16_t* right,
+                             int64_t nsamples, double* win_sums, int32_t* win_idx, int64_t nwin_cap, int32_t* hist,
+                             double* title_db, int32_t* stats) {
+  return debug_replaygain(channels, samplerate, kbps, flags, left, right, nsamples, win_sums, win_idx, nwin_cap, hist, title_db, stats);
+}
+int mp3b200_debug_replaygain_f32(int channels, int samplerate, int kbps, int flags, const float* left, const float* right,
+                                 int64_t nsamples, double* win_sums, int32_t* win_idx, int64_t nwin_cap, int32_t* hist,
+                                 double* title_db, int32_t* stats) {
+  return debug_replaygain(channels, samplerate, kbps, flags, left, right, nsamples, win_sums, win_idx, nwin_cap, hist, title_db, stats);
+}
 }  // extern "C"
-
-/* ---- container / metadata step (SURVEY.md 8(f3)): music CRC on the device, tag frames on the host ---- */
-namespace {
-CrcTables g_crc_host;                              /* byte table + zero-byte powers (k_tag.cuh), built once */
-bool g_crc_host_ready = false;
-CrcTables* g_crc_dev[MP3_MAX_DEVICES] = {};        /* per device copy */
-
-const CrcTables& crc_host() {
-  std::lock_guard<std::mutex> lk(g_mu);
-  if (!g_crc_host_ready) { crc_host_tables(&g_crc_host); g_crc_host_ready = true; }
-  return g_crc_host;
-}
-
-/* uploads the CRC tables to `device` on first use there (g_crc_dev) */
-int crc_tables_on(int device) {
-  const CrcTables& ht = crc_host();
-  std::lock_guard<std::mutex> lk(g_mu);
-  if (!g_crc_dev[device]) {
-    CK(cudaMalloc(&g_crc_dev[device], sizeof(CrcTables)));
-    CK(cudaMemcpy(g_crc_dev[device], &ht, sizeof(CrcTables), cudaMemcpyHostToDevice));
-  }
-  return 0;
-}
-
-/* Queues on c.st, behind whatever wrote the bytes, the music CRC (CRC-16, start 0) of the byte ranges [at[r], at[r] + len[r])
- * (absolute device addresses, like the packer's output offsets) into c.crc[r]: one k_music_crc launch per 65535 ranges.
- * The ranges go up through upload(); the CRC tables must already be on the device (crc_tables_on). */
-int queue_music_crc(ThreadCtx& c, const std::vector<long long>& at, const std::vector<long long>& len) {
-  const int R = (int)at.size();
-  if (R == 0) return 0;
-  std::vector<long long> ranges((size_t)2 * R);
-  long long longest = 0;
-  for (int i = 0; i < R; i++) { ranges[i] = at[i]; ranges[(size_t)R + i] = len[i]; longest = len[i] > longest ? len[i] : longest; }
-  int rc = 0;
-  if ((rc = c.crc_ranges.fit((size_t)2 * R)) || (rc = c.crc.fit((size_t)R)) ||
-      (rc = upload(c, c.crc_ranges.p, ranges.data(), sizeof(long long) * ranges.size())))
-    return rc;
-  CK(cudaMemsetAsync(c.crc.p, 0, sizeof(unsigned) * (size_t)R, c.st));
-  const long long pieces = (longest + CRC_PIECE_BYTES - 1) / CRC_PIECE_BYTES;
-  for (int r0 = 0; r0 < R && longest > 0; r0 += 65535) {
-    const int nr = R - r0 < 65535 ? R - r0 : 65535;
-    dim3 grid((unsigned)((pieces + CRC_WARPS - 1) / CRC_WARPS), (unsigned)nr);
-    k_music_crc<<<grid, CRC_WARPS * 32, 0, c.st>>>(nullptr, c.crc_ranges.p + r0, c.crc_ranges.p + R + r0, g_crc_dev[c.device], c.crc.p + r0);
-    g_launches++;
-  }
-  return 0;
-}
-
-/* mp3b200_lametag_build(_ex): `field` is the tag's Radio Replay Gain field, 0 for a stream nobody analysed */
-int build_lametag(int channels, int samplerate, int kbps, int flags, int64_t nframes, int64_t music_bytes, int music_crc,
-                  int encoder_padding, int field, uint8_t* buf, int cap) {
-  const Config* c = host_config(channels, samplerate, kbps, flags);
-  if (!c) return MP3B200_ERR_CONFIG;
-  const Mp3TagParams& p = c->tag;
-  if (!p.fits || nframes <= 0) return 0;
-  if (!buf || cap < p.frame_bytes) return p.frame_bytes;              /* like getLameTagFrame: the size it needs */
-  Mp3SeekBag* bag = new Mp3SeekBag();
-  bag->reset();
-  bag->add_frames(nframes, p.kbps);
-  const int n = mp3_tag_frame(p, *bag, music_bytes, (unsigned)music_crc, encoder_padding, buf, field);
-  delete bag;
-  return n;
-}
-}  // namespace
 
 extern "C" {
 
@@ -1739,353 +1998,10 @@ int mp3b200_lametag_build(int channels, int samplerate, int kbps, int64_t nframe
   return build_lametag(channels, samplerate, kbps, 0, nframes, music_bytes, music_crc, encoder_padding, 0, buf, cap);
 }
 
-int mp3b200_encode_streams_tagged(int channels, int samplerate, int kbps, int nstreams, const int16_t* const* left,
-                                  const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
-                                  const int64_t* cap, int64_t* out_bytes) {
-  return mp3b200_encode_streams_tagged_ex(channels, samplerate, kbps, 0, nstreams, left, right, nsamples, out, cap, out_bytes,
-                                          nullptr, nullptr);
-}
-
-}  // extern "C"
-
-namespace {
-/* What is known about tagged whole streams before anything runs, in closed form from the lamejs FIFO: each stream's frames,
- * its end padding and the size of its tag frame (tfs, or 0: no frame), and, with `rg`, the pieces the analysis sees
- * (rg->specs), whether or not the tag fits. */
-struct TaggedPlan {
-  int tfs = 0;
-  std::vector<long long> frames;
-  std::vector<int> padding, tag;
-};
-TaggedPlan stream_plan(const Config* cfg, int nstreams, const int64_t* nsamples, RgJob* rg) {
-  TaggedPlan pl;
-  pl.tfs = cfg->tag.fits ? cfg->tag.frame_bytes : 0;
-  if (rg) rg->specs.assign((size_t)nstreams, RgSpec());
-  pl.frames.resize((size_t)nstreams); pl.padding.resize((size_t)nstreams); pl.tag.resize((size_t)nstreams);
-  for (int s = 0; s < nstreams; s++) {
-    LameFifo fifo(cfg->host.mode_gr, cfg->rs.ratio);
-    if (rg) { rg->specs[s].stream = s; fifo.pieces = &rg->specs[s].pieces; }
-    const long long fed = fifo.feed(nsamples[s]);
-    const FifoFlush fl = fifo.flush();
-    pl.frames[s] = fed + fl.frames;
-    pl.padding[s] = fl.end_padding;
-    pl.tag[s] = pl.tfs > 0 && pl.frames[s] > 0 ? pl.tfs : 0;
-  }
-  return pl;
-}
-
-/* stream_plan for the tagged encodes: `rg` is reset to NULL where lamejs does not analyse, which it does only when the tag
- * is written (Lame.js:911-916) */
-TaggedPlan tagged_plan(const Config* cfg, int nstreams, const int64_t* nsamples, RgJob*& rg) {
-  if (rg && !cfg->tag.fits) rg = nullptr;
-  return stream_plan(cfg, nstreams, nsamples, rg);
-}
-
-/* Queues, behind the packer on c.st, what turns the audio of tagged whole streams into files: the music CRC of each stream
- * where its audio lies (sds[i].out_base, an absolute address), and k_tag_finish, which completes each template frame with
- * it and with the field of gain[i] (device; NULL: nothing was analysed, the field is 0) and writes it to d_out + out_off[i].
- * The templates are mp3_tag_frame with music CRC 0 and gain field 0.  Every upload goes through upload(). */
-int finish_tagged(ThreadCtx& c, Config* cfg, const TaggedPlan& plan, const std::vector<StreamDesc>& sds, const std::vector<long long>& audio,
-                  uint8_t* d_out, const int64_t* out_off, const double* gain) {
-  const int S = (int)sds.size();
-  const Mp3TagParams& p = cfg->tag;
-  int ntags = 0;
-  for (int i = 0; i < S; i++) ntags += plan.tag[i] ? 1 : 0;
-  if (ntags == 0) return 0;
-  std::vector<long long> at((size_t)S);
-  for (int i = 0; i < S; i++) at[i] = sds[i].out_base;
-  int rc = queue_music_crc(c, at, audio);
-  if (rc) return rc;
-  /* the template frames: everything but the music CRC, the gain field and the frame's own CRC */
-  const size_t tfs = (size_t)plan.tfs;
-  std::vector<TagDest> dst((size_t)ntags);
-  std::vector<uint8_t> frames(tfs * (size_t)ntags);
-  Mp3SeekBag* bag = new Mp3SeekBag();
-  for (int i = 0, k = 0; i < S; i++) {
-    if (!plan.tag[i]) continue;
-    bag->reset();
-    bag->add_frames(plan.frames[i], p.kbps);
-    mp3_tag_frame(p, *bag, audio[i], 0, plan.padding[i], frames.data() + tfs * (size_t)k, 0);
-    dst[k].at = d_out + out_off[i]; dst[k].stream = i;
-    k++;
-  }
-  delete bag;
-  const size_t dst_bytes = (sizeof(TagDest) * (size_t)ntags + 255) & ~(size_t)255;
-  if ((rc = c.tags.fit(dst_bytes + frames.size())) || (rc = upload(c, c.tags.p, dst.data(), sizeof(TagDest) * dst.size())) ||
-      (rc = upload(c, c.tags.p + dst_bytes, frames.data(), frames.size())))
-    return rc;
-  k_tag_finish<<<ntags, TAG_FINISH_THREADS, 0, c.st>>>(reinterpret_cast<const TagDest*>(c.tags.p), c.tags.p + dst_bytes, p, c.crc.p, gain);
-  g_launches++;
-  CK(cudaGetLastError());
-  return 0;
-}
-
-/* The tag step of the synchronous tagged whole streams, once their audio lies at sds[s].out_base (audio[s] bytes, queued
- * on t_ctx.st or already there): finish_tagged with gain[s] (device; NULL: field 0), out_bytes[s] = the file's length, and
- * with `out` each file copied from d_out + out_off[s] into out[s].  Returns with t_ctx.st drained. */
-int finish_files(Config* cfg, const TaggedPlan& plan, const std::vector<StreamDesc>& sds, const std::vector<long long>& audio,
-                 uint8_t* d_out, const int64_t* out_off, const double* gain, uint8_t* const* out, int64_t* out_bytes) {
-  int rc = crc_tables_on(t_ctx.device);
-  if (rc || (rc = finish_tagged(t_ctx, cfg, plan, sds, audio, d_out, out_off, gain))) return rc;
-  for (size_t s = 0; s < sds.size(); s++) {
-    out_bytes[s] = audio[s] + plan.tag[s];
-    if (out) CK(cudaMemcpyAsync(out[s], d_out + out_off[s], (size_t)out_bytes[s], cudaMemcpyDeviceToHost, t_ctx.st));
-  }
-  CK(cudaStreamSynchronize(t_ctx.st));
-  CK(cudaGetLastError());
-  return 0;
-}
-
-/* The synchronous tagged whole streams (encodeBuffer(everything) + flush() on fresh encoders with the tag on), once their PCM
- * is on the device: `sds` are the batch's whole_streams descriptors, and o.arrival / o.f32_in say how their rows arrive.
- * File s -- its tag frame (plan.tag[s] bytes), then its audio -- is written at d_out + out_off[s]; with `out` (host callers,
- * d_out in t_ctx.out) it is then copied into out[s].  out_bytes[s] receives the file's length, `rg` (as tagged_plan left
- * it) the analysis, and title_db[s] / album_db (optional) its gains, RG_NOT_ENOUGH_SAMPLES where nothing ran. */
-int encode_tagged(Config* cfg, const TaggedPlan& plan, RgJob* rg, std::vector<StreamDesc>& sds, LaunchOpts o, uint8_t* d_out,
-                  const int64_t* out_off, uint8_t* const* out, int64_t* out_bytes, double* title_db, double* album_db) {
-  const int S = (int)sds.size();
-  if (S > 0) {
-    /* The packer gets a null base and each stream's absolute output address, its audio behind the room of its tag frame */
-    std::vector<long long> audio((size_t)S);
-    for (int s = 0; s < S; s++) {
-      sds[s].out_base = (long long)(uintptr_t)(d_out + out_off[s] + plan.tag[s]);
-      audio[s] = bytes_of_frames(cfg->host, 0, sds[s].nframes);
-    }
-    o.rg = rg;
-    int rc = launch_streams(t_ctx, cfg, sds, nullptr, o);     /* returns with the refusals checked: no tag for a refused call */
-    if (rc || (rc = finish_files(cfg, plan, sds, audio, d_out, out_off, rg ? t_ctx.rg_gain.p : nullptr, out, out_bytes))) return rc;
-  }
-  const bool ran = rg && (int)rg->title_db.size() == S && S > 0;
-  for (int s = 0; title_db && s < S; s++) title_db[s] = ran ? rg->title_db[s] : RG_NOT_ENOUGH_SAMPLES;
-  if (album_db) *album_db = ran ? rg->album_db : RG_NOT_ENOUGH_SAMPLES;
-  return 0;
-}
-
-/* The checks a synchronous tagged call starts with, and its configuration */
-int tagged_config(int channels, int samplerate, int kbps, int flags, int nstreams, Config** cfg) {
-  if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
-  if (flags & ~(MP3B200_RESAMPLE | MP3B200_REPLAYGAIN)) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
-  return get_config(channels, samplerate, kbps, flags & MP3B200_RESAMPLE, cfg);
-}
-
-/* Host rows in, host files out: the PCM is checked and uploaded as mp3b200_encode_streams does it, and out[s] (cap[s] bytes)
- * receives file s.  With MP3B200_REPLAYGAIN, `job` receives the analysis. */
-template <class T>
-int encode_tagged_host(int channels, int samplerate, int kbps, int flags, int nstreams, const T* const* left, const T* const* right,
-                       const int64_t* nsamples, uint8_t* const* out, const int64_t* cap, int64_t* out_bytes, double* title_db,
-                       double* album_db, RgJob& job) {
-  Config* cfg;
-  int rc = tagged_config(channels, samplerate, kbps, flags, nstreams, &cfg);
-  if (rc || (rc = check_input(cfg, nstreams, left, right, nsamples))) return rc;
-  RgJob* rg = flags & MP3B200_REPLAYGAIN ? &job : nullptr;
-  const TaggedPlan plan = tagged_plan(cfg, nstreams, nsamples, rg);
-  std::vector<int64_t> file_off;
-  std::vector<StreamDesc> sds;
-  PcmArrival arr;
-  if ((rc = stage_host_streams(cfg, nstreams, left, right, nsamples, cap, plan.tag.data(), out_bytes, file_off, sds, arr))) return rc;
-  LaunchOpts o;
-  o.arrival = &arr;
-  o.f32_in = std::is_same_v<T, float>;
-  return encode_tagged(cfg, plan, rg, sds, o, t_ctx.out.p, file_off.data(), out, out_bytes, title_db, album_db);
-}
-
-/* Device rows in (laid out as mp3b200_encode_streams_device reads them), device files out: file s at d_out + out_off[s] */
-template <class T>
-int encode_tagged_device(int channels, int samplerate, int kbps, int flags, int nstreams, const T* d_pcm, const int64_t* pcm_off,
-                         const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off, int64_t* out_bytes, double* title_db,
-                         double* album_db) {
-  Config* cfg;
-  const int rc = tagged_config(channels, samplerate, kbps, flags, nstreams, &cfg);
-  if (rc) return rc;
-  RgJob job;
-  RgJob* rg = flags & MP3B200_REPLAYGAIN ? &job : nullptr;
-  const TaggedPlan plan = tagged_plan(cfg, nstreams, nsamples, rg);
-  std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off, nsamples, out_off);
-  LaunchOpts o;
-  o.f32_in = std::is_same_v<T, float>;
-  return encode_tagged(cfg, plan, rg, sds, o, d_out, out_off, nullptr, out_bytes, title_db, album_db);
-}
-
-/* The argument checks of the standalone analysis and tag step, made before anything touches the device: `rows` is the
- * call's row array (left, or d_pcm / d_files) and `offs` its offsets, which host rows (host_rows) do not have */
-int whole_stream_args(int nstreams, int flags, const void* rows, const int64_t* offs, bool host_rows, const int64_t* nsamples) {
-  if (nstreams < 0) { g_err = "negative stream count"; return MP3B200_ERR_HANDLE; }
-  if (flags & ~MP3B200_RESAMPLE) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
-  if (nstreams == 0) return MP3B200_OK;
-  if (!rows || !nsamples || (!host_rows && !offs)) { g_err = "null array"; return MP3B200_ERR_HANDLE; }
-  for (int s = 0; s < nstreams; s++)
-    if (nsamples[s] < 0) { g_err = "negative sample count"; return MP3B200_ERR_HANDLE; }
-  return MP3B200_OK;
-}
-
-/* The ReplayGain analysis of whole streams (descriptors `sds` from whole_streams) without the encoder: the RgSpecs of the
- * tagged whole-stream path (stream_plan), analysed by launch_streams on the staged or resampled rows (o.analyse_only) */
-int analyse_streams(Config* cfg, int nstreams, const int64_t* nsamples, std::vector<StreamDesc>& sds, LaunchOpts o,
-                    double* title_db, double* album_db) {
-  RgJob job;
-  stream_plan(cfg, nstreams, nsamples, &job);
-  o.rg = &job;
-  o.analyse_only = true;
-  const int rc = launch_streams(t_ctx, cfg, sds, nullptr, o);
-  if (rc) return rc;
-  const bool ran = (int)job.title_db.size() == nstreams && nstreams > 0;
-  for (int s = 0; title_db && s < nstreams; s++) title_db[s] = ran ? job.title_db[s] : RG_NOT_ENOUGH_SAMPLES;
-  if (album_db) *album_db = ran ? job.album_db : RG_NOT_ENOUGH_SAMPLES;
-  return 0;
-}
-
-template <class T>
-int replaygain_host(int channels, int samplerate, int kbps, int flags, int nstreams, const T* const* left, const T* const* right,
-                    const int64_t* nsamples, double* title_db, double* album_db) {
-  int rc = whole_stream_args(nstreams, flags, left, nullptr, true, nsamples);
-  if (rc) return rc;
-  for (int s = 0; s < nstreams; s++)
-    if (!left[s]) { g_err = "null row"; return MP3B200_ERR_HANDLE; }
-  Config* cfg;
-  if ((rc = get_config(channels, samplerate, kbps, flags, &cfg)) || (rc = check_input(cfg, nstreams, left, right, nsamples))) return rc;
-  std::vector<int64_t> pcm_off, out_off((size_t)nstreams, 0);
-  T* d_pcm = nullptr;
-  PcmArrival arr;
-  if (nstreams > 0 && (rc = upload_host_rows(cfg, nstreams, left, right, nsamples, pcm_off, d_pcm, arr))) return rc;
-  std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off.data(), nsamples, out_off.data());
-  LaunchOpts o;
-  o.arrival = nstreams > 0 ? &arr : nullptr;
-  o.f32_in = std::is_same_v<T, float>;
-  return analyse_streams(cfg, nstreams, nsamples, sds, o, title_db, album_db);
-}
-
-template <class T>
-int replaygain_device(int channels, int samplerate, int kbps, int flags, int nstreams, const T* d_pcm, const int64_t* pcm_off,
-                      const int64_t* nsamples, double* title_db, double* album_db) {
-  int rc = whole_stream_args(nstreams, flags, d_pcm, pcm_off, false, nsamples);
-  if (rc) return rc;
-  Config* cfg;
-  if ((rc = get_config(channels, samplerate, kbps, flags, &cfg))) return rc;
-  std::vector<int64_t> out_off((size_t)nstreams, 0);
-  std::vector<StreamDesc> sds = whole_streams(cfg, nstreams, d_pcm, pcm_off, nsamples, out_off.data());
-  LaunchOpts o;
-  o.f32_in = std::is_same_v<T, float>;
-  return analyse_streams(cfg, nstreams, nsamples, sds, o, title_db, album_db);
-}
-}  // namespace
-
-extern "C" {
-
-int mp3b200_encode_streams_tagged_ex(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
-                                     const int16_t* const* right, const int64_t* nsamples, uint8_t* const* out,
-                                     const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db) {
-  RgJob job;
-  return encode_tagged_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, title_db, album_db, job);
-}
-int mp3b200_encode_streams_tagged_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* const* left,
-                                      const float* const* right, const int64_t* nsamples, uint8_t* const* out,
-                                      const int64_t* cap, int64_t* out_bytes, double* title_db, double* album_db) {
-  RgJob job;
-  return encode_tagged_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, out, cap, out_bytes, title_db, album_db, job);
-}
-
-int mp3b200_encode_streams_tagged_device(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
-                                         const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off,
-                                         int64_t* out_bytes, double* title_db, double* album_db) {
-  return encode_tagged_device(channels, samplerate, kbps, flags, nstreams, d_pcm, pcm_off, nsamples, d_out, out_off, out_bytes,
-                              title_db, album_db);
-}
-int mp3b200_encode_streams_tagged_device_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* d_pcm,
-                                             const int64_t* pcm_off, const int64_t* nsamples, uint8_t* d_out, const int64_t* out_off,
-                                             int64_t* out_bytes, double* title_db, double* album_db) {
-  return encode_tagged_device(channels, samplerate, kbps, flags, nstreams, d_pcm, pcm_off, nsamples, d_out, out_off, out_bytes,
-                              title_db, album_db);
-}
-
 int mp3b200_lametag_build_ex(int channels, int samplerate, int kbps, int flags, int64_t nframes, int64_t music_bytes, int music_crc,
                              int encoder_padding, int radio_gain, uint8_t* buf, int cap) {
   return build_lametag(channels, samplerate, kbps, flags, nframes, music_bytes, music_crc, encoder_padding,
                        mp3_radio_gain_field(radio_gain), buf, cap);
-}
-
-int mp3b200_replaygain_streams(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* const* left,
-                               const int16_t* const* right, const int64_t* nsamples, double* title_db, double* album_db) {
-  return replaygain_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, title_db, album_db);
-}
-int mp3b200_replaygain_streams_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* const* left,
-                                   const float* const* right, const int64_t* nsamples, double* title_db, double* album_db) {
-  return replaygain_host(channels, samplerate, kbps, flags, nstreams, left, right, nsamples, title_db, album_db);
-}
-int mp3b200_replaygain_streams_device(int channels, int samplerate, int kbps, int flags, int nstreams, const int16_t* d_pcm,
-                                      const int64_t* pcm_off, const int64_t* nsamples, double* title_db, double* album_db) {
-  return replaygain_device(channels, samplerate, kbps, flags, nstreams, d_pcm, pcm_off, nsamples, title_db, album_db);
-}
-int mp3b200_replaygain_streams_device_f32(int channels, int samplerate, int kbps, int flags, int nstreams, const float* d_pcm,
-                                          const int64_t* pcm_off, const int64_t* nsamples, double* title_db, double* album_db) {
-  return replaygain_device(channels, samplerate, kbps, flags, nstreams, d_pcm, pcm_off, nsamples, title_db, album_db);
-}
-
-int mp3b200_finish_tags_device(int channels, int samplerate, int kbps, int flags, int nstreams, uint8_t* d_files,
-                               const int64_t* file_off, const int64_t* nsamples, const double* title_db, int64_t* file_bytes) {
-  int rc = whole_stream_args(nstreams, flags, d_files, file_off, false, nsamples);
-  if (rc) return rc;
-  if (nstreams > 0 && !file_bytes) { g_err = "file_bytes is NULL"; return MP3B200_ERR_HANDLE; }
-  Config* cfg;
-  if ((rc = get_config(channels, samplerate, kbps, flags, &cfg)) || (rc = wait_legacy(t_ctx))) return rc;
-  const TaggedPlan plan = stream_plan(cfg, nstreams, nsamples, nullptr);
-  std::vector<StreamDesc> sds((size_t)nstreams);
-  std::vector<long long> audio((size_t)nstreams);
-  for (int s = 0; s < nstreams; s++) {
-    memset(&sds[s], 0, sizeof(StreamDesc));
-    sds[s].out_base = (long long)(uintptr_t)(d_files + file_off[s] + plan.tag[s]);
-    audio[s] = bytes_of_frames(cfg->host, 0, plan.frames[s]);
-  }
-  const double* gain = nullptr;
-  if (title_db && nstreams > 0) {
-    if ((rc = t_ctx.rg_gain.fit((size_t)nstreams)) || (rc = upload(t_ctx, t_ctx.rg_gain.p, title_db, sizeof(double) * (size_t)nstreams)))
-      return rc;
-    gain = t_ctx.rg_gain.p;
-  }
-  return finish_files(cfg, plan, sds, audio, d_files, file_off, gain, nullptr, file_bytes);
-}
-
-}  // extern "C"
-
-namespace {
-template <class T>
-int debug_replaygain(int channels, int samplerate, int kbps, int flags, const T* left, const T* right, int64_t nsamples,
-                     double* win_sums, int32_t* win_idx, int64_t nwin_cap, int32_t* hist, double* title_db, int32_t* stats) {
-  if (nsamples < 0 || !left) return MP3B200_ERR_HANDLE;
-  RgJob job;
-  job.want_windows = true;
-  const Config* c = encodable_config(channels, samplerate, kbps, flags & MP3B200_RESAMPLE);
-  if (!c) { g_err = "unsupported configuration"; return MP3B200_ERR_CONFIG; }
-  if (!c->tag.fits) { g_err = "the tag does not fit: no ReplayGain"; return MP3B200_ERR_CONFIG; }
-  const int64_t cap = bytes_of_frames(c->host, 0, frames_for(nsamples, c->host.mode_gr, c->rs.ratio)) + c->tag.frame_bytes;
-  std::vector<uint8_t> out((size_t)cap);
-  uint8_t* outp = out.data();
-  int64_t ob = 0;
-  const int rc = encode_tagged_host(channels, samplerate, kbps, (flags & MP3B200_RESAMPLE) | MP3B200_REPLAYGAIN, 1, &left, &right,
-                                    &nsamples, &outp, &cap, &ob, nullptr, nullptr, job);
-  if (rc) return rc;
-  const long long n = (long long)job.win_idx.size();
-  for (long long w = 0; w < n && w < nwin_cap; w++) {
-    if (win_sums) { win_sums[2 * w] = job.win_sum[2 * w]; win_sums[2 * w + 1] = job.win_sum[2 * w + 1]; }
-    if (win_idx) win_idx[w] = job.win_idx[w];
-  }
-  if (hist && !job.hist0.empty()) memcpy(hist, job.hist0.data(), sizeof(int32_t) * RG_HIST);
-  if (title_db) *title_db = job.title_db[0];
-  if (stats) { stats[0] = (int32_t)n; stats[1] = job.passes; stats[2] = job.reruns; memcpy(stats + 3, &job.ms, sizeof(float)); }
-  return 0;
-}
-}  // namespace
-
-extern "C" {
-
-int mp3b200_debug_replaygain(int channels, int samplerate, int kbps, int flags, const int16_t* left, const int16_t* right,
-                             int64_t nsamples, double* win_sums, int32_t* win_idx, int64_t nwin_cap, int32_t* hist,
-                             double* title_db, int32_t* stats) {
-  return debug_replaygain(channels, samplerate, kbps, flags, left, right, nsamples, win_sums, win_idx, nwin_cap, hist, title_db, stats);
-}
-int mp3b200_debug_replaygain_f32(int channels, int samplerate, int kbps, int flags, const float* left, const float* right,
-                                 int64_t nsamples, double* win_sums, int32_t* win_idx, int64_t nwin_cap, int32_t* hist,
-                                 double* title_db, int32_t* stats) {
-  return debug_replaygain(channels, samplerate, kbps, flags, left, right, nsamples, win_sums, win_idx, nwin_cap, hist, title_db, stats);
 }
 
 }  // extern "C"

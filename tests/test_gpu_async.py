@@ -287,12 +287,14 @@ def test_refusals(M):
         assert async_once(M, good, sess)[0] == ref
         # refused before anything is queued, with the synchronous call's errors
         i16 = Batch(M, 2, 44100, 128, signals(2, 44100, [3000], 0xBAD1))
-        for cfg, flags in (((2, 44100, 128), M.REPLAYGAIN), ((2, 44100, 128), 8), ((3, 44100, 128), 0), ((2, 44100, 7), 0)):
+        neg = np.array([-5], dtype=np.int64)
+        ok, c2 = (i16.pcm_off.ctypes.data, i16.ns.ctypes.data), (2, 44100, 128)
+        for cfg, flags, rows in ((c2, M.REPLAYGAIN, ok), (c2, 8, ok), ((3, 44100, 128), 0, ok), ((2, 44100, 7), 0, ok),
+                                 (c2, 0, (None, ok[1])), (c2, 0, (ok[0], None)), (c2, 0, (ok[0], neg.ctypes.data))):
             for fn in (M.lib().mp3b200_encode_streams_async, M.lib().mp3b200_encode_streams_device_ex):
                 o = i16.out()
                 st = torch.zeros(4, dtype=torch.int32, device="cuda")
-                args = (*cfg, flags, 1, i16.pcm.data_ptr(), i16.pcm_off.ctypes.data, i16.ns.ctypes.data, o.data_ptr(),
-                        i16.out_off.ctypes.data)
+                args = (*cfg, flags, 1, i16.pcm.data_ptr(), *rows, o.data_ptr(), i16.out_off.ctypes.data)
                 rc = fn(sess._h, *args, st.data_ptr()) if fn is M.lib().mp3b200_encode_streams_async else fn(*args, None)
                 msg = M.lib().mp3b200_last_error()
                 if fn is M.lib().mp3b200_encode_streams_async:

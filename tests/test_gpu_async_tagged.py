@@ -369,12 +369,14 @@ def test_refusals(M):
         # refused before anything is queued, with the synchronous call's codes and texts
         i16 = Tagged(M, 2, 44100, 128, signals(2, 44100, [3000], 0xBAD3))
         ob = np.zeros(1, dtype=np.int64)
-        for cfg, flags in (((2, 44100, 128), 4), ((2, 44100, 128), 8 | M.REPLAYGAIN), ((3, 44100, 128), 0), ((2, 44100, 7), M.REPLAYGAIN)):
+        neg = np.array([-5], dtype=np.int64)
+        ok, c2 = (i16.pcm_off.ctypes.data, i16.ns.ctypes.data), (2, 44100, 128)
+        for cfg, flags, rows in ((c2, 4, ok), (c2, 8 | M.REPLAYGAIN, ok), ((3, 44100, 128), 0, ok), ((2, 44100, 7), M.REPLAYGAIN, ok),
+                                 (c2, M.REPLAYGAIN, (None, ok[1])), (c2, 0, (ok[0], None)), (c2, M.REPLAYGAIN, (ok[0], neg.ctypes.data))):
             o = i16.out()
             st = torch.zeros(8, dtype=torch.int32, device="cuda")
             gains = torch.zeros(2, dtype=torch.float64, device="cuda")
-            args = (*cfg, flags, 1, i16.pcm.data_ptr(), i16.pcm_off.ctypes.data, i16.ns.ctypes.data, o.data_ptr(), i16.out_off.ctypes.data,
-                    ob.ctypes.data)
+            args = (*cfg, flags, 1, i16.pcm.data_ptr(), *rows, o.data_ptr(), i16.out_off.ctypes.data, ob.ctypes.data)
             rc_async = L.mp3b200_encode_streams_tagged_async(sess._h, *args, gains.data_ptr(), st.data_ptr())
             msg_async = L.mp3b200_last_error()
             torch.cuda.synchronize()

@@ -111,37 +111,80 @@ def L():
     return encoder.lib()
 
 
+# Every synchronous whole-stream entry point: its arguments in order (F: flags, N: nstreams, or a buffer role), and which
+# flag bits it takes.  MP3B200_REPLAYGAIN (2) belongs to the tagged encodes alone.
+HOST = ("left", "right", "nsamples")
+DEVICE = ("d_pcm", "pcm_off", "nsamples")
+ENTRIES = {
+    "mp3b200_encode_streams": (("N",) + HOST + ("out", "cap", "out_bytes"), None),
+    "mp3b200_encode_streams_ex": (("F", "N") + HOST + ("out", "cap", "out_bytes"), 1),
+    "mp3b200_encode_streams_f32": (("F", "N") + HOST + ("out", "cap", "out_bytes"), 1),
+    "mp3b200_encode_streams_tagged": (("N",) + HOST + ("out", "cap", "out_bytes"), None),
+    "mp3b200_encode_streams_tagged_ex": (("F", "N") + HOST + ("out", "cap", "out_bytes", "title", "album"), 3),
+    "mp3b200_encode_streams_tagged_f32": (("F", "N") + HOST + ("out", "cap", "out_bytes", "title", "album"), 3),
+    "mp3b200_replaygain_streams": (("F", "N") + HOST + ("title", "album"), 1),
+    "mp3b200_replaygain_streams_f32": (("F", "N") + HOST + ("title", "album"), 1),
+    "mp3b200_encode_streams_device": (("N",) + DEVICE + ("d_out", "out_off", "timings"), None),
+    "mp3b200_encode_streams_device_ex": (("F", "N") + DEVICE + ("d_out", "out_off", "timings"), 1),
+    "mp3b200_encode_streams_device_f32": (("F", "N") + DEVICE + ("d_out", "out_off", "timings"), 1),
+    "mp3b200_encode_streams_tagged_device": (("F", "N") + DEVICE + ("d_out", "out_off", "out_bytes", "title", "album"), 3),
+    "mp3b200_encode_streams_tagged_device_f32": (("F", "N") + DEVICE + ("d_out", "out_off", "out_bytes", "title", "album"), 3),
+    "mp3b200_replaygain_streams_device": (("F", "N") + DEVICE + ("title", "album"), 1),
+    "mp3b200_replaygain_streams_device_f32": (("F", "N") + DEVICE + ("title", "album"), 1),
+    "mp3b200_finish_tags_device": (("F", "N", "d_pcm", "pcm_off", "nsamples", "title", "out_bytes"), 1),
+}
+# what each entry cannot do without: the rows, the offsets of device rows, and the arrays it writes
+OPTIONAL = {"right", "d_out", "title", "album", "timings"}
+
+
 def test_c_entries_refuse_bad_arguments_before_the_device(L):
+    """every bad argument of a whole-stream call is refused by one gate before the configuration and before any CUDA call,
+    so a machine without a device answers with the gate's code, never MP3B200_ERR_CUDA"""
+    import torch
+
     vp = ctypes.c_void_p
-    one = np.array([1000], dtype=np.int64)
-    row = np.zeros(1000, dtype=np.int16)
-    rows = (vp * 1)(row.ctypes.data)
-    title = np.zeros(1, dtype=np.float64)
-    got = np.zeros(1, dtype=np.int64)
-    for host in ("mp3b200_replaygain_streams", "mp3b200_replaygain_streams_f32"):
-        fn = getattr(L, host)
-        assert fn(2, 44100, 128, 0, -1, rows, None, one.ctypes.data, title.ctypes.data, None) == -3
-        assert fn(2, 44100, 128, 0, 1, None, None, one.ctypes.data, title.ctypes.data, None) == -3
-        assert fn(2, 44100, 128, 0, 1, rows, None, None, title.ctypes.data, None) == -3
-        assert fn(2, 44100, 128, 0, 1, (vp * 1)(None), None, one.ctypes.data, title.ctypes.data, None) == -3
-        assert fn(2, 44100, 128, 4, 1, rows, None, one.ctypes.data, title.ctypes.data, None) == -1
-        assert fn(2, 44100, 128, 2, 1, rows, None, one.ctypes.data, title.ctypes.data, None) == -1      # REPLAYGAIN is implied
-        assert fn(2, 44100, 128, 0, 1, rows, None, np.array([-5], np.int64).ctypes.data, title.ctypes.data, None) == -3
-    off = np.zeros(1, dtype=np.int64)
-    for dev in ("mp3b200_replaygain_streams_device", "mp3b200_replaygain_streams_device_f32"):
-        fn = getattr(L, dev)
-        assert fn(2, 44100, 128, 0, -1, row.ctypes.data, off.ctypes.data, one.ctypes.data, None, None) == -3
-        assert fn(2, 44100, 128, 0, 1, None, off.ctypes.data, one.ctypes.data, None, None) == -3
-        assert fn(2, 44100, 128, 0, 1, row.ctypes.data, None, one.ctypes.data, None, None) == -3
-        assert fn(2, 44100, 128, 0, 1, row.ctypes.data, off.ctypes.data, None, None, None) == -3
-        assert fn(2, 44100, 128, 8, 1, row.ctypes.data, off.ctypes.data, one.ctypes.data, None, None) == -1
-    fn = L.mp3b200_finish_tags_device
-    assert fn(2, 44100, 128, 0, -1, row.ctypes.data, off.ctypes.data, one.ctypes.data, None, got.ctypes.data) == -3
-    assert fn(2, 44100, 128, 0, 1, None, off.ctypes.data, one.ctypes.data, None, got.ctypes.data) == -3
-    assert fn(2, 44100, 128, 0, 1, row.ctypes.data, None, one.ctypes.data, None, got.ctypes.data) == -3
-    assert fn(2, 44100, 128, 0, 1, row.ctypes.data, off.ctypes.data, None, None, got.ctypes.data) == -3
-    assert fn(2, 44100, 128, 0, 1, row.ctypes.data, off.ctypes.data, one.ctypes.data, None, None) == -3
-    assert fn(2, 44100, 128, 2, 1, row.ctypes.data, off.ctypes.data, one.ctypes.data, None, got.ctypes.data) == -1
+    C = ctypes.CDLL(L._name)                      # a handle of our own: argtypes set here leave the binding's alone
+    i16, f32 = np.zeros(2000, np.int16), np.zeros(2000, np.float32)
+    bufs = {"nsamples": np.array([1000], np.int64), "pcm_off": np.zeros(1, np.int64), "out_off": np.zeros(1, np.int64),
+            "cap": np.array([1 << 16], np.int64), "out_bytes": np.zeros(1, np.int64), "title": np.zeros(1, np.float64),
+            "album": np.zeros(1, np.float64), "timings": np.zeros(16, np.float32), "d_out": np.zeros(1 << 16, np.uint8)}
+    out = np.zeros(1 << 16, np.uint8)
+    for name, (roles, takes) in ENTRIES.items():
+        rows = f32 if name.endswith("_f32") else i16
+        fn = getattr(C, name)
+        fn.argtypes = [ctypes.c_int] * 3 + [ctypes.c_int if r in ("F", "N") else vp for r in roles]
+
+        def call(n=1, flags=0, **over):
+            host = {"left": (vp * 1)(rows.ctypes.data), "right": None, "d_pcm": rows.ctypes.data, "out": (vp * 1)(out.ctypes.data)}
+            args = []
+            for r in roles:
+                v = {"F": flags, "N": n}.get(r, host.get(r, bufs[r].ctypes.data if r in bufs else None))
+                args.append(over.get(r, v))
+            return fn(2, 44100, 128, *args)
+
+        if not torch.cuda.is_available():             # the base call is valid: only the missing device refuses it
+            assert call() == -100, name
+        assert call(n=-1) == -3 and L.mp3b200_last_error() == b"negative stream count", name
+        for r in roles:
+            if r in ("F", "N") or r in OPTIONAL:
+                continue
+            want = {"out_bytes": b"file_bytes is NULL" if "finish_tags" in name else b"out_bytes is NULL"}.get(r, b"null array")
+            assert call(**{r: None}) == -3 and L.mp3b200_last_error() == want, (name, r)
+        if "left" in roles:
+            assert call(left=(vp * 1)(None)) == -3 and L.mp3b200_last_error() == b"null row", name
+        assert call(nsamples=np.array([-5], np.int64).ctypes.data) == -3, name
+        assert L.mp3b200_last_error() == b"negative sample count", name
+        if takes is not None:
+            for flags in (4, 8, 1 << 30, 2 | 4, 2):
+                if flags & ~takes:
+                    assert call(flags=flags) == -1 and L.mp3b200_last_error() == b"unknown flags", (name, flags)
+    for name in ("mp3b200_debug_replaygain", "mp3b200_debug_replaygain_f32"):       # one stream of its own
+        fn = getattr(C, name)
+        fn.argtypes = [ctypes.c_int] * 4 + [vp, vp, ctypes.c_int64, vp, vp, ctypes.c_int64, vp, vp, vp]
+        rows = f32 if name.endswith("_f32") else i16
+        assert fn(2, 44100, 128, 0, None, None, 1000, None, None, 0, None, None, None) == -3, name
+        assert L.mp3b200_last_error() == b"null row", name
+        assert fn(2, 44100, 128, 0, rows.ctypes.data, None, -5, None, None, 0, None, None, None) == -3, name
 
 
 def test_resampled_configuration_is_refused_for_segments():
