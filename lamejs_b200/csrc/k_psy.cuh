@@ -9,7 +9,8 @@
  * state from call to call.  Here the work is split by what it depends on:
  *   k_psy_analysis   pure function of PCM, every unit: fs/4 HPF + 9 sub-block peaks, 1024-pt FHT, line energies,
  *                    long partition energies / tonality index
- *                    (and the ordered 512-term loudness sum, psycho_loudness_approx: terms in parallel, additions on one thread)
+ *                    (and the ordered 512-term loudness sum, psycho_loudness_approx: terms in parallel, additions on one
+ *                    thread per unit); PSY_UNITS consecutive units of one channel per block
  *   k_attack_prepass pure function of two consecutive units: attack candidates (before the lastAttacks FSM)
  *   k_stream_scan    the only sequential part: per stream, the attack / block-type FSM and the ATH-adjust IIR
  *   k_psy_short_list after the scan: the units whose short-block half is read (psy_short_read, DESIGN.md 2)
@@ -26,8 +27,7 @@
 #include "mp3_tables.h"
 
 #ifndef PSY_THREADS
-#define PSY_THREADS 128     /* 4 warps per (unit, channel): faster than 256 (cheaper block barriers,
-                               better-filled rounds); sections written for 256 "virtual threads" loop over them */
+#define PSY_THREADS 128     /* k_psy_short: 4 warps per (unit, channel) task */
 #endif
 #define MASK_THREADS 128
 
@@ -65,6 +65,11 @@ static int psy_upload_constants() {
     1.29083, 1.19746, 1.11084, 1.03826};
   static const double fir_half[10] = {-8.65163e-18, -0.00851586, -6.74764e-18, 0.0209036, -3.36639e-17, -0.0438162,
     -1.54175e-17, 0.0931738, -5.52212e-17, -0.313819};
+  for (int j = 0; j < 128; j++) {    /* k_psy_analysis reads fft_rv[j] as 2 rev7(j) */
+    int r = 0;
+    for (int bit = 0; bit < 7; bit++) r |= (j >> bit & 1) << (6 - bit);
+    if (MP3_FFT_RV[j] != 2 * r) return -100;
+  }
   double t1[25], t2[10], t3[14], fir[10];
   for (int i = 0; i < 25; i++) t1[i] = r1[i] * r1[i];       /* PsyModel.js:378-398 spells them as x*x */
   for (int i = 0; i < 10; i++) t2[i] = r2[i] * r2[i];
@@ -168,9 +173,9 @@ __device__ __forceinline__ void fht_task(f32w* fz, int stage, int task, const do
 /* psy row of (stream z, relative unit u >= -1): unit_base + z + u + 1 */
 __device__ __forceinline__ size_t psy_row(const StreamDesc& sd, int z, int u) { return (size_t)sd.unit_base + z + u + 1; }
 
-/* the unit's PCM span [x0, x0 + 1024) widened to double (zero outside the stream), all of a thread's loads in flight at once
+/* the PCM span [x0, x0 + N) widened to double (zero outside the stream), all of a thread's loads in flight at once
  * (they were one dependent HBM round trip per iteration) */
-template <bool F32_PCM, int NT>
+template <bool F32_PCM, int NT, int N = 1024>
 __device__ __forceinline__ void psy_load_span(const Mp3Tables* __restrict__ T, const StreamDesc& sd, int ch, long long x0, double* xs) {
   using Sample = pcm_sample_t<F32_PCM>;
   const int tid = threadIdx.x;
@@ -178,156 +183,240 @@ __device__ __forceinline__ void psy_load_span(const Mp3Tables* __restrict__ T, c
   const double scale = T->scale;
   const Sample* __restrict__ pbuf = static_cast<const Sample*>(sd.pcm[ch]);
   const long long pbase = sd.pcm_base, pend = sd.pcm_end;
-  constexpr int NB = (1024 + NT - 1) / NT;
+  constexpr int NB = (N + NT - 1) / NT;
   Sample v[NB];
 #pragma unroll
   for (int k = 0; k < NB; k++) {
     const int j = tid + k * NT;
     const long long i = x0 + j;
-    v[k] = (j < 1024 && i >= 0 && i < pend) ? __ldg(&pbuf[i - pbase]) : (Sample)0;
+    v[k] = (j < N && i >= 0 && i < pend) ? __ldg(&pbuf[i - pbase]) : (Sample)0;
   }
 #pragma unroll
   for (int k = 0; k < NB; k++) {
     const int j = tid + k * NT;
-    if (j < 1024) xs[j] = pcm_value(v[k], scale_applied, scale);
+    if (j < N) xs[j] = pcm_value(v[k], scale_applied, scale);
   }
 }
 
-/* grid (max_units + 1, nch, nstreams).  F32_PCM: sd.pcm[ch] points at Float32 samples already at the encoding rate and
- * scaled (the resampler's output, k_resample) instead of Int16 input. */
-#ifndef PSY_MIN_BLOCKS
-#define PSY_MIN_BLOCKS 12     /* C2 step on an H100 SXM (400 W): 8 / 10 / 12 blocks -> 5.18 / 5.15 / 5.13 ms */
+/* Block shape of k_psy_analysis: PSY_UNITS consecutive units of one channel per block.  Consecutive units overlap by 448
+ * of their 1024 samples, so the block loads and widens the union span (576 (U - 1) + 1024 samples) once; the FHTs and the
+ * partition phases of its units share one set of barriers.  PSY_UNIT_THREADS (P) >= 64 threads per unit: unit k's
+ * partitions run on threads P k .. P k + npart_l - 1, its loudness chain on thread P k + P - 1 (one warp per unit holds it,
+ * idle in the partition phases when npart_l < P). */
+#ifndef PSY_UNITS
+#define PSY_UNITS 2
 #endif
+#ifndef PSY_UNIT_THREADS
+#define PSY_UNIT_THREADS 64
+#endif
+#define PSY_A_THREADS (PSY_UNITS * PSY_UNIT_THREADS)
+#ifndef PSY_MIN_BLOCKS
+#define PSY_MIN_BLOCKS 8      /* 2 units x 64 threads: 58 / 64 registers (<false> / <true>), no spills, 26 112 B shared memory
+                                 -> 8 blocks (32 warps) per SM.  C2 on an H100 80GB HBM3 (700 W), `psy` phase 0.458 ms; with
+                                 1 unit x 128 threads, 12 blocks, 0.456 ms (DESIGN.md 6) */
+#endif
+static_assert(PSY_UNIT_THREADS >= 64 && PSY_UNIT_THREADS % 32 == 0, "one thread per long partition of each unit");
+
+#ifdef PSY_PHASESTAT
+/* tuning build: clock64() at the phase boundaries of every PSY_STAT_EVERY-th block of channel 0 of stream 0 (tools/psy_phasestat.py) */
+#define PSY_STAT_EVERY 16
+#define PSY_STAT_ROWS 4096
+#define PSY_STAT_COLS 13
+__device__ long long g_psystat[PSY_STAT_ROWS][PSY_STAT_COLS];
+#define PSY_CLOCK(col, who) do { if (stat_row >= 0 && (who)) g_psystat[stat_row][col] = clock64(); } while (0)
+#else
+#define PSY_CLOCK(col, who) do { } while (0)
+#endif
+
+/* a unit belongs to the upload slice `chunk` of `nchunks` (the host uploads every stream's PCM in time slices and launches
+ * this kernel once per slice as it lands) when that slice holds the last sample of its 1024-sample window */
+__device__ __forceinline__ bool psy_unit_in_slice(const StreamDesc& sd, long long c, int chunk, int nchunks) {
+  if (nchunks <= 1) return true;
+  const long long n = sd.pcm_end - sd.pcm_base;
+  long long last = 576 * c - 224 + 1023 - sd.pcm_base;
+  if (last > n - 1) last = n - 1;
+  int mine = 0;
+  while (mine < nchunks - 1 && last >= n * (mine + 1) / nchunks) mine++;
+  return mine == chunk;
+}
+
+/* grid (ceil((max_units + 1) / PSY_UNITS), nch, nstreams).  F32_PCM: sd.pcm[ch] points at Float32 samples already at the
+ * encoding rate and scaled (the resampler's output, k_resample) instead of Int16 input.  Every unit of the block is
+ * computed; only the units that exist and belong to this slice are written. */
 template <bool F32_PCM>
-__global__ void __launch_bounds__(PSY_THREADS, PSY_MIN_BLOCKS)
+__global__ void __launch_bounds__(PSY_A_THREADS, PSY_MIN_BLOCKS)
 k_psy_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ streams, PsyUnit* __restrict__ out,
                int chunk, int nchunks, int u_base) {
+  constexpr int U = PSY_UNITS, NT = PSY_A_THREADS;
   const int z = blockIdx.z;
   const StreamDesc& sd = streams[z];
-  const int u = (int)blockIdx.x + u_base;             /* relative unit, -1 = halo */
-  if (u >= T->mode_gr * sd.nframes) return;
+  const int u0 = (int)blockIdx.x * U + u_base;        /* relative unit of the block's first unit, -1 = halo */
   const int ch = blockIdx.y;
   const int nch = T->nch;
-  const long long c = (long long)T->mode_gr * sd.frame0 + u;   /* absolute psy call index (one call per granule) */
-  if (nchunks > 1) {
-    /* the host uploads every stream's PCM in `nchunks` time slices and launches this kernel once per slice as it
-     * lands: a unit belongs to the slice that holds the last sample of its 1024-sample window */
-    const long long n = sd.pcm_end - sd.pcm_base;
-    long long last = 576 * c - 224 + 1023 - sd.pcm_base;
-    if (last > n - 1) last = n - 1;
-    int mine = 0;
-    while (mine < nchunks - 1 && last >= n * (mine + 1) / nchunks) mine++;
-    if (mine != chunk) return;
-  }
-  PsyUnit* o = out + psy_row(sd, z, u) * nch + ch;
+  const int nunits = T->mode_gr * sd.nframes;
+  const long long c0 = (long long)T->mode_gr * sd.frame0 + u0;   /* absolute psy call index (one call per granule) */
   const int tid = threadIdx.x;
+  PsyUnit* const o0 = out + psy_row(sd, z, u0) * nch + ch;        /* unit k's row: o0 + k * nch */
+#ifdef PSY_PHASESTAT
+  const int stat_row = (z == 0 && ch == 0 && blockIdx.x % PSY_STAT_EVERY == 0 && blockIdx.x / PSY_STAT_EVERY < PSY_STAT_ROWS)
+                       ? (int)blockIdx.x / PSY_STAT_EVERY : -1;
+#endif
+  PSY_CLOCK(0, tid == 0);
 
-  if (c < 0) {   /* before the first call: psymodel_init values (PsyModel.js:2573-2595) */
-    if (tid < MP3_CBANDS) { o->eb_l[tid] = 0.0f; o->mask_idx[tid] = 0; }
-    if (tid < 9) o->peaks[tid] = 10.0f;
-    if (tid == 0) o->loudness = 0.0f;
-    if (tid < 4) o->attack[tid] = 0;
-    return;
-  }
-
-  /* xs (the PCM span widened once; the HPF reads each sample 21 times) is dead after the high-pass and the first radix-4
-   * pass; the line / partition energies are first written after the last FHT stage: they share its storage */
-  __shared__ __align__(16) unsigned char s_u[sizeof(double) * 1024];
-  double* const xs = reinterpret_cast<double*>(s_u);
-  f32s* const fe = reinterpret_cast<f32s*>(s_u);                                  /* [513] */
-  f32s* const s_max = reinterpret_cast<f32s*>(s_u + 2064);                        /* [64] */
-  f32s* const s_avg = s_max + MP3_CBANDS;                                         /* [64] */
-  /* psycho_loudness_approx (PsyModel.js:241-249) is ONE ordered 512-term double sum per unit.  Its terms energy[i] * eql_w[i]
-   * are computed by the threads that produce the energies (double products, 2 x 256 of them parked in shared memory that is
-   * dead by then: the high-pass output and the tail of the PCM span); the thread that owns no partition then only walks the
-   * additions -- an 8-cycle step instead of the 60-cycle load / convert / multiply / add step that stalled the block when
-   * the whole sum sat on one thread (measured slower) -- half in each of the two partition phases. */
-  constexpr int PROD_HI_OFF = 2064 + 2 * 4 * MP3_CBANDS;
-  static_assert(PROD_HI_OFF % 8 == 0 && PROD_HI_OFF + 256 * 8 <= (int)sizeof(s_u), "second half of the loudness terms");
-  double* const prod_hi = reinterpret_cast<double*>(s_u + PROD_HI_OFF);                /* terms 256..511 */
-  __shared__ f32w wl[1024 + 64];
-  __shared__ __align__(8) f32s hp[576];
-  double* const prod_lo = reinterpret_cast<double*>(hp);                               /* terms 0..255 (hp is dead by then) */
-  static_assert(sizeof(f32s) * 576 >= 256 * 8, "first half of the loudness terms");
-  __shared__ int s_peak[9];
-  if (tid < 9) s_peak[tid] = __float_as_int(1.0f);
-
-  psy_load_span<F32_PCM, PSY_THREADS>(T, sd, ch, 576 * c - 224, xs);
-  __syncthreads();
-
-  /* fs/4 high-pass (PsyModel.js:1051-1069): firbuf index = bufPos + 397 + i + j */
-  for (int i = tid; i < 576; i += PSY_THREADS) {
-    const double* fb = xs + 397 + i;
-    double sum1 = fb[10], sum2 = 0.0;
+  unsigned act = 0;                                   /* bit k: unit k is written by this block */
 #pragma unroll
-    for (int j = 0; j < 9; j += 2) {
-      sum1 += c_fircoef[j] * (fb[j] + fb[21 - j]);
-      sum2 += c_fircoef[j + 1] * (fb[j + 1] + fb[21 - j - 1]);
+  for (int k = 0; k < U; k++) {
+    const int u = u0 + k;
+    if (u >= nunits || !psy_unit_in_slice(sd, c0 + k, chunk, nchunks)) continue;
+    if (c0 + k < 0) {   /* before the first call: psymodel_init values (PsyModel.js:2573-2595) */
+      PsyUnit* o = o0 + k * nch;
+      if (tid < MP3_CBANDS) { o->eb_l[tid] = 0.0f; o->mask_idx[tid] = 0; }
+      if (tid < 9) o->peaks[tid] = 10.0f;
+      if (tid == 0) o->loudness = 0.0f;
+      if (tid < 4) o->attack[tid] = 0;
+      continue;
     }
-    hp[i] = sum1 + sum2;
+    act |= 1u << k;
   }
-  /* windowing + first radix-4 pass of fft_long (FFT.js:185-224): iteration jj writes y[4jj..4jj+3], y[512+4jj..] */
-  for (int jj = tid; jj < 128; jj += PSY_THREADS) {
-    const int i = c_fft_rv[jj], x = 4 * jj;
+  if (act == 0) return;
+
+  /* Region A holds the PCM span widened once (the HPF reads each sample 21 times) and the high-pass output; the span is
+   * dead after the first radix-4 pass, the high-pass output after the peaks (FHT stage 0).  From the line energies on it
+   * holds, per unit: the energies fe[513], the partition max / avg, and the 512 loudness terms energy[i] * eql_w[i]
+   * (double products, computed by the threads that produce the energies). */
+  constexpr int SPAN = 576 * (U - 1) + 1024;
+  constexpr int HP_OFF = SPAN * 8;
+  constexpr int POST = 2064 + 2 * 4 * MP3_CBANDS + 512 * 8;        /* fe, s_max, s_avg, loudness terms */
+  constexpr int A_BYTES = HP_OFF + U * 576 * 4 > U * POST ? HP_OFF + U * 576 * 4 : U * POST;
+  static_assert(POST % 16 == 0 && (2064 + 2 * 4 * MP3_CBANDS) % 8 == 0, "per-unit layout of region A");
+  __shared__ __align__(16) unsigned char s_a[A_BYTES];
+  double* const xs = reinterpret_cast<double*>(s_a);
+  f32s* const hp = reinterpret_cast<f32s*>(s_a + HP_OFF);                          /* unit k: hp + 576 k */
+  __shared__ f32w wl[U][1024 + 64];
+
+  psy_load_span<F32_PCM, NT, SPAN>(T, sd, ch, 576 * c0 - 224, xs);
+  __syncthreads();
+  PSY_CLOCK(1, tid == 0);
+
+  /* fs/4 high-pass (PsyModel.js:1051-1069): firbuf index = bufPos + 397 + i + j; unit k's output i is q = 576 k + i.
+   * Each thread computes the outputs q = 2p and 2p + 1 from the 24 samples xs[396 + 2p ..], read as 16-byte pairs: the
+   * reads were 22 8-byte loads per output, and shared-memory wavefronts are what this kernel runs out of first. */
+  for (int p = tid; p < U * 288; p += NT) {
+    double v[24];
+    const double2* src = reinterpret_cast<const double2*>(xs + 396 + 2 * p);
+#pragma unroll
+    for (int t = 0; t < 12; t++) { const double2 d = src[t]; v[2 * t] = d.x; v[2 * t + 1] = d.y; }
+#pragma unroll
+    for (int r = 0; r < 2; r++) {
+      const double* fb = v + 1 + r;
+      double sum1 = fb[10], sum2 = 0.0;
+#pragma unroll
+      for (int j = 0; j < 9; j += 2) {
+        sum1 += c_fircoef[j] * (fb[j] + fb[21 - j]);
+        sum2 += c_fircoef[j + 1] * (fb[j + 1] + fb[21 - j - 1]);
+      }
+      hp[2 * p + r] = sum1 + sum2;
+    }
+  }
+  /* windowing + first radix-4 pass of fft_long (FFT.js:185-224): iteration jj writes y[4jj..4jj+3], y[512+4jj..] and reads
+   * the samples from i = fft_rv[jj] = 2 rev7(jj) on (psy_upload_constants checks the table).  Thread p runs iteration
+   * jj = rev7(p), so that a warp reads consecutive samples and window values (in table order a warp's 32 reads of xs lie
+   * multiples of 64 bytes apart, in two pairs of banks) and writes y conflict-free (x = 4 jj spreads over the padded banks). */
+  for (int q = tid; q < U * 128; q += NT) {
+    const int k = q >> 7, p = q & 127, jj = (int)(__brev((unsigned)p) >> 25);
+    const int i = 2 * p, x = 4 * jj;
     const float* w = T->fft_window;
+    const double* xu = xs + 576 * k;
+    f32w* const y = wl[k];
     double f0, f1, f2, f3, wv;
-    f0 = (double)w[i] * (double)xs[i];
-    wv = (double)w[i + 0x200] * (double)xs[i + 0x200];
+    f0 = (double)w[i] * (double)xu[i];
+    wv = (double)w[i + 0x200] * (double)xu[i + 0x200];
     f1 = f0 - wv; f0 = f0 + wv;
-    f2 = (double)w[i + 0x100] * (double)xs[i + 0x100];
-    wv = (double)w[i + 0x300] * (double)xs[i + 0x300];
+    f2 = (double)w[i + 0x100] * (double)xu[i + 0x100];
+    wv = (double)w[i + 0x300] * (double)xu[i + 0x300];
     f3 = f2 - wv; f2 = f2 + wv;
-    wl[FHT_PAD(x + 0)] = f0 + f2; wl[FHT_PAD(x + 2)] = f0 - f2; wl[FHT_PAD(x + 1)] = f1 + f3; wl[FHT_PAD(x + 3)] = f1 - f3;
-    f0 = (double)w[i + 0x001] * (double)xs[i + 0x001];
-    wv = (double)w[i + 0x201] * (double)xs[i + 0x201];
+    y[FHT_PAD(x + 0)] = f0 + f2; y[FHT_PAD(x + 2)] = f0 - f2; y[FHT_PAD(x + 1)] = f1 + f3; y[FHT_PAD(x + 3)] = f1 - f3;
+    f0 = (double)w[i + 0x001] * (double)xu[i + 0x001];
+    wv = (double)w[i + 0x201] * (double)xu[i + 0x201];
     f1 = f0 - wv; f0 = f0 + wv;
-    f2 = (double)w[i + 0x101] * (double)xs[i + 0x101];
-    wv = (double)w[i + 0x301] * (double)xs[i + 0x301];
+    f2 = (double)w[i + 0x101] * (double)xu[i + 0x101];
+    wv = (double)w[i + 0x301] * (double)xu[i + 0x301];
     f3 = f2 - wv; f2 = f2 + wv;
-    wl[FHT_PAD(x + 512 + 0)] = f0 + f2; wl[FHT_PAD(x + 512 + 2)] = f0 - f2; wl[FHT_PAD(x + 512 + 1)] = f1 + f3; wl[FHT_PAD(x + 512 + 3)] = f1 - f3;
+    y[FHT_PAD(x + 512 + 0)] = f0 + f2; y[FHT_PAD(x + 512 + 2)] = f0 - f2; y[FHT_PAD(x + 512 + 1)] = f1 + f3; y[FHT_PAD(x + 512 + 3)] = f1 - f3;
   }
   __syncthreads();
+  PSY_CLOCK(2, tid == 0);
 
-  /* 9 sub-block peaks of the high-passed signal (PsyModel.js:1125-1132): max(1, |hp|) over 64 samples each; the
-   * values are non-negative float32, whose order is the order of their bit patterns */
-  for (int i = tid; i < 576; i += PSY_THREADS) atomicMax(&s_peak[i >> 6], __float_as_int(fabsf(hp[i].v)));
-  /* FHT stages: 128 tasks per stage (task numbers map to butterflies by shifts: the earlier enumeration needed integer
-   * divisions, 16 % of this kernel's instructions) */
+  /* 9 sub-block peaks of the high-passed signal per unit (PsyModel.js:1125-1132): max(1, |hp|) over 64 samples each, one
+   * warp per sub-block (unit k's sub-block s is sb = 9 k + s, its samples hp[64 sb ..]); the values are non-negative
+   * float32, whose order is the order of their bit patterns, so a warp max of the bits is the exact max */
+  for (int sb = tid >> 5; sb < 9 * U; sb += NT / 32) {
+    const int lane = tid & 31;
+    const unsigned m = __reduce_max_sync(0xffffffffu, max(__float_as_uint(fabsf(hp[64 * sb + lane].v)),
+                                                          __float_as_uint(fabsf(hp[64 * sb + 32 + lane].v))));
+    const int k = sb / 9;
+    if (lane == 0 && (act >> k & 1)) o0[k * nch].peaks[sb - 9 * k] = __uint_as_float(max(m, __float_as_uint(1.0f)));
+  }
+  /* FHT stages: 128 tasks per unit and stage (task numbers map to butterflies by shifts) */
 #pragma unroll
   for (int stage = 0; stage < 4; stage++) {
-    for (int t = tid; t < 128; t += PSY_THREADS) fht_task(wl, stage, t, T->tw, T->tw_off);
+    for (int t = tid; t < U * 128; t += NT) fht_task(wl[t >> 7], stage, t & 127, T->tw, T->tw_off);
     __syncthreads();
+    PSY_CLOCK(3 + stage, tid == 0);
   }
 
-  /* line energies (PsyModel.js:278-298) */
-  for (int j = tid; j < 512; j += PSY_THREADS) {
-    const double re = wl[FHT_PAD(512 - j)], im = wl[FHT_PAD(512 + j)];
+  /* line energies (PsyModel.js:278-298) and the loudness terms */
+  for (int q = tid; q < U * 512; q += NT) {
+    const int k = q >> 9, j = q & 511;
+    unsigned char* const pk = s_a + k * POST;
+    f32s* const fe = reinterpret_cast<f32s*>(pk);
+    double* const prod = reinterpret_cast<double*>(pk + 2064 + 2 * 4 * MP3_CBANDS);
+    const double re = wl[k][FHT_PAD(512 - j)], im = wl[k][FHT_PAD(512 + j)];
     f32s e; e = (re * re + im * im) * 0.5;
     fe[512 - j] = (double)e;
-    const int k = 512 - j;                              /* 1..512; the loudness sum runs over 0..511 */
-    if (k < 512) { const double p = (double)e * (double)T->eql_w[k]; if (k < 256) prod_lo[k] = p; else prod_hi[k - 256] = p; }
+    if (j > 0) prod[512 - j] = (double)e * (double)T->eql_w[512 - j];   /* the loudness sum runs over 0..511 */
   }
-  if (tid == 0) { f32s t0; t0 = (double)wl[0]; t0 *= (double)t0; fe[0] = (double)t0; prod_lo[0] = (double)t0 * (double)T->eql_w[0]; }
+  if (tid < U) {
+    unsigned char* const pk = s_a + tid * POST;
+    f32s* const fe = reinterpret_cast<f32s*>(pk);
+    double* const prod = reinterpret_cast<double*>(pk + 2064 + 2 * 4 * MP3_CBANDS);
+    f32s t0; t0 = (double)wl[tid][0]; t0 *= (double)t0; fe[0] = (double)t0; prod[0] = (double)t0 * (double)T->eql_w[0];
+  }
   __syncthreads();
+  PSY_CLOCK(7, tid == 0);
 
+  /* partition phases: unit k = tid / PSY_UNIT_THREADS, partition b = tid % PSY_UNIT_THREADS */
+  const int k = tid / PSY_UNIT_THREADS, b = tid % PSY_UNIT_THREADS;
   const int npl = T->npart_l;
-  for (int b = tid; b < npl; b += PSY_THREADS) {     /* calc_energy (PsyModel.js:906-928) */
+  unsigned char* const pk = s_a + k * POST;
+  f32s* const fe = reinterpret_cast<f32s*>(pk);
+  f32s* const s_max = reinterpret_cast<f32s*>(pk + 2064);
+  f32s* const s_avg = s_max + MP3_CBANDS;
+  const double* const prod = reinterpret_cast<const double*>(pk + 2064 + 2 * 4 * MP3_CBANDS);
+  const bool mine = act >> k & 1;
+  PsyUnit* const o = o0 + k * nch;
+  if (b < npl) {     /* calc_energy (PsyModel.js:906-928) */
     double ebb = 0, m = 0;
     const int l0 = T->line0_l[b], l1 = T->line0_l[b + 1];
     for (int j = l0; j < l1; j++) { const double el = fe[j]; ebb += el; if (m < el) m = el; }
-    o->eb_l[b] = (float)ebb;
+    if (mine) o->eb_l[b] = (float)ebb;
     s_max[b] = m;
     s_avg[b] = ebb * (double)T->rnumlines_l[b];
   }
+  /* psycho_loudness_approx (PsyModel.js:241-249): ONE ordered 512-term double sum per unit, half in each partition phase,
+   * on a thread of its own per unit (in different warps), so that the units' chains run side by side */
+  const bool chain = b == PSY_UNIT_THREADS - 1 && mine;
   double loud = 0.0;
-  if (tid == PSY_THREADS - 1) {
+  if (chain) {
 #pragma unroll 8
-    for (int i = 0; i < 256; ++i) loud += prod_lo[i];
+    for (int i = 0; i < 256; ++i) loud += prod[i];
   }
-  if (tid < 9) o->peaks[tid] = __int_as_float(s_peak[tid]);
+  PSY_CLOCK(11, chain && k == 0);
+  PSY_CLOCK(8, tid == 0);
   __syncthreads();
+  PSY_CLOCK(9, tid == 0);
 
-  for (int b = tid; b < npl; b += PSY_THREADS) {     /* calc_mask_index_l (PsyModel.js:930-992) */
+  if (b < npl) {     /* calc_mask_index_l (PsyModel.js:930-992) */
     const int lo = b > 0 ? b - 1 : b, hi = b < npl - 1 ? b + 1 : b;
     double a = 0; double m = 0; int lines = 0;
     for (int q = lo; q <= hi; q++) {
@@ -335,21 +424,23 @@ k_psy_analysis(const Mp3Tables* __restrict__ T, const StreamDesc* __restrict__ s
       else { a = a + (double)s_avg[q]; if (m < (double)s_max[q]) m = (double)s_max[q]; }
       lines += T->numlines_l[q];
     }
-    int k = 0;
+    int kk = 0;
     if (a > 0.0) {
       const double cnt = (double)(hi - lo + 1);
       a = 20.0 * (m * cnt - a) / (a * (lines - 1));
-      k = js_trunc<DOM_TRUNC_MASK_IDX>(a);
-      if (k > 8) k = 8;
+      kk = js_trunc<DOM_TRUNC_MASK_IDX>(a);
+      if (kk > 8) kk = 8;
     }
-    o->mask_idx[b] = (unsigned char)k;
+    if (mine) o->mask_idx[b] = (unsigned char)kk;
   }
-  if (tid == PSY_THREADS - 1) {
+  PSY_CLOCK(10, tid == 0);
+  if (chain) {
 #pragma unroll 8
-    for (int i = 0; i < 256; ++i) loud += prod_hi[i];
+    for (int i = 256; i < 512; ++i) loud += prod[i];
     loud *= (1. / (14752. * 14752.) / 512);
     o->loudness = (float)loud;
   }
+  PSY_CLOCK(12, chain && k == 0);
 }
 
 /* ---- the short-block half (PsyModel.js:1000-1383 for shortblock, compute_masking_s :740-761) --------------------------

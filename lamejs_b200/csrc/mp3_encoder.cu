@@ -553,7 +553,7 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, const 
   }
   CK(cudaEventRecord(ev[0], st));
 
-  /* K2: psy analysis, one block per (granule incl. 1 halo, channel, stream) */
+  /* K2: psy analysis, one block per (PSY_UNITS consecutive granules incl. 1 halo, channel, stream) */
   {
     const int nchunks = arrival ? arrival->chunks : 1;
     /* units (relative index, -1 = halo) each upload slice completes, over all streams: the kernel's own rule
@@ -578,9 +578,9 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, const 
     for (int j = 0; j < nchunks; j++) {
       if (arrival) CK(cudaStreamWaitEvent(st, arrival->ready[j], 0));
       if (u_hi[j] <= u_lo[j]) continue;
-      dim3 gridj(u_hi[j] - u_lo[j], nch, S);
-      if (f32_pcm) k_psy_analysis<true><<<gridj, PSY_THREADS, 0, st>>>(tab, ws.streams.p, ws.psy.p, j, nchunks, u_lo[j]);
-      else k_psy_analysis<false><<<gridj, PSY_THREADS, 0, st>>>(tab, ws.streams.p, ws.psy.p, j, nchunks, u_lo[j]);
+      dim3 gridj((u_hi[j] - u_lo[j] + PSY_UNITS - 1) / PSY_UNITS, nch, S);
+      if (f32_pcm) k_psy_analysis<true><<<gridj, PSY_A_THREADS, 0, st>>>(tab, ws.streams.p, ws.psy.p, j, nchunks, u_lo[j]);
+      else k_psy_analysis<false><<<gridj, PSY_A_THREADS, 0, st>>>(tab, ws.streams.p, ws.psy.p, j, nchunks, u_lo[j]);
       g_launches++;
       DBG("k_psy_analysis");
     }
@@ -2014,6 +2014,13 @@ int mp3b200_lametag_build_ex(int channels, int samplerate, int kbps, int flags, 
 extern "C" int mp3b200_debug_taskstat(int* out, int rows) {
   if (rows > (1 << 16)) rows = 1 << 16;
   return cudaMemcpyFromSymbol(out, g_taskstat, sizeof(int) * 8 * (size_t)rows) == cudaSuccess ? 0 : -1;
+}
+#endif
+
+#ifdef PSY_PHASESTAT
+extern "C" int mp3b200_debug_psystat(long long* out, int rows) {
+  if (rows > PSY_STAT_ROWS) rows = PSY_STAT_ROWS;
+  return cudaMemcpyFromSymbol(out, g_psystat, sizeof(long long) * PSY_STAT_COLS * (size_t)rows) == cudaSuccess ? rows : -1;
 }
 #endif
 
