@@ -519,6 +519,90 @@ int wait_legacy(ThreadCtx& c) {
 struct Rows { bool f32; int scale_applied; };
 constexpr Rows SCALED_F32 = {true, 0};
 
+/* Debug psy-row capture (mp3b200_debug_psy_capture).  While it is on, every pipeline launch poisons the psy rows it uses
+ * before k_psy_analysis, so that a row the launch forgets to write cannot pass for one written by an earlier launch, and
+ * records them after k_attack_prepass (PsyUnit) and after k_psy_short (the short list and its PsyShort rows).  The launch
+ * synchronises its stream at both points; with capture off it does nothing at all. */
+std::atomic<int> g_psy_capture{0};
+std::mutex g_psy_mu;                      /* guards g_psy_rec, g_psy_launch */
+std::vector<unsigned char> g_psy_rec;     /* records: int32[8] header + payload (include/mp3b200.h) */
+int g_psy_launch = 0;
+
+void psy_rec_append(const int32_t (&h)[8], const void* a, size_t na, const void* b = nullptr, size_t nb = 0) {
+  std::lock_guard<std::mutex> lk(g_psy_mu);
+  const unsigned char* hp = reinterpret_cast<const unsigned char*>(h);
+  g_psy_rec.insert(g_psy_rec.end(), hp, hp + sizeof h);
+  if (na) g_psy_rec.insert(g_psy_rec.end(), static_cast<const unsigned char*>(a), static_cast<const unsigned char*>(a) + na);
+  if (nb) g_psy_rec.insert(g_psy_rec.end(), static_cast<const unsigned char*>(b), static_cast<const unsigned char*>(b) + nb);
+}
+
+/* Fills the launch's rows: floats with a quiet NaN, bytes with values that stay valid table indices (mask_idx 8, attack 0),
+ * so that reading an unwritten row changes results without ever indexing out of bounds. */
+int psy_poison(ThreadCtx& c, size_t rows, int* launch) {
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  CK(cudaStreamIsCapturing(c.st, &cs));
+  if (cs != cudaStreamCaptureStatusNone) { g_err = "psy-row capture inside CUDA stream capture"; return MP3B200_ERR_CUDA; }
+  {
+    std::lock_guard<std::mutex> lk(g_psy_mu);
+    *launch = g_psy_launch++;
+  }
+  const uint32_t qbits = 0x7fc00000u;
+  float qnan;
+  memcpy(&qnan, &qbits, sizeof qnan);
+  PsyUnit pu;
+  for (float& v : pu.eb_l) v = qnan;
+  for (float& v : pu.peaks) v = qnan;
+  pu.loudness = qnan;
+  memset(pu.mask_idx, 8, sizeof pu.mask_idx);
+  memset(pu.attack, 0, sizeof pu.attack);
+  pu.pad_ = 0;
+  PsyShort ps;
+  for (int s = 0; s < 3; s++)
+    for (int b = 0; b < MP3_CBANDS; b++) { ps.ecb_s[s][b] = (double)qnan; ps.eb_s[s][b] = qnan; }
+  std::vector<PsyUnit> u(rows, pu);
+  std::vector<PsyShort> sh(rows, ps);
+  CK(cudaMemcpyAsync(c.ws.psy.p, u.data(), rows * sizeof(PsyUnit), cudaMemcpyHostToDevice, c.st));
+  CK(cudaMemcpyAsync(c.ws.psy_s.p, sh.data(), rows * sizeof(PsyShort), cudaMemcpyHostToDevice, c.st));
+  CK(cudaStreamSynchronize(c.st));
+  return 0;
+}
+
+/* After k_attack_prepass: each stream's rows u = -1 .. G nframes - 1 */
+int psy_record_units(ThreadCtx& c, const StreamDesc* sds, int S, int nch, int G, int launch) {
+  CK(cudaStreamSynchronize(c.st));
+  for (int z = 0; z < S; z++) {
+    const StreamDesc& sd = sds[z];
+    const size_t n = ((size_t)G * sd.nframes + 1) * nch;
+    std::vector<PsyUnit> rows(n);
+    CK(cudaMemcpyAsync(rows.data(), c.ws.psy.p + ((size_t)sd.unit_base + z) * nch, n * sizeof(PsyUnit), cudaMemcpyDeviceToHost, c.st));
+    CK(cudaStreamSynchronize(c.st));
+    const int32_t h[8] = {1, launch, z, sd.frame0, sd.nframes, nch, G, (int32_t)sizeof(PsyUnit)};
+    psy_rec_append(h, rows.data(), n * sizeof(PsyUnit));
+  }
+  return 0;
+}
+
+/* After k_psy_short: the short list in list order and the PsyShort row of each entry */
+int psy_record_short(ThreadCtx& c, const StreamDesc* sds, int nch, int G, int launch, int k2_launches) {
+  CK(cudaStreamSynchronize(c.st));
+  int count = 0;
+  CK(cudaMemcpyAsync(&count, c.ws.short_count.p, sizeof count, cudaMemcpyDeviceToHost, c.st));
+  CK(cudaStreamSynchronize(c.st));
+  std::vector<int2> list((size_t)count);
+  std::vector<PsyShort> rows((size_t)count);
+  if (count) CK(cudaMemcpyAsync(list.data(), c.ws.short_list.p, count * sizeof(int2), cudaMemcpyDeviceToHost, c.st));
+  CK(cudaStreamSynchronize(c.st));
+  for (int i = 0; i < count; i++) {
+    const int z = list[i].x, u = (list[i].y >> 1) - 1, ch = list[i].y & 1;
+    const size_t row = ((size_t)sds[z].unit_base + z + u + 1) * nch + ch;
+    CK(cudaMemcpyAsync(&rows[i], c.ws.psy_s.p + row, sizeof(PsyShort), cudaMemcpyDeviceToHost, c.st));
+  }
+  CK(cudaStreamSynchronize(c.st));
+  const int32_t h[8] = {2, launch, count, nch, G, k2_launches, 0, (int32_t)sizeof(PsyShort)};
+  psy_rec_append(h, list.data(), count * sizeof(int2), rows.data(), count * sizeof(PsyShort));
+  return 0;
+}
+
 /* One pipeline launch for the streams sds[0 .. S) (at most MP3_MAX_LAUNCH_STREAMS, unit / frame bases set, the workspace
  * large enough).  All launches go to the context's stream (c.st: the calling thread's, t_ctx.st, or a session's), which
  * first waits for whatever the caller queued on the legacy default stream (wait_legacy); with o.sync the call returns after
@@ -551,6 +635,9 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, const 
     g_launches++;
     DBG("k_handle_carry_in");
   }
+  int psy_launch = -1, k2_launches = 0;
+  if (g_psy_capture.load(std::memory_order_relaxed) &&
+      (rc = psy_poison(c, ((size_t)cfg->host.mode_gr * total_frames + S) * nch, &psy_launch))) return rc;
   CK(cudaEventRecord(ev[0], st));
 
   /* K2: psy analysis, one block per (PSY_UNITS consecutive granules incl. 1 halo, channel, stream) */
@@ -582,6 +669,7 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, const 
       if (f32_pcm) k_psy_analysis<true><<<gridj, PSY_A_THREADS, 0, st>>>(tab, ws.streams.p, ws.psy.p, j, nchunks, u_lo[j]);
       else k_psy_analysis<false><<<gridj, PSY_A_THREADS, 0, st>>>(tab, ws.streams.p, ws.psy.p, j, nchunks, u_lo[j]);
       g_launches++;
+      k2_launches++;
       DBG("k_psy_analysis");
     }
   }
@@ -591,6 +679,7 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, const 
     dim3 grid((cfg->host.mode_gr * max_frames + 127) / 128, 1, S);
     k_attack_prepass<<<grid, 128, 0, st>>>(tab, ws.streams.p, ws.psy.p, ws.scan_in.p);
     DBG("k_attack_prepass");
+    if (psy_launch >= 0 && (rc = psy_record_units(c, h_streams, S, nch, cfg->host.mode_gr, psy_launch))) return rc;
     k_stream_scan<<<S, SCAN_THREADS, 0, st>>>(tab, ws.streams.p, S, ws.scan_in.p, ws.bt_final.p, ws.bt_prev.p, ws.ath_psy.p, ws.ath_q.p, ws.scan.p);
     g_launches += 2;
     DBG("k_stream_scan");
@@ -639,6 +728,7 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, const 
     else k_psy_short<false><<<blocks, PSY_THREADS, 0, st>>>(tab, ws.streams.p, ws.psy_s.p, ws.short_list.p, ws.short_count.p);
     g_launches += 2;
     DBG("k_psy_short");
+    if (psy_launch >= 0 && (rc = psy_record_short(c, h_streams, nch, cfg->host.mode_gr, psy_launch, k2_launches))) return rc;
   }
   /* K3b: masking thresholds */
   {
@@ -1170,6 +1260,21 @@ int mp3b200_debug_qstats(unsigned long long* out16, int reset) {
 }
 #endif
 int64_t mp3b200_launch_count(void) { return g_launches; }
+int mp3b200_debug_psy_capture(int on) {
+  std::lock_guard<std::mutex> lk(g_psy_mu);
+  if (on) { g_psy_rec.clear(); g_psy_launch = 0; }
+  g_psy_capture.store(on ? 1 : 0);
+  return 0;
+}
+int64_t mp3b200_debug_psy_take(void* buf, int64_t cap) {
+  std::lock_guard<std::mutex> lk(g_psy_mu);
+  const int64_t n = (int64_t)g_psy_rec.size();
+  if (buf && cap >= n) {
+    memcpy(buf, g_psy_rec.data(), (size_t)n);
+    g_psy_rec.clear();
+  }
+  return n;
+}
 int64_t mp3b200_debug_short_units(void) {
   if (!t_ctx.ws.short_count.p) return -1;
   int n = 0;

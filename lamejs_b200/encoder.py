@@ -1,3 +1,4 @@
+import contextlib
 import ctypes
 import os
 
@@ -970,6 +971,76 @@ def debug_short_units():
     f = lib().mp3b200_debug_short_units
     f.restype = ctypes.c_int64
     return f()
+
+
+# the rows mp3b200_debug_psy_take hands out (include/mp3b200.h)
+PSY_UNIT_DTYPE = np.dtype({"names": ["eb_l", "peaks", "loudness", "mask_idx", "attack"],
+                           "formats": [(np.float32, 64), (np.float32, 9), np.float32, (np.uint8, 64), (np.uint8, 4)],
+                           "offsets": [0, 256, 292, 296, 360], "itemsize": 368})
+PSY_SHORT_DTYPE = np.dtype({"names": ["ecb_s", "eb_s"], "formats": [(np.float64, (3, 64)), (np.float32, (3, 64))],
+                            "offsets": [0, 1536], "itemsize": 2304})
+
+
+class PsyCapture:
+    """What debug_psy_capture recorded: `launches`, one dict per pipeline launch in launch order, filled when the block ends:
+    "streams": per stream of the launch {"z", "frame0", "nframes", "rows"} with rows PSY_UNIT_DTYPE[G nframes + 1][nch] for
+    u = -1 .. G nframes - 1; "short": the short list as an int array [count][3] of (stream, u, channel) in list order;
+    "short_rows": PSY_SHORT_DTYPE[count]; "k2_launches": how many k_psy_analysis launches the pipeline made."""
+
+    def __init__(self):
+        self.launches = []
+
+    def _parse(self, raw):
+        by = {}
+        off = 0
+        while off < len(raw):
+            h = np.frombuffer(raw, dtype=np.int32, count=8, offset=off)
+            off += 32
+            kind, launch = int(h[0]), int(h[1])
+            rec = by.setdefault(launch, {"streams": [], "short": None, "short_rows": None, "k2_launches": None})
+            if kind == 1:
+                z, frame0, nframes, nch, G, rb = (int(v) for v in h[2:])
+                assert rb == PSY_UNIT_DTYPE.itemsize, rb
+                n = (G * nframes + 1) * nch
+                rows = np.frombuffer(raw, dtype=PSY_UNIT_DTYPE, count=n, offset=off).reshape(-1, nch).copy()
+                off += n * rb
+                rec["streams"].append({"z": z, "frame0": frame0, "nframes": nframes, "G": G, "rows": rows})
+            else:
+                assert kind == 2, kind
+                count, nch, G, k2, _, rb = (int(v) for v in h[2:])
+                assert rb == PSY_SHORT_DTYPE.itemsize, rb
+                pairs = np.frombuffer(raw, dtype=np.int32, count=2 * count, offset=off).reshape(-1, 2)
+                off += 8 * count
+                rec["short"] = np.stack([pairs[:, 0], (pairs[:, 1] >> 1) - 1, pairs[:, 1] & 1], axis=1) if count else np.zeros((0, 3), np.int64)
+                rec["short_rows"] = np.frombuffer(raw, dtype=PSY_SHORT_DTYPE, count=count, offset=off).copy()
+                off += count * rb
+                rec["k2_launches"] = k2
+        for k in sorted(by):
+            by[k]["streams"].sort(key=lambda s: s["z"])
+            self.launches.append(by[k])
+
+
+@contextlib.contextmanager
+def debug_psy_capture():
+    """Debug only: while the block runs, every pipeline launch (any thread, any session) poisons its psy rows before the
+    long-block analysis and records them after the attack pre-pass and the short-block analysis (mp3b200_debug_psy_capture;
+    each launch synchronises its stream at those points).  Yields a PsyCapture, filled when the block ends."""
+    L = lib()
+    L.mp3b200_debug_psy_capture.argtypes = [ctypes.c_int]
+    L.mp3b200_debug_psy_take.argtypes = [ctypes.c_void_p, ctypes.c_int64]
+    L.mp3b200_debug_psy_take.restype = ctypes.c_int64
+    cap = PsyCapture()
+    _check(L.mp3b200_debug_psy_capture(1))
+    try:
+        yield cap
+    finally:
+        L.mp3b200_debug_psy_capture(0)
+        while True:
+            n = L.mp3b200_debug_psy_take(None, 0)
+            buf = np.empty(n, dtype=np.uint8)
+            if L.mp3b200_debug_psy_take(buf.ctypes.data, n) == n:
+                break
+        cap._parse(buf.tobytes())
 
 
 def debug_stages(channels, samplerate, kbps, left, right=None, force_blocktype=None, want=("xr",), resample=False,

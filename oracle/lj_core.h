@@ -126,6 +126,23 @@ struct LjQuantTrace {
   int   old_value_mid[2], cur_step_mid[2];   /* MPEG-1: OldValue / CurrentStep after gr0, where gr1's search starts; 0 for LSF */
 };
 
+/* per-frame record of the psy model's per-granule analysis (lj_set_psy_trace), [gr][ch] = psy call G k + gr of frame k.  A
+ * record of its own, like LjQuantTrace.  Only the first npart_l / npart_s partitions are defined (0 beyond).
+ *   eb_l, mask_idx_l  calc_energy's partition energies and calc_mask_index_l's indices
+ *   peaks             en_subshort[3..11]: max(1, |high-passed sample|) over each 64-sample sub-block
+ *   loudness          loudness_sq_save[ch] after the call (psycho_loudness_approx of this granule)
+ *   attack            ns_attacks after the `ratio < 1.7` pass, before the lastAttacks rule
+ *   eb_s, ecb_s       compute_masking_s of each short block: its partition energies and the spreading sum it stores into nb_s1 */
+struct LjPsyTrace {
+  float eb_l[2][2][CBANDS];
+  float peaks[2][2][9];
+  float loudness[2][2];
+  float eb_s[2][2][3][CBANDS];
+  float ecb_s[2][2][3][CBANDS];
+  int   mask_idx_l[2][2][CBANDS];
+  int   attack[2][2][4];
+};
+
 /* what an encoder carries from one call to the next (lj_get_state) */
 struct LjState {
   double ath_adjust, ath_adjust_limit;

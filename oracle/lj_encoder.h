@@ -102,6 +102,8 @@ struct LjEnc {
   LjFrameTrace* trace; int trace_cap, trace_n;
   LjQuantTrace* qtrace; int qtrace_cap;
   LjQuantTrace* qtrace_cur;      /* the quantizer row of the frame being encoded while tracing, else NULL (lj_quant.cpp) */
+  LjPsyTrace* ptrace; int ptrace_cap, ptrace_n;
+  LjPsyTrace* ptrace_cur;        /* the psy row of the frame being encoded while tracing, else NULL (lj_psy_trace_*) */
   /* Xing / LAME tag state (VBRSeekInfo.js, LameInternalFlags.js:170; lj_vbrtag.cpp).  nMusicCRC and nBytesWritten are
    * maintained by copy_buffer on every call whether or not a tag is written (BitStream.js:924-935). */
   int nMusicCRC; long long nBytesWritten;
@@ -128,6 +130,11 @@ int  lj_psycho_anal_ns(LjEnc* e, const F32* buf0, const F32* buf1, int bufPos, i
                        PsyRatio masking_ratio[2][2], PsyRatio masking_MS_ratio[2][2], double* percep_entropy,
                        double* percep_MS_entropy, F32* energy, int* blocktype_d);
 void lj_psymodel_init(LjEnc* e);
+/* lj_init.cpp: the psy trace's row of psy call (gr, chn) of the frame being encoded (lj_set_psy_trace); no-ops when the
+ * trace is off and for the mid / side channels.  Kept out of lj_psy.cpp, whose per-frame branches the tests account for. */
+void lj_psy_trace_attacks(LjEnc* e, int gr, int chn, const F32* en_subshort, const int* ns_attacks);
+void lj_psy_trace_long(LjEnc* e, int gr, int chn, const F32* eb_l, const int* mask_idx_l);
+void lj_psy_trace_short(LjEnc* e, int gr, int chn, int sblock, const F32* eb_s);
 double lj_ATHformula(double f, const LjEnc* e);
 /* lj_quant.cpp */
 void lj_iteration_init(LjEnc* e);

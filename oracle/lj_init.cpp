@@ -333,6 +333,26 @@ static void adjust_ATH(LjEnc* e) {
   }
 }
 
+/* the psy trace (lj_set_psy_trace): called by lj_psycho_anal_ns at the points each field is final */
+void lj_psy_trace_attacks(LjEnc* e, int gr, int chn, const F32* en_subshort, const int* ns_attacks) {
+  LjPsyTrace* const t = e->ptrace_cur;
+  if (!t || chn >= 2) return;
+  for (int i = 0; i < 9; i++) t->peaks[gr][chn][i] = en_subshort[i + 3].v;
+  for (int i = 0; i < 4; i++) t->attack[gr][chn][i] = ns_attacks[i];
+}
+void lj_psy_trace_long(LjEnc* e, int gr, int chn, const F32* eb_l, const int* mask_idx_l) {
+  LjPsyTrace* const t = e->ptrace_cur;
+  if (!t || chn >= 2) return;
+  t->loudness[gr][chn] = e->loudness_sq_save[chn].v;
+  for (int b = 0; b < e->npart_l; b++) { t->eb_l[gr][chn][b] = eb_l[b].v; t->mask_idx_l[gr][chn][b] = mask_idx_l[b]; }
+}
+/* after compute_masking_s of short block sblock: its partition energies and the spreading sums it stored into nb_s1 */
+void lj_psy_trace_short(LjEnc* e, int gr, int chn, int sblock, const F32* eb_s) {
+  LjPsyTrace* const t = e->ptrace_cur;
+  if (!t || chn >= 2) return;
+  for (int b = 0; b < e->npart_s; b++) { t->eb_s[gr][chn][sblock][b] = eb_s[b].v; t->ecb_s[gr][chn][sblock][b] = e->nb_s1[chn][b].v; }
+}
+
 /* Encoder.js:287-326 */
 static void encode_frame_init(LjEnc* e) {
   if (e->frame_init_done) return;
@@ -368,6 +388,8 @@ static int encode_mp3_frame(LjEnc* e, uint8_t* mp3buf, int mp3buf_size) {
   if ((e->slot_lag -= e->frac_SpF) < 0) { e->slot_lag += e->out_samplerate; e->padding = 1; }
 
   int blocktype[2];
+  e->ptrace_cur = (e->ptrace && e->ptrace_n < e->ptrace_cap) ? &e->ptrace[e->ptrace_n++] : NULL;
+  if (e->ptrace_cur) memset(e->ptrace_cur, 0, sizeof *e->ptrace_cur);
   for (int gr = 0; gr < e->mode_gr; gr++) {
     int bufpPos = 576 + gr * 576 - FFTOFFSET;
     int ret = lj_psycho_anal_ns(e, e->mfbuf[0], e->mfbuf[1], bufpPos, gr, masking_LR, masking_MS, pe[gr], pe_MS[gr], tot_ener[gr], blocktype);
@@ -381,6 +403,7 @@ static int encode_mp3_frame(LjEnc* e, uint8_t* mp3buf, int mp3buf_size) {
       e->tt[gr][ch].mixed_block_flag = 0;
     }
   }
+  e->ptrace_cur = NULL;
   adjust_ATH(e);
   lj_mdct_sub48(e, e->mfbuf[0], e->mfbuf[1]);
   e->mode_ext = 0; /* MPG_MD_LR_LR */
@@ -699,6 +722,15 @@ void lj_set_trace(LjEnc* e, LjFrameTrace* buf, int cap) { e->trace = buf; e->tra
 /* quantizer rows next to the frame trace: row k is filled together with lj_set_trace's row k (call it after lj_set_trace) */
 void lj_set_quant_trace(LjEnc* e, LjQuantTrace* buf, int cap) { e->qtrace = buf; e->qtrace_cap = cap; }
 int lj_quant_trace_size(void) { return (int)sizeof(LjQuantTrace); }
+/* psy rows, one per frame encoded from now on (independent of lj_set_trace) */
+void lj_set_psy_trace(LjEnc* e, LjPsyTrace* buf, int cap) { e->ptrace = buf; e->ptrace_cap = cap; e->ptrace_n = 0; }
+int lj_psy_trace_count(const LjEnc* e) { return e->ptrace_n; }
+int lj_psy_trace_size(void) { return (int)sizeof(LjPsyTrace); }
+/* the attack threshold of the long-block channels (NsPsy attackthre, the preset's st_lrm) */
+double lj_psy_attack_threshold(const LjEnc* e) { return e->attackthre; }
+double lj_ath_aa_sensitivity(const LjEnc* e) { return e->ath_aaSensitivityP; }
+/* partitions of the long (shortblock 0) or short blocks: the defined prefix of the psy trace's partition rows */
+int lj_psy_npart(const LjEnc* e, int shortblock) { return shortblock ? e->npart_s : e->npart_l; }
 int lj_trace_count(const LjEnc* e) { return e->trace_n; }
 int lj_trace_size(void) { return (int)sizeof(LjFrameTrace); }
 int lj_state_size(void) { return (int)sizeof(LjState); }

@@ -652,6 +652,7 @@ int lj_psycho_anal_ns(LjEnc* e, const F32* buf0, const F32* buf1, int bufPos, in
         if (i == 1) ns_attacks[0] = 0;
       }
     }
+    lj_psy_trace_attacks(e, gr_out, chn, en_subshort, ns_attacks);
     if (ns_attacks[0] != 0 && e->lastAttacks[chn] != 0) ns_attacks[0] = 0;
     if (e->lastAttacks[chn] == 3 || (ns_attacks[0] + ns_attacks[1] + ns_attacks[2] + ns_attacks[3]) != 0) {
       ns_uselongblock = 0;
@@ -666,9 +667,11 @@ int lj_psycho_anal_ns(LjEnc* e, const F32* buf0, const F32* buf1, int bufPos, in
     compute_ffts(e, fftenergy, fftenergy_s, wsamp_L, wsamp_S, gr_out, chn, buffer, bufPos);
     calc_energy(e, fftenergy, eb_l, max, avg);
     calc_mask_index_l(e, max, avg, mask_idx_l);
+    lj_psy_trace_long(e, gr_out, chn, eb_l, mask_idx_l);
     for (sblock = 0; sblock < 3; sblock++) {
       double enn, thmm;
       compute_masking_s(e, fftenergy_s, eb_s, thr, chn, sblock);
+      lj_psy_trace_short(e, gr_out, chn, sblock, eb_s);
       convert_partition2scalefac_s(e, eb_s, thr, chn, sblock);
       for (sb = 0; sb < SBMAX_s; sb++) {
         thmm = e->thm[chn].s[sb][sblock];

@@ -69,6 +69,7 @@ def bind(so):
     L.lj_gain_clamps.argtypes = [vp]
     L.lj_get_scale.restype = ctypes.c_double
     assert L.lj_trace_size() == oracle_lib.TRACE_DTYPE.itemsize
+    oracle_lib.bind_psy_trace(L)
     return L
 
 
@@ -80,12 +81,13 @@ class Encoder:
     """Mp3Encoder of the oracle whose encode_buffer takes Int16 arrays (lj_encode) or floating arrays (lj_encode_f32: rounded
     to Float32 once, like lamejs's store)."""
 
-    def __init__(self, channels, samplerate, kbps, trace_frames=0, write_vbr_tag=False):
+    def __init__(self, channels, samplerate, kbps, trace_frames=0, write_vbr_tag=False, psy_trace=False):
         self.L = lib()
         self.h = self.L.lj_create(channels, samplerate, kbps)
         if not self.h:
             raise ValueError("unsupported configuration")
         self.channels = channels
+        self.psy = oracle_lib.PsyTraceRows(self.L, self.h) if psy_trace else None
         self.tag_on = bool(write_vbr_tag) and self.L.lj_enable_vbr_tag(self.h) == 1
         self.trace = self.qtrace = None
         if trace_frames:
@@ -102,6 +104,8 @@ class Encoder:
         left, right = np.ascontiguousarray(left, dtype=dt), np.ascontiguousarray(right, dtype=dt)
         cap = int(1.25 * len(left) + 7200) + 2880
         buf = np.empty(cap, dtype=np.uint8)
+        if self.psy:
+            self.psy.before_call(len(left) // 576 + 4)
         fn = self.L.lj_encode_f32 if f32 else self.L.lj_encode
         k = oracle_lib.check(fn(self.h, left.ctypes.data, right.ctypes.data, len(left), buf.ctypes.data, cap), "lj_encode")
         return buf[:k].tobytes()
@@ -109,6 +113,8 @@ class Encoder:
     def flush(self):
         cap = 7200 + 4 * 1440 + 2880
         buf = np.empty(cap, dtype=np.uint8)
+        if self.psy:
+            self.psy.before_call(8)
         k = oracle_lib.check(self.L.lj_flush(self.h, buf.ctypes.data, cap), "lj_flush")
         return buf[:k].tobytes()
 
@@ -116,6 +122,12 @@ class Encoder:
         buf = np.zeros(2880, dtype=np.uint8)
         k = self.L.lj_get_lametag_frame(self.h, buf.ctypes.data, 2880)
         return buf[:k].tobytes()
+
+    def psy_traces(self):
+        return self.psy.rows()
+
+    def npart(self):
+        return self.L.lj_psy_npart(self.h, 0), self.L.lj_psy_npart(self.h, 1)
 
     def traces(self):
         n = self.L.lj_trace_count(self.h)

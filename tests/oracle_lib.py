@@ -60,6 +60,21 @@ QTRACE_DTYPE = np.dtype(
     align=True,
 )
 
+# lj_set_psy_trace: the psy model's per-granule analysis, one row per frame, [gr][ch] = psy call G k + gr of frame k; only the
+# first npart_l / npart_s partitions are defined
+PSY_TRACE_DTYPE = np.dtype(
+    [
+        ("eb_l", np.float32, (2, 2, 64)),                 # calc_energy
+        ("peaks", np.float32, (2, 2, 9)),                 # en_subshort[3..11]: max(1, |high-pass|) per 64 samples
+        ("loudness", np.float32, (2, 2)),                 # loudness_sq_save after the call
+        ("eb_s", np.float32, (2, 2, 3, 64)),              # compute_masking_s per short block: partition energies
+        ("ecb_s", np.float32, (2, 2, 3, 64)),             # ... and the spreading sum stored into nb_s1
+        ("mask_idx_l", np.int32, (2, 2, 64)),             # calc_mask_index_l
+        ("attack", np.int32, (2, 2, 4)),                  # ns_attacks after the ratio < 1.7 pass, before the lastAttacks rule
+    ],
+    align=True,
+)
+
 # what OracleEncoder.traces() returns: the fields of both records
 FULL_TRACE_DTYPE = np.dtype([(n, TRACE_DTYPE.fields[n][0]) for n in TRACE_DTYPE.names] +
                             [(n, QTRACE_DTYPE.fields[n][0]) for n in QTRACE_DTYPE.names])
@@ -126,8 +141,44 @@ def lib():
         assert L.lj_trace_size() == TRACE_DTYPE.itemsize, (L.lj_trace_size(), TRACE_DTYPE.itemsize)
         assert L.lj_quant_trace_size() == QTRACE_DTYPE.itemsize, (L.lj_quant_trace_size(), QTRACE_DTYPE.itemsize)
         assert L.lj_state_size() == STATE_DTYPE.itemsize, (L.lj_state_size(), STATE_DTYPE.itemsize)
+        bind_psy_trace(L)
         _lib = L
     return _lib
+
+
+def bind_psy_trace(L):
+    """ctypes signatures of the psy trace (the oracle's library or the Float32 build of its sources)"""
+    vp = ctypes.c_void_p
+    L.lj_set_psy_trace.argtypes = [vp, vp, ctypes.c_int]
+    L.lj_psy_trace_count.argtypes = [vp]
+    L.lj_psy_attack_threshold.argtypes = [vp]
+    L.lj_psy_attack_threshold.restype = ctypes.c_double
+    L.lj_ath_aa_sensitivity.argtypes = [vp]
+    L.lj_ath_aa_sensitivity.restype = ctypes.c_double
+    L.lj_psy_npart.argtypes = [vp, ctypes.c_int]
+    assert L.lj_psy_trace_size() == PSY_TRACE_DTYPE.itemsize, (L.lj_psy_trace_size(), PSY_TRACE_DTYPE.itemsize)
+
+
+class PsyTraceRows:
+    """The psy trace of one encoder, growing across its calls (lj_set_psy_trace); shared by OracleEncoder and oracle_f32."""
+
+    def __init__(self, L, h, cap=64):
+        self.L, self.h = L, h
+        self.buf = np.zeros(cap, dtype=PSY_TRACE_DTYPE)
+        self.done = []
+        L.lj_set_psy_trace(h, self.buf.ctypes.data, cap)
+
+    def before_call(self, max_frames):
+        """room for max_frames more rows: rows already written move to `done` and the buffer starts over"""
+        n = self.L.lj_psy_trace_count(self.h)
+        if n + max_frames > len(self.buf):
+            self.done.append(self.buf[:n].copy())
+            self.buf = np.zeros(max(max_frames, 64), dtype=PSY_TRACE_DTYPE)
+            self.L.lj_set_psy_trace(self.h, self.buf.ctypes.data, len(self.buf))
+
+    def rows(self):
+        n = self.L.lj_psy_trace_count(self.h)
+        return np.concatenate(self.done + [self.buf[:n]])
 
 
 ERR_BITSTREAM = -10          # LJ_ERR_BITSTREAM (oracle/lj_encoder.h)
@@ -155,12 +206,14 @@ def out_samplerate(channels, samplerate, kbps):
 class OracleEncoder:
     """Mirror of lamejs.Mp3Encoder (src/js/index.js:66-136) backed by the C++ restatement."""
 
-    def __init__(self, channels, samplerate, kbps, trace_frames=0, write_vbr_tag=False, reservoir=False, joint_stereo=False):
+    def __init__(self, channels, samplerate, kbps, trace_frames=0, write_vbr_tag=False, reservoir=False, joint_stereo=False,
+                 psy_trace=False):
         self.L = lib()
         self.h = self.L.lj_create(channels, samplerate, kbps)
         if not self.h:
             raise ValueError("unsupported configuration")
         self.channels = channels
+        self.psy = PsyTraceRows(self.L, self.h) if psy_trace else None
         if joint_stereo:                   # gfp.mode = JOINT_STEREO (SURVEY 8(f2); Mp3Encoder uses STEREO)
             assert self.L.lj_enable_joint_stereo(self.h) == 0
         if reservoir == "java":            # NOT lamejs: integer byte counts as in Reservoir.java (decodable streams)
@@ -181,12 +234,16 @@ class OracleEncoder:
         assert len(left) == len(right)
         cap = int(1.25 * len(left) + 7200)
         buf = np.empty(cap, dtype=np.uint8)
+        if self.psy:
+            self.psy.before_call(len(left) // 576 + 4)
         k = check(self.L.lj_encode(self.h, left.ctypes.data, right.ctypes.data, len(left), buf.ctypes.data, cap), "lj_encode")
         return buf[:k].tobytes()
 
     def flush(self):
         cap = 7200 + 4 * 1440
         buf = np.empty(cap, dtype=np.uint8)
+        if self.psy:
+            self.psy.before_call(8)
         k = check(self.L.lj_flush(self.h, buf.ctypes.data, cap), "lj_flush")
         return buf[:k].tobytes()
 
@@ -198,6 +255,20 @@ class OracleEncoder:
             for k in rec.dtype.names:
                 out[k] = rec[k][:n]
         return out
+
+    def psy_traces(self):
+        """every psy row since the encoder was made (PSY_TRACE_DTYPE, one per frame), across all calls"""
+        return self.psy.rows()
+
+    def attack_threshold(self):
+        return self.L.lj_psy_attack_threshold(self.h)
+
+    def ath_aa_sensitivity(self):
+        return self.L.lj_ath_aa_sensitivity(self.h)
+
+    def npart(self):
+        """(npart_l, npart_s): the defined prefix of the psy trace's partition rows"""
+        return self.L.lj_psy_npart(self.h, 0), self.L.lj_psy_npart(self.h, 1)
 
     def state(self):
         """The state carried into the next call: one STATE_DTYPE record (ATH adjust and its limit, blocktype_old,
