@@ -443,15 +443,21 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* t);
  * its first launch */
 int64_t mp3b200_debug_short_units(void);
 /* Debug psy-row capture, off by default.  on != 0 clears the records and turns capture on for every thread and session;
- * 0 turns it off (the records stay until taken).  While it is on, each pipeline launch fills its psy rows with a poison
- * pattern before the long-block analysis (float fields a quiet NaN, mask_idx 8, attack 0), synchronises its stream after the
- * attack pre-pass and after the short-block analysis, and records the rows there; a launch inside CUDA stream capture
- * fails with MP3B200_ERR_CUDA.  Launches are numbered from 0 in the order they start.  Each record is an int32[8] header
- * and its payload:
+ * 0 turns it off (the records stay until taken).  While it is on, each pipeline launch fills its front-end rows with a
+ * poison pattern before the long-block analysis (float and double fields a quiet NaN, mask_idx 8, attack 0, both block-type
+ * rows 1 = START), synchronises its stream after the attack pre-pass, after the short-block analysis and after the MDCT, and
+ * records the rows there; a launch inside CUDA stream capture fails with MP3B200_ERR_CUDA.  Launches are numbered from 0 in
+ * the order they start.  Each record is an int32[8] header and its payload:
  *   {1, launch, stream, frame0, nframes, nch, G, row_bytes}: the stream's long rows u = -1 .. G nframes - 1, nch per unit
  *     (eb_l float[64], peaks float[9], loudness float, mask_idx uint8[64], attack uint8[4], one pad byte; row_bytes each)
  *   {2, launch, count, nch, G, k_psy_analysis launches, 0, row_bytes}: the short list, count int32 pairs (stream,
- *     ((u + 1) << 1) | channel) in list order, then each entry's short row (ecb_s double[3][64], eb_s float[3][64]) */
+ *     ((u + 1) << 1) | channel) in list order, then each entry's short row (ecb_s double[3][64], eb_s float[3][64])
+ *   {3, launch, stream, frame0, nframes, nch, G, row_bytes}: the stream's rows after the MDCT, with n = G nframes:
+ *     ATH.adjust seen by the psy calls of each frame (double[nframes]), the adjustment the quantizer uses (double[nframes]),
+ *     the masking rows u = -1 .. n - 1, nch per unit (en_l float[22], thm_l float[22], en_s float[13][3],
+ *     thm_s float[13][3]; row_bytes each; row u is what granule u + 1 uses), xr float[n][nch][576], the final block type
+ *     int8[n][2] and the block type the psy call of the unit saw before it (int8[n][2]; both hold 2 per unit whatever nch),
+ *     then zero bytes up to a multiple of 8 */
 int mp3b200_debug_psy_capture(int on);
 /* Copies the records held (bytes) to buf and clears them when cap is large enough; returns their size either way. */
 int64_t mp3b200_debug_psy_take(void* buf, int64_t cap);

@@ -21,7 +21,9 @@
 #define MP3B200_K_FILTERBANK_CUH
 #include "mp3_device.cuh"
 
+#ifndef FB_G
 #define FB_G 8                                   /* granules per block */
+#endif
 #define FB_SPAN (576 * FB_G + 1055)              /* PCM samples a block touches */
 #define FB_PCM_WORDS (FB_SPAN + (FB_SPAN >> 5) + 2)   /* doubles: Int16 -> scaled float32 -> double is converted ONCE */
 #define FB_SLAB_STRIDE 33

@@ -627,7 +627,9 @@ __global__ void k_attack_prepass(const Mp3Tables* __restrict__ T, const StreamDe
  * reset the ATH state to (1, 1)), so each 16-frame chunk is run from a guessed in-state by its own thread, the
  * guesses are checked against the predecessor's out-state, and only wrong chunks are redone until nothing changes.
  * The result equals the sequential scan exactly; the worst case degenerates to it.  One block per stream. */
+#ifndef SCAN_FRAMES
 #define SCAN_FRAMES 16
+#endif
 #define SCAN_THREADS 1024
 /* The in-state every chunk but a stream's first starts from: lastAttacks and blocktype_old of both channels, and the ATH
  * (adjust, adjustLimit) pair.  Only the number of redo rounds depends on it (tests/test_gpu_speculation.py builds the

@@ -519,10 +519,11 @@ int wait_legacy(ThreadCtx& c) {
 struct Rows { bool f32; int scale_applied; };
 constexpr Rows SCALED_F32 = {true, 0};
 
-/* Debug psy-row capture (mp3b200_debug_psy_capture).  While it is on, every pipeline launch poisons the psy rows it uses
- * before k_psy_analysis, so that a row the launch forgets to write cannot pass for one written by an earlier launch, and
- * records them after k_attack_prepass (PsyUnit) and after k_psy_short (the short list and its PsyShort rows).  The launch
- * synchronises its stream at both points; with capture off it does nothing at all. */
+/* Debug psy-row capture (mp3b200_debug_psy_capture).  While it is on, every pipeline launch poisons the front-end rows it
+ * uses before k_psy_analysis, so that a row the launch forgets to write cannot pass for one written by an earlier launch, and
+ * records them after k_attack_prepass (PsyUnit), after k_psy_short (the short list and its PsyShort rows) and after k_mdct
+ * (block types, ATH adjustments, masking and xr).  The launch synchronises its stream at those points; with capture off it
+ * does nothing at all. */
 std::atomic<int> g_psy_capture{0};
 std::mutex g_psy_mu;                      /* guards g_psy_rec, g_psy_launch */
 std::vector<unsigned char> g_psy_rec;     /* records: int32[8] header + payload (include/mp3b200.h) */
@@ -536,9 +537,10 @@ void psy_rec_append(const int32_t (&h)[8], const void* a, size_t na, const void*
   if (nb) g_psy_rec.insert(g_psy_rec.end(), static_cast<const unsigned char*>(b), static_cast<const unsigned char*>(b) + nb);
 }
 
-/* Fills the launch's rows: floats with a quiet NaN, bytes with values that stay valid table indices (mask_idx 8, attack 0),
- * so that reading an unwritten row changes results without ever indexing out of bounds. */
-int psy_poison(ThreadCtx& c, size_t rows, int* launch) {
+/* Fills the launch's rows: floats with a quiet NaN, bytes with values that stay valid table indices (mask_idx 8, attack 0,
+ * block types BT_START), so that reading an unwritten row changes results without ever indexing out of bounds.  bt_prev never
+ * holds BT_START when written (the scan stores NORM, STOP or SHORT there). */
+int psy_poison(ThreadCtx& c, int G, long long total_frames, int S, int nch, int* launch) {
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
   CK(cudaStreamIsCapturing(c.st, &cs));
   if (cs != cudaStreamCaptureStatusNone) { g_err = "psy-row capture inside CUDA stream capture"; return MP3B200_ERR_CUDA; }
@@ -559,10 +561,25 @@ int psy_poison(ThreadCtx& c, size_t rows, int* launch) {
   PsyShort ps;
   for (int s = 0; s < 3; s++)
     for (int b = 0; b < MP3_CBANDS; b++) { ps.ecb_s[s][b] = (double)qnan; ps.eb_s[s][b] = qnan; }
+  const size_t units = (size_t)G * total_frames, rows = (units + S) * nch;
   std::vector<PsyUnit> u(rows, pu);
   std::vector<PsyShort> sh(rows, ps);
+  std::vector<float> f(rows * 576, qnan);             /* slab rows; the ratio and xr rows take a prefix */
+  const uint64_t dbits = 0x7ff8000000000000ull;
+  double dnan;
+  memcpy(&dnan, &dbits, sizeof dnan);
+  std::vector<double> d((size_t)total_frames, dnan);
   CK(cudaMemcpyAsync(c.ws.psy.p, u.data(), rows * sizeof(PsyUnit), cudaMemcpyHostToDevice, c.st));
   CK(cudaMemcpyAsync(c.ws.psy_s.p, sh.data(), rows * sizeof(PsyShort), cudaMemcpyHostToDevice, c.st));
+  CK(cudaMemcpyAsync(c.ws.ratio.p, f.data(), rows * sizeof(PsyRatioDev), cudaMemcpyHostToDevice, c.st));
+  CK(cudaMemcpyAsync(c.ws.slab.p, f.data(), rows * 576 * sizeof(float), cudaMemcpyHostToDevice, c.st));
+  CK(cudaMemcpyAsync(c.ws.xr.p, f.data(), units * nch * 576 * sizeof(float), cudaMemcpyHostToDevice, c.st));
+  if (total_frames) {
+    CK(cudaMemcpyAsync(c.ws.ath_psy.p, d.data(), d.size() * sizeof(double), cudaMemcpyHostToDevice, c.st));
+    CK(cudaMemcpyAsync(c.ws.ath_q.p, d.data(), d.size() * sizeof(double), cudaMemcpyHostToDevice, c.st));
+  }
+  CK(cudaMemsetAsync(c.ws.bt_final.p, BT_START, units * 2, c.st));
+  CK(cudaMemsetAsync(c.ws.bt_prev.p, BT_START, units * 2, c.st));
   CK(cudaStreamSynchronize(c.st));
   return 0;
 }
@@ -603,6 +620,36 @@ int psy_record_short(ThreadCtx& c, const StreamDesc* sds, int nch, int G, int la
   return 0;
 }
 
+/* After k_mdct: per stream, ath_psy and ath_q of its frames, the ratio rows u = -1 .. G nframes - 1, the xr rows, bt_final
+ * and bt_prev of its units (two per unit, as the workspace holds them), zero bytes up to a multiple of 8 */
+int psy_record_front(ThreadCtx& c, const StreamDesc* sds, int S, int nch, int G, int launch) {
+  CK(cudaStreamSynchronize(c.st));
+  for (int z = 0; z < S; z++) {
+    const StreamDesc& sd = sds[z];
+    const size_t F = (size_t)sd.nframes, n = (size_t)G * sd.nframes;
+    const size_t b_ath = 2 * F * sizeof(double), b_ratio = (n + 1) * nch * sizeof(PsyRatioDev);
+    const size_t b_xr = n * nch * 576 * sizeof(float), b_bt = 2 * n * 2;
+    std::vector<unsigned char> p(b_ath + b_ratio + b_xr + ((b_bt + 7) & ~(size_t)7), 0);
+    unsigned char* q = p.data();
+    if (F) {
+      CK(cudaMemcpyAsync(q, c.ws.ath_psy.p + sd.frame_base, F * sizeof(double), cudaMemcpyDeviceToHost, c.st));
+      CK(cudaMemcpyAsync(q + F * sizeof(double), c.ws.ath_q.p + sd.frame_base, F * sizeof(double), cudaMemcpyDeviceToHost, c.st));
+    }
+    q += b_ath;
+    CK(cudaMemcpyAsync(q, c.ws.ratio.p + ((size_t)sd.unit_base + z) * nch, b_ratio, cudaMemcpyDeviceToHost, c.st));
+    q += b_ratio;
+    if (n) {
+      CK(cudaMemcpyAsync(q, c.ws.xr.p + (size_t)sd.unit_base * nch * 576, b_xr, cudaMemcpyDeviceToHost, c.st));
+      CK(cudaMemcpyAsync(q + b_xr, c.ws.bt_final.p + (size_t)sd.unit_base * 2, n * 2, cudaMemcpyDeviceToHost, c.st));
+      CK(cudaMemcpyAsync(q + b_xr + n * 2, c.ws.bt_prev.p + (size_t)sd.unit_base * 2, n * 2, cudaMemcpyDeviceToHost, c.st));
+    }
+    CK(cudaStreamSynchronize(c.st));
+    const int32_t h[8] = {3, launch, z, sd.frame0, sd.nframes, nch, G, (int32_t)sizeof(PsyRatioDev)};
+    psy_rec_append(h, p.data(), p.size());
+  }
+  return 0;
+}
+
 /* One pipeline launch for the streams sds[0 .. S) (at most MP3_MAX_LAUNCH_STREAMS, unit / frame bases set, the workspace
  * large enough).  All launches go to the context's stream (c.st: the calling thread's, t_ctx.st, or a session's), which
  * first waits for whatever the caller queued on the legacy default stream (wait_legacy); with o.sync the call returns after
@@ -637,7 +684,7 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, const 
   }
   int psy_launch = -1, k2_launches = 0;
   if (g_psy_capture.load(std::memory_order_relaxed) &&
-      (rc = psy_poison(c, ((size_t)cfg->host.mode_gr * total_frames + S) * nch, &psy_launch))) return rc;
+      (rc = psy_poison(c, cfg->host.mode_gr, total_frames, S, nch, &psy_launch))) return rc;
   CK(cudaEventRecord(ev[0], st));
 
   /* K2: psy analysis, one block per (PSY_UNITS consecutive granules incl. 1 halo, channel, stream) */
@@ -746,6 +793,7 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, const 
     k_mdct<<<grid, FB_G * 32, 0, st>>>(tab, ws.streams.p, ws.slab.p, ws.bt_final.p, ws.xr.p);
     g_launches++;
     DBG("k_mdct");
+    if (psy_launch >= 0 && (rc = psy_record_front(c, h_streams, S, nch, cfg->host.mode_gr, psy_launch))) return rc;
   }
   CK(cudaEventRecord(ev[4], st));
   int passes = 0;

@@ -979,19 +979,24 @@ PSY_UNIT_DTYPE = np.dtype({"names": ["eb_l", "peaks", "loudness", "mask_idx", "a
                            "offsets": [0, 256, 292, 296, 360], "itemsize": 368})
 PSY_SHORT_DTYPE = np.dtype({"names": ["ecb_s", "eb_s"], "formats": [(np.float64, (3, 64)), (np.float32, (3, 64))],
                             "offsets": [0, 1536], "itemsize": 2304})
+PSY_RATIO_DTYPE = np.dtype([("en_l", np.float32, 22), ("thm_l", np.float32, 22), ("en_s", np.float32, (13, 3)),
+                            ("thm_s", np.float32, (13, 3))])
 
 
 class PsyCapture:
     """What debug_psy_capture recorded: `launches`, one dict per pipeline launch in launch order, filled when the block ends:
     "streams": per stream of the launch {"z", "frame0", "nframes", "rows"} with rows PSY_UNIT_DTYPE[G nframes + 1][nch] for
-    u = -1 .. G nframes - 1; "short": the short list as an int array [count][3] of (stream, u, channel) in list order;
-    "short_rows": PSY_SHORT_DTYPE[count]; "k2_launches": how many k_psy_analysis launches the pipeline made."""
+    u = -1 .. G nframes - 1, and the rows after the MDCT: "bt" and "bt_prev" int8[G nframes][nch] (the final block type and
+    the one the unit's psy call saw), "ath_psy" and "ath_q" float64[nframes], "ratio" PSY_RATIO_DTYPE[G nframes + 1][nch]
+    for u = -1 .. G nframes - 1 (row u is the masking granule u + 1 uses) and "xr" float32[G nframes][nch][576]; "short": the
+    short list as an int array [count][3] of (stream, u, channel) in list order; "short_rows": PSY_SHORT_DTYPE[count];
+    "k2_launches": how many k_psy_analysis launches the pipeline made."""
 
     def __init__(self):
         self.launches = []
 
     def _parse(self, raw):
-        by = {}
+        by, front = {}, {}
         off = 0
         while off < len(raw):
             h = np.frombuffer(raw, dtype=np.int32, count=8, offset=off)
@@ -1005,6 +1010,23 @@ class PsyCapture:
                 rows = np.frombuffer(raw, dtype=PSY_UNIT_DTYPE, count=n, offset=off).reshape(-1, nch).copy()
                 off += n * rb
                 rec["streams"].append({"z": z, "frame0": frame0, "nframes": nframes, "G": G, "rows": rows})
+            elif kind == 3:
+                z, frame0, nframes, nch, G, rb = (int(v) for v in h[2:])
+                assert rb == PSY_RATIO_DTYPE.itemsize, rb
+                n = G * nframes
+                s = {}
+                for k in ("ath_psy", "ath_q"):
+                    s[k] = np.frombuffer(raw, dtype=np.float64, count=nframes, offset=off).copy()
+                    off += 8 * nframes
+                s["ratio"] = np.frombuffer(raw, dtype=PSY_RATIO_DTYPE, count=(n + 1) * nch, offset=off).reshape(-1, nch).copy()
+                off += (n + 1) * nch * rb
+                s["xr"] = np.frombuffer(raw, dtype=np.float32, count=n * nch * 576, offset=off).reshape(n, nch, 576).copy()
+                off += 4 * n * nch * 576
+                for k in ("bt", "bt_prev"):
+                    s[k] = np.frombuffer(raw, dtype=np.int8, count=2 * n, offset=off).reshape(n, 2)[:, :nch].copy()
+                    off += 2 * n
+                off += -(4 * n) % 8
+                front.setdefault(launch, {})[z] = s
             else:
                 assert kind == 2, kind
                 count, nch, G, k2, _, rb = (int(v) for v in h[2:])
@@ -1017,14 +1039,17 @@ class PsyCapture:
                 rec["k2_launches"] = k2
         for k in sorted(by):
             by[k]["streams"].sort(key=lambda s: s["z"])
+            for s in by[k]["streams"]:
+                s.update(front.get(k, {}).get(s["z"], {}))
             self.launches.append(by[k])
 
 
 @contextlib.contextmanager
 def debug_psy_capture():
-    """Debug only: while the block runs, every pipeline launch (any thread, any session) poisons its psy rows before the
-    long-block analysis and records them after the attack pre-pass and the short-block analysis (mp3b200_debug_psy_capture;
-    each launch synchronises its stream at those points).  Yields a PsyCapture, filled when the block ends."""
+    """Debug only: while the block runs, every pipeline launch (any thread, any session) poisons its front-end rows before
+    the long-block analysis (psy rows, short rows, subband slabs, masking, xr, ATH adjustments, block types) and records them
+    after the attack pre-pass, the short-block analysis and the MDCT (mp3b200_debug_psy_capture; each launch synchronises
+    its stream at those points).  Yields a PsyCapture, filled when the block ends."""
     L = lib()
     L.mp3b200_debug_psy_capture.argtypes = [ctypes.c_int]
     L.mp3b200_debug_psy_take.argtypes = [ctypes.c_void_p, ctypes.c_int64]

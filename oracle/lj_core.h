@@ -143,6 +143,14 @@ struct LjPsyTrace {
   int   attack[2][2][4];
 };
 
+/* per-frame record of the block type each psy call found (lj_set_psy_block_trace), row k belonging to LjPsyTrace row k.  A
+ * record of its own, like LjQuantTrace, so that LjPsyTrace keeps its layout.
+ *   blocktype_old     gfc.blocktype_old as call G k + gr found it: what compute_masking_s and the long-block thresholds read,
+ *                     before block_type_set turns it into the granule's block type */
+struct LjPsyBlockTrace {
+  int   blocktype_old[2][2];
+};
+
 /* what an encoder carries from one call to the next (lj_get_state) */
 struct LjState {
   double ath_adjust, ath_adjust_limit;

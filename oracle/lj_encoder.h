@@ -104,6 +104,7 @@ struct LjEnc {
   LjQuantTrace* qtrace_cur;      /* the quantizer row of the frame being encoded while tracing, else NULL (lj_quant.cpp) */
   LjPsyTrace* ptrace; int ptrace_cap, ptrace_n;
   LjPsyTrace* ptrace_cur;        /* the psy row of the frame being encoded while tracing, else NULL (lj_psy_trace_*) */
+  LjPsyBlockTrace* pbtrace; int pbtrace_cap;   /* rows beside ptrace's (lj_set_psy_block_trace), or NULL */
   /* Xing / LAME tag state (VBRSeekInfo.js, LameInternalFlags.js:170; lj_vbrtag.cpp).  nMusicCRC and nBytesWritten are
    * maintained by copy_buffer on every call whether or not a tag is written (BitStream.js:924-935). */
   int nMusicCRC; long long nBytesWritten;

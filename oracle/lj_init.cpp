@@ -339,6 +339,8 @@ void lj_psy_trace_attacks(LjEnc* e, int gr, int chn, const F32* en_subshort, con
   if (!t || chn >= 2) return;
   for (int i = 0; i < 9; i++) t->peaks[gr][chn][i] = en_subshort[i + 3].v;
   for (int i = 0; i < 4; i++) t->attack[gr][chn][i] = ns_attacks[i];
+  const int row = (int)(t - e->ptrace);
+  if (e->pbtrace && row < e->pbtrace_cap) e->pbtrace[row].blocktype_old[gr][chn] = e->blocktype_old[chn];
 }
 void lj_psy_trace_long(LjEnc* e, int gr, int chn, const F32* eb_l, const int* mask_idx_l) {
   LjPsyTrace* const t = e->ptrace_cur;
@@ -723,7 +725,13 @@ void lj_set_trace(LjEnc* e, LjFrameTrace* buf, int cap) { e->trace = buf; e->tra
 void lj_set_quant_trace(LjEnc* e, LjQuantTrace* buf, int cap) { e->qtrace = buf; e->qtrace_cap = cap; }
 int lj_quant_trace_size(void) { return (int)sizeof(LjQuantTrace); }
 /* psy rows, one per frame encoded from now on (independent of lj_set_trace) */
-void lj_set_psy_trace(LjEnc* e, LjPsyTrace* buf, int cap) { e->ptrace = buf; e->ptrace_cap = cap; e->ptrace_n = 0; }
+void lj_set_psy_trace(LjEnc* e, LjPsyTrace* buf, int cap) {
+  e->ptrace = buf; e->ptrace_cap = cap; e->ptrace_n = 0;
+  e->pbtrace = NULL; e->pbtrace_cap = 0;
+}
+/* block types beside the psy rows: row k is filled together with lj_set_psy_trace's row k (call it after lj_set_psy_trace) */
+void lj_set_psy_block_trace(LjEnc* e, LjPsyBlockTrace* buf, int cap) { e->pbtrace = buf; e->pbtrace_cap = cap; }
+int lj_psy_block_trace_size(void) { return (int)sizeof(LjPsyBlockTrace); }
 int lj_psy_trace_count(const LjEnc* e) { return e->ptrace_n; }
 int lj_psy_trace_size(void) { return (int)sizeof(LjPsyTrace); }
 /* the attack threshold of the long-block channels (NsPsy attackthre, the preset's st_lrm) */

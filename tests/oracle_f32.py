@@ -68,7 +68,9 @@ def bind(so):
     L.lj_get_scale.argtypes = [vp]
     L.lj_gain_clamps.argtypes = [vp]
     L.lj_get_scale.restype = ctypes.c_double
+    L.lj_get_state.argtypes = [vp, vp]
     assert L.lj_trace_size() == oracle_lib.TRACE_DTYPE.itemsize
+    assert L.lj_state_size() == oracle_lib.STATE_DTYPE.itemsize
     oracle_lib.bind_psy_trace(L)
     return L
 
@@ -126,8 +128,17 @@ class Encoder:
     def psy_traces(self):
         return self.psy.rows()
 
+    def psy_block_traces(self):
+        return self.psy.block_rows()
+
     def npart(self):
         return self.L.lj_psy_npart(self.h, 0), self.L.lj_psy_npart(self.h, 1)
+
+    def state(self):
+        """the state carried into the next call (oracle_lib.OracleEncoder.state)"""
+        s = np.zeros((), dtype=oracle_lib.STATE_DTYPE)
+        self.L.lj_get_state(self.h, s.ctypes.data)
+        return s
 
     def traces(self):
         n = self.L.lj_trace_count(self.h)

@@ -75,6 +75,9 @@ PSY_TRACE_DTYPE = np.dtype(
     align=True,
 )
 
+# lj_set_psy_block_trace: beside each psy row, blocktype_old as each psy call found it ([gr][ch]), before block_type_set
+PSY_BLOCK_TRACE_DTYPE = np.dtype([("blocktype_old", np.int32, (2, 2))])
+
 # what OracleEncoder.traces() returns: the fields of both records
 FULL_TRACE_DTYPE = np.dtype([(n, TRACE_DTYPE.fields[n][0]) for n in TRACE_DTYPE.names] +
                             [(n, QTRACE_DTYPE.fields[n][0]) for n in QTRACE_DTYPE.names])
@@ -156,29 +159,42 @@ def bind_psy_trace(L):
     L.lj_ath_aa_sensitivity.argtypes = [vp]
     L.lj_ath_aa_sensitivity.restype = ctypes.c_double
     L.lj_psy_npart.argtypes = [vp, ctypes.c_int]
+    L.lj_set_psy_block_trace.argtypes = [vp, vp, ctypes.c_int]
     assert L.lj_psy_trace_size() == PSY_TRACE_DTYPE.itemsize, (L.lj_psy_trace_size(), PSY_TRACE_DTYPE.itemsize)
+    assert L.lj_psy_block_trace_size() == PSY_BLOCK_TRACE_DTYPE.itemsize, (L.lj_psy_block_trace_size(), PSY_BLOCK_TRACE_DTYPE.itemsize)
 
 
 class PsyTraceRows:
-    """The psy trace of one encoder, growing across its calls (lj_set_psy_trace); shared by OracleEncoder and oracle_f32."""
+    """The psy trace of one encoder and the block types beside it, growing across its calls (lj_set_psy_trace,
+    lj_set_psy_block_trace); shared by OracleEncoder and oracle_f32."""
 
     def __init__(self, L, h, cap=64):
         self.L, self.h = L, h
+        self.done, self.bt_done = [], []
+        self._set(cap)
+
+    def _set(self, cap):
         self.buf = np.zeros(cap, dtype=PSY_TRACE_DTYPE)
-        self.done = []
-        L.lj_set_psy_trace(h, self.buf.ctypes.data, cap)
+        self.bt_buf = np.zeros(cap, dtype=PSY_BLOCK_TRACE_DTYPE)
+        self.L.lj_set_psy_trace(self.h, self.buf.ctypes.data, cap)
+        self.L.lj_set_psy_block_trace(self.h, self.bt_buf.ctypes.data, cap)
 
     def before_call(self, max_frames):
-        """room for max_frames more rows: rows already written move to `done` and the buffer starts over"""
+        """room for max_frames more rows: rows already written move to `done` and the buffers start over"""
         n = self.L.lj_psy_trace_count(self.h)
         if n + max_frames > len(self.buf):
             self.done.append(self.buf[:n].copy())
-            self.buf = np.zeros(max(max_frames, 64), dtype=PSY_TRACE_DTYPE)
-            self.L.lj_set_psy_trace(self.h, self.buf.ctypes.data, len(self.buf))
+            self.bt_done.append(self.bt_buf[:n].copy())
+            self._set(max(max_frames, 64))
 
     def rows(self):
         n = self.L.lj_psy_trace_count(self.h)
         return np.concatenate(self.done + [self.buf[:n]])
+
+    def block_rows(self):
+        """blocktype_old [frame][gr][ch] of every psy row"""
+        n = self.L.lj_psy_trace_count(self.h)
+        return np.concatenate(self.bt_done + [self.bt_buf[:n]])["blocktype_old"]
 
 
 ERR_BITSTREAM = -10          # LJ_ERR_BITSTREAM (oracle/lj_encoder.h)
@@ -259,6 +275,10 @@ class OracleEncoder:
     def psy_traces(self):
         """every psy row since the encoder was made (PSY_TRACE_DTYPE, one per frame), across all calls"""
         return self.psy.rows()
+
+    def psy_block_traces(self):
+        """blocktype_old as each psy call found it, int32 [frame][gr][ch], beside psy_traces()"""
+        return self.psy.block_rows()
 
     def attack_threshold(self):
         return self.L.lj_psy_attack_threshold(self.h)

@@ -25,7 +25,8 @@ PCM_SLICES = 8              # MP3_MAX_PCM_CHUNKS: host calls of <= 8 streams and
 
 
 class Ref:
-    """the oracle encoder of one stream, fed the same calls as the GPU: psy rows, block types and bytes across all calls"""
+    """the oracle encoder of one stream, fed the same calls as the GPU: psy rows, block types and bytes across all calls, and
+    `states`: the state after each call (oracle_lib.STATE_DTYPE) by the number of frames encoded so far"""
 
     def __init__(self, ch, sr, kb, f32=False, trace_frames=4096):
         self.ch = ch
@@ -33,26 +34,31 @@ class Ref:
         self.enc = (oracle_f32.Encoder(ch, sr, kb, trace_frames=trace_frames, psy_trace=True) if mod else
                     oracle_lib.OracleEncoder(ch, sr, kb, trace_frames=trace_frames, psy_trace=True))
         self.out = []
+        self.states = {}
+
+    def _after_call(self, b):
+        st = self.enc.state()
+        self.states[int(st["frames_done"])] = st
+        self.out.append(b)
+        return b
 
     def call(self, l, r=None):
-        b = self.enc.encode_buffer(l, r)
-        self.out.append(b)
-        return b
+        return self._after_call(self.enc.encode_buffer(l, r))
 
     def flush(self):
-        b = self.enc.flush()
-        self.out.append(b)
-        return b
+        return self._after_call(self.enc.flush())
 
     def stream(self, l, r=None):
         """one whole stream (encodeBuffer once, flush): its bytes"""
         return self.call(l, r) + self.flush() if len(l) else self.flush()
 
     def done(self):
-        """psy rows, block types [unit][ch] and partition counts of everything encoded so far"""
+        """psy rows, blocktype_old per psy call (`bt_old`), frame trace (`tr`), block types [unit][ch] and partition counts of
+        everything encoded so far"""
         self.psy = self.enc.psy_traces()
+        self.bt_old = self.enc.psy_block_traces()
         G = self.G = 2 if self.sr_out >= 32000 else 1
-        tr = self.enc.traces()
+        tr = self.tr = self.enc.traces()
         self.bt = tr["blocktype"][:, :G, :self.ch].reshape(-1, self.ch)
         self.npl, self.nps = self.enc.npart()
         return self
@@ -225,8 +231,9 @@ def capture_call(M, fn):
     return res, cap.launches
 
 
-def whole_streams(M, ch, sr, kb, sigs, label, fail, f32=False, resample=False):
-    """one host call over `sigs` (a batch when several); rows and bytes against one oracle per stream"""
+def whole_streams(M, ch, sr, kb, sigs, label, fail, f32=False, resample=False, check=None):
+    """one host call over `sigs` (a batch when several); rows (`check`, default check_launch) and bytes against one oracle
+    per stream"""
     refs = [make_ref(ch, sr, kb, f32) for _ in sigs]
     want = [rf.stream(l, r if ch == 2 else None) for rf, (l, r) in zip(refs, sigs)]
     for rf in refs:
@@ -239,7 +246,7 @@ def whole_streams(M, ch, sr, kb, sigs, label, fail, f32=False, resample=False):
     base = 0
     for rec in launches:
         k = len(rec["streams"])
-        check_launch(rec, refs[base:base + k], label, fail)
+        (check or check_launch)(rec, refs[base:base + k], label, fail)
         base += k
     if base != len(sigs):
         fail.append("%s: %d streams recorded, %d encoded" % (label, base, len(sigs)))
@@ -253,12 +260,13 @@ def stream_lengths(M, ch, sr, kb):
     return [0, 1, 575, 576, 1376, 1377, 12 * fs + 300, 13 * fs + 300]
 
 
-def shape_whole(M, fail, configs=None):
+def shape_whole(M, fail, configs=None, check=None):
     for j, (ch, sr, kb) in enumerate(configs or native_configs()):
         lens = stream_lengths(M, ch, sr, kb)
         for i, n in enumerate(lens):
             kind = K2_KINDS[(i + j) % len(K2_KINDS)]
-            whole_streams(M, ch, sr, kb, [k2_signal(kind, n, 100 * j + i)], "whole %d/%d/%d n=%d %s" % (ch, sr, kb, n, kind), fail)
+            whole_streams(M, ch, sr, kb, [k2_signal(kind, n, 100 * j + i)], "whole %d/%d/%d n=%d %s" % (ch, sr, kb, n, kind), fail,
+                          check=check)
 
 
 BATCHES = [
@@ -269,11 +277,11 @@ BATCHES = [
 ]
 
 
-def shape_batches(M, fail):
+def shape_batches(M, fail, check=None):
     for (ch, sr, kb), lens in BATCHES:
         sigs = [k2_signal(K2_KINDS[i % len(K2_KINDS)], n, 300 + i) if i % 2 else make_signal("burst", n, sr, 300 + i)
                 for i, n in enumerate(lens)]
-        whole_streams(M, ch, sr, kb, sigs, "batch %d/%d/%d" % (ch, sr, kb), fail)
+        whole_streams(M, ch, sr, kb, sigs, "batch %d/%d/%d" % (ch, sr, kb), fail, check=check)
 
 
 def slice_of(c, pcm_base, n, nchunks=PCM_SLICES):
@@ -326,11 +334,11 @@ def slice_lengths(M, ch, sr, kb, nstreams, seed):
     raise AssertionError("no slicing found")
 
 
-def shape_slices(M, fail):
+def shape_slices(M, fail, check=None):
     for (ch, sr, kb), nstreams in (((2, 44100, 128), 1), ((1, 22050, 64), 3)):
         lens = slice_lengths(M, ch, sr, kb, nstreams, 7 + nstreams)
         sigs = [k2_signal("mixed", n, 500 + i) for i, n in enumerate(lens)]
-        launches = whole_streams(M, ch, sr, kb, sigs, "slices %d/%d/%d" % (ch, sr, kb), fail)
+        launches = whole_streams(M, ch, sr, kb, sigs, "slices %d/%d/%d" % (ch, sr, kb), fail, check=check)
         G = M.granules_per_frame(ch, sr, kb)
         want = len({slice_of(u, 0, n) for n in lens for u in range(-1, G * M.stream_frames(n, ch, sr, kb))})
         for rec in launches:

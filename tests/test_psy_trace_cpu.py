@@ -33,7 +33,7 @@ def encode(oracle, ch, sr, kb, l, r):
     L = enc.L
     L.lj_get_scale.argtypes = [ctypes.c_void_p]
     L.lj_get_scale.restype = ctypes.c_double
-    out = dict(psy=enc.psy_traces(), tr=enc.traces(), thr=enc.attack_threshold(), sens=enc.ath_aa_sensitivity(),
+    out = dict(psy=enc.psy_traces(), bt_old=enc.psy_block_traces(), tr=enc.traces(), thr=enc.attack_threshold(), sens=enc.ath_aa_sensitivity(),
                scale=L.lj_get_scale(enc.h))
     enc.close()
     assert len(out["psy"]) == len(out["tr"])
@@ -150,6 +150,27 @@ def check_ath_adjust(o, G, nch):
         assert np.float64(adjust).tobytes() == np.float64(tr["ath_adjust"][k]).tobytes(), (k, adjust, tr["ath_adjust"][k])
 
 
+NORM, START, SHORT, STOP = 0, 1, 2, 3
+
+
+def check_block_types(o, G, nch):
+    """blocktype_old as each psy call found it, tied to the traced block types (block_type_set, PsyModel.js:784-826): the
+    stream starts from NORM; a unit is short exactly when the next call finds SHORT, and then its block type is blocktype_old
+    promoted (NORM -> START, STOP -> SHORT), else blocktype_old itself; a long unit hands on STOP after SHORT, NORM otherwise"""
+    psy, tr = o["psy"], o["tr"]
+    U = G * len(psy)
+    assert len(o["bt_old"]) == len(psy)
+    prev = o["bt_old"][:, :G, :nch].reshape(U, nch)
+    bt = tr["blocktype"][:, :G, :nch].reshape(U, nch)
+    assert (prev[0] == NORM).all()
+    assert np.isin(prev, (NORM, SHORT, STOP)).all(), np.unique(prev)
+    for c in range(U - 1):
+        short = prev[c + 1] == SHORT
+        promoted = np.where(prev[c] == NORM, START, np.where(prev[c] == STOP, SHORT, prev[c]))
+        assert (bt[c] == np.where(short, promoted, prev[c])).all(), (c, bt[c], prev[c], prev[c + 1])
+        assert (short | (prev[c + 1] == np.where(prev[c] == SHORT, STOP, NORM))).all(), (c, prev[c], prev[c + 1])
+
+
 def run_case(oracle, ch, sr, kb, l, r):
     assert oracle.out_samplerate(ch, sr, kb) == sr
     G = 2 if sr >= 32000 else 1
@@ -168,7 +189,8 @@ def run_case(oracle, ch, sr, kb, l, r):
 def test_trace_of_the_edge_corpus(oracle, case):
     _, ch, sr, kb, _ = case
     l, r = edge_signals.signal(case)
-    run_case(oracle, ch, sr, kb, l, r if ch == 2 else None)
+    o = run_case(oracle, ch, sr, kb, l, r if ch == 2 else None)
+    check_block_types(o, 2 if sr >= 32000 else 1, ch)
 
 
 @pytest.mark.parametrize("lsb,ch,sr,kb", QUIET)
