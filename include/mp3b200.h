@@ -177,7 +177,8 @@ int mp3b200_encode_streams_ex(int channels, int samplerate, int kbps, int flags,
  * [11] k_q_finish (gr0 + gr1), [12] k_q_pack, [13] the re-validation folded into the first pass (verify + repaired
  * searches / rate loops of the few frames whose speculated start did not stand); [14..15] reserved (0).
  * More than 65535 streams run as consecutive launches of at most 65535 streams: the times are summed over them, [7] is the
- * largest pass count of any of them.
+ * largest pass count of any of them.  The passes after the first run on the device, as a CUDA graph with a conditional
+ * WHILE node (DESIGN.md 5, 14): [7] is read from the device with the times, and a new launch shape costs one capture.
  * The call runs on a stream of its own that first waits for work already queued on the legacy default stream (where torch /
  * plain CUDA callers produced d_pcm) and returns after that stream has drained.  Arguments as for every whole-stream call
  * (above). */
@@ -529,8 +530,8 @@ int mp3b200_debug_replaygain_f32(int channels, int samplerate, int kbps, int fla
  * The call does not wait for the device, except: on the first use of a configuration on the device (its tables are
  * uploaded), when the session's workspace or pinned staging grows (which may synchronise the device), and when
  * MP3B200_SESSION_SLOTS calls of the session are still in flight (it waits for the oldest).  A session that has seen a
- * launch shape before never waits.  The quantizer's re-validation loop runs on the device (a CUDA graph with a conditional
- * WHILE node, captured once per launch shape and kept by the session).
+ * launch shape before never waits.  The quantizer's re-validation loop runs on the device, as in every call (a CUDA graph
+ * with a conditional WHILE node, captured once per launch shape and kept by the session, at most 32 of them).
  * One call runs at a time per session; sessions share no buffer, so several may be used from one thread or from many.
  * The buffers must stay alive until the stream has reached the call's end.  mp3b200_session_destroy waits for the session's
  * queued work, then frees it. */

@@ -16,7 +16,7 @@
  *
  * Cross-frame recurrence: bin_search_StepSize starts from gfc.OldValue/CurrentStep left by the previous frame.
  * Frames are encoded in parallel from a speculated in-state, the out-states are compared with the successor's
- * assumption and mismatching frames are redone (host loop in quant_run) until a fixed point -- byte-identical to
+ * assumption and mismatching frames are redone (a device loop in quant_run) until a fixed point -- byte-identical to
  * the sequential order.
  */
 #ifndef MP3B200_K_QUANT_CUH
@@ -2118,10 +2118,10 @@ __global__ void k_qstate_commit(StreamDesc* __restrict__ streams, int nstreams, 
 }
 
 /* The fixed-point loop as a CUDA graph (QuantLoop): runs after each k_qstate_verify of the graph's WHILE body and decides
- * whether the body goes on.  st[2] counts the passes of the launch group as quant_run's host loop counts them (2 after the
- * first pass, +1 for each re-validation that found work), st[0] keeps the largest count of the call.  A count beyond
- * max_passes (the host loop's bound, which cannot be reached) stops the loop with st[1] = 1 and an empty work list, so the
- * rest of the body has nothing to do. */
+ * whether the body goes on.  st[2] counts the passes of the launch group (2 after the first pass, +1 for each re-validation
+ * that found work), st[0] keeps the largest count of the call.  A count beyond max_passes (which cannot be reached: each
+ * pass fixes at least the first dirty frame) stops the loop with st[1] = 1 and an empty work list, so the rest of the body
+ * has nothing to do. */
 __global__ void k_qstate_loop_cond(cudaGraphConditionalHandle loop, int* __restrict__ count, int* __restrict__ st, int max_passes) {
   const int n = *count;
   int passes = st[2];
@@ -2145,7 +2145,7 @@ struct QuantBuffers {
 #define Q_REPAIR_BLOCKS 16
 enum { QE_START, QE_PREP, QE_S0, QE_O0, QE_F0, QE_S1, QE_MID, QE_O1, QE_F1, QE_PK, QE_COUNT };   /* timing event slots */
 
-/* The fixed-point loop on the device, for launches that must not wait for the host: a graph of a memset (st[2] = 2) and a
+/* The fixed-point loop on the device, so that no launch waits for the host: a graph of a memset (st[2] = 2) and a
  * conditional WHILE node whose body is one re-validation pass -- the counter memsets, k_qstate_verify, k_qstate_loop_cond,
  * then the searches, rate loops and finishes of the listed frames and k_q_pack, every launch taking its count from the
  * device and sized for all F frames.  quant_run launches `exec` on the main stream; when it is null it first captures and
@@ -2159,8 +2159,7 @@ struct QuantLoop {
 
 static int quant_run(const Mp3Tables* dT, const Mp3Tables& hT, StreamDesc* d_streams, int S, int nstreams_with_frames, int max_frames, long long F,
                      const QuantBuffers& B, cudaStream_t st_main, cudaStream_t st_repair, cudaEvent_t ev_fork, cudaEvent_t ev_join,
-                     cudaEvent_t ev_pass1, cudaEvent_t* evq, int* evq_pred, int* passes_out, std::atomic<long long>* launches,
-                     QuantLoop* dloop = nullptr) {
+                     cudaEvent_t ev_pass1, cudaEvent_t* evq, int* evq_pred, std::atomic<long long>* launches, QuantLoop& loop) {
   cudaStream_t st = st_main;       /* the launch helpers below use `st`; the repair chain temporarily points it at st_repair */
   static std::mutex attr_mu;
   static bool attr_done[64] = {};
@@ -2179,7 +2178,7 @@ static int quant_run(const Mp3Tables* dT, const Mp3Tables& hT, StreamDesc* d_str
       attr_done[dev] = true;
     }
   }
-  if (F <= 0) { *passes_out = 0; return 0; }
+  if (F <= 0) return 0;
   const int nch = hT.nch;
   int next_counter = Q_NCOUNTERS;                 /* forces the first memset */
   auto fresh_counter = [&]() -> int* {            /* a zeroed task counter for the next launch */
@@ -2302,72 +2301,57 @@ static int quant_run(const Mp3Tables* dT, const Mp3Tables& hT, StreamDesc* d_str
   }
   pack(nullptr, nullptr, F, 0); mark(QE_PK);
   if (cudaEventRecord(ev_pass1, st) != cudaSuccess) return -100;
-  int passes = 2;
   /* ---- fixed point: a repaired frame may hand its successor a different in-state than the one it was verified with ----
-   * One re-validation pass over the frames verify() listed: `count` of them (count1 == nullptr), or as many as
-   * counter[0] says on the device (count = F, the worst case). */
-  auto revalidate = [&](const int* count1, long long count) {
-    search(0, list1, count1, count, 1);
-    outer(0, list2, B.counter + 1, count, 1);
-    finish(0, list2, B.counter + 1, count, 1);
-    if (G == 2) {
-      search(1, list2, B.counter + 1, count, 1);
-      outer(1, list2, B.counter + 1, count, 1);
-      finish(1, list2, B.counter + 1, count, 1);
-    }
-    pack(list2, B.counter + 1, count, 1);
-  };
-  if (dloop && speculated) {
-    if (!dloop->exec) {
+   * The loop's graph (QuantLoop), captured here for this launch's shape when the caller has none.  Its body is one
+   * re-validation pass over the frames verify() listed, as many as counter[0] says on the device (grids sized for all F). */
+  if (speculated) {
+    if (!loop.exec) {
       cudaGraph_t g = nullptr;
       cudaGraphConditionalHandle cond;
-      cudaGraphNode_t reset, loop;
+      cudaGraphNode_t reset, node;
       cudaMemsetParams mp = {};
-      mp.dst = dloop->st + 2; mp.value = 2; mp.elementSize = sizeof(int); mp.width = 1; mp.height = 1;
+      mp.dst = loop.st + 2; mp.value = 2; mp.elementSize = sizeof(int); mp.width = 1; mp.height = 1;
       cudaGraphNodeParams cp = {};
       cp.type = cudaGraphNodeTypeConditional;
       if (cudaGraphCreate(&g, 0) != cudaSuccess) return -100;
       bool ok = cudaGraphConditionalHandleCreate(&cond, g, 1, cudaGraphCondAssignDefault) == cudaSuccess &&
                 cudaGraphAddMemsetNode(&reset, g, nullptr, 0, &mp) == cudaSuccess;
       cp.conditional.handle = cond; cp.conditional.type = cudaGraphCondTypeWhile; cp.conditional.size = 1;
-      ok = ok && cudaGraphAddNode(&loop, g, &reset, 1, &cp) == cudaSuccess;
+      ok = ok && cudaGraphAddNode(&node, g, &reset, 1, &cp) == cudaSuccess;
       cudaGraph_t body = ok ? cp.conditional.phGraph_out[0] : nullptr;
-      if (ok && cudaStreamBeginCaptureToGraph(dloop->capture, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
+      if (ok && cudaStreamBeginCaptureToGraph(loop.capture, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
         std::atomic<long long> captured{0};        /* launches are counted when the graph runs, not when it is captured */
         std::atomic<long long>* const counted = launches;
         launches = &captured;
-        st = dloop->capture;
+        st = loop.capture;
         next_counter = Q_NCOUNTERS;                /* the body zeroes its own task counters */
         verify();
-        k_qstate_loop_cond<<<1, 1, 0, st>>>(cond, B.counter, dloop->st, max_frames + 3);
-        revalidate(B.counter, F);
+        k_qstate_loop_cond<<<1, 1, 0, st>>>(cond, B.counter, loop.st, max_frames + 3);
+        search(0, list1, B.counter, F, 1);
+        outer(0, list2, B.counter + 1, F, 1);
+        finish(0, list2, B.counter + 1, F, 1);
+        if (G == 2) {
+          search(1, list2, B.counter + 1, F, 1);
+          outer(1, list2, B.counter + 1, F, 1);
+          finish(1, list2, B.counter + 1, F, 1);
+        }
+        pack(list2, B.counter + 1, F, 1);
         st = st_main;
         launches = counted;
         cudaGraph_t captured_body = nullptr;
-        ok = cudaStreamEndCapture(dloop->capture, &captured_body) == cudaSuccess && captured_body == body &&
-             cudaGraphInstantiate(&dloop->exec, g, 0) == cudaSuccess;
+        ok = cudaStreamEndCapture(loop.capture, &captured_body) == cudaSuccess && captured_body == body &&
+             cudaGraphInstantiate(&loop.exec, g, 0) == cudaSuccess;
       } else {
         ok = false;
       }
       cudaGraphDestroy(g);
-      if (!ok) { dloop->exec = nullptr; return -100; }
+      if (!ok) { loop.exec = nullptr; return -100; }
     }
-    if (cudaGraphLaunch(dloop->exec, st) != cudaSuccess) return -100;
+    if (cudaGraphLaunch(loop.exec, st) != cudaSuccess) return -100;
     (*launches)++;
-  }
-  for (; speculated && !dloop;) {
-    verify();
-    int h_count = 0;
-    if (cudaMemcpyAsync(&h_count, B.counter, sizeof(int), cudaMemcpyDeviceToHost, st) != cudaSuccess) return -100;
-    if (cudaStreamSynchronize(st) != cudaSuccess) return -100;
-    if (h_count == 0) break;
-    revalidate(nullptr, h_count);
-    passes++;
-    if (passes > max_frames + 3) return -100;   /* cannot happen: each pass fixes at least the first dirty frame */
   }
   k_qstate_commit<<<(S + 63) / 64, 64, 0, st>>>(d_streams, S, B.qs);
   (*launches)++;
-  *passes_out = passes;
   return 0;
 }
 

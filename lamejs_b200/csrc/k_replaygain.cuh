@@ -37,7 +37,7 @@
 #define RG_GUESS 0                      /* 0: a chunk starts from the zero state; 1: from a deliberately wrong state (tests) */
 #endif
 #ifndef RG_QUEUED_PASSES
-#define RG_QUEUED_PASSES 4              /* repair passes queued without waiting for the host (more run if needed; speed only) */
+#define RG_QUEUED_PASSES 4              /* repair passes queued ahead of the loop graph (more run if needed; speed only) */
 #endif
 #define RG_THREADS 64
 #define RG_HIST 12000
@@ -296,7 +296,7 @@ __device__ __forceinline__ void rg_check_pass(const RgParams& p, int pass, long 
 __global__ void __launch_bounds__(RG_THREADS) k_rg_repair(RgParams p, int pass) { rg_repair_pass<false>(p, pass, nullptr); }
 __global__ void k_rg_check(RgParams p, int pass, long long rows) { rg_check_pass(p, pass, rows); }
 
-/* ---- the repair loop on the device (an encode session's tagged calls: no host round trip per pass) ----
+/* ---- the repair loop on the device (rg_finish: no host round trip per pass) ----
  * A CUDA graph whose conditional WHILE node has one pass as its body: k_rg_repair_at and k_rg_check_at, which are k_rg_repair
  * and k_rg_check taking the pass index from device memory, then k_rg_loop_cond.  loop[0] is that index (the host sets it to
  * RG_QUEUED_PASSES, the passes queued ahead of the graph); k_rg_report leaves the counts of the call in loop[1 .. 2]. */
@@ -304,8 +304,8 @@ __global__ void __launch_bounds__(RG_THREADS) k_rg_repair_at(RgParams p, const i
 __global__ void k_rg_check_at(RgParams p, const int* __restrict__ loop, long long rows) { rg_check_pass(p, loop[0], rows); }
 
 /* one thread, after each pass of the body: counts it and lets the body run again unless a pass has changed nothing.  With
- * max_passes run and still no such pass (the bound of the host loop, rg_finish, which cannot be reached) it ends the loop
- * with *fault = RG_FAULT. */
+ * max_passes run and still no such pass (a bound that cannot be reached: each pass settles at least one more chunk) it
+ * ends the loop with *fault = RG_FAULT. */
 #define RG_FAULT 2
 __global__ void k_rg_loop_cond(cudaGraphConditionalHandle handle, int* __restrict__ loop, int* __restrict__ done, int max_passes,
                                int* __restrict__ fault) {
@@ -316,7 +316,7 @@ __global__ void k_rg_loop_cond(cudaGraphConditionalHandle handle, int* __restric
   cudaGraphSetConditional(handle, more ? 1u : 0u);
 }
 
-/* one thread, after the loop: loop[1] = the passes the analysis needed, counted like rg_finish counts them -- up to and
+/* one thread, after the loop: loop[1] = the passes the analysis needed -- up to and
  * including the first of the loop[0] passes run that changed nothing (later ones returned at once); loop[2] = chunks run again */
 __global__ void k_rg_report(int* __restrict__ loop, const int* __restrict__ pass_changed, const int* __restrict__ reruns) {
   int used = 0;

@@ -214,6 +214,15 @@ template <class T, bool Pinned = false> struct Buf {
 };
 
 /* ------------------------------------------------------------------------------------------------ */
+/* The status words of a call (Workspace::refusals): [0] a Float32 sample was refused (k_stage_f32), [1] frames over their
+ * bit budget (k_q_pack), [2] the call's largest quantizer pass count, [3] a fixed-point loop hit its bound -- the four
+ * status words, which a session's call copies to the caller's d_status -- [4] the pass count of the current launch group
+ * (k_qstate_loop_cond), [5] the pass index of the ReplayGain repair loop (k_rg_loop_cond), and [6 .. 10) the four further
+ * status words of a tagged call: the analysis's passes and reruns (k_rg_report) and two zeros.  A handle call uses [6] and
+ * [7] itself (k_handle_commit), so the repair loop of a tagged handle call keeps its pass index, passes and reruns in
+ * [10 .. 13). */
+enum { MP3_SESSION_WORDS = 13, MP3_STATUS_WORDS = 4, MP3_TAGGED_WORDS_AT = 6, MP3_HANDLE_RG_WORDS_AT = 10 };
+
 /* Per-launch device workspace (U granule rows, F frame rows, S streams of nch channels).                */
 struct Workspace {
   Buf<StreamDesc> streams;
@@ -243,8 +252,7 @@ struct Workspace {
   Buf<float> rs_y;                        /* resampled batches: the resampler's output rows, the PCM the pipeline reads */
   Buf<StageDesc> st_desc;                 /* Float32 input: [S] */
   Buf<float> st_y;                        /* Float32 input: the staged (scaled) rows */
-  Buf<int> refusals;                      /* [2]: [0] set by k_stage_f32 when a Float32 sample is refused (non-finite or beyond
-                                             MP3_F32_MAX_SAMPLE), [1] frames whose bits do not fit their slot (k_q_pack) */
+  Buf<int> refusals;                      /* [MP3_SESSION_WORDS]: the call's status words (reset_words) */
   int fit(int S, int nch, long long U, long long F) {
     const size_t gc = (size_t)U * nch, rows = (size_t)(U + S) * nch, f = (size_t)F + 1;
     const bool failed = streams.fit(S) || bt_final.fit((size_t)U * 2 + 16) || bt_prev.fit((size_t)U * 2 + 16) ||
@@ -280,6 +288,57 @@ struct PinnedArena { uint8_t* p = nullptr; size_t cap = 0, used = 0; };
  * An encode session (mp3b200_session) holds one too, bound to the caller's stream instead (session = true): its launches
  * are ordered by that stream alone, with no wait for the legacy default stream, and upload their descriptors from `arena`. */
 enum { MP3_MAX_PCM_CHUNKS = 8 };
+/* The graphs of a context's device loops: the quantizer's fixed-point loop (QuantLoop), one per launch shape (configuration,
+ * streams, frames, longest stream's frames), and the ReplayGain repair loop (rg_finish), one per (configuration, Float32
+ * rows, titles, longest title's chunks, chunk rows, loop words) -- what RgParams and the launch grids are made of.  They
+ * hold the buffers' addresses, so the quantizer's are all dropped when the workspace's generation changes and the
+ * ReplayGain ones when the context's rg_generation does.  A context sees arbitrary shapes: at most MP3_LOOP_GRAPHS graphs
+ * are kept, the least recently used going first. */
+enum { MP3_LOOP_GRAPHS = 32 };
+struct LoopGraphs {
+  /* (configuration, 0 for the quantizer or 1 + Float32 for the ReplayGain loop, then the shape), and the loop words */
+  using Key = std::tuple<const Config*, int, long long, long long, long long, const int*>;
+  struct Graph { cudaGraphExec_t exec = nullptr; unsigned long long used = 0; };
+  cudaStream_t capture = nullptr;        /* only captured on */
+  size_t generation = 0, rg_generation = 0;
+  long long instantiated = 0;            /* graphs instantiated over the context's life (mp3b200_session_graph_instantiations) */
+  unsigned long long tick = 0;
+  std::map<Key, Graph> graphs;
+  /* the cached graph of `key`, or null */
+  cudaGraphExec_t find(const Key& key) {
+    const auto e = graphs.find(key);
+    if (e == graphs.end()) return nullptr;
+    e->second.used = ++tick;
+    return e->second.exec;
+  }
+  /* keeps the graph just instantiated for `key` */
+  void put(const Key& key, cudaGraphExec_t exec) {
+    if (graphs.size() >= MP3_LOOP_GRAPHS) {
+      auto lru = graphs.begin();
+      for (auto e = graphs.begin(); e != graphs.end(); ++e) if (e->second.used < lru->second.used) lru = e;
+      cudaGraphExecDestroy(lru->second.exec);
+      graphs.erase(lru);
+    }
+    graphs[key] = {exec, ++tick};
+    instantiated++;
+  }
+  /* drops the graphs of one kind when the generation of the buffers they hold has changed */
+  void renew(bool rg, size_t now) {
+    size_t& gen = rg ? rg_generation : generation;
+    if (gen == now) return;
+    gen = now;
+    for (auto e = graphs.begin(); e != graphs.end();) {
+      if ((std::get<1>(e->first) != 0) != rg) { ++e; continue; }
+      cudaGraphExecDestroy(e->second.exec);
+      e = graphs.erase(e);
+    }
+  }
+  void release() {
+    for (auto& e : graphs) cudaGraphExecDestroy(e.second.exec);
+    graphs.clear();
+    if (capture) { cudaStreamDestroy(capture); capture = nullptr; }
+  }
+};
 /* The stream index is a grid y / z coordinate of several kernels (CUDA limit 65535): larger batches run in groups */
 enum { MP3_MAX_LAUNCH_STREAMS = 65535 };
 struct ThreadCtx {
@@ -290,6 +349,7 @@ struct ThreadCtx {
   cudaEvent_t ev[8] = {}, evq[QE_COUNT] = {}, ev_in = nullptr, ev_fork = nullptr, ev_join = nullptr, ready[MP3_MAX_PCM_CHUNKS] = {};
   cudaEvent_t ev_rs[2] = {};              /* around k_resample */
   Workspace ws;
+  LoopGraphs loops;
   int evq_pred[QE_COUNT] = {};
   Buf<uint8_t> pcm;                       /* staged PCM of host callers (Int16 or Float32 rows) */
   Buf<uint8_t> out;                       /* encoded bytes of host callers */
@@ -318,6 +378,7 @@ struct ThreadCtx {
   void release() {
     if (device < 0) return;
     cudaSetDevice(device);
+    loops.release();
     ws.release(); pcm.release(); out.release(); pin.release(); crc_ranges.release(); crc.release(); tags.release();
     hdesc.release(); rg_stage.release(); hrows.release(); halo_scratch.release(); hpin.release();
     rg_titles.release(); rg_piece.release(); rg_sum.release(); rg_gain.release(); rg_wstate.release(); rg_cstart.release();
@@ -355,6 +416,7 @@ struct ThreadCtx {
   int create(int dev) {
     CK(cudaStreamCreateWithFlags(&up_st, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&rg_st, cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(&loops.capture, cudaStreamNonBlocking));
     for (auto& e : ev_rg) CK(cudaEventCreate(&e));
     for (auto& e : ev) CK(cudaEventCreate(&e));
     for (auto& e : evq) CK(cudaEventCreate(&e));
@@ -421,15 +483,15 @@ bool debug_sync() { static int v = -1; if (v < 0) { const char* e = getenv("MP3B
     }                                                                                       \
   } while (0)
 
-struct Timings { float psy = 0, scan = 0, mask = 0, fb = 0, q1 = 0, qn = 0, total = 0; int passes = 0;
+struct Timings { float psy = 0, scan = 0, mask = 0, fb = 0, q1 = 0, qn = 0, total = 0;
                  float q_prepare = 0, q_search = 0, q_outer = 0, q_finish = 0, q_pack = 0, q_mid = 0; };
 
 /* chunks > 1: the caller uploads each stream's PCM in that many time slices on another stream and records ready[j] after
  * slice j; the psy analysis of slice j starts as soon as it has landed. */
 struct PcmArrival { int chunks = 1; cudaEvent_t* ready = nullptr; };
 
-/* The error of a launch whose ws.refusals read refused / over_budget (and, for an asynchronous call, fault: its device
- * fixed-point loop hit the bound), with g_err set; 0 when the output stands. */
+/* The error of a call whose status words read refused / over_budget / fault (a device loop hit its bound), with g_err
+ * set; 0 when the output stands. */
 int refusal_error(int refused, int over_budget, int fault) {
   if (refused) { g_err = "non-finite input sample (or one beyond 2^40 once scaled)"; return MP3B200_ERR_CONFIG; }
   if (over_budget) { g_err = "frame over its bit budget (input too loud to encode)"; return MP3B200_ERR_CONFIG; }
@@ -438,14 +500,14 @@ int refusal_error(int refused, int over_budget, int fault) {
   return 0;
 }
 
-/* After a launch has drained, one read-back of ws.refusals: MP3B200_ERR_CONFIG when k_stage_f32 refused a Float32 sample,
- * or when a frame's bits did not fit its slot (k_q_pack left it unpacked), where lamejs throws out of the call
- * (BitStream.js:856-885).  The call's output must not be used. */
+/* Once the call's work has joined c.st, one read-back of the status words: MP3B200_ERR_CONFIG when k_stage_f32 refused a
+ * Float32 sample, or when a frame's bits did not fit its slot (k_q_pack left it unpacked), where lamejs throws out of the
+ * call (BitStream.js:856-885); MP3B200_ERR_CUDA when a device loop hit its bound.  The call's output must not be used. */
 int check_refusals(ThreadCtx& c) {
-  int r[2] = {0, 0};
+  int r[MP3_STATUS_WORDS] = {};
   CK(cudaMemcpyAsync(r, c.ws.refusals.p, sizeof r, cudaMemcpyDeviceToHost, c.st));
   CK(cudaStreamSynchronize(c.st));
-  return refusal_error(r[0], r[1], 0);
+  return refusal_error(r[0], r[1], r[3]);
 }
 
 /* Options of launch_streams */
@@ -459,36 +521,15 @@ struct LaunchOpts {
   struct RgJob* rg = nullptr;            /* ReplayGain of every stream, beside the encoder (one launch group only) */
   bool f32_in = false;                   /* the descriptors point at the caller's Float32 rows (k_stage_f32 stages them); with
                                             sync, a non-finite sample makes the launch return MP3B200_ERR_CONFIG */
-  struct LoopGraphs* loops = nullptr;    /* run the quantizer's fixed-point loop on the device, as the cached graphs of a session
-                                            (no host round trip; needs !sync) */
   const struct HandleCarry* carry = nullptr;   /* streaming handles: their carried state is on the device (k_handle_carry_in;
                                                   one launch group only) */
-  int* rg_loop = nullptr;                /* a session's three words of the ReplayGain loop (rg_finish_queued); NULL: ws.refusals + 5 */
+  int* rg_loop = nullptr;                /* the three words of the ReplayGain loop (rg_finish) of a handle call; NULL: ws.refusals + 5 */
   bool analyse_only = false;             /* stop after staging, resampling and the ReplayGain analysis of o.rg: no encoder
                                             kernels, no bytes, no workspace beyond the staged rows */
 };
 
 /* LaunchOpts::carry: recs[z] is the record of stream z (device array); halo_scratch takes the masking of refused handles */
 struct HandleCarry { HandleRecord* const* recs; float* halo_scratch; };
-
-/* The quantizer's fixed-point loop graphs of a session (QuantLoop), one per launch shape: (configuration, streams, frames,
- * longest stream's frames).  They hold the workspace's addresses, so they are all dropped when its generation changes.
- * The graphs of the ReplayGain repair loop (rg_finish_queued) are kept the same way: one per (configuration, Float32 rows,
- * titles, longest title's chunks, chunk rows, loop words) -- what RgParams and the launch grids are made of -- dropped when
- * the context's rg_generation changes.  Streaming handles vary those shapes far more than whole streams do, so at most
- * MP3_RG_GRAPHS of them are kept, the least recently used going first. */
-enum { MP3_RG_GRAPHS = 32 };
-struct LoopGraphs {
-  cudaStream_t capture = nullptr;
-  size_t generation = 0, rg_generation = 0;
-  long long instantiated = 0;            /* graphs instantiated over the session's life (mp3b200_session_graph_instantiations) */
-  unsigned long long rg_tick = 0;
-  std::map<std::tuple<const Config*, int, long long, int>, cudaGraphExec_t> exec;
-  struct RgGraph { cudaGraphExec_t exec = nullptr; unsigned long long used = 0; };
-  std::map<std::tuple<const Config*, bool, int, int, long long, const int*>, RgGraph> rg_exec;
-  void clear_rg() { for (auto& e : rg_exec) cudaGraphExecDestroy(e.second.exec); rg_exec.clear(); }
-  void clear() { for (auto& e : exec) cudaGraphExecDestroy(e.second); exec.clear(); }
-};
 
 /* Queues the copy of n bytes of host descriptors to dst on `on` (NULL: c.st).  A session's call stages them in its pinned
  * slot first, so the copy never waits for the device; a thread's context copies from `src` (pageable) as it is. */
@@ -503,6 +544,16 @@ int upload(ThreadCtx& c, void* dst, const void* src, size_t n, cudaStream_t on =
   }
   CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, on ? on : c.st));
   return 0;
+}
+
+/* Resets the status words (ws.refusals) for a call of `nstreams` streams on c.st: [0 .. 2) zero, then the start words --
+ * [2] is the pass count of launch groups that speculate nothing -- and zeros */
+int reset_words(ThreadCtx& c, int nstreams) {
+  int rc = c.ws.refusals.fit(MP3_SESSION_WORDS);
+  if (rc) return rc;
+  CK(cudaMemsetAsync(c.ws.refusals.p, 0, 2 * sizeof(int), c.st));
+  const int start[MP3_SESSION_WORDS - 2] = {nstreams > 0 ? 2 : 0};
+  return upload(c, c.ws.refusals.p + 2, start, sizeof start);
 }
 
 /* Makes c.st wait for the work the caller queued on the legacy default stream (torch and plain CUDA callers produce their
@@ -796,27 +847,20 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, const 
     if (psy_launch >= 0 && (rc = psy_record_front(c, h_streams, S, nch, cfg->host.mode_gr, psy_launch))) return rc;
   }
   CK(cudaEventRecord(ev[4], st));
-  int passes = 0;
   if (!o.stop_after_mdct) {
     QuantBuffers qb;
     qb.xr = ws.xr.p; qb.ratio = ws.ratio.p; qb.bt = ws.bt_final.p; qb.ath_q = ws.ath_q.p; qb.qs = ws.qstate.p; qb.ginfo = ws.ginfo.p;
     qb.l3enc = ws.l3enc.p; qb.xrq = ws.xrq.p; qb.xrpow = ws.xrpow.p; qb.neg = ws.neg.p; qb.prep = ws.prep.p; qb.list = ws.dirty.p; qb.counter = ws.counter.p;
     qb.over_budget = ws.refusals.p + 1;
-    QuantLoop dloop;
-    cudaGraphExec_t* cached = nullptr;
-    if (o.loops) {                         /* the session's graph for this shape, captured by quant_run if there is none */
-      LoopGraphs& lg = *o.loops;
-      if (lg.generation != ws.generation()) { lg.clear(); lg.generation = ws.generation(); }
-      cached = &lg.exec[std::make_tuple((const Config*)cfg, S, total_frames, max_frames)];
-      dloop.capture = lg.capture; dloop.st = ws.refusals.p + 2; dloop.exec = *cached;
-    }
-    rc = quant_run(tab, cfg->host, ws.streams.p, S, streams_with_frames, max_frames, total_frames, qb, st, c.aux_st, c.ev_fork, c.ev_join, ev[5], c.evq, c.evq_pred, &passes, &g_launches,
-                   o.loops ? &dloop : nullptr);
-    if (cached) {
-      if (!*cached && dloop.exec) o.loops->instantiated++;
-      *cached = dloop.exec;
-      if (!dloop.exec) o.loops->exec.erase(std::make_tuple((const Config*)cfg, S, total_frames, max_frames));
-    }
+    LoopGraphs& lg = c.loops;              /* the graph for this shape, captured by quant_run if there is none */
+    lg.renew(false, ws.generation());
+    const LoopGraphs::Key key = {cfg, 0, S, total_frames, max_frames, nullptr};
+    QuantLoop loop;
+    loop.capture = lg.capture; loop.st = ws.refusals.p + 2; loop.exec = lg.find(key);
+    const bool cached = loop.exec != nullptr;
+    rc = quant_run(tab, cfg->host, ws.streams.p, S, streams_with_frames, max_frames, total_frames, qb, st, c.aux_st, c.ev_fork, c.ev_join,
+                   ev[5], c.evq, c.evq_pred, &g_launches, loop);
+    if (!cached && loop.exec) lg.put(key, loop.exec);
     if (rc) { g_err = "quantizer stage failed: " + std::string(cudaGetErrorString(cudaGetLastError())); return rc; }
   } else {
     CK(cudaEventRecord(ev[5], st));
@@ -833,8 +877,7 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, const 
     cudaEventElapsedTime(&tm->q1, ev[4], ev[5]);
     cudaEventElapsedTime(&tm->qn, ev[5], ev[6]);
     cudaEventElapsedTime(&tm->total, ev[0], ev[6]);
-    tm->passes = passes;
-    if (!o.stop_after_mdct && passes > 0) {
+    if (!o.stop_after_mdct) {
       auto span = [&](int slot) { float v = 0; const int p = c.evq_pred[slot]; if (p >= 0) cudaEventElapsedTime(&v, c.evq[p], c.evq[slot]); return v; };
       tm->q_prepare = span(QE_PREP);
       tm->q_search = span(QE_S0) + span(QE_S1);
@@ -1091,26 +1134,20 @@ int rg_queue_results(ThreadCtx& c, RgJob& job) {
   return 0;
 }
 
-/* rg_finish for a session, which must not wait for the device: the repair loop runs as a graph on c.rg_st (k_rg_loop_cond),
- * kept in `lg` per shape and captured here when there is none; then the same results and carries.  `loop` is three words
- * of device memory: the pass index, and what k_rg_report leaves there (RgJob::passes and reruns of rg_finish); *fault is
- * set to RG_FAULT if the loop hits rg_finish's bound.  Nothing is read back. */
-int rg_finish_queued(ThreadCtx& c, Config* cfg, RgJob& job, LoopGraphs& lg, int* loop, int* fault) {
+/* After the encoder has been queued: the repair loop runs as a graph on c.rg_st (k_rg_loop_cond), kept in c.loops per
+ * shape and captured here when there is none; then the histograms, the gains of the titles that end (c.rg_gain) and the
+ * carries.  `loop` is three words of device memory: the pass index, and what k_rg_report leaves there (the passes the
+ * analysis needed and the chunks it ran again); *fault is set to RG_FAULT if the loop hits its bound.  Nothing is read
+ * back (rg_read). */
+int rg_finish(ThreadCtx& c, Config* cfg, RgJob& job, int* loop, int* fault) {
   cudaStream_t st = c.rg_st;
   RgParams& p = job.prm;
   const int nch = cfg->host.nch, T = (int)job.specs.size();
   if (job.max_chunks > 0) {
-    if (lg.rg_generation != c.rg_generation()) { lg.clear_rg(); lg.rg_generation = c.rg_generation(); }
-    const auto key = std::make_tuple((const Config*)cfg, p.f32 != 0, T, job.max_chunks, job.chunk_rows, (const int*)loop);
-    if (!lg.rg_exec.count(key) && lg.rg_exec.size() >= MP3_RG_GRAPHS) {
-      auto lru = lg.rg_exec.begin();
-      for (auto e = lg.rg_exec.begin(); e != lg.rg_exec.end(); ++e) if (e->second.used < lru->second.used) lru = e;
-      cudaGraphExecDestroy(lru->second.exec);
-      lg.rg_exec.erase(lru);
-    }
-    LoopGraphs::RgGraph& slot = lg.rg_exec[key];
-    slot.used = ++lg.rg_tick;
-    cudaGraphExec_t& exec = slot.exec;
+    LoopGraphs& lg = c.loops;
+    lg.renew(true, c.rg_generation());
+    const LoopGraphs::Key key = {cfg, 1 + (p.f32 != 0), T, job.max_chunks, job.chunk_rows, loop};
+    cudaGraphExec_t exec = lg.find(key);
     if (!exec) {
       cudaGraph_t g = nullptr;
       cudaGraphConditionalHandle cond;
@@ -1135,12 +1172,10 @@ int rg_finish_queued(ThreadCtx& c, Config* cfg, RgJob& job, LoopGraphs& lg, int*
       }
       if (g) cudaGraphDestroy(g);
       if (!ok) {
-        exec = nullptr;
-        lg.rg_exec.erase(key);
         g_err = "ReplayGain loop graph failed: " + std::string(cudaGetErrorString(cudaGetLastError()));
         return MP3B200_ERR_CUDA;
       }
-      lg.instantiated++;
+      lg.put(key, exec);
     }
     const int first = RG_QUEUED_PASSES;              /* the pass index the graph starts at */
     int rc = upload(c, loop, &first, sizeof first, st);
@@ -1157,61 +1192,31 @@ int rg_finish_queued(ThreadCtx& c, Config* cfg, RgJob& job, LoopGraphs& lg, int*
   return 0;
 }
 
-/* after the encoder has been queued: runs repair passes until one changes nothing, then the histograms, the gains of the
- * titles that end and the carries; reads the results.  Returns with c.rg_st drained. */
-int rg_finish(ThreadCtx& c, Config* cfg, RgJob& job) {
-  cudaStream_t st = c.rg_st;
-  RgParams& p = job.prm;
-  const int nch = cfg->host.nch, T = (int)job.specs.size();
-  int rc = 0;
-  if (job.max_chunks > 0) {
-    dim3 grid((unsigned)((job.max_chunks * nch + RG_THREADS - 1) / RG_THREADS), (unsigned)T);
-    for (;;) {
-      int done = 0;
-      CK(cudaMemcpyAsync(&done, p.done, sizeof(int), cudaMemcpyDeviceToHost, st));
-      CK(cudaStreamSynchronize(st));
-      if (done) break;
-      if (job.passes >= job.max_chunks + RG_QUEUED_PASSES + 1) { g_err = "ReplayGain repair did not converge"; return MP3B200_ERR_CUDA; }
-      k_rg_repair<<<grid, RG_THREADS, 0, st>>>(p, job.passes);
-      k_rg_check<<<(unsigned)((job.chunk_rows + 255) / 256), 256, 0, st>>>(p, job.passes, job.chunk_rows);
-      job.passes++;
-      g_launches += 2;
-    }
-    CK(cudaMemcpyAsync(&job.reruns, p.reruns, sizeof(int), cudaMemcpyDeviceToHost, st));
-    /* the pass that found nothing to change: the first with pass_changed == 0 (later queued ones returned at once) */
-    std::vector<int> pc((size_t)job.passes);
-    CK(cudaMemcpyAsync(pc.data(), p.pass_changed, sizeof(int) * (size_t)job.passes, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    int used = 0;
-    while (used < job.passes && pc[used] != 0) used++;
-    job.passes = used + 1;
-  }
-  rc = rg_queue_results(c, job);
-  if (rc) return rc;
-  std::vector<int> hist0;
-  if (job.want_windows && T > 0) {
-    job.hist0.assign(RG_HIST, 0);
-    RgTitle t0;
-    CK(cudaMemcpyAsync(&t0, p.titles, sizeof t0, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    CK(cudaMemcpyAsync(job.hist0.data(), t0.hist, sizeof(int) * RG_HIST, cudaMemcpyDeviceToHost, st));
-  }
-  k_rg_finish<<<T, 256, 0, st>>>(p.titles, p.end_in, nch);
-  g_launches++;
-  CK(cudaEventRecord(c.ev_rg[2], st));
+/* A synchronous call's results of the analysis, once rg_finish's work has drained: the gains, the passes and reruns from
+ * the loop words `loop`, the analysis's time and (want_windows) spec 0's windows and histogram A. */
+int rg_read(ThreadCtx& c, RgJob& job, const int* loop) {
+  const int T = (int)job.specs.size();
+  auto fetch = [&](void* dst, const void* src, size_t bytes) { return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c.st); };
   std::vector<double> g((size_t)T + 1);
-  CK(cudaMemcpyAsync(g.data(), c.rg_gain.p, sizeof(double) * (size_t)(T + 1), cudaMemcpyDeviceToHost, st));
-  if (job.want_windows) {
+  int counts[2] = {0, 0};
+  CK(fetch(g.data(), c.rg_gain.p, sizeof(double) * (size_t)(T + 1)));
+  if (job.max_chunks > 0) CK(fetch(counts, loop + 1, sizeof counts));
+  if (job.want_windows) {                          /* a whole stream's A is the workspace's (RgSpec::hist NULL) */
     job.win_sum.assign((size_t)job.nwin0 * 2, 0.0);
     job.win_idx.assign((size_t)job.nwin0, 0);
     if (job.nwin0 > 0) {
-      CK(cudaMemcpyAsync(job.win_sum.data(), c.rg_sum.p, sizeof(double) * 2 * (size_t)job.nwin0, cudaMemcpyDeviceToHost, st));
-      CK(cudaMemcpyAsync(job.win_idx.data(), c.rg_idx.p, sizeof(int) * (size_t)job.nwin0, cudaMemcpyDeviceToHost, st));
+      CK(fetch(job.win_sum.data(), c.rg_sum.p, sizeof(double) * 2 * (size_t)job.nwin0));
+      CK(fetch(job.win_idx.data(), c.rg_idx.p, sizeof(int) * (size_t)job.nwin0));
+    }
+    if (T > 0) {
+      job.hist0.assign(RG_HIST, 0);
+      CK(fetch(job.hist0.data(), c.rg_hist.p, sizeof(int) * RG_HIST));
     }
   }
-  CK(cudaStreamSynchronize(st));
-  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(c.st));
   CK(cudaEventElapsedTime(&job.ms, c.ev_rg[1], c.ev_rg[2]));
+  job.passes = counts[0];
+  job.reruns = counts[1];
   job.title_db.assign((size_t)T, (double)RG_NOT_ENOUGH_SAMPLES);
   for (int i = 0; i < T; i++) if (job.specs[i].title_end) job.title_db[i] = g[i];
   job.album_db = g[T];
@@ -1222,7 +1227,8 @@ int rg_finish(ThreadCtx& c, Config* cfg, RgJob& job) {
  * device address of its bytes) and carried state; this assigns unit_base / frame_base, grows the context's workspace and runs the pipeline.
  * The stream index is a grid y / z coordinate of several kernels (CUDA limit 65535): a larger batch runs as consecutive
  * launches of at most MP3_MAX_LAUNCH_STREAMS streams on the context's stream, the later ones behind every PCM upload.
- * Timings add up over the launches; the pass count is the largest any of them needed.
+ * Timings add up over the launches; the pass count (ws.refusals[2]) is the largest any of them needed.  The caller has
+ * reset the status words (reset_words); with o.sync the call returns with its work drained and the words checked.
  * With resampling (cfg->rs.ratio > 1) the descriptors hold the caller's input as resample_streams describes; each launch
  * first resamples it (timing slot 14). */
 int launch_streams(ThreadCtx& c, Config* cfg, std::vector<StreamDesc>& sds, const LaunchOpts& o) {
@@ -1230,11 +1236,6 @@ int launch_streams(ThreadCtx& c, Config* cfg, std::vector<StreamDesc>& sds, cons
   const PcmArrival* arrival = o.arrival;
   const int nstreams = (int)sds.size();
   if (o.rg && nstreams > MP3_MAX_LAUNCH_STREAMS) { g_err = "ReplayGain batches hold at most 65535 streams"; return MP3B200_ERR_HANDLE; }
-  {
-    int rc = c.ws.refusals.fit(2);
-    if (rc) return rc;
-    CK(cudaMemsetAsync(c.ws.refusals.p, 0, 2 * sizeof(int), c.st));
-  }
   /* Before anything reads the descriptors' rows: the caller's device rows may come from the legacy default stream, and
    * rg_queue forks the analysis stream from c.st ahead of run_pipeline's own wait (Int16 rows that are neither staged
    * nor resampled are read by k_rg_pass1 where the caller left them). */
@@ -1277,10 +1278,12 @@ int launch_streams(ThreadCtx& c, Config* cfg, std::vector<StreamDesc>& sds, cons
     Timings tm;
     rc = o.analyse_only ? 0 : run_pipeline(c, cfg, group, n, o, arrival, rows, &tm);
     if (rc) return rc;
-    if (o.rg) {                                /* a session: ws.refusals[3] is its fault word, [5 .. 8) the loop's words */
-      rc = o.loops ? rg_finish_queued(c, cfg, *o.rg, *o.loops, o.rg_loop ? o.rg_loop : c.ws.refusals.p + 5, c.ws.refusals.p + 3)
-                   : rg_finish(c, cfg, *o.rg);
+    if (o.rg) {                                /* ws.refusals[3] is the fault word, [5 .. 8) the loop's words */
+      rc = rg_finish(c, cfg, *o.rg, o.rg_loop ? o.rg_loop : c.ws.refusals.p + 5, c.ws.refusals.p + 3);
       if (rc) return rc;
+      /* the analysis joins the call before anything reads what it wrote */
+      CK(cudaEventRecord(c.ev_rg[2], c.rg_st));
+      CK(cudaStreamWaitEvent(c.st, c.ev_rg[2], 0));
     }
     arrival = nullptr;
     float rs_ms = 0.0f;
@@ -1289,8 +1292,13 @@ int launch_streams(ThreadCtx& c, Config* cfg, std::vector<StreamDesc>& sds, cons
       const float t[16] = {tm.psy, tm.scan, tm.mask, tm.fb, tm.q1, tm.qn, tm.total, 0.0f,
                            tm.q_prepare, tm.q_search, tm.q_outer, tm.q_finish, tm.q_pack, tm.q_mid, rs_ms, 0.0f};
       for (int i = 0; i < 16; i++) o.timings_ms[i] += t[i];
-      if ((float)tm.passes > o.timings_ms[7]) o.timings_ms[7] = (float)tm.passes;
     }
+  }
+  if (o.timings_ms && o.sync && !o.stop_after_mdct && !o.analyse_only) {
+    int passes = 0;
+    CK(cudaMemcpyAsync(&passes, c.ws.refusals.p + 2, sizeof passes, cudaMemcpyDeviceToHost, c.st));
+    CK(cudaStreamSynchronize(c.st));
+    o.timings_ms[7] = (float)passes;
   }
   return o.sync && (o.f32_in || !o.stop_after_mdct) ? check_refusals(c) : 0;
 }
@@ -1652,8 +1660,8 @@ int upload_host_rows(const Config* cfg, int nstreams, const T* const* left, cons
 }
 
 /* The body of every whole-stream call, on context c once it is planned (pl): stages host rows (upload_host_rows), describes
- * the streams (whole_streams), encodes and / or analyses them (launch_streams; o.arrival, o.rg and o.analyse_only are set
- * here) and writes the tag frames (finish_tagged).  The files lie at k.d_out + k.out_off[s] on the device; k.out_bytes[s]
+ * the streams (whole_streams), resets the status words, encodes and / or analyses them (launch_streams; o.arrival, o.rg and
+ * o.analyse_only are set here) and writes the tag frames (finish_tagged).  The files lie at k.d_out + k.out_off[s] on the device; k.out_bytes[s]
  * (optional) receives each file's length. */
 template <class T>
 int whole_run(ThreadCtx& c, Config* cfg, const WholeCall<T>& k, const StreamPlan& pl, LaunchOpts o) {
@@ -1673,12 +1681,8 @@ int whole_run(ThreadCtx& c, Config* cfg, const WholeCall<T>& k, const StreamPlan
   o.analyse_only = !k.encode;
   /* launch_streams returns with the refusals checked when it synchronises: no tag for a refused call.  The tag step alone
    * waits for the caller's files as a launch waits for its rows. */
-  int rc = k.encode || pl.rg ? launch_streams(c, cfg, sds, o) : wait_legacy(c);
-  if (!rc && pl.rg && !o.sync) {         /* the analysis, still queued on c.rg_st, joins the call before its gains are read */
-    if (cudaEventRecord(c.ev_rg[2], c.rg_st) != cudaSuccess || cudaStreamWaitEvent(c.st, c.ev_rg[2], 0) != cudaSuccess) {
-      g_err = "ReplayGain join failed"; rc = MP3B200_ERR_CUDA;
-    }
-  }
+  int rc = reset_words(c, S);
+  if (!rc) rc = k.encode || pl.rg ? launch_streams(c, cfg, sds, o) : wait_legacy(c);
   if (rc || !k.tagged) return rc;
   const double* gain = pl.rg ? c.rg_gain.p : nullptr;
   if (k.title_in && S > 0) {
@@ -1723,6 +1727,7 @@ int whole_sync(WholeCall<T> k) {
     CK(cudaStreamSynchronize(t_ctx.st));
     CK(cudaGetLastError());
   }
+  if (pl.rg && S > 0 && (rc = rg_read(t_ctx, *pl.rg, t_ctx.ws.refusals.p + 5))) return rc;
   const bool ran = pl.rg && (int)pl.rg->title_db.size() == S && S > 0;
   for (int s = 0; k.title_db && s < S; s++) k.title_db[s] = ran ? pl.rg->title_db[s] : RG_NOT_ENOUGH_SAMPLES;
   if (k.album_db) *k.album_db = ran ? pl.rg->album_db : RG_NOT_ENOUGH_SAMPLES;
@@ -1907,7 +1912,8 @@ int debug_stages(const mp3b200_debug_taps* tp, const T* left, const T* right) {
   opts.all_short = !(tp->flags & MP3B200_DEBUG_SKIP_SHORT);
   opts.stop_after_mdct = !(l3_enc || bytes_out || want_gi || want_prep || want_q);
   opts.arrival = &arr;
-  rc = launch_streams(t_ctx, cfg, sds, opts);
+  rc = reset_words(t_ctx, 1);
+  if (!rc) rc = launch_streams(t_ctx, cfg, sds, opts);
   /* read-back on the thread's stream (the launch has drained it) */
   auto fetch = [](void* dst, const void* src, size_t bytes) {
     const cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, t_ctx.st);
@@ -2016,7 +2022,7 @@ int debug_resample(int channels, int samplerate, int kbps, const T* left, const 
   sd.pcm_end = nsamples;
   Rows rows = {false, cfg->host.scale_applied};
   if (std::is_same_v<T, float>) {                   /* the launch path's staging: Float32(x * scale) rows */
-    rc = t_ctx.ws.refusals.fit(2);
+    rc = t_ctx.ws.refusals.fit(MP3_SESSION_WORDS);
     if (rc) return rc;
     rc = stage_streams(t_ctx, cfg, &sd, 1);
     if (rc) return rc;

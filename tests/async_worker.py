@@ -1,7 +1,8 @@
 """Runs in a subprocess of tests/test_gpu_async.py with MP3B200_LIB naming a library built with bad speculation guesses and
 no folded repair (lamejs_b200.lib() is a process singleton, so one process per library): every wrong guess is repaired by
-the fixed-point loop, which an encode session runs on the device.  Encodes ragged batches through a session, compares
-with the oracle and with encode_streams_device's pass count, and prints one JSON line:
+the fixed-point loop, which runs on the device for every call.  Encodes ragged batches through a session, compares with
+the oracle and with encode_streams_device's pass count and launch count (a graph launch counts once, however many passes
+it runs), and prints one JSON line:
 {"fail": [what differed, ...], "passes": {workload: quantizer passes}}."""
 import json
 import os
@@ -21,6 +22,7 @@ def main():
 
     import lamejs_b200 as M
 
+    launches = M.lib().mp3b200_launch_count
     assert os.path.samefile(M.lib()._name, os.environ["MP3B200_LIB"])
     fail, passes = [], {}
     sess = M.EncodeSession(torch.cuda.Stream())
@@ -38,16 +40,22 @@ def main():
         out_off = np.cumsum([0] + nb)[:-1]
         d_pcm = torch.from_numpy(pcm).cuda()
         ref_out = torch.zeros(sum(nb) + 8, dtype=torch.uint8, device="cuda")
+        n0 = launches()
         tm = M.encode_streams_device(ch, sr, kbps, d_pcm.data_ptr(), pcm_off, ns, ref_out.data_ptr(), out_off, resample=rs)
+        sync_launches = launches() - n0
         sess.stream.wait_stream(torch.cuda.current_stream())
         for rep in range(2):                             # the second call of the shape reuses the captured graph
             with torch.cuda.stream(sess.stream):
                 d_out = torch.zeros(sum(nb) + 8, dtype=torch.uint8, device="cuda")
+            n0 = launches()
             st = sess.encode_streams(ch, sr, kbps, d_pcm, pcm_off, ns, d_out, out_off, resample=rs)
+            n = launches() - n0
+            if n != sync_launches:
+                fail.append("%s#%d: %d launches in the session, %d in the synchronous call" % (tag, rep, n, sync_launches))
             p = M.check_status(st)
             passes["%s#%d" % (tag, rep)] = p
             if p != int(tm[7]):
-                fail.append("%s: %d passes on the device, %d on the host" % (tag, p, int(tm[7])))
+                fail.append("%s: %d passes in the session, %d in the synchronous call" % (tag, p, int(tm[7])))
             out = d_out.cpu().numpy()
             for i, ((l, r), o, b) in enumerate(zip(sigs, out_off, nb)):
                 if out[o:o + b].tobytes() != O.encode_stream(ch, sr, kbps, l, r if ch == 2 else None)[0]:

@@ -132,7 +132,8 @@ def test_more_than_65535_streams(M):
 
 
 def test_the_device_loop_iterates(M, tmp_path):
-    """with every speculated frame landing on gain 255 and no folded repair, the graph's WHILE loop does all the repair"""
+    """with every speculated frame landing on gain 255 and no folded repair, the graph's WHILE loop does all the repair, in
+    the session and in the synchronous call alike: the same passes and the same launch count"""
     from lamejs_b200 import build
     lib = build.build(variant="async_nofold", defines=["Q_SPEC_START=255", "Q_SPEC_STEP=1", "Q_SPEC_FOLD=0"], out_dir=str(tmp_path))
     env = dict(os.environ, MP3B200_LIB=lib)

@@ -1,5 +1,5 @@
 """The ReplayGain speculation under hostile knobs (k_replaygain.cuh): one-window chunks, a deliberately wrong guess for every
-chunk's start state and no repair pass queued ahead, so that every chunk is repaired by passes the host starts.  The knobs
+chunk's start state and no repair pass queued ahead, so that every chunk is repaired by the repair loop's graph.  The knobs
 change the speed only: each variant must give the restatement's window bits, gains, tags and album gain on whole streams and
 on live handles under a random call schedule (tests/replaygain_worker.py, one subprocess per library)."""
 import json
