@@ -389,6 +389,73 @@ int mp3b200_debug_music_crc(const uint8_t* d_buf, const int64_t* off, const int6
 typedef struct mp3b200_wav_header { int64_t data_offset, data_len; int32_t channels; uint32_t sample_rate; } mp3b200_wav_header;
 int mp3b200_wav_read_header(const uint8_t* data, int64_t len, mp3b200_wav_header* out);
 
+/* ---- WAV files in, MP3 files out (DESIGN.md 18) ---------------------------------------------------------------------------
+ * A batch of whole WAV files encoded as lamejs's worker-example/worker.js encodes one, but with the whole file in one call:
+ *   w = WavHeader.readHeader(f); v = new Int16Array(f.buffer, w.dataOffset, w.dataLen / 2);
+ *   stereo: left[i] = v[2 i], right[i] = v[2 i + 1] for i < dataLen / 4 (new Int16Array(dataLen / (2 channels)));
+ *   e = new Mp3Encoder(w.channels, w.sampleRate, kbps); file = e.encodeBuffer(left, right) ++ e.flush().
+ * (worker.js feeds 1152-sample calls and drops the last n mod 1152 samples: that is its loop, not the encoder's; every
+ * sample is encoded here.)  Typed-array lengths truncate: the view holds floor(dataLen / 2) samples, a channel
+ * floor(dataLen / 2) (mono) or floor(dataLen / 4) (stereo).  Each file gets a status; the first that applies:
+ *   MP3B200_WAV_NOT_WAV         readHeader returns undefined (not RIFF / not WAVE / "fmt " not first)
+ *   MP3B200_WAV_EXTENDED_FMT    readHeader throws 'extended fmt chunk not implemented' (fmt length other than 16 or 18)
+ *   MP3B200_WAV_RANGE_ERROR     a RangeError: the header runs past the end of the file, or the view does (odd dataOffset, or
+ *                               dataOffset + 2 floor(dataLen / 2) > length: truncated files, streaming WAVs whose dataLen is
+ *                               0xFFFFFFFF), or new Int16Array(dataLen / 0) of a file with 0 channels and data
+ *   MP3B200_WAV_NOT_PCM16       the fmt chunk's format tag is not 1 (PCM) or its bits per sample not 16.  A deliberate
+ *                               deviation: lamejs never reads these fields and encodes such data as Int16 noise
+ *   MP3B200_WAV_UNSUPPORTED     a configuration mp3b200_create_ex(channels, sampleRate, kbps, flags & MP3B200_RESAMPLE)
+ *                               refuses (channels other than 1 or 2, a rate lamejs resamples without MP3B200_RESAMPLE, a
+ *                               non-integer ratio)
+ *   MP3B200_WAV_ENCODED         encoded.
+ * A file that is not encoded changes nothing about the bytes, status or gains of the others. */
+#define MP3B200_WAV_ENCODED 0
+#define MP3B200_WAV_NOT_WAV 1
+#define MP3B200_WAV_EXTENDED_FMT 2
+#define MP3B200_WAV_RANGE_ERROR 3
+#define MP3B200_WAV_NOT_PCM16 4
+#define MP3B200_WAV_UNSUPPORTED 5
+/* mp3b200_wav_plan only: size the files as mp3b200_encode_wav_tagged writes them (its tag frame included) */
+#define MP3B200_WAV_TAG 4
+typedef struct mp3b200_wav_plan_entry {
+  int32_t status;               /* MP3B200_WAV_* */
+  int32_t channels;             /* from the header (0 where readHeader gave none) */
+  int32_t sample_rate;          /* the header's rate (values above 2^31 - 1 read as -1) */
+  int32_t out_samplerate;       /* the rate the file is encoded at (!= sample_rate: resampled); 0 unless encoded */
+  int64_t data_offset;          /* where the PCM starts in the file (0 where readHeader gave none) */
+  int64_t nsamples;             /* samples per channel once the view and the split have succeeded, else 0 */
+  int64_t out_bytes;            /* the exact size of the MP3 file: mp3b200_stream_bytes_ex, + mp3b200_lametag_size_ex with
+                                   MP3B200_WAV_TAG; 0 unless encoded */
+} mp3b200_wav_plan_entry;
+/* files[s]: file_len[s] bytes of file s.  flags within MP3B200_RESAMPLE | MP3B200_WAV_TAG.  Fills plan[s] for every file
+ * and returns 0.  Pure host arithmetic: the same answer without a device. */
+int mp3b200_wav_plan(int kbps, int flags, int nfiles, const uint8_t* const* files, const int64_t* file_len,
+                     mp3b200_wav_plan_entry* plan);
+/* Encodes the files whose status is MP3B200_WAV_ENCODED: out[s] receives out_bytes[s] bytes (cap[s] >= plan out_bytes;
+ * a smaller cap for a file that is encoded returns MP3B200_ERR_BUFFER before anything runs), status[s] the file's status
+ * (out_bytes[s] = 0 for a file that is not encoded).  flags within MP3B200_RESAMPLE.  The bytes of every file are those
+ * mp3b200_encode_streams_ex returns for its channels.  The data regions are copied to the GPU as they are, one copy per file
+ * (per upload slice of large batches), and de-interleaved there (k_stage_wav); the files of each (channels, sampleRate)
+ * run as one whole-stream encode, one configuration after another.
+ * Arguments as for every whole-stream call (above), checked before any CUDA call: nfiles < 0, a NULL files / file_len /
+ * out / cap / out_bytes / status array (nfiles > 0), a NULL files[s] or a negative file_len[s] return MP3B200_ERR_HANDLE; an
+ * unknown flag MP3B200_ERR_CONFIG; with MP3B200_REPLAYGAIN, more than 65535 files MP3B200_ERR_HANDLE.  A bad file is
+ * reported in status[s], never by failing the call. */
+int mp3b200_encode_wav(int kbps, int flags, int nfiles, const uint8_t* const* files, const int64_t* file_len, uint8_t* const* out,
+                       const int64_t* cap, int64_t* out_bytes, int32_t* status);
+/* The same with the Info / LAME tag: every encoded file is what mp3b200_encode_streams_tagged_ex returns for it.  flags within
+ * MP3B200_RESAMPLE | MP3B200_REPLAYGAIN.  title_db[s] (optional) is that call's title gain of file s (-24601 for a file not
+ * encoded); album_db (optional) GetAlbumGain over the summed histograms of every file analysed in the call, whatever their
+ * configurations (the rule of mp3b200_album_gain). */
+int mp3b200_encode_wav_tagged(int kbps, int flags, int nfiles, const uint8_t* const* files, const int64_t* file_len,
+                              uint8_t* const* out, const int64_t* cap, int64_t* out_bytes, int32_t* status, double* title_db,
+                              double* album_db);
+/* Test tap of k_stage_wav: stages the files (encodable, all of one configuration; flags within MP3B200_RESAMPLE) as
+ * mp3b200_encode_wav does, on rows filled with 0x7f bytes first, and copies the staged rows back: file after file, its left
+ * row, then (stereo) its right row.  slices (optional) receives the number of upload slices used. */
+int mp3b200_debug_stage_wav(int kbps, int flags, int nfiles, const uint8_t* const* files, const int64_t* file_len, int16_t* rows,
+                            int64_t cap, int32_t* slices);
+
 /* ---- stage taps for parity tests (one stream, whole-stream semantics) -----------------------------------
  * Run the pipeline for one stream given host PCM and copy intermediate results back.  Any output pointer may be
  * NULL.  Shapes ([F] = mp3b200_stream_frames(n)):

@@ -13,3 +13,4 @@ from .encoder import REPLAYGAIN, GAIN_NOT_ENOUGH_SAMPLES, radio_gain, lametag_bu
 from .encoder import DOMAIN_SITES, debug_domain_hits  # noqa: F401
 from .encoder import EncodeSession, check_status  # noqa: F401
 from .encoder import replay_gain_streams, replay_gain_streams_device, finish_tags_device  # noqa: F401
+from .encoder import encode_wav_files, wav_plan, WAV_ENCODED, WAV_NOT_WAV, WAV_EXTENDED_FMT, WAV_RANGE_ERROR, WAV_NOT_PCM16, WAV_UNSUPPORTED  # noqa: F401

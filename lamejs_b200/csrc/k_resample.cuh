@@ -106,4 +106,46 @@ k_stage_f32(const StageDesc* __restrict__ descs, int scale_applied, double scale
   if (bad) atomicOr(refused, 1);
 }
 
+/* ---- stereo WAV data: interleaved little-endian Int16 frames (L R L R ...) to the planar rows whole streams read ----
+ * worker.js:31-38 splits the data chunk the same way: left[i] = view[2 i], right[i] = view[2 i + 1].  The samples are
+ * copied as they are (the Int16 path applies lamejs's scale itself).  Mono data regions already are rows and are not staged.
+ * Slice j of nchunks stages the frames [n j / nchunks, n (j + 1) / nchunks) of every file, the rule the sliced upload and
+ * k_psy_analysis share, so slice j reads only bytes that slice j's copy has landed. */
+#define WAV_STAGE_THREADS 256
+struct WavStageDesc {
+  const uint8_t* x;         /* the file's data region, 16-byte aligned: frame i at x + 4 i */
+  int16_t* y[2];            /* left row (8-byte aligned), right row */
+  long long n;              /* frames (samples per channel) */
+};
+
+/* grid (ceil(max groups of 4 frames in a slice / WAV_STAGE_THREADS), files); thread = 4 frames at 4 g .. 4 g + 3 */
+__global__ void __launch_bounds__(WAV_STAGE_THREADS)
+k_stage_wav(const WavStageDesc* __restrict__ descs, int j, int nchunks) {
+  const WavStageDesc& d = descs[blockIdx.y];
+  const long long lo = d.n * j / nchunks, hi = d.n * (j + 1) / nchunks;
+  const long long g = (lo >> 2) + (long long)blockIdx.x * WAV_STAGE_THREADS + threadIdx.x, i0 = 4 * g;
+  if (i0 >= hi) return;
+  int16_t* __restrict__ yl = d.y[0] + i0;
+  int16_t* __restrict__ yr = d.y[1] + i0;
+  if (i0 >= lo && i0 + 4 <= hi) {         /* the whole group is in the slice: one 16-byte load, two 8-byte rows */
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>(d.x) + g);
+    const uint2 l = make_uint2(__byte_perm(v.x, v.y, 0x5410), __byte_perm(v.z, v.w, 0x5410));
+    const uint2 r = make_uint2(__byte_perm(v.x, v.y, 0x7632), __byte_perm(v.z, v.w, 0x7632));
+    *reinterpret_cast<uint2*>(yl) = l;
+    if ((reinterpret_cast<uintptr_t>(yr) & 7) == 0) {
+      *reinterpret_cast<uint2*>(yr) = r;
+    } else {
+      yr[0] = (int16_t)(r.x & 0xffff); yr[1] = (int16_t)(r.x >> 16); yr[2] = (int16_t)(r.y & 0xffff); yr[3] = (int16_t)(r.y >> 16);
+    }
+    return;
+  }
+  for (int k = 0; k < 4; k++) {           /* a group cut by the slice's ends: its frames one by one */
+    const long long i = i0 + k;
+    if (i < lo || i >= hi) continue;
+    const unsigned w = __ldg(reinterpret_cast<const unsigned*>(d.x) + i);
+    yl[k] = (int16_t)(w & 0xffff);
+    yr[k] = (int16_t)(w >> 16);
+  }
+}
+
 #endif

@@ -1626,6 +1626,12 @@ int check_input(const Config* cfg, int nstreams, const float* const* left, const
   return MP3B200_OK;
 }
 
+/* Host PCM is uploaded in time slices on a copy stream; the psy analysis of a slice starts when it has landed, so only the
+ * first slice's transfer is exposed.  Many small streams are uploaded whole (one slice): per-copy overhead would win. */
+int upload_slices(int nstreams, long long tot_samples) {
+  return (nstreams <= 8 && tot_samples >= (1 << 20)) ? MP3_MAX_PCM_CHUNKS : 1;
+}
+
 /* Stages the rows of host streams (Int16 or Float32) in the thread's buffer, stream s at d_pcm + pcm_off[s] laid out as
  * whole_streams reads it, and fills the upload's arrival `arr`.  Stereo input with right == NULL or right[s] == NULL takes
  * left[s] for both channels. */
@@ -1641,9 +1647,7 @@ int upload_host_rows(const Config* cfg, int nstreams, const T* const* left, cons
   }
   d_pcm = staging_pcm<T>((size_t)tot_samples + 8);
   if (!d_pcm) return MP3B200_ERR_CUDA;
-  /* Upload in time slices on a copy stream; the psy analysis of a slice starts when it has landed, so only the first
-   * slice's transfer is exposed.  Many small streams are uploaded whole (one slice): per-copy overhead would win. */
-  arr.chunks = (nstreams <= 8 && tot_samples >= (1 << 20)) ? MP3_MAX_PCM_CHUNKS : 1;
+  arr.chunks = upload_slices(nstreams, tot_samples);
   arr.ready = t_ctx.ready;
   for (int j = 0; j < arr.chunks; j++) {
     for (int s = 0; s < nstreams; s++) {
@@ -1692,14 +1696,26 @@ int whole_run(ThreadCtx& c, Config* cfg, const WholeCall<T>& k, const StreamPlan
   return finish_tagged(c, cfg, pl, sds, k.d_out, k.out_off, gain);
 }
 
+template <class T>
+int whole_sync_run(WholeCall<T> k, Config* cfg, const PcmArrival* arrival = nullptr, int* album_hist = nullptr);
+
 /* The synchronous driver, on the calling thread's context: host files are laid out in t_ctx.out and copied into out[s];
  * returns with every result on the host. */
 template <class T>
 int whole_sync(WholeCall<T> k) {
   Config* cfg = nullptr;
   int rc = whole_args(k);
-  if (rc || (rc = get_config(k.channels, k.samplerate, k.kbps, k.flags & MP3B200_RESAMPLE, &cfg)) ||
-      (k.left && (rc = check_input(cfg, k.nstreams, k.left, k.right, k.nsamples))) || (k.tagged && (rc = crc_tables_on(t_ctx.device))))
+  if (rc || (rc = get_config(k.channels, k.samplerate, k.kbps, k.flags & MP3B200_RESAMPLE, &cfg))) return rc;
+  return whole_sync_run(k, cfg);
+}
+
+/* whole_sync once the arguments are checked and the configuration is bound.  Device rows (k.d_pcm) may be written to host
+ * files (k.out): the WAV calls stage their rows themselves and pass the upload's `arrival`.  album_hist (optional, RG_HIST
+ * ints) receives the album histogram of the streams analysed (zeros where none were). */
+template <class T>
+int whole_sync_run(WholeCall<T> k, Config* cfg, const PcmArrival* arrival, int* album_hist) {
+  int rc = 0;
+  if ((k.left && (rc = check_input(cfg, k.nstreams, k.left, k.right, k.nsamples))) || (k.tagged && (rc = crc_tables_on(t_ctx.device))))
     return rc;
   const int S = k.nstreams;
   RgJob job;
@@ -1720,6 +1736,7 @@ int whole_sync(WholeCall<T> k) {
   LaunchOpts o;
   o.f32_in = std::is_same_v<T, float>;
   o.timings_ms = k.timings_ms;
+  o.arrival = arrival;
   if ((rc = whole_run(t_ctx, cfg, k, pl, o))) return rc;
   if (k.out || k.tagged) {               /* the copies and the tag step are still queued */
     for (int s = 0; k.out && s < S; s++)
@@ -1731,6 +1748,10 @@ int whole_sync(WholeCall<T> k) {
   const bool ran = pl.rg && (int)pl.rg->title_db.size() == S && S > 0;
   for (int s = 0; k.title_db && s < S; s++) k.title_db[s] = ran ? pl.rg->title_db[s] : RG_NOT_ENOUGH_SAMPLES;
   if (k.album_db) *k.album_db = ran ? pl.rg->album_db : RG_NOT_ENOUGH_SAMPLES;
+  if (album_hist) {                      /* rg_queue_results left the album's histogram behind the titles' */
+    if (ran) CK(cudaMemcpy(album_hist, t_ctx.rg_hist.p + (size_t)S * RG_HIST, sizeof(int) * RG_HIST, cudaMemcpyDeviceToHost));
+    else memset(album_hist, 0, sizeof(int) * RG_HIST);
+  }
   return MP3B200_OK;
 }
 }  // namespace
@@ -2095,7 +2116,222 @@ int mp3b200_debug_replaygain_f32(int channels, int samplerate, int kbps, int fla
 }
 }  // extern "C"
 
+namespace {
+/* ---- WAV files (include/mp3b200.h "WAV files in, MP3 files out", DESIGN.md 18) ---- */
+
+/* One file's outcome from its bytes alone (host arithmetic): lamejs's header, view and split, then the 16-bit PCM rule and
+ * the configuration. */
+mp3b200_wav_plan_entry wav_plan_file(int kbps, int flags, bool tagged, const uint8_t* f, long long len) {
+  mp3b200_wav_plan_entry e;
+  memset(&e, 0, sizeof e);
+  long long off = 0, dl = 0;
+  int ch = 0;
+  unsigned sr = 0;
+  const int hdr = mp3_wav_read_header(f, len, &off, &dl, &ch, &sr);
+  if (hdr == 0) { e.status = MP3B200_WAV_NOT_WAV; return e; }
+  if (hdr == -1) { e.status = MP3B200_WAV_EXTENDED_FMT; return e; }
+  if (hdr != 1) { e.status = MP3B200_WAV_RANGE_ERROR; return e; }
+  e.channels = ch;
+  e.sample_rate = sr > 0x7fffffffu ? -1 : (int32_t)sr;
+  e.data_offset = off;
+  /* new Int16Array(buffer, dataOffset, dataLen / 2): the length truncates; an odd offset or a view past the end throws.
+   * new Int16Array(dataLen / (2 channels)) throws for 0 channels with data (length Infinity; 0 / 0 is NaN, length 0). */
+  const long long view = dl / 2;
+  if ((off & 1) || off + 2 * view > len || (ch == 0 && dl > 0)) { e.status = MP3B200_WAV_RANGE_ERROR; return e; }
+  e.nsamples = ch == 1 ? view : ch == 0 ? 0 : dl / (2LL * ch);
+  const unsigned tag = (unsigned)f[20] | ((unsigned)f[21] << 8), bits = (unsigned)f[34] | ((unsigned)f[35] << 8);
+  if (tag != 1 || bits != 16) { e.status = MP3B200_WAV_NOT_PCM16; return e; }
+  const Config* c = e.sample_rate > 0 ? encodable_config(ch, e.sample_rate, kbps, flags & MP3B200_RESAMPLE) : nullptr;
+  if (!c) { e.status = MP3B200_WAV_UNSUPPORTED; return e; }
+  e.status = MP3B200_WAV_ENCODED;
+  e.out_samplerate = c->host.samplerate;
+  e.out_bytes = bytes_of_frames(c->host, 0, frames_for(e.nsamples, c->host.mode_gr, c->rs.ratio));
+  if (tagged && c->tag.fits) e.out_bytes += c->tag.frame_bytes;
+  return e;
+}
+
+/* The argument rules of the WAV calls, the whole-stream calls' rules on their arrays, before any CUDA call */
+int wav_args(int flags, int allowed, int nfiles, const uint8_t* const* files, const int64_t* file_len, bool encode,
+             uint8_t* const* out, const int64_t* cap, const int64_t* out_bytes, const int32_t* status) {
+  auto refuse = [](const char* why) { g_err = why; return MP3B200_ERR_HANDLE; };
+  if (nfiles < 0) return refuse("negative stream count");
+  if (flags & ~allowed) { g_err = "unknown flags"; return MP3B200_ERR_CONFIG; }
+  if ((flags & MP3B200_REPLAYGAIN) && nfiles > MP3_MAX_LAUNCH_STREAMS) return refuse("ReplayGain batches hold at most 65535 streams");
+  if (nfiles == 0) return MP3B200_OK;
+  if (!files || !file_len || (encode && (!out || !cap || !out_bytes || !status))) return refuse("null array");
+  for (int s = 0; s < nfiles; s++) {
+    if (!files[s]) return refuse("null file");
+    if (file_len[s] < 0) return refuse("negative file length");
+  }
+  return MP3B200_OK;
+}
+
+/* Uploads the data regions of the files `idx` (one configuration: cfg) as they are, one copy per file and upload slice on
+ * t_ctx.up_st, and stages them as the rows whole_streams reads: file i's left row at rows + pcm_off[i], its right row behind
+ * it.  Mono regions are copied straight into their rows; stereo regions land in a raw area behind the rows and k_stage_wav
+ * splits each slice on the copy stream once it has landed, so arr.ready[j] means slice j's rows are there. */
+int upload_wav_rows(const Config* cfg, const uint8_t* const* files, const std::vector<mp3b200_wav_plan_entry>& plan,
+                    const std::vector<int>& idx, std::vector<int64_t>& pcm_off, int16_t*& rows, PcmArrival& arr, bool poison = false) {
+  const int n = (int)idx.size(), nch = cfg->host.nch;
+  pcm_off.assign((size_t)n, 0);
+  std::vector<long long> raw_off((size_t)n, 0);
+  long long tot = 0, raw = 0;
+  for (int i = 0; i < n; i++) {
+    const long long ns = plan[idx[i]].nsamples;
+    pcm_off[i] = tot;
+    tot += (ns * nch + 7) & ~7LL;                    /* rows 16-byte aligned: k_stage_wav's 8-byte left stores */
+    if (nch == 2) { raw_off[i] = raw; raw += (4 * ns + 15) & ~15LL; }
+  }
+  const size_t rows_bytes = ((size_t)tot * 2 + 16 + 255) & ~(size_t)255, raw_bytes = ((size_t)raw + 255) & ~(size_t)255;
+  const size_t desc_bytes = nch == 2 ? sizeof(WavStageDesc) * (size_t)n : 0;
+  if (t_ctx.pcm.fit(rows_bytes + raw_bytes + desc_bytes)) return MP3B200_ERR_CUDA;
+  rows = reinterpret_cast<int16_t*>(t_ctx.pcm.p);
+  uint8_t* d_raw = t_ctx.pcm.p + rows_bytes;
+  WavStageDesc* d_desc = reinterpret_cast<WavStageDesc*>(d_raw + raw_bytes);
+  if (poison) CK(cudaMemsetAsync(rows, 0x7f, rows_bytes, t_ctx.up_st));   /* debug tap: rows of 0x7f7f until written */
+  long long max_n = 0;
+  if (nch == 2) {
+    std::vector<WavStageDesc> d((size_t)n);
+    for (int i = 0; i < n; i++) {
+      d[i].x = d_raw + raw_off[i];
+      d[i].y[0] = rows + pcm_off[i];
+      d[i].y[1] = d[i].y[0] + plan[idx[i]].nsamples;
+      d[i].n = plan[idx[i]].nsamples;
+      max_n = d[i].n > max_n ? d[i].n : max_n;
+    }
+    const int rc = upload(t_ctx, d_desc, d.data(), desc_bytes, t_ctx.up_st);
+    if (rc) return rc;
+  }
+  arr.chunks = upload_slices(n, tot);
+  arr.ready = t_ctx.ready;
+  for (int j = 0; j < arr.chunks; j++) {
+    long long max_groups = 0;
+    for (int i = 0; i < n; i++) {
+      const mp3b200_wav_plan_entry& e = plan[idx[i]];
+      const long long lo = e.nsamples * j / arr.chunks, hi = e.nsamples * (j + 1) / arr.chunks;
+      if (hi <= lo) continue;
+      const uint8_t* src = files[idx[i]] + e.data_offset;
+      if (nch == 1) CK(cudaMemcpyAsync(rows + pcm_off[i] + lo, src + 2 * lo, 2 * (hi - lo), cudaMemcpyHostToDevice, t_ctx.up_st));
+      else CK(cudaMemcpyAsync(d_raw + raw_off[i] + 4 * lo, src + 4 * lo, 4 * (hi - lo), cudaMemcpyHostToDevice, t_ctx.up_st));
+      const long long groups = ((hi + 3) >> 2) - (lo >> 2);
+      max_groups = groups > max_groups ? groups : max_groups;
+    }
+    for (int f0 = 0; nch == 2 && max_groups > 0 && f0 < n; f0 += MP3_MAX_LAUNCH_STREAMS) {
+      const int nf = n - f0 < MP3_MAX_LAUNCH_STREAMS ? n - f0 : MP3_MAX_LAUNCH_STREAMS;
+      dim3 grid((unsigned)((max_groups + WAV_STAGE_THREADS - 1) / WAV_STAGE_THREADS), (unsigned)nf);
+      k_stage_wav<<<grid, WAV_STAGE_THREADS, 0, t_ctx.up_st>>>(d_desc + f0, j, arr.chunks);
+      g_launches++;
+      CK(cudaGetLastError());
+    }
+    CK(cudaEventRecord(t_ctx.ready[j], t_ctx.up_st));
+  }
+  return MP3B200_OK;
+}
+
+/* The body of mp3b200_encode_wav / _tagged: plan every file, then one whole-stream encode per (channels, sampleRate) on the
+ * rows upload_wav_rows stages.  Output order is input order whatever the group order. */
+int encode_wav(int kbps, int flags, bool tagged, int nfiles, const uint8_t* const* files, const int64_t* file_len,
+               uint8_t* const* out, const int64_t* cap, int64_t* out_bytes, int32_t* status, double* title_db, double* album_db) {
+  int rc = wav_args(flags, MP3B200_RESAMPLE | (tagged ? MP3B200_REPLAYGAIN : 0), nfiles, files, file_len, true, out, cap, out_bytes,
+                    status);
+  if (rc) return rc;
+  std::vector<mp3b200_wav_plan_entry> plan((size_t)nfiles);
+  std::map<std::pair<int, int>, std::vector<int>> groups;
+  for (int s = 0; s < nfiles; s++) {
+    plan[s] = wav_plan_file(kbps, flags, tagged, files[s], file_len[s]);
+    if (plan[s].status == MP3B200_WAV_ENCODED) {
+      if (cap[s] < plan[s].out_bytes) { g_err = "output buffer too small"; return MP3B200_ERR_BUFFER; }
+      groups[{plan[s].channels, plan[s].sample_rate}].push_back(s);
+    }
+  }
+  for (int s = 0; s < nfiles; s++) {
+    status[s] = plan[s].status;
+    out_bytes[s] = 0;
+    if (title_db) title_db[s] = RG_NOT_ENOUGH_SAMPLES;
+  }
+  const bool analyse = tagged && (flags & MP3B200_REPLAYGAIN);
+  std::vector<int> album(RG_HIST, 0), hist(RG_HIST);
+  for (const auto& g : groups) {
+    const std::vector<int>& idx = g.second;
+    const int n = (int)idx.size();
+    Config* cfg = nullptr;
+    if ((rc = get_config(g.first.first, g.first.second, kbps, flags & MP3B200_RESAMPLE, &cfg))) return rc;
+    std::vector<int64_t> pcm_off, ns((size_t)n), caps((size_t)n), nb((size_t)n);
+    std::vector<uint8_t*> outs((size_t)n);
+    std::vector<double> title((size_t)n);
+    for (int i = 0; i < n; i++) { ns[i] = plan[idx[i]].nsamples; outs[i] = out[idx[i]]; caps[i] = cap[idx[i]]; }
+    int16_t* rows = nullptr;
+    PcmArrival arr;
+    if ((rc = upload_wav_rows(cfg, files, plan, idx, pcm_off, rows, arr))) return rc;
+    WholeCall<int16_t> k = {.channels = g.first.first, .samplerate = g.first.second, .kbps = kbps, .flags = flags, .nstreams = n,
+                            .d_pcm = rows, .pcm_off = pcm_off.data(), .nsamples = ns.data(), .tagged = tagged, .analyse = analyse,
+                            .out = outs.data(), .cap = caps.data(), .out_bytes = nb.data(), .title_db = title.data()};
+    if ((rc = whole_sync_run(k, cfg, &arr, analyse ? hist.data() : nullptr))) return rc;
+    for (int i = 0; i < n; i++) {
+      out_bytes[idx[i]] = nb[i];
+      if (title_db) title_db[idx[i]] = analyse ? title[i] : RG_NOT_ENOUGH_SAMPLES;
+    }
+    for (int b = 0; analyse && b < RG_HIST; b++) album[b] += hist[b];
+  }
+  if (album_db) *album_db = analyse ? rg_analyze_result(album.data()) : RG_NOT_ENOUGH_SAMPLES;
+  return MP3B200_OK;
+}
+}  // namespace
+
 extern "C" {
+
+int mp3b200_wav_plan(int kbps, int flags, int nfiles, const uint8_t* const* files, const int64_t* file_len,
+                     mp3b200_wav_plan_entry* plan) {
+  const int rc = wav_args(flags, MP3B200_RESAMPLE | MP3B200_WAV_TAG, nfiles, files, file_len, false, nullptr, nullptr, nullptr, nullptr);
+  if (rc) return rc;
+  if (nfiles > 0 && !plan) { g_err = "null array"; return MP3B200_ERR_HANDLE; }
+  for (int s = 0; s < nfiles; s++) plan[s] = wav_plan_file(kbps, flags, (flags & MP3B200_WAV_TAG) != 0, files[s], file_len[s]);
+  return MP3B200_OK;
+}
+
+int mp3b200_encode_wav(int kbps, int flags, int nfiles, const uint8_t* const* files, const int64_t* file_len, uint8_t* const* out,
+                       const int64_t* cap, int64_t* out_bytes, int32_t* status) {
+  return encode_wav(kbps, flags, false, nfiles, files, file_len, out, cap, out_bytes, status, nullptr, nullptr);
+}
+
+int mp3b200_encode_wav_tagged(int kbps, int flags, int nfiles, const uint8_t* const* files, const int64_t* file_len,
+                              uint8_t* const* out, const int64_t* cap, int64_t* out_bytes, int32_t* status, double* title_db,
+                              double* album_db) {
+  return encode_wav(kbps, flags, true, nfiles, files, file_len, out, cap, out_bytes, status, title_db, album_db);
+}
+
+int mp3b200_debug_stage_wav(int kbps, int flags, int nfiles, const uint8_t* const* files, const int64_t* file_len, int16_t* rows,
+                            int64_t cap, int32_t* slices) {
+  int rc = wav_args(flags, MP3B200_RESAMPLE, nfiles, files, file_len, false, nullptr, nullptr, nullptr, nullptr);
+  if (rc || nfiles == 0) return rc;
+  std::vector<mp3b200_wav_plan_entry> plan((size_t)nfiles);
+  std::vector<int> idx((size_t)nfiles);
+  long long tot = 0;
+  for (int s = 0; s < nfiles; s++) {
+    plan[s] = wav_plan_file(kbps, flags, false, files[s], file_len[s]);
+    idx[s] = s;
+    if (plan[s].status != MP3B200_WAV_ENCODED || plan[s].channels != plan[0].channels || plan[s].sample_rate != plan[0].sample_rate) {
+      g_err = "the tap takes encodable files of one configuration"; return MP3B200_ERR_CONFIG;
+    }
+    tot += plan[s].nsamples * plan[s].channels;
+  }
+  if (!rows || cap < tot) { g_err = "output buffer too small"; return MP3B200_ERR_BUFFER; }
+  Config* cfg = nullptr;
+  if ((rc = get_config(plan[0].channels, plan[0].sample_rate, kbps, flags, &cfg))) return rc;
+  std::vector<int64_t> pcm_off;
+  int16_t* d_rows = nullptr;
+  PcmArrival arr;
+  if ((rc = upload_wav_rows(cfg, files, plan, idx, pcm_off, d_rows, arr, true))) return rc;
+  CK(cudaStreamSynchronize(t_ctx.up_st));
+  long long at = 0;
+  for (int s = 0; s < nfiles; s++) {
+    const size_t n = (size_t)(plan[s].nsamples * plan[s].channels);
+    CK(cudaMemcpy(rows + at, d_rows + pcm_off[s], sizeof(int16_t) * n, cudaMemcpyDeviceToHost));
+    at += (long long)n;
+  }
+  if (slices) *slices = arr.chunks;
+  return MP3B200_OK;
+}
 
 int mp3b200_wav_read_header(const uint8_t* data, int64_t len, mp3b200_wav_header* out) {
   if (!out || len < 0 || (len > 0 && !data)) return MP3B200_ERR_HANDLE;

@@ -130,6 +130,10 @@ def lib():
         getattr(L, name).argtypes = [c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp]
     L.mp3b200_finish_tags_device.argtypes = [c_int, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp]
     L.mp3b200_session_tail_capacity.restype = c_i64
+    L.mp3b200_wav_plan.argtypes = [c_int, c_int, c_int, vp, vp, vp]
+    L.mp3b200_encode_wav.argtypes = [c_int, c_int, c_int, vp, vp, vp, vp, vp, vp]
+    L.mp3b200_encode_wav_tagged.argtypes = [c_int, c_int, c_int, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.mp3b200_debug_stage_wav.argtypes = [c_int, c_int, c_int, vp, vp, vp, c_i64, vp]
     _lib = L
     return L
 
@@ -600,6 +604,71 @@ def album_gain(encoders):
 
 
 GAIN_NOT_ENOUGH_SAMPLES = -24601
+
+# the status of a file in encode_wav_files / wav_plan (MP3B200_WAV_*, include/mp3b200.h)
+WAV_ENCODED, WAV_NOT_WAV, WAV_EXTENDED_FMT, WAV_RANGE_ERROR, WAV_NOT_PCM16, WAV_UNSUPPORTED = range(6)
+WAV_TAG = 4      # MP3B200_WAV_TAG
+
+
+class WavPlanEntry(ctypes.Structure):
+    """mp3b200_wav_plan_entry (include/mp3b200.h)"""
+    _fields_ = [("status", ctypes.c_int32), ("channels", ctypes.c_int32), ("sample_rate", ctypes.c_int32),
+                ("out_samplerate", ctypes.c_int32), ("data_offset", ctypes.c_int64), ("nsamples", ctypes.c_int64),
+                ("out_bytes", ctypes.c_int64)]
+
+
+def _wav_files(files):
+    """the files as contiguous uint8 arrays (bytes, bytearray, or uint8 arrays), their pointer and length arrays"""
+    arrs = [np.frombuffer(f, dtype=np.uint8) if isinstance(f, (bytes, bytearray, memoryview)) else np.ascontiguousarray(f, dtype=np.uint8)
+            for f in files]
+    empty = np.zeros(1, dtype=np.uint8)              # a file of no bytes still needs a pointer
+    ptrs = (ctypes.c_void_p * max(len(arrs), 1))(*[(a if len(a) else empty).ctypes.data for a in arrs])
+    lens = np.array([len(a) for a in arrs] or [0], dtype=np.int64)
+    return arrs, ptrs, lens
+
+
+def wav_plan(files, kbps, resample=False, write_vbr_tag=False):
+    """What encode_wav_files does with each file, from its bytes alone (mp3b200_wav_plan, no device): a list of dicts with
+    status (WAV_*), channels, sample_rate, out_samplerate, data_offset, nsamples (per channel) and out_bytes (the MP3 file's
+    exact size; with write_vbr_tag its tag frame included)."""
+    arrs, ptrs, lens = _wav_files(files)
+    plan = (WavPlanEntry * max(len(arrs), 1))()
+    flags = (RESAMPLE if resample else 0) | (WAV_TAG if write_vbr_tag else 0)
+    _check(lib().mp3b200_wav_plan(int(kbps), flags, len(arrs), ptrs, lens.ctypes.data, plan))
+    return [{k: getattr(p, k) for k, _ in WavPlanEntry._fields_} for p in plan[:len(arrs)]]
+
+
+def encode_wav_files(files, kbps, resample=False, write_vbr_tag=False, find_replay_gain=False):
+    """WAV files in, MP3 files out: each file encoded as lamejs's worker-example does it with the whole file in one
+    encodeBuffer + flush (WavHeader.readHeader, the Int16 view of the data chunk, new Mp3Encoder(channels, sampleRate, kbps)).
+    `files` are bytes, bytearray or uint8 arrays of whole WAV files.  Returns (mp3s, status): mp3s[s] is the file's MP3
+    bytes, or None when status[s] != WAV_ENCODED.  write_vbr_tag: every file starts with its Info / LAME tag frame, as from
+    encode_streams_tagged.  find_replay_gain (implies the tag): returns (mp3s, status, title_db, album_db) with the gains of
+    encode_streams_replaygain; the album covers every analysed file, whatever its configuration."""
+    tagged = write_vbr_tag or find_replay_gain
+    plan = wav_plan(files, kbps, resample, tagged)
+    arrs, ptrs, lens = _wav_files(files)
+    S = len(arrs)
+    outs = [np.empty(max(p["out_bytes"], 1), dtype=np.uint8) for p in plan]
+    op = (ctypes.c_void_p * max(S, 1))(*[o.ctypes.data for o in outs])
+    caps = np.array([p["out_bytes"] for p in plan] or [0], dtype=np.int64)
+    got = np.zeros(max(S, 1), dtype=np.int64)
+    status = np.zeros(max(S, 1), dtype=np.int32)
+    flags = RESAMPLE if resample else 0
+    if tagged:
+        title = np.zeros(max(S, 1), dtype=np.float64)
+        album = ctypes.c_double(0.0)
+        flags |= REPLAYGAIN if find_replay_gain else 0
+        _check(lib().mp3b200_encode_wav_tagged(int(kbps), flags, S, ptrs, lens.ctypes.data, op, caps.ctypes.data, got.ctypes.data,
+                                               status.ctypes.data, title.ctypes.data, ctypes.byref(album)))
+    else:
+        _check(lib().mp3b200_encode_wav(int(kbps), flags, S, ptrs, lens.ctypes.data, op, caps.ctypes.data, got.ctypes.data,
+                                        status.ctypes.data))
+    mp3s = [o[: int(g)].tobytes() if st == WAV_ENCODED else None for o, g, st in zip(outs, got, status)]
+    st = [int(x) for x in status[:S]]
+    if find_replay_gain:
+        return mp3s, st, [float(t) for t in title[:S]], float(album.value)
+    return mp3s, st
 
 
 def radio_gain(title_db):
