@@ -492,9 +492,7 @@ int mp3b200_debug_stages(int channels, int samplerate, int kbps, const int16_t* 
  * is that of the output rate ([F] = mp3b200_stream_frames_ex(..., flags, nsamples), [G] = mp3b200_granules_per_frame_ex).
  * Any output pointer may be NULL.
  * The encoder computes the short-block half of the psy model (en_s / thm_s) only for the units whose masking a short
- * granule reads, and for each stream's last unit (DESIGN.md 2); the taps compute it for every unit, unless `flags` holds
- * MP3B200_DEBUG_SKIP_SHORT: then en_s / thm_s are defined for those units only, as in an encode. */
-#define MP3B200_DEBUG_SKIP_SHORT 0x10000
+ * granule reads, and for each stream's last unit (DESIGN.md 2); the taps compute it for every unit. */
 typedef struct mp3b200_debug_taps {
   int32_t size, channels, samplerate, kbps;
   const int16_t *left, *right;
@@ -507,9 +505,6 @@ typedef struct mp3b200_debug_taps {
   int32_t flags;
 } mp3b200_debug_taps;
 int mp3b200_debug_stages_ex(const mp3b200_debug_taps* t);
-/* (unit, channel) pairs the calling thread's last launch ran the short-block psy half for (halo units included); -1 before
- * its first launch */
-int64_t mp3b200_debug_short_units(void);
 /* Debug psy-row capture, off by default.  on != 0 clears the records and turns capture on for every thread and session;
  * 0 turns it off (the records stay until taken).  While it is on, each pipeline launch fills its front-end rows with a
  * poison pattern before the long-block analysis (float and double fields a quiet NaN, mask_idx 8, attack 0, both block-type

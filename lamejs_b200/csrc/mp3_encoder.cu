@@ -1331,13 +1331,6 @@ int64_t mp3b200_debug_psy_take(void* buf, int64_t cap) {
   }
   return n;
 }
-int64_t mp3b200_debug_short_units(void) {
-  if (!t_ctx.ws.short_count.p) return -1;
-  int n = 0;
-  CK(cudaMemcpyAsync(&n, t_ctx.ws.short_count.p, sizeof n, cudaMemcpyDeviceToHost, t_ctx.st));
-  CK(cudaStreamSynchronize(t_ctx.st));
-  return n;
-}
 
 int mp3b200_set_device(int device) {
   int n = 0;
@@ -1909,7 +1902,7 @@ int debug_stages(const mp3b200_debug_taps* tp, const T* left, const T* right) {
   uint8_t* bytes_out = tp->bytes_out;
   const int64_t bytes_cap = tp->bytes_cap;
   Config* cfg;
-  int rc = get_config(channels, tp->samplerate, tp->kbps, tp->flags & ~MP3B200_DEBUG_SKIP_SHORT, &cfg);
+  int rc = get_config(channels, tp->samplerate, tp->kbps, tp->flags, &cfg);
   if (rc || (rc = check_input(cfg, 1, &left, &right, &nsamples))) return rc;
   const int nch = cfg->host.nch;
   const int G = cfg->host.mode_gr;
@@ -1930,7 +1923,7 @@ int debug_stages(const mp3b200_debug_taps* tp, const T* left, const T* right) {
   LaunchOpts opts;
   opts.f32_in = std::is_same_v<T, float>;
   opts.force_bt = force_blocktype;
-  opts.all_short = !(tp->flags & MP3B200_DEBUG_SKIP_SHORT);
+  opts.all_short = true;
   opts.stop_after_mdct = !(l3_enc || bytes_out || want_gi || want_prep || want_q);
   opts.arrival = &arr;
   rc = reset_words(t_ctx, 1);

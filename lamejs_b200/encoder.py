@@ -1032,16 +1032,6 @@ def debug_resample(channels, samplerate, kbps, left, right=None, ny=None):
     return y
 
 
-DEBUG_SKIP_SHORT = 0x10000    # mp3b200_debug_taps.flags: the short-block psy half only where an encode computes it
-
-
-def debug_short_units():
-    """(unit, channel) pairs the calling thread's last launch ran the short-block psy half for (halo units included)."""
-    f = lib().mp3b200_debug_short_units
-    f.restype = ctypes.c_int64
-    return f()
-
-
 # the rows mp3b200_debug_psy_take hands out (include/mp3b200.h)
 PSY_UNIT_DTYPE = np.dtype({"names": ["eb_l", "peaks", "loudness", "mask_idx", "attack"],
                            "formats": [(np.float32, 64), (np.float32, 9), np.float32, (np.uint8, 64), (np.uint8, 4)],
@@ -1137,14 +1127,12 @@ def debug_psy_capture():
         cap._parse(buf.tobytes())
 
 
-def debug_stages(channels, samplerate, kbps, left, right=None, force_blocktype=None, want=("xr",), resample=False,
-                 skip_short=False):
+def debug_stages(channels, samplerate, kbps, left, right=None, force_blocktype=None, want=("xr",), resample=False):
     """Stage taps for parity tests: returns a dict of numpy arrays (see include/mp3b200.h).  `want` names any of xr,
     blocktype, en_l, thm_l, en_s, thm_s, ath_adjust, l3_enc, ginfo, bytes, scalefac, subblock_gain, xmin, max_nonzero_coeff,
     xrpow_max, scfsi, old_value and cur_step (the last two [F][3][nch]: frame start, after gr0, frame end).  resample=True
     also accepts the configurations lamejs resamples by an integer ratio: left / right are input samples, the taps are
-    those of the output rate, after k_resample.  skip_short=True: en_s / thm_s are defined only for the units whose short
-    thresholds an encode computes (include/mp3b200.h), as the encoder runs; the others hold whatever was there."""
+    those of the output rate, after k_resample."""
     L = lib()
     (left,), (right,), f32 = _rows([left], [None if channels == 1 else right])
     n = len(left)
@@ -1186,7 +1174,7 @@ def debug_stages(channels, samplerate, kbps, left, right=None, force_blocktype=N
                   xmin=alloc("xmin", (F, G, nch, 39), np.float32), max_nonzero_coeff=alloc("max_nonzero_coeff", (F, G, nch), np.int32),
                   xrpow_max=alloc("xrpow_max", (F, G, nch), np.float64), scfsi=alloc("scfsi", (F, nch, 4), np.int32),
                   old_value=alloc("old_value", (F, 3, nch), np.int32), cur_step=alloc("cur_step", (F, 3, nch), np.int32),
-                  flags=(RESAMPLE if resample else 0) | (DEBUG_SKIP_SHORT if skip_short else 0))
+                  flags=RESAMPLE if resample else 0)
     if f32:
         _check(L.mp3b200_debug_stages_f32(ctypes.byref(t), left.ctypes.data, right.ctypes.data))
     else:

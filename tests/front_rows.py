@@ -1,8 +1,8 @@
-"""The front end's remaining rows against the oracle, row for row and bit for bit (tests/test_gpu_front_rows.py): the block
-types and ATH adjustments of k_stream_scan, the masking rows of k_psy_masking and the xr rows of k_mdct, as the debug capture
-records them after k_mdct.  The launch poisons them (and the subband slabs k_mdct reads) before the psy analysis, so a row
-it forgets to write shows as NaN, or as block type START where the scan never stores one.  The shapes, the oracle and the
-whole-stream driver are tests/psy_rows.py's.
+"""The front end's remaining rows against the oracle, row for row and bit for bit (tests/test_gpu_front_end_rows.py): the
+block types and ATH adjustments of k_stream_scan, the masking rows of k_psy_masking and the xr rows of k_mdct, as the debug
+capture records them after k_mdct.  The launch poisons them (and the subband slabs k_mdct reads) before the psy analysis, so
+a row it forgets to write shows as NaN, or as block type START where the scan never stores one.  The shapes, the oracle and
+the whole-stream driver are tests/psy_rows.py's.
 
 What is compared, for stream unit u (absolute granule c = G frame0 + u) of a launch:
   bt[u]          the oracle's block type of granule c
@@ -13,8 +13,8 @@ What is compared, for stream unit u (absolute granule c = G frame0 + u) of a lau
   last row       (u = G nframes - 1) in all 122 floats: the oracle's gfc.en / gfc.thm after the call, the masking handed on
   xr[u]          the frame trace's xr of granule c, all 576 lines
 
-Run as a script (MP3B200_LIB set to a variant build) it checks the whole-stream, ragged-batch and upload-slice shapes and
-prints one JSON line {"fail": [first differences], "nfail": n}."""
+Run as a script (MP3B200_LIB set to a variant build) it checks every row (check_rows) in the whole-stream, ragged-batch and
+upload-slice shapes and prints one JSON line {"fail": [first differences], "nfail": n}."""
 import json
 import os
 import sys
@@ -108,6 +108,12 @@ def check_front(rec, refs, label, fail):
                 label, z, f, frame0 + f, s["ath_psy"][f], want_psy[f], s["ath_q"][f], want_q[f]))
 
 
+def check_rows(rec, refs, label, fail):
+    """every front-end row of one launch: the psy rows and the short list (psy_rows.check_launch), then the rows after k_mdct"""
+    P.check_launch(rec, refs, label, fail)
+    check_front(rec, refs, label, fail)
+
+
 def read_rows(bt):
     """R(u) of a launch's stream from its own block types bt [n][nch]: u is the last unit or granule u + 1 is short"""
     n = len(bt)
@@ -141,9 +147,9 @@ def main():
 
     assert os.path.samefile(M.lib()._name, os.environ["MP3B200_LIB"])
     fail = []
-    P.shape_whole(M, fail, check=check_front)
-    P.shape_batches(M, fail, check=check_front)
-    P.shape_slices(M, fail, check=check_front)
+    P.shape_whole(M, fail, check_rows)
+    P.shape_batches(M, fail, check_rows)
+    P.shape_slices(M, fail, check_rows)
     print(json.dumps({"fail": fail[:50], "nfail": len(fail)}))
 
 

@@ -1,24 +1,14 @@
 """The psy rows of k_psy_analysis / k_attack_prepass / k_psy_short against the oracle's psy trace, row for row and bit for bit
-(tests/test_gpu_psy_rows.py).  Every call runs under lamejs_b200.debug_psy_capture(): the launch poisons the rows before
-the analysis, so a row it forgets to write shows as NaN (or as mask_idx 8), and the bytes of the call must still equal the
-oracle's, which shows that no kernel read a row the launch did not write.
-
-Run as a script (MP3B200_LIB set to a variant build) it checks the whole-stream, ragged-batch and upload-slice shapes and
-prints one JSON line {"fail": [first differences], "nfail": n}."""
-import json
-import os
-import sys
-
+(tests/test_gpu_front_end_rows.py), and the launch shapes every front-end row is checked in.  Every call runs under
+lamejs_b200.debug_psy_capture(): the launch poisons the rows before the analysis, so a row it forgets to write shows as NaN
+(or as mask_idx 8), and the bytes of the call must still equal the oracle's, which shows that no kernel read a row the
+launch did not write."""
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, os.path.dirname(HERE))
-sys.path.insert(0, HERE)
-
-import oracle_f32  # noqa: E402
-import oracle_inputs  # noqa: E402
-import oracle_lib  # noqa: E402
-from synth import make_signal  # noqa: E402
+import oracle_f32
+import oracle_inputs
+import oracle_lib
+from synth import make_signal
 
 BT_SHORT = 2
 PCM_SLICES = 8              # MP3_MAX_PCM_CHUNKS: host calls of <= 8 streams and >= 2^20 samples upload in 8 time slices
@@ -231,9 +221,8 @@ def capture_call(M, fn):
     return res, cap.launches
 
 
-def whole_streams(M, ch, sr, kb, sigs, label, fail, f32=False, resample=False, check=None):
-    """one host call over `sigs` (a batch when several); rows (`check`, default check_launch) and bytes against one oracle
-    per stream"""
+def whole_streams(M, ch, sr, kb, sigs, label, fail, check, f32=False, resample=False):
+    """one host call over `sigs` (a batch when several); rows (`check`) and bytes against one oracle per stream"""
     refs = [make_ref(ch, sr, kb, f32) for _ in sigs]
     want = [rf.stream(l, r if ch == 2 else None) for rf, (l, r) in zip(refs, sigs)]
     for rf in refs:
@@ -246,7 +235,7 @@ def whole_streams(M, ch, sr, kb, sigs, label, fail, f32=False, resample=False, c
     base = 0
     for rec in launches:
         k = len(rec["streams"])
-        (check or check_launch)(rec, refs[base:base + k], label, fail)
+        check(rec, refs[base:base + k], label, fail)
         base += k
     if base != len(sigs):
         fail.append("%s: %d streams recorded, %d encoded" % (label, base, len(sigs)))
@@ -260,13 +249,13 @@ def stream_lengths(M, ch, sr, kb):
     return [0, 1, 575, 576, 1376, 1377, 12 * fs + 300, 13 * fs + 300]
 
 
-def shape_whole(M, fail, configs=None, check=None):
-    for j, (ch, sr, kb) in enumerate(configs or native_configs()):
+def shape_whole(M, fail, check):
+    for j, (ch, sr, kb) in enumerate(native_configs()):
         lens = stream_lengths(M, ch, sr, kb)
         for i, n in enumerate(lens):
             kind = K2_KINDS[(i + j) % len(K2_KINDS)]
             whole_streams(M, ch, sr, kb, [k2_signal(kind, n, 100 * j + i)], "whole %d/%d/%d n=%d %s" % (ch, sr, kb, n, kind), fail,
-                          check=check)
+                          check)
 
 
 BATCHES = [
@@ -277,11 +266,11 @@ BATCHES = [
 ]
 
 
-def shape_batches(M, fail, check=None):
+def shape_batches(M, fail, check):
     for (ch, sr, kb), lens in BATCHES:
         sigs = [k2_signal(K2_KINDS[i % len(K2_KINDS)], n, 300 + i) if i % 2 else make_signal("burst", n, sr, 300 + i)
                 for i, n in enumerate(lens)]
-        whole_streams(M, ch, sr, kb, sigs, "batch %d/%d/%d" % (ch, sr, kb), fail, check=check)
+        whole_streams(M, ch, sr, kb, sigs, "batch %d/%d/%d" % (ch, sr, kb), fail, check)
 
 
 def slice_of(c, pcm_base, n, nchunks=PCM_SLICES):
@@ -334,28 +323,13 @@ def slice_lengths(M, ch, sr, kb, nstreams, seed):
     raise AssertionError("no slicing found")
 
 
-def shape_slices(M, fail, check=None):
+def shape_slices(M, fail, check):
     for (ch, sr, kb), nstreams in (((2, 44100, 128), 1), ((1, 22050, 64), 3)):
         lens = slice_lengths(M, ch, sr, kb, nstreams, 7 + nstreams)
         sigs = [k2_signal("mixed", n, 500 + i) for i, n in enumerate(lens)]
-        launches = whole_streams(M, ch, sr, kb, sigs, "slices %d/%d/%d" % (ch, sr, kb), fail, check=check)
+        launches = whole_streams(M, ch, sr, kb, sigs, "slices %d/%d/%d" % (ch, sr, kb), fail, check)
         G = M.granules_per_frame(ch, sr, kb)
         want = len({slice_of(u, 0, n) for n in lens for u in range(-1, G * M.stream_frames(n, ch, sr, kb))})
         for rec in launches:
             if rec["k2_launches"] != want:
                 fail.append("slices %d/%d/%d: %d k_psy_analysis launches, %d slices hold units" % (ch, sr, kb, rec["k2_launches"], want))
-
-
-def main():
-    import lamejs_b200 as M
-
-    assert os.path.samefile(M.lib()._name, os.environ["MP3B200_LIB"])
-    fail = []
-    shape_whole(M, fail)
-    shape_batches(M, fail)
-    shape_slices(M, fail)
-    print(json.dumps({"fail": fail[:50], "nfail": len(fail)}))
-
-
-if __name__ == "__main__":
-    main()

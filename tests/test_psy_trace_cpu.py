@@ -1,6 +1,7 @@
 """The oracle's psy trace means what it says: its peaks, attack candidates and loudness are recomputed in plain numpy from the
-same PCM and tied to the values the encoder consumes (the ath_adjust of the frame trace).  tests/test_gpu_psy_rows.py
-compares the GPU's psy rows with this trace, so a trace that recorded the wrong thing would let a wrong kernel pass."""
+same PCM and tied to the values the encoder consumes (the ath_adjust of the frame trace).
+tests/test_gpu_front_end_rows.py compares the GPU's psy rows with this trace, so a trace that recorded the wrong thing would
+let a wrong kernel pass."""
 import ctypes
 
 import numpy as np
