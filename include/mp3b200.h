@@ -508,9 +508,12 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* t);
 /* Debug psy-row capture, off by default.  on != 0 clears the records and turns capture on for every thread and session;
  * 0 turns it off (the records stay until taken).  While it is on, each pipeline launch fills its front-end rows with a
  * poison pattern before the long-block analysis (float and double fields a quiet NaN, mask_idx 8, attack 0, both block-type
- * rows 1 = START), synchronises its stream after the attack pre-pass, after the short-block analysis and after the MDCT, and
- * records the rows there; a launch inside CUDA stream capture fails with MP3B200_ERR_CUDA.  Launches are numbered from 0 in
- * the order they start.  Each record is an int32[8] header and its payload:
+ * rows 1 = START) and its quantizer rows with finite values the quantizer can run on (xrq and xrpow 1.0f, sign masks
+ * 0xAAAAAAAA, quantised lines 1, prepared rows and side info of a long block with global_gain 1, frame states of stream 0
+ * frame 0 with OldValue 180 / CurrentStep 4 and valid 0), synchronises its stream after the attack pre-pass, after the
+ * short-block analysis, after the MDCT and after the quantizer, and records the rows there; a launch inside CUDA stream
+ * capture fails with MP3B200_ERR_CUDA.  Launches are numbered from 0 in the order they start.  Each record is an int32[8]
+ * header and its payload:
  *   {1, launch, stream, frame0, nframes, nch, G, row_bytes}: the stream's long rows u = -1 .. G nframes - 1, nch per unit
  *     (eb_l float[64], peaks float[9], loudness float, mask_idx uint8[64], attack uint8[4], one pad byte; row_bytes each)
  *   {2, launch, count, nch, G, k_psy_analysis launches, 0, row_bytes}: the short list, count int32 pairs (stream,
@@ -520,7 +523,12 @@ int mp3b200_debug_stages_ex(const mp3b200_debug_taps* t);
  *     the masking rows u = -1 .. n - 1, nch per unit (en_l float[22], thm_l float[22], en_s float[13][3],
  *     thm_s float[13][3]; row_bytes each; row u is what granule u + 1 uses), xr float[n][nch][576], the final block type
  *     int8[n][2] and the block type the psy call of the unit saw before it (int8[n][2]; both hold 2 per unit whatever nch),
- *     then zero bytes up to a multiple of 8 */
+ *     then zero bytes up to a multiple of 8
+ *   {4, launch, stream, frame0, nframes, nch, G, 0}: the stream's quantizer rows after the fixed point, with g = G nframes nch
+ *     granule-channels in (unit, channel) order: the row sizes int32[4] {frame state, prepared row, side info, 0}, the
+ *     frame states (QuantFrameState of k_quant.cuh, nframes rows), the prepared rows (GcPrep: xmin float[39], have, mnz,
+ *     block type, xrpow_max double; g rows), the side info (GranuleInfoDev; g rows), the quantised lines short[g][576],
+ *     xrq and xrpow float[g][576] (xr as the quantizer sees it and |xr|^(3/4)) and the sign masks uint32[g][18] */
 int mp3b200_debug_psy_capture(int on);
 /* Copies the records held (bytes) to buf and clears them when cap is large enough; returns their size either way. */
 int64_t mp3b200_debug_psy_take(void* buf, int64_t cap);

@@ -2142,7 +2142,9 @@ struct QuantBuffers {
                                      counter[2..Q_NCOUNTERS): task counters, one per launch */
 };
 #define Q_NCOUNTERS 256
-#define Q_REPAIR_BLOCKS 16
+#ifndef Q_REPAIR_BLOCKS
+#define Q_REPAIR_BLOCKS 16        /* blocks of each repair-stream kernel, and block slots the main stream leaves them */
+#endif
 enum { QE_START, QE_PREP, QE_S0, QE_O0, QE_F0, QE_S1, QE_MID, QE_O1, QE_F1, QE_PK, QE_COUNT };   /* timing event slots */
 
 /* The fixed-point loop on the device, so that no launch waits for the host: a graph of a memset (st[2] = 2) and a

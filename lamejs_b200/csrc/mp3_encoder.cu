@@ -570,11 +570,11 @@ int wait_legacy(ThreadCtx& c) {
 struct Rows { bool f32; int scale_applied; };
 constexpr Rows SCALED_F32 = {true, 0};
 
-/* Debug psy-row capture (mp3b200_debug_psy_capture).  While it is on, every pipeline launch poisons the front-end rows it
- * uses before k_psy_analysis, so that a row the launch forgets to write cannot pass for one written by an earlier launch, and
- * records them after k_attack_prepass (PsyUnit), after k_psy_short (the short list and its PsyShort rows) and after k_mdct
- * (block types, ATH adjustments, masking and xr).  The launch synchronises its stream at those points; with capture off it
- * does nothing at all. */
+/* Debug psy-row capture (mp3b200_debug_psy_capture).  While it is on, every pipeline launch poisons the front-end and
+ * quantizer rows it uses before k_psy_analysis, so that a row the launch forgets to write cannot pass for one written by an
+ * earlier launch, and records them after k_attack_prepass (PsyUnit), after k_psy_short (the short list and its PsyShort
+ * rows), after k_mdct (block types, ATH adjustments, masking and xr) and after the quantizer's fixed point (its frame states
+ * and hand-over rows).  The launch synchronises its stream at those points; with capture off it does nothing at all. */
 std::atomic<int> g_psy_capture{0};
 std::mutex g_psy_mu;                      /* guards g_psy_rec, g_psy_launch */
 std::vector<unsigned char> g_psy_rec;     /* records: int32[8] header + payload (include/mp3b200.h) */
@@ -588,9 +588,56 @@ void psy_rec_append(const int32_t (&h)[8], const void* a, size_t na, const void*
   if (nb) g_psy_rec.insert(g_psy_rec.end(), static_cast<const unsigned char*>(b), static_cast<const unsigned char*>(b) + nb);
 }
 
-/* Fills the launch's rows: floats with a quiet NaN, bytes with values that stay valid table indices (mask_idx 8, attack 0,
- * block types BT_START), so that reading an unwritten row changes results without ever indexing out of bounds.  bt_prev never
- * holds BT_START when written (the scan stores NORM, STOP or SHORT there). */
+/* The quantizer's rows of a launch (gcs granule-channels, nframes frame states), each value chosen so that a kernel reading
+ * an unwritten row runs on and changes what the record or the bytes show, without indexing out of bounds or looping forever:
+ *   xrq, xrpow  1.0f: finite and positive, so every adj43 index and every bin search stays in range; real rows are zeroed
+ *               above the analog silence and are rarely exactly 1.0 anywhere else
+ *   neg         0xAAAAAAAA: every other line negative, which flips the sign of half the packed lines
+ *   l3enc       1 on every line: counted and packed like a real quantised row, never all zero as a silent granule's is
+ *   prep        xmin 1.0f, have 1, mnz 575, block type NORM, xrpow_max 1.0: a granule with energy and valid long-block bands
+ *   ginfo       gi_init_w's long-block template over that prep, but global_gain 1 where the template has 210; every other
+ *               field 0, so part2_3_length 0 and table 0 everywhere (valid for the packer)
+ *   qstate      stream 0, rel_frame 0 (k_qstate_verify skips a first frame instead of reading row -1), every carried state
+ *               (180, 4) as at a stream's start, used0 0, valid 0, redo 0 */
+int q_poison(ThreadCtx& c, size_t gcs, long long nframes) {
+  if (!gcs) return 0;
+  std::vector<float> one(gcs * 576, 1.0f);
+  std::vector<unsigned> neg(gcs * 18, 0xAAAAAAAAu);
+  std::vector<short> ix(gcs * 576, 1);
+  GcPrep pr;
+  memset(&pr, 0, sizeof pr);
+  for (float& v : pr.xmin) v = 1.0f;
+  pr.have = 1; pr.mnz = 575; pr.block_type = BT_NORM; pr.xrpow_max = 1.0;
+  GranuleInfoDev gi;
+  memset(&gi, 0, sizeof gi);
+  gi.global_gain = 1; gi.block_type = BT_NORM;
+  gi.sfb_lmax = 21; gi.sfb_smin = 12; gi.psy_lmax = 21; gi.psymax = 21; gi.sfbmax = 21; gi.sfbdivide = 11;
+  gi.max_nonzero_coeff = 575; gi.xrpow_max = 1.0;
+  QuantFrameState qs;
+  memset(&qs, 0, sizeof qs);
+  for (int ch = 0; ch < 2; ch++) {
+    qs.in_old[ch] = qs.out_old[ch] = qs.bs_gain0[ch] = 180;
+    qs.in_step[ch] = qs.out_step[ch] = qs.bs_step0[ch] = 4;
+  }
+  std::vector<GcPrep> prs(gcs, pr);
+  std::vector<GranuleInfoDev> gis(gcs, gi);
+  std::vector<QuantFrameState> qss((size_t)nframes, qs);
+  CK(cudaMemcpyAsync(c.ws.xrq.p, one.data(), one.size() * sizeof(float), cudaMemcpyHostToDevice, c.st));
+  CK(cudaMemcpyAsync(c.ws.xrpow.p, one.data(), one.size() * sizeof(float), cudaMemcpyHostToDevice, c.st));
+  CK(cudaMemcpyAsync(c.ws.neg.p, neg.data(), neg.size() * sizeof(unsigned), cudaMemcpyHostToDevice, c.st));
+  CK(cudaMemcpyAsync(c.ws.l3enc.p, ix.data(), ix.size() * sizeof(short), cudaMemcpyHostToDevice, c.st));
+  CK(cudaMemcpyAsync(c.ws.prep.p, prs.data(), gcs * sizeof(GcPrep), cudaMemcpyHostToDevice, c.st));
+  CK(cudaMemcpyAsync(c.ws.ginfo.p, gis.data(), gcs * sizeof(GranuleInfoDev), cudaMemcpyHostToDevice, c.st));
+  CK(cudaMemcpyAsync(c.ws.qstate.p, qss.data(), qss.size() * sizeof(QuantFrameState), cudaMemcpyHostToDevice, c.st));
+  CK(cudaStreamSynchronize(c.st));
+  return 0;
+}
+
+/* Fills the launch's rows: front-end floats with a quiet NaN, bytes with values that stay valid table indices (mask_idx 8,
+ * attack 0, block types BT_START), so that reading an unwritten row changes results without ever indexing out of bounds.
+ * bt_prev never holds BT_START when written (the scan stores NORM, STOP or SHORT there).
+ * The quantizer's rows get finite values its kernels can run on (q_poison): a NaN or negative xrpow would index adj43 out of
+ * range, and a zero search step would never end a bin search. */
 int psy_poison(ThreadCtx& c, int G, long long total_frames, int S, int nch, int* launch) {
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
   CK(cudaStreamIsCapturing(c.st, &cs));
@@ -632,7 +679,7 @@ int psy_poison(ThreadCtx& c, int G, long long total_frames, int S, int nch, int*
   CK(cudaMemsetAsync(c.ws.bt_final.p, BT_START, units * 2, c.st));
   CK(cudaMemsetAsync(c.ws.bt_prev.p, BT_START, units * 2, c.st));
   CK(cudaStreamSynchronize(c.st));
-  return 0;
+  return q_poison(c, units * nch, total_frames);
 }
 
 /* After k_attack_prepass: each stream's rows u = -1 .. G nframes - 1 */
@@ -696,6 +743,44 @@ int psy_record_front(ThreadCtx& c, const StreamDesc* sds, int S, int nch, int G,
     }
     CK(cudaStreamSynchronize(c.st));
     const int32_t h[8] = {3, launch, z, sd.frame0, sd.nframes, nch, G, (int32_t)sizeof(PsyRatioDev)};
+    psy_rec_append(h, p.data(), p.size());
+  }
+  return 0;
+}
+
+/* After the quantizer's fixed point and k_qstate_commit: per stream, the row sizes int32[4] {QuantFrameState, GcPrep,
+ * GranuleInfoDev, 0}, its frames' QuantFrameState rows, then for its n nch granule-channels (n = G nframes) the GcPrep and
+ * GranuleInfoDev rows, l3enc short[576], xrq and xrpow float[576] and neg unsigned[18] of each (every size a multiple of 8).
+ * k_q_prepare's rows are never rewritten, so this one record sees what every later kernel read. */
+int q_record(ThreadCtx& c, const StreamDesc* sds, int S, int nch, int G, int launch) {
+  CK(cudaStreamSynchronize(c.st));
+  const int32_t sizes[4] = {(int32_t)sizeof(QuantFrameState), (int32_t)sizeof(GcPrep), (int32_t)sizeof(GranuleInfoDev), 0};
+  for (int z = 0; z < S; z++) {
+    const StreamDesc& sd = sds[z];
+    const size_t F = (size_t)sd.nframes, g = (size_t)G * sd.nframes * nch, g0 = (size_t)sd.unit_base * nch;
+    const size_t b_qs = F * sizeof(QuantFrameState), b_prep = g * sizeof(GcPrep), b_gi = g * sizeof(GranuleInfoDev);
+    const size_t b_ix = g * 576 * sizeof(short), b_row = g * 576 * sizeof(float), b_neg = g * 18 * sizeof(unsigned);
+    std::vector<unsigned char> p(sizeof sizes + b_qs + b_prep + b_gi + b_ix + 2 * b_row + b_neg);
+    unsigned char* q = p.data();
+    memcpy(q, sizes, sizeof sizes);
+    q += sizeof sizes;
+    if (F) {
+      CK(cudaMemcpyAsync(q, c.ws.qstate.p + sd.frame_base, b_qs, cudaMemcpyDeviceToHost, c.st));
+      q += b_qs;
+      CK(cudaMemcpyAsync(q, c.ws.prep.p + g0, b_prep, cudaMemcpyDeviceToHost, c.st));
+      q += b_prep;
+      CK(cudaMemcpyAsync(q, c.ws.ginfo.p + g0, b_gi, cudaMemcpyDeviceToHost, c.st));
+      q += b_gi;
+      CK(cudaMemcpyAsync(q, c.ws.l3enc.p + g0 * 576, b_ix, cudaMemcpyDeviceToHost, c.st));
+      q += b_ix;
+      CK(cudaMemcpyAsync(q, c.ws.xrq.p + g0 * 576, b_row, cudaMemcpyDeviceToHost, c.st));
+      q += b_row;
+      CK(cudaMemcpyAsync(q, c.ws.xrpow.p + g0 * 576, b_row, cudaMemcpyDeviceToHost, c.st));
+      q += b_row;
+      CK(cudaMemcpyAsync(q, c.ws.neg.p + g0 * 18, b_neg, cudaMemcpyDeviceToHost, c.st));
+    }
+    CK(cudaStreamSynchronize(c.st));
+    const int32_t h[8] = {4, launch, z, sd.frame0, sd.nframes, nch, G, 0};
     psy_rec_append(h, p.data(), p.size());
   }
   return 0;
@@ -862,6 +947,7 @@ int run_pipeline(ThreadCtx& c, Config* cfg, StreamDesc* h_streams, int S, const 
                    ev[5], c.evq, c.evq_pred, &g_launches, loop);
     if (!cached && loop.exec) lg.put(key, loop.exec);
     if (rc) { g_err = "quantizer stage failed: " + std::string(cudaGetErrorString(cudaGetLastError())); return rc; }
+    if (psy_launch >= 0 && (rc = q_record(c, h_streams, S, nch, cfg->host.mode_gr, psy_launch))) return rc;
   } else {
     CK(cudaEventRecord(ev[5], st));
   }

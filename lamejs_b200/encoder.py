@@ -1040,6 +1040,23 @@ PSY_SHORT_DTYPE = np.dtype({"names": ["ecb_s", "eb_s"], "formats": [(np.float64,
                             "offsets": [0, 1536], "itemsize": 2304})
 PSY_RATIO_DTYPE = np.dtype([("en_l", np.float32, 22), ("thm_l", np.float32, 22), ("en_s", np.float32, (13, 3)),
                             ("thm_s", np.float32, (13, 3))])
+# the quantizer's rows (k_quant.cuh: QuantFrameState, GcPrep, GranuleInfoDev)
+Q_STATE_DTYPE = np.dtype([("stream", np.int32), ("rel_frame", np.int32), ("in_old", np.int32, 2), ("in_step", np.int32, 2),
+                          ("out_old", np.int32, 2), ("out_step", np.int32, 2), ("bs_gain0", np.int32, 2), ("bs_step0", np.int32, 2),
+                          ("used0", np.int32, 2), ("bs_hash", np.uint64, (2, 2)), ("scfsi", np.int32, (2, 4)), ("redo", np.int32),
+                          ("valid", np.int32)], align=True)
+Q_PREP_DTYPE = np.dtype([("xmin", np.float32, 39), ("have", np.int32), ("mnz", np.int32), ("block_type", np.int32),
+                         ("xrpow_max", np.float64)], align=True)
+Q_GINFO_DTYPE = np.dtype([(k, np.int32) for k in ("global_gain", "part2_3_length", "part2_length", "big_values", "count1",
+                                                   "scalefac_compress")] +
+                         [("table_select", np.int32, 3)] +
+                         [(k, np.int32) for k in ("region0_count", "region1_count", "preflag", "scalefac_scale",
+                                                   "count1table_select", "block_type")] +
+                         [("subblock_gain", np.int32, 4)] +
+                         [(k, np.int32) for k in ("count1bits", "sfbmax", "sfbdivide", "sfb_lmax", "psymax", "psy_lmax", "sfb_smin",
+                                                   "max_nonzero_coeff")] +
+                         [("scalefac", np.int32, 39), ("slen", np.int32, 4), ("part_row", np.int32), ("pad_", np.int32),
+                          ("xrpow_max", np.float64)], align=True)
 
 
 class PsyCapture:
@@ -1047,15 +1064,18 @@ class PsyCapture:
     "streams": per stream of the launch {"z", "frame0", "nframes", "rows"} with rows PSY_UNIT_DTYPE[G nframes + 1][nch] for
     u = -1 .. G nframes - 1, and the rows after the MDCT: "bt" and "bt_prev" int8[G nframes][nch] (the final block type and
     the one the unit's psy call saw), "ath_psy" and "ath_q" float64[nframes], "ratio" PSY_RATIO_DTYPE[G nframes + 1][nch]
-    for u = -1 .. G nframes - 1 (row u is the masking granule u + 1 uses) and "xr" float32[G nframes][nch][576]; "short": the
-    short list as an int array [count][3] of (stream, u, channel) in list order; "short_rows": PSY_SHORT_DTYPE[count];
-    "k2_launches": how many k_psy_analysis launches the pipeline made."""
+    for u = -1 .. G nframes - 1 (row u is the masking granule u + 1 uses) and "xr" float32[G nframes][nch][576]; the
+    quantizer's rows after its fixed point (launches that ran it): "qstate" Q_STATE_DTYPE[nframes], and per unit and channel
+    "prep" Q_PREP_DTYPE and "ginfo" Q_GINFO_DTYPE [G nframes][nch], "l3enc" int16, "xrq" and "xrpow" float32
+    [G nframes][nch][576], "neg" uint32[G nframes][nch][18]; "short": the short list as an int array [count][3] of (stream,
+    u, channel) in list order; "short_rows": PSY_SHORT_DTYPE[count]; "k2_launches": how many k_psy_analysis launches the
+    pipeline made."""
 
     def __init__(self):
         self.launches = []
 
     def _parse(self, raw):
-        by, front = {}, {}
+        by, front, quant = {}, {}, {}
         off = 0
         while off < len(raw):
             h = np.frombuffer(raw, dtype=np.int32, count=8, offset=off)
@@ -1086,6 +1106,20 @@ class PsyCapture:
                     off += 2 * n
                 off += -(4 * n) % 8
                 front.setdefault(launch, {})[z] = s
+            elif kind == 4:
+                z, frame0, nframes, nch, G, _ = (int(v) for v in h[2:])
+                sizes = [int(v) for v in np.frombuffer(raw, dtype=np.int32, count=4, offset=off)]
+                assert sizes[:3] == [Q_STATE_DTYPE.itemsize, Q_PREP_DTYPE.itemsize, Q_GINFO_DTYPE.itemsize], sizes
+                off += 16
+                g = G * nframes * nch
+                s = {}
+                for k, dt, count, shape in (("qstate", Q_STATE_DTYPE, nframes, (nframes,)), ("prep", Q_PREP_DTYPE, g, (-1, nch)),
+                                            ("ginfo", Q_GINFO_DTYPE, g, (-1, nch)), ("l3enc", np.int16, g * 576, (-1, nch, 576)),
+                                            ("xrq", np.float32, g * 576, (-1, nch, 576)), ("xrpow", np.float32, g * 576, (-1, nch, 576)),
+                                            ("neg", np.uint32, g * 18, (-1, nch, 18))):
+                    s[k] = np.frombuffer(raw, dtype=dt, count=count, offset=off).reshape(shape).copy()
+                    off += count * np.dtype(dt).itemsize
+                quant.setdefault(launch, {})[z] = s
             else:
                 assert kind == 2, kind
                 count, nch, G, k2, _, rb = (int(v) for v in h[2:])
@@ -1100,15 +1134,17 @@ class PsyCapture:
             by[k]["streams"].sort(key=lambda s: s["z"])
             for s in by[k]["streams"]:
                 s.update(front.get(k, {}).get(s["z"], {}))
+                s.update(quant.get(k, {}).get(s["z"], {}))
             self.launches.append(by[k])
 
 
 @contextlib.contextmanager
 def debug_psy_capture():
     """Debug only: while the block runs, every pipeline launch (any thread, any session) poisons its front-end rows before
-    the long-block analysis (psy rows, short rows, subband slabs, masking, xr, ATH adjustments, block types) and records them
-    after the attack pre-pass, the short-block analysis and the MDCT (mp3b200_debug_psy_capture; each launch synchronises
-    its stream at those points).  Yields a PsyCapture, filled when the block ends."""
+    the long-block analysis (psy rows, short rows, subband slabs, masking, xr, ATH adjustments, block types, and the
+    quantizer's frame states and hand-over rows) and records them after the attack pre-pass, the short-block analysis, the
+    MDCT and the quantizer (mp3b200_debug_psy_capture; each launch synchronises its stream at those points).  Yields a
+    PsyCapture, filled when the block ends."""
     L = lib()
     L.mp3b200_debug_psy_capture.argtypes = [ctypes.c_int]
     L.mp3b200_debug_psy_take.argtypes = [ctypes.c_void_p, ctypes.c_int64]

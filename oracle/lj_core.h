@@ -126,6 +126,17 @@ struct LjQuantTrace {
   int   old_value_mid[2], cur_step_mid[2];   /* MPEG-1: OldValue / CurrentStep after gr0, where gr1's search starts; 0 for LSF */
 };
 
+/* per-frame record of the rows lj_iteration_loop hands outer_loop (lj_set_quant_row_trace), row k belonging to LjQuantTrace
+ * row k.  A record of its own, so that LjQuantTrace, which callers size their buffers by, keeps its layout.
+ *   xrq    cod_info.xr as outer_loop receives it: short blocks in the quantizer's band order, analog silence zeroed
+ *   xrpow  init_xrpow's |xr|^(3/4), every line (the rate loop rescales it later)
+ *   have   init_xrpow's result: 0 for a granule without energy, which skips calc_xmin and outer_loop */
+struct LjQuantRowTrace {
+  float xrq[2][2][576];
+  float xrpow[2][2][576];
+  int   have[2][2];
+};
+
 /* per-frame record of the psy model's per-granule analysis (lj_set_psy_trace), [gr][ch] = psy call G k + gr of frame k.  A
  * record of its own, like LjQuantTrace.  Only the first npart_l / npart_s partitions are defined (0 beyond).
  *   eb_l, mask_idx_l  calc_energy's partition energies and calc_mask_index_l's indices

@@ -102,6 +102,7 @@ struct LjEnc {
   LjFrameTrace* trace; int trace_cap, trace_n;
   LjQuantTrace* qtrace; int qtrace_cap;
   LjQuantTrace* qtrace_cur;      /* the quantizer row of the frame being encoded while tracing, else NULL (lj_quant.cpp) */
+  LjQuantRowTrace* qrtrace; int qrtrace_cap;   /* rows beside qtrace's (lj_set_quant_row_trace), or NULL */
   LjPsyTrace* ptrace; int ptrace_cap, ptrace_n;
   LjPsyTrace* ptrace_cur;        /* the psy row of the frame being encoded while tracing, else NULL (lj_psy_trace_*) */
   LjPsyBlockTrace* pbtrace; int pbtrace_cap;   /* rows beside ptrace's (lj_set_psy_block_trace), or NULL */
@@ -136,6 +137,10 @@ void lj_psymodel_init(LjEnc* e);
 void lj_psy_trace_attacks(LjEnc* e, int gr, int chn, const F32* en_subshort, const int* ns_attacks);
 void lj_psy_trace_long(LjEnc* e, int gr, int chn, const F32* eb_l, const int* mask_idx_l);
 void lj_psy_trace_short(LjEnc* e, int gr, int chn, int sblock, const F32* eb_s);
+/* lj_init.cpp: the hand-over rows of granule (gr, ch) beside the quant trace's row t (LjQuantRowTrace); a no-op when t is
+ * NULL (the trace is off) or no row trace is set.  Kept out of lj_quant.cpp for the same reason; its caller is a tap line
+ * there. */
+void lj_quant_trace_rows(LjEnc* e, const LjQuantTrace* t, int gr, int ch, const GrInfo* cod_info, const F32* xrpow, bool have);
 double lj_ATHformula(double f, const LjEnc* e);
 /* lj_quant.cpp */
 void lj_iteration_init(LjEnc* e);

@@ -354,6 +354,15 @@ void lj_psy_trace_short(LjEnc* e, int gr, int chn, int sblock, const F32* eb_s) 
   if (!t || chn >= 2) return;
   for (int b = 0; b < e->npart_s; b++) { t->eb_s[gr][chn][sblock][b] = eb_s[b].v; t->ecb_s[gr][chn][sblock][b] = e->nb_s1[chn][b].v; }
 }
+/* the quantizer trace (lj_set_quant_trace): what lj_iteration_loop hands outer_loop, after init_xrpow */
+void lj_quant_trace_rows(LjEnc* e, const LjQuantTrace* t, int gr, int ch, const GrInfo* cod_info, const F32* xrpow, bool have) {
+  if (!t || ch >= 2) return;
+  const int row = (int)(t - e->qtrace);
+  if (!e->qrtrace || row >= e->qrtrace_cap) return;
+  LjQuantRowTrace* const r = &e->qrtrace[row];
+  for (int i = 0; i < 576; i++) { r->xrq[gr][ch][i] = cod_info->xr[i].v; r->xrpow[gr][ch][i] = xrpow[i].v; }
+  r->have[gr][ch] = have ? 1 : 0;
+}
 
 /* Encoder.js:287-326 */
 static void encode_frame_init(LjEnc* e) {
@@ -449,6 +458,7 @@ static int encode_mp3_frame(LjEnc* e, uint8_t* mp3buf, int mp3buf_size) {
   }
   e->qtrace_cur = (tracing && e->qtrace && e->trace_n < e->qtrace_cap) ? &e->qtrace[e->trace_n] : NULL;
   if (e->qtrace_cur) memset(e->qtrace_cur, 0, sizeof *e->qtrace_cur);
+  if (e->qtrace_cur && e->qrtrace && e->trace_n < e->qrtrace_cap) memset(&e->qrtrace[e->trace_n], 0, sizeof *e->qrtrace);
   lj_iteration_loop(e, pe_use, ms_ener_ratio, masking);
   e->qtrace_cur = NULL;
   lj_format_bitstream(e);
@@ -724,6 +734,10 @@ void lj_set_trace(LjEnc* e, LjFrameTrace* buf, int cap) { e->trace = buf; e->tra
 /* quantizer rows next to the frame trace: row k is filled together with lj_set_trace's row k (call it after lj_set_trace) */
 void lj_set_quant_trace(LjEnc* e, LjQuantTrace* buf, int cap) { e->qtrace = buf; e->qtrace_cap = cap; }
 int lj_quant_trace_size(void) { return (int)sizeof(LjQuantTrace); }
+/* the rows lj_iteration_loop hands outer_loop, beside the quantizer rows: row k is filled together with lj_set_quant_trace's
+ * row k (call it after lj_set_quant_trace) */
+void lj_set_quant_row_trace(LjEnc* e, LjQuantRowTrace* buf, int cap) { e->qrtrace = buf; e->qrtrace_cap = cap; }
+int lj_quant_row_trace_size(void) { return (int)sizeof(LjQuantRowTrace); }
 /* psy rows, one per frame encoded from now on (independent of lj_set_trace) */
 void lj_set_psy_trace(LjEnc* e, LjPsyTrace* buf, int cap) {
   e->ptrace = buf; e->ptrace_cap = cap; e->ptrace_n = 0;

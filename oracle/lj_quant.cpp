@@ -1364,6 +1364,7 @@ void lj_iteration_loop(LjEnc* e, double pe[2][2], const double* ms_ener_ratio, P
         t->max_nonzero_coeff[gr][ch] = cod_info->max_nonzero_coeff;
         t->xrpow_max[gr][ch] = cod_info->xrpow_max;
         for (int i = 0; i < SFBMAX; i++) t->xmin[gr][ch][i] = (have && i < cod_info->psymax) ? l3_xmin[i].v : 0.0f;
+        lj_quant_trace_rows(e, e->qtrace_cur, gr, ch, cod_info, xrpow, have);
       }
       if (have) outer_loop(e, cod_info, l3_xmin, xrpow, ch, targ_bits[ch]);
       iteration_finish_one(e, gr, ch);

@@ -13,8 +13,11 @@ What is compared, for stream unit u (absolute granule c = G frame0 + u) of a lau
   last row       (u = G nframes - 1) in all 122 floats: the oracle's gfc.en / gfc.thm after the call, the masking handed on
   xr[u]          the frame trace's xr of granule c, all 576 lines
 
-Run as a script (MP3B200_LIB set to a variant build) it checks every row (check_rows) in the whole-stream, ragged-batch and
-upload-slice shapes and prints one JSON line {"fail": [first differences], "nfail": n}."""
+check_rows also runs the psy rows' check before these and the quantizer rows' check after them (tests/quant_rows.py).
+
+Run as a script (MP3B200_LIB set to a variant build) it checks every row (check_rows) in the shapes named on its command line
+(SHAPES: whole, batches, slices, edges; the first three by default) and prints one JSON line {"fail": [first differences],
+"nfail": n, "frames": .., "repaired": ..} (main)."""
 import json
 import os
 import sys
@@ -26,6 +29,7 @@ sys.path.insert(0, os.path.dirname(HERE))
 sys.path.insert(0, HERE)
 
 import psy_rows as P  # noqa: E402
+import quant_rows as Q  # noqa: E402
 
 BT_START, BT_SHORT = 1, 2
 ATH_START = 0.01            # ATH.adjust before the first adjust_ATH (lamejs's start value)
@@ -109,9 +113,11 @@ def check_front(rec, refs, label, fail):
 
 
 def check_rows(rec, refs, label, fail):
-    """every front-end row of one launch: the psy rows and the short list (psy_rows.check_launch), then the rows after k_mdct"""
+    """every row of one launch: the psy rows and the short list (psy_rows.check_launch), the rows after k_mdct, then the
+    quantizer's rows (quant_rows.check_quant)"""
     P.check_launch(rec, refs, label, fail)
     check_front(rec, refs, label, fail)
+    Q.check_quant(rec, refs, label, fail)
 
 
 def read_rows(bt):
@@ -122,8 +128,9 @@ def read_rows(bt):
 
 def check_unpoisoned(rec, label, fail, halo_start=False):
     """Without an oracle (a seeked handle): every row the launch writes holds no NaN and no block type the scan never stores
-    there; with halo_start, the halo row is the stream-start masking (1e20) and the first frame's psy calls saw ATH.adjust
-    0.01."""
+    there, and no quantizer row holds its poison (quant_rows.check_unpoisoned); with halo_start, the halo row is the
+    stream-start masking (1e20) and the first frame's psy calls saw ATH.adjust 0.01."""
+    Q.check_unpoisoned(rec, label, fail)
     for s in rec["streams"]:
         z, n = s["z"], s["G"] * s["nframes"]
         if not n:
@@ -142,16 +149,40 @@ def check_unpoisoned(rec, label, fail, halo_start=False):
                 fail.append("%s: stream %d: %s" % (label, z, what))
 
 
-def main():
+def shape_edges(M, fail, check):
+    """every case of the edge corpus as one whole stream"""
+    import edge_signals
+
+    for case in edge_signals.CASES:
+        l, r = edge_signals.signal(case)
+        P.whole_streams(M, case[1], case[2], case[3], [(l, r)], edge_signals.case_id(case), fail, check)
+
+
+SHAPES = {"whole": P.shape_whole, "batches": P.shape_batches, "slices": P.shape_slices, "edges": shape_edges}
+Q_R0_ANY = 3                # QuantFrameState.redo: gr0's rate loop was redone on the repair stream (k_quant.cuh)
+
+
+def main(shapes=("whole", "batches", "slices")):
+    """checks every row of every launch in `shapes` (names of SHAPES) and prints one JSON line: the first differences, their
+    number, and over the frames after the first of each MPEG-1 stream, how many there are and how many ended with gr0
+    repaired (redo & Q_R0_ANY)"""
     import lamejs_b200 as M
 
     assert os.path.samefile(M.lib()._name, os.environ["MP3B200_LIB"])
     fail = []
-    P.shape_whole(M, fail, check_rows)
-    P.shape_batches(M, fail, check_rows)
-    P.shape_slices(M, fail, check_rows)
-    print(json.dumps({"fail": fail[:50], "nfail": len(fail)}))
+    stats = {"frames": 0, "repaired": 0}
+
+    def check(rec, refs, label, fail):
+        check_rows(rec, refs, label, fail)
+        for s in rec["streams"]:
+            if s["G"] == 2 and "qstate" in s:
+                q = s["qstate"][1:]
+                stats["frames"] += len(q)
+                stats["repaired"] += int((q["redo"] & Q_R0_ANY != 0).sum())
+    for name in shapes:
+        SHAPES[name](M, fail, check)
+    print(json.dumps(dict(stats, fail=fail[:50], nfail=len(fail))))
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1:] or ("whole", "batches", "slices"))

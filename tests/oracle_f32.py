@@ -72,6 +72,7 @@ def bind(so):
     assert L.lj_trace_size() == oracle_lib.TRACE_DTYPE.itemsize
     assert L.lj_state_size() == oracle_lib.STATE_DTYPE.itemsize
     oracle_lib.bind_psy_trace(L)
+    oracle_lib.bind_quant_row_trace(L)
     return L
 
 
@@ -91,12 +92,7 @@ class Encoder:
         self.channels = channels
         self.psy = oracle_lib.PsyTraceRows(self.L, self.h) if psy_trace else None
         self.tag_on = bool(write_vbr_tag) and self.L.lj_enable_vbr_tag(self.h) == 1
-        self.trace = self.qtrace = None
-        if trace_frames:
-            self.trace = np.zeros(trace_frames, dtype=oracle_lib.TRACE_DTYPE)
-            self.qtrace = np.zeros(trace_frames, dtype=oracle_lib.QTRACE_DTYPE)
-            self.L.lj_set_trace(self.h, self.trace.ctypes.data, trace_frames)
-            self.L.lj_set_quant_trace(self.h, self.qtrace.ctypes.data, trace_frames)
+        self.trace, self.qtrace, self.qrtrace = oracle_lib.set_traces(self.L, self.h, trace_frames) if trace_frames else (None,) * 3
 
     def encode_buffer(self, left, right=None):
         if right is None or self.channels == 1:
@@ -141,12 +137,7 @@ class Encoder:
         return s
 
     def traces(self):
-        n = self.L.lj_trace_count(self.h)
-        out = np.empty(n, dtype=oracle_lib.FULL_TRACE_DTYPE)
-        for rec in (self.trace, self.qtrace):
-            for k in rec.dtype.names:
-                out[k] = rec[k][:n]
-        return out
+        return oracle_lib.merged_traces(self.L, self.h, (self.trace, self.qtrace, self.qrtrace))
 
     def close(self):
         if self.h:

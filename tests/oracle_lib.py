@@ -60,6 +60,17 @@ QTRACE_DTYPE = np.dtype(
     align=True,
 )
 
+# lj_set_quant_row_trace: beside each QTRACE_DTYPE row, the rows lj_iteration_loop hands outer_loop
+QROW_TRACE_DTYPE = np.dtype(
+    [
+        ("xrq", np.float32, (2, 2, 576)),                 # cod_info.xr as outer_loop receives it (short blocks reordered,
+                                                          # analog silence zeroed)
+        ("xrpow", np.float32, (2, 2, 576)),               # init_xrpow's rows
+        ("have", np.int32, (2, 2)),                       # init_xrpow's result: the granule has energy
+    ],
+    align=True,
+)
+
 # lj_set_psy_trace: the psy model's per-granule analysis, one row per frame, [gr][ch] = psy call G k + gr of frame k; only the
 # first npart_l / npart_s partitions are defined
 PSY_TRACE_DTYPE = np.dtype(
@@ -78,9 +89,8 @@ PSY_TRACE_DTYPE = np.dtype(
 # lj_set_psy_block_trace: beside each psy row, blocktype_old as each psy call found it ([gr][ch]), before block_type_set
 PSY_BLOCK_TRACE_DTYPE = np.dtype([("blocktype_old", np.int32, (2, 2))])
 
-# what OracleEncoder.traces() returns: the fields of both records
-FULL_TRACE_DTYPE = np.dtype([(n, TRACE_DTYPE.fields[n][0]) for n in TRACE_DTYPE.names] +
-                            [(n, QTRACE_DTYPE.fields[n][0]) for n in QTRACE_DTYPE.names])
+# what OracleEncoder.traces() returns: the fields of the three records
+FULL_TRACE_DTYPE = np.dtype([(n, d.fields[n][0]) for d in (TRACE_DTYPE, QTRACE_DTYPE, QROW_TRACE_DTYPE) for n in d.names])
 
 # lj_get_state: what an encoder carries from one call to the next
 STATE_DTYPE = np.dtype(
@@ -145,8 +155,35 @@ def lib():
         assert L.lj_quant_trace_size() == QTRACE_DTYPE.itemsize, (L.lj_quant_trace_size(), QTRACE_DTYPE.itemsize)
         assert L.lj_state_size() == STATE_DTYPE.itemsize, (L.lj_state_size(), STATE_DTYPE.itemsize)
         bind_psy_trace(L)
+        bind_quant_row_trace(L)
         _lib = L
     return _lib
+
+
+def bind_quant_row_trace(L):
+    """ctypes signature of the quantizer's row trace (the oracle's library or the Float32 build of its sources)"""
+    L.lj_set_quant_row_trace.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]
+    assert L.lj_quant_row_trace_size() == QROW_TRACE_DTYPE.itemsize, (L.lj_quant_row_trace_size(), QROW_TRACE_DTYPE.itemsize)
+
+
+def set_traces(L, h, trace_frames):
+    """the frame, quantizer and quantizer row traces of encoder h, trace_frames rows each (the three records of traces())"""
+    recs = (np.zeros(trace_frames, dtype=TRACE_DTYPE), np.zeros(trace_frames, dtype=QTRACE_DTYPE),
+            np.zeros(trace_frames, dtype=QROW_TRACE_DTYPE))
+    L.lj_set_trace(h, recs[0].ctypes.data, trace_frames)
+    L.lj_set_quant_trace(h, recs[1].ctypes.data, trace_frames)
+    L.lj_set_quant_row_trace(h, recs[2].ctypes.data, trace_frames)
+    return recs
+
+
+def merged_traces(L, h, recs):
+    """the traced frames so far: FULL_TRACE_DTYPE rows (the records of set_traces side by side)"""
+    n = L.lj_trace_count(h)
+    out = np.empty(n, dtype=FULL_TRACE_DTYPE)
+    for rec in recs:
+        for k in rec.dtype.names:
+            out[k] = rec[k][:n]
+    return out
 
 
 def bind_psy_trace(L):
@@ -237,12 +274,7 @@ class OracleEncoder:
         elif reservoir:                    # gfp.disable_reservoir = false (SURVEY 8(f2); Mp3Encoder never does this)
             assert self.L.lj_enable_reservoir(self.h) == 0
         self.tag_on = bool(write_vbr_tag) and self.L.lj_enable_vbr_tag(self.h) == 1   # gfp.bWriteVbrTag (InitVbrTag may refuse)
-        self.trace = self.qtrace = None
-        if trace_frames:
-            self.trace = np.zeros(trace_frames, dtype=TRACE_DTYPE)
-            self.qtrace = np.zeros(trace_frames, dtype=QTRACE_DTYPE)
-            self.L.lj_set_trace(self.h, self.trace.ctypes.data, trace_frames)
-            self.L.lj_set_quant_trace(self.h, self.qtrace.ctypes.data, trace_frames)
+        self.trace, self.qtrace, self.qrtrace = set_traces(self.L, self.h, trace_frames) if trace_frames else (None,) * 3
 
     def encode_buffer(self, left, right=None):
         left = np.ascontiguousarray(left, dtype=np.int16)
@@ -264,13 +296,8 @@ class OracleEncoder:
         return buf[:k].tobytes()
 
     def traces(self):
-        """the traced frames so far: FULL_TRACE_DTYPE rows (the frame trace and the quantizer trace side by side)"""
-        n = self.L.lj_trace_count(self.h)
-        out = np.empty(n, dtype=FULL_TRACE_DTYPE)
-        for rec in (self.trace, self.qtrace):
-            for k in rec.dtype.names:
-                out[k] = rec[k][:n]
-        return out
+        """the traced frames so far: FULL_TRACE_DTYPE rows (the frame trace and the quantizer traces side by side)"""
+        return merged_traces(self.L, self.h, (self.trace, self.qtrace, self.qrtrace))
 
     def psy_traces(self):
         """every psy row since the encoder was made (PSY_TRACE_DTYPE, one per frame), across all calls"""
